@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- whole-job throughput of the B200 baseline-JPEG decode path on BASELINE.json's metric.
+"""bench.py -- whole-job throughput of the H100 baseline-JPEG decode path on BASELINE.json's metric.
 
     python bench.py --gpus N --steps K --warmup W            (N > 1: launched by torch.distributed.run)
     python bench.py --impl reference --gpus N --steps K --warmup W
@@ -9,9 +9,10 @@
 Workloads (config.workload; tools/bench_inputs.py): the synthetic source images S(w,h,seed) of SURVEY.md 8d encoded by the
 REFERENCE ENCODER (oracle/_ref/jpeg, named in config.encoder; the repo's own generator only where that binary is absent),
 `--distinct` distinct frames tiled over the batch.
-  cfg3 (default): 3840x2160 4:2:0 q75 baseline, DRI = 240.  One step = one pass of the hot path over 840 frames per GPU
-        (840 x 135 restart intervals = one full wave of the persistent entropy kernel); cfg3's 4096-frame batch is 4.9 steps
-        of one GPU.  Weak scaling (840 frames per GPU per step) unless --global-batch is given.
+  cfg3 (default): 3840x2160 4:2:0 q75 baseline, DRI = 240.  One step = one pass of the hot path over 750 frames per GPU
+        (750 x 135 restart intervals = one full wave of the persistent entropy kernel: 132 SMs x 768 lanes on an H100; 840
+        frames, 1.12 waves, measured 11 % fewer frames/s); cfg3's 4096-frame batch is 5.5 steps of one GPU.  Weak scaling (750
+        frames per GPU per step) unless --global-batch is given.
   cfg2: 1920x1080 4:2:0 q75, DRI = 120, 4096 frames per step on one GPU (BASELINE configs[1]).
   cfg4: 3840x2160 4:2:0 q75 progressive (ten scans), 1024 frames per step on one GPU (BASELINE configs[3]).
   cfg3n: cfg3 without restart markers (DRI-less streams).
@@ -29,7 +30,6 @@ roofline: the dominant stage by time. Reconstruction: algorithmic bytes = 128 B 
          over its CUDA-event duration against MEASURED_PEAKS.json hbm_gbs, plus `int32`: the same launches against the
          measured int32 issue rate (b200jpg_microbench_int32), the roofline north_star names for this stage.
          roofline_entropy: stage a (unstuff + entropy kernels), algorithmic bytes = ECS bytes + 128 B x stored blocks.
-         `traffic` = DRAM bytes per launch measured by ncu (profiles/), scaled from the per-frame figure of the captured run.
 cpu_baseline / --impl reference: the unmodified reference (oracle/_ref/refharness: public API, memory hook, 8-row stripes)
          as forked worker processes on a bounded sample of the same frames; reports the processes used, the physical cores,
          CPU model, affinity and cgroup quota of the box, and the parallelism the box actually delivered.
@@ -50,18 +50,12 @@ if ROOT not in sys.path:
 
 from tools import bench_inputs  # noqa: E402
 
-DEFAULT_FRAMES = {"cfg3": 840, "cfg2": 4096, "cfg4": 1024, "cfg3n": 840, "cfg2n": 4096, "cfg1": 8192, "cfg5": 24}
-# DRAM bytes per cfg3 frame measured with ncu --set full (dram__bytes_read.sum + dram__bytes_write.sum); see profiles/
-NCU_DRAM_BYTES_PER_FRAME = {"cfg3": {"entropy": None, "recon": None}}
-try:
-    NCU_DRAM_BYTES_PER_FRAME.update(json.load(open(os.path.join(ROOT, "profiles", "dram_bytes_per_frame.json"))))
-except Exception:
-    pass
+DEFAULT_FRAMES = {"cfg3": 750, "cfg2": 4096, "cfg4": 1024, "cfg3n": 750, "cfg2n": 4096, "cfg1": 8192, "cfg5": 24}
 INT_OPS_PER_PIXEL_420 = 520e6 / (3840 * 2160)  # SURVEY.md 8d: IDCT 205 M + upsample 133 M + colour 182 M per 4K 4:2:0 frame
 
 
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (B200_PROFILING.md): NVML polled every 5 ms from a
+    """SM clock and throttle reasons sampled DURING the timed region: NVML polled every 5 ms from a
     thread (nvidia-smi's loop mode needs seconds to deliver its first line -- longer than a timed region of a few steps)."""
 
     def __init__(self, index):
@@ -72,16 +66,9 @@ class ClockSampler:
         self.thread = None
         self.max_mhz = None
 
-    def _handle(self):
-        import pynvml
-        pynvml.nvmlInit()
-        vis = os.environ.get("CUDA_VISIBLE_DEVICES")
-        phys = int(vis.split(",")[self.index]) if vis and vis.split(",")[self.index].isdigit() else self.index
-        return pynvml, pynvml.nvmlDeviceGetHandleByIndex(phys)
-
     def start(self):
         try:
-            nv, h = self._handle()
+            nv, h = nvml_handle(self.index)
             self.max_mhz = float(nv.nvmlDeviceGetMaxClockInfo(h, nv.NVML_CLOCK_SM))
         except Exception:
             return
@@ -114,14 +101,35 @@ class ClockSampler:
                 "reasons": sorted(self.reasons), "samples": len(self.samples), "how": "NVML, 5 ms period, during the timed region"}
 
 
+def nvml_handle(index):
+    """(pynvml, NVML handle) of CUDA device `index`, matched by UUID: CUDA_VISIBLE_DEVICES and CUDA_DEVICE_ORDER can make CUDA's
+    numbering differ from NVML's."""
+    import pynvml
+    import torch
+    pynvml.nvmlInit()
+    return pynvml, pynvml.nvmlDeviceGetHandleByUUID("GPU-%s" % torch.cuda.get_device_properties(index).uuid)
+
+
+def gpu_facts(index):
+    """The card the numbers were measured on: its name and power limit (a card limited below 700 W runs at lower clocks)."""
+    import torch
+    facts = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        nv, h = nvml_handle(index)
+        facts["power_limit_w"] = nv.nvmlDeviceGetPowerManagementLimit(h) / 1000.0
+    except Exception:
+        pass
+    return facts
+
+
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         try:
-            return json.load(open(p)), "measured"
+            return json.load(open(p)), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
         except Exception:
             pass
-    return {"hbm_gbs": 6650.0}, "fallback"
+    return {"hbm_gbs": 3350.0}, "H100 SXM data sheet, not measured"
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -242,12 +250,8 @@ def bind_to_gpu_numa_node(index):
     if os.environ.get("B200JPG_NO_AFFINITY"):
         return "off"
     try:
-        import pynvml
-        pynvml.nvmlInit()
-        vis = os.environ.get("CUDA_VISIBLE_DEVICES")
-        phys = int(vis.split(",")[index]) if vis and vis.split(",")[index].isdigit() else index
-        h = pynvml.nvmlDeviceGetHandleByIndex(phys)
-        words = pynvml.nvmlDeviceGetCpuAffinity(h, (os.cpu_count() + 63) // 64)
+        nv, h = nvml_handle(index)
+        words = nv.nvmlDeviceGetCpuAffinity(h, (os.cpu_count() + 63) // 64)
         cpus = [64 * w + b for w, m in enumerate(words) for b in range(64) if (m >> b) & 1]
         if cpus:
             os.sched_setaffinity(0, cpus)
@@ -255,6 +259,31 @@ def bind_to_gpu_numa_node(index):
     except Exception as e:  # no NVML, no permission: run unpinned
         return "unavailable: %s" % type(e).__name__
     return "none"
+
+
+def dump_outputs(path, dec, out, sampled_frames=16, samples_per_frame=1 << 18, seed=0):
+    """The samples the last timed step decoded, for comparing two builds output for output. A 4K frame alone is 25 MB, so:
+    frame_sums.npy [frames, 2] float64 = per frame the exact sum and sum of squares of all its samples;
+    frame_sample.npy [k, samples_per_frame] float32 = samples at seeded positions of k seeded frames, whose indices are in
+    frame_sample_index.npy (float64)."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    torch.cuda.synchronize()
+    sums = np.zeros((dec.n, 2), dtype=np.float64)
+    for i in range(dec.n):
+        v = dec.frame_view(out, i).reshape(-1).to(torch.int64)
+        sums[i] = (float(v.sum()), float((v * v).sum()))
+    rng = np.random.default_rng(seed)
+    picks = np.sort(rng.choice(dec.n, size=min(sampled_frames, dec.n), replace=False))
+    sample = np.zeros((len(picks), samples_per_frame), dtype=np.float32)
+    for row, i in enumerate(picks):
+        v = dec.frame_view(out, int(i)).reshape(-1)
+        pos = torch.from_numpy(rng.integers(0, v.numel(), size=samples_per_frame)).to(v.device)
+        sample[row] = v[pos].float().cpu().numpy()
+    np.save(os.path.join(path, "frame_sums.npy"), sums)
+    np.save(os.path.join(path, "frame_sample.npy"), sample)
+    np.save(os.path.join(path, "frame_sample_index.npy"), picks.astype(np.float64))
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -274,7 +303,12 @@ def main():
     ap.add_argument("--p2d-chunks", type=int, default=2, help="pinned_to_device_rgb: chunks per step (each: H2D + index + kernels on its own stream)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="write what the last timed step decoded (per-frame sums and a fixed seeded sample of samples) as DIR/*.npy; "
+                         "with several GPUs, rank 0's shard")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -293,7 +327,7 @@ def main():
     mb_codestream = {"cfg2": 0.37, "cfg2n": 0.37, "cfg1": 0.25, "cfg5": 54.0}.get(args.workload, 1.45)
     config = {"workload": desc, "encoder": bench_inputs.encoder_name(args.workload), "frames_per_gpu": nf, "global_batch": global_batch,
               "distinct_frames": args.distinct, "parallelism": "frames sharded over %d GPU(s), no data-path collective" % world,
-              "l2": "inputs larger than L2 (no flush needed): about %.1f GB codestreams + %.1f GB coefficients per step vs 126 MB L2"
+              "l2": "inputs larger than L2 (no flush needed): about %.1f GB codestreams + %.1f GB coefficients per step vs 50 MB L2"
                     % (nf * mb_codestream * 1e-3, nf * W * H * 3e-9)}
 
     if args.impl == "reference":
@@ -328,6 +362,7 @@ def main():
     from libjpeg_b200 import native
     assert torch.cuda.is_available(), "bench.py needs a CUDA device (there is no CPU fallback)"
     torch.cuda.set_device(local_rank)
+    config["gpu"] = gpu_facts(local_rank)
     config["cpu_affinity"] = bind_to_gpu_numa_node(local_rank)
     dist = None
     if world > 1:
@@ -381,6 +416,8 @@ def main():
     barrier()
     clocks = sampler.stop()
     total_ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dec, out)
     t = torch.tensor([total_ms], device="cuda")
     if dist is not None:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -421,14 +458,12 @@ def main():
     uns = statistics.mean(uns_ms)
 
     peaks, peak_kind = measured_peaks()
-    ncu = NCU_DRAM_BYTES_PER_FRAME.get(args.workload, {})
     algo_a = dec.ecs_bytes + 128 * dec.stored_blocks
     roof_a = {"bound": "hbm", "kernel": "stage a = unstuff_kernel + %s" % ("pf_dc_kernel + pf_ac_kernel per component (all scans of a block in one pass)" if PROG else
                                                                ("unstuff_long_kernel + spec_sync_kernel + entropy_decode_kernel<indexed>" if args.workload.endswith("n") else "entropy_decode_kernel")),
               "ms_unstuff": uns, "ms_decode": ent - uns,
               "achieved": algo_a / (ent * 1e-3) / 1e9, "peak": peaks["hbm_gbs"],
-              "peak_source": peak_kind + " (MEASURED_PEAKS.json hbm_gbs, burst copy)", "unit": "GB/s",
-              "traffic": ncu["entropy"] * nf if ncu.get("entropy") else None,
+              "peak_source": peak_kind, "unit": "GB/s",
               "algorithmic_bytes_per_launch": algo_a, "ms_per_launch": ent, "share_of_step": ent / (ent + rec)}
     roof_a["frac"] = roof_a["achieved"] / roof_a["peak"]
     import ctypes
@@ -440,8 +475,7 @@ def main():
     roof_b = {"bound": "hbm", "kernel": ("stage b = idct_planes_kernel<int> of base + residual image, generic_reconstruct_kernel: upsampling + JPEG XT merge + store"
                                          if args.workload == "cfg5" else "stage b = reconstruction kernel(s): IDCT + upsampling + colour + store"),
               "achieved": algo_b / (rec * 1e-3) / 1e9, "peak": peaks["hbm_gbs"],
-              "peak_source": peak_kind + " (MEASURED_PEAKS.json hbm_gbs, burst copy)", "unit": "GB/s",
-              "traffic": ncu["recon"] * nf if ncu.get("recon") else None,
+              "peak_source": peak_kind, "unit": "GB/s",
               "algorithmic_bytes_per_launch": algo_b, "ms_per_launch": rec, "share_of_step": rec / (ent + rec),
               "int32": {"unit": "Gop/s", "achieved": int_ops / (rec * 1e-3) / 1e9, "peak": int_peak,
                         "peak_source": "measured here: b200jpg_microbench_int32 (imad %.0f, alu %.0f, mix %.0f Gop/s; multiply-add = 2 ops)"
@@ -479,7 +513,7 @@ def main():
         for _ in range(2):
             p2d_step()
         barrier()
-        psteps = max(2, min(args.steps, 5))
+        psteps = args.steps
         t0 = time.perf_counter()
         for _ in range(psteps):
             p2d_step()
@@ -517,8 +551,8 @@ def main():
                   "host": torch.empty(ob, dtype=torch.uint8).pin_memory()} for _ in range(nslots)]
         counters = {"h2d": 0, "d2h": 0}
 
-        # measured (profiles/README.md): one GPU 2.13 k frames/s with one thread, 2.05 k with two; four GPUs 4.85 k / 5.73 k; eight GPUs
-        # 9.66 k / 9.35 k (eight ranks x two threads x 16 parsing threads oversubscribe the host)
+        # two threads pay off only on two to four GPUs: one GPU does not need a second, and eight ranks x two threads x 16 parsing
+        # threads oversubscribe the host
         nprod = args.e2e_producers if args.e2e_producers > 0 else (2 if 2 <= world <= 4 else 1)
 
         def e2e_step(keep_last=False):
@@ -574,7 +608,7 @@ def main():
         barrier()
         counters["h2d"] = counters["d2h"] = 0
         t0 = time.perf_counter()
-        esteps = max(2, min(args.steps, 5))
+        esteps = args.steps
         for i in range(esteps):
             last_bd = e2e_step(keep_last=(i == esteps - 1))
         barrier()

@@ -1,5 +1,5 @@
 /*
- * b200jpg.h -- the C ABI of the B200-native baseline-JPEG decode path.
+ * b200jpg.h -- the C ABI of the H100-native baseline-JPEG decode path.
  *
  * This is the drop-in boundary beneath the reference's C++ interface (include/interface/jpeg.hpp restates
  * thorfdbg/libjpeg's interface/jpeg.hpp:79-250): plain pointers and sizes, no C++ and no torch types.

@@ -1,7 +1,7 @@
 // jpeg.hpp -- the library object of the JPEG interface (reference: interface/jpeg.hpp:79-250).
 //
 // Same public surface as the reference's `class JPEG`, so a client written against thorfdbg/libjpeg compiles
-// unchanged; behind it sits the B200 decode path (include/b200jpg.h).  Supported here: decoding of baseline /
+// unchanged; behind it sits the GPU decode path (include/b200jpg.h).  Supported here: decoding of baseline /
 // extended-sequential Huffman codestreams (Construct, Read, GetInformation, DisplayRectangle, LastError,
 // LastWarning, Destruct).  The encoder entry points and the marker peek/read/skip calls exist for link
 // compatibility and fail with JPGERR_NOT_IMPLEMENTED.

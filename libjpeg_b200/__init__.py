@@ -1,4 +1,4 @@
-"""libjpeg_b200 -- a B200-native (sm_100a) baseline-JPEG decode path behind the thorfdbg/libjpeg interface.
+"""libjpeg_b200 -- a H100-native (sm_90a) baseline-JPEG decode path behind the thorfdbg/libjpeg interface.
 
 The product is the shared library ``libb200jpg.so`` (hand-written CUDA kernels + C ABI + the C++ ``class JPEG``
 shim, see ``include/``).  This Python package is the thin host layer used by the tests and the benchmark:

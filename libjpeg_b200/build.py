@@ -1,4 +1,4 @@
-"""Builds libjpeg_b200/libb200jpg.so (CUDA kernels for sm_100a + C ABI + C++ JPEG shim) in-tree with nvcc.
+"""Builds libjpeg_b200/libb200jpg.so (CUDA kernels for sm_90a + C ABI + C++ JPEG shim) in-tree with nvcc.
 
 The shared object travels to the GPU box with the repo snapshot; nothing is JIT-compiled at run time.
 """
@@ -14,7 +14,7 @@ OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libb200jpg.so")
 SYNTH_LIB = os.path.join(HERE, "libb200jpg_synth.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden",
           "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
@@ -48,11 +48,12 @@ def _run(cmd, verbose):
 
 
 def build(force=False, verbose=False, ptxas_info=False):
-    """Compile every translation unit for sm_100a and link the shared objects. Returns the library path."""
+    """Compile every translation unit for sm_90a and link the shared objects. Returns the library path."""
     nvcc = _nvcc()
     os.makedirs(OBJ, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".hpp")]
     headers += [os.path.join(ROOT, "include", "b200jpg.h")]
+    headers += [os.path.abspath(__file__)]  # the flags (ARCH, COMMON) live here: objects built with other flags are stale
     idir = os.path.join(ROOT, "include", "interface")
     if os.path.isdir(idir):
         headers += [os.path.join(idir, f) for f in os.listdir(idir)]

@@ -276,7 +276,7 @@ static int parse_residual(const ParsedFrame &base, ParsedFrame &rf, std::string 
     const b200jpg_frame_info &bi = base.info, &ri = rf.info;
     if (rst == 0 && (rf.xt.present || ri.width != bi.width || ri.height != bi.height || ri.ncomp != bi.ncomp || ri.precision != 8)) {
         rst = B200JPG_ERR_NOT_IMPLEMENTED;
-        err = "outside the JPEG XT profile of the B200 path (8-bit DCT residual of the frame's size)";
+        err = "outside the JPEG XT profile of the GPU path (8-bit DCT residual of the frame's size)";
     }
     if (rst != 0) err = "residual codestream: " + err;
     return rst;
@@ -332,7 +332,7 @@ int b200jpg_create(int device, b200jpg_ctx **out) {
     cudaError_t e = cudaGetDeviceCount(&count);
     if (e != cudaSuccess || count == 0) {
         g_tls_code = B200JPG_ERR_NO_DEVICE;
-        g_tls_error = "no CUDA device available: the B200 JPEG decode path has no CPU fallback";
+        g_tls_error = "no CUDA device available: the H100 JPEG decode path has no CPU fallback";
         return B200JPG_ERR_NO_DEVICE;
     }
     if (device < 0) {
@@ -346,9 +346,9 @@ int b200jpg_create(int device, b200jpg_ctx **out) {
     }
     cudaDeviceProp prop;
     e = cudaGetDeviceProperties(&prop, device);
-    if (e != cudaSuccess || prop.major < 10) {
+    if (e != cudaSuccess || prop.major != 9 || prop.minor != 0) {
         g_tls_code = B200JPG_ERR_NO_DEVICE;
-        g_tls_error = "device is not a Blackwell (sm_100a) GPU: the kernels are built for sm_100a only";
+        g_tls_error = "device is not a Hopper (sm_90a) GPU: the kernels are built for sm_90a only";
         return B200JPG_ERR_NO_DEVICE;
     }
     auto *c = new b200jpg_ctx();
@@ -521,7 +521,7 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
                 for (int c = 0; c < fi.ncomp; c++) {
                     if (fi.frame_type != 2 && seen[c] > 1) {
                         st = B200JPG_ERR_NOT_IMPLEMENTED;
-                        errs[i] = "sequential frame codes a component more than once, not supported by the B200 path";
+                        errs[i] = "sequential frame codes a component more than once, not supported by the GPU path";
                     }
                     if (seen[c] == 0) b->clear_coef = true;
                 }

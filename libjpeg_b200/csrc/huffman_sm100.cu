@@ -1,4 +1,4 @@
-// huffman_sm100.cu -- stage (a): sequential-scan Huffman decode + dequantisation on sm_100a.
+// huffman_sm100.cu -- stage (a): sequential-scan Huffman decode + dequantisation on sm_90a.
 //
 // Replaces the reference's entropy path for SOF0/SOF1 Huffman scans:
 //   SequentialScan::ParseMCU / DecodeBlock / Restart   codestream/sequentialscan.cpp:381-428, 678-773, 266-274

@@ -1,4 +1,4 @@
-// internal.hpp -- shared declarations of the B200 baseline-JPEG decode path (host parser <-> CUDA stages).
+// internal.hpp -- shared declarations of the GPU baseline-JPEG decode path (host parser <-> CUDA stages).
 //
 // Data layout in HBM (one "batch" = n codestreams decoded by the same launches):
 //   bytes      : the codestreams, each copied whole at a 16-byte aligned offset and followed by FF D9 + zero

@@ -1,4 +1,4 @@
-// jpeg_shim.cpp -- the reference's C++ interface (`class JPEG`, `JPG_TagItem`) on top of the B200 C ABI.
+// jpeg_shim.cpp -- the reference's C++ interface (`class JPEG`, `JPG_TagItem`) on top of the C ABI.
 //
 // Restates the client-visible protocol of thorfdbg/libjpeg:
 //   JPG_TagItem traversal           interface/tagitem.cpp:63-324
@@ -346,7 +346,7 @@ JPG_LONG JPEG::DisplayRectangle(struct JPG_TagItem *tags) {
     // a subset of the components: the identity transformation works component by component; through YCbCr->RGB the reference
     // feeds zeros for the components left out (blockbitmaprequester.cpp:1046-1051) -- not offered here
     if ((firstc != 0 || lastc != s.info.ncomp - 1) && colortrafo && s.info.ycbcr)
-        return s.fail(JPGERR_NOT_IMPLEMENTED, "a subset of the components through the colour transformation is not supported by the B200 path");
+        return s.fail(JPGERR_NOT_IMPLEMENTED, "a subset of the components through the colour transformation is not supported by the GPU path");
     const int sample_bytes = s.info.precision > 8 ? 2 : 1;
     // planes mode: plane offsets (in samples) and sizes of the components at their own resolution
     size_t plane_at[B200JPG_MAX_COMPONENTS + 1] = {0};
@@ -462,7 +462,7 @@ JPG_LONG JPEG::DisplayRectangle(struct JPG_TagItem *tags) {
     // colortransformerfactory.cpp:613-632: bytes only hold 8-bit frames; 16-bit samples hold any precision of this path
     const bool deep = s.info.precision > 8;
     if (common_type != 0 && common_type != CTYP_UBYTE && common_type != CTYP_UWORD)
-        return s.fail(JPGERR_INVALID_PARAMETER, "only CTYP_UBYTE and CTYP_UWORD pixels are supported by the B200 path");
+        return s.fail(JPGERR_INVALID_PARAMETER, "only CTYP_UBYTE and CTYP_UWORD pixels are supported by the GPU path");
     if (deep && common_type == CTYP_UBYTE)
         return s.fail(JPGERR_OVERFLOW_PARAMETER, "invalid data type selected for the image, image precision is deeper than 8 bits");
     const bool wide_out = common_type == CTYP_UWORD;
@@ -552,21 +552,21 @@ JPG_LONG JPEG::LastWarning(const char *&warning) {
 }
 
 // encoder side and marker access: present for link compatibility only
-JPG_LONG JPEG::Write(struct JPG_TagItem *) { return m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "encoding is not part of the B200 decode path"); }
-JPG_LONG JPEG::ProvideImage(struct JPG_TagItem *) { return m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "encoding is not part of the B200 decode path"); }
+JPG_LONG JPEG::Write(struct JPG_TagItem *) { return m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "encoding is not part of the GPU decode path"); }
+JPG_LONG JPEG::ProvideImage(struct JPG_TagItem *) { return m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "encoding is not part of the GPU decode path"); }
 JPG_LONG JPEG::PeekMarker(struct JPG_TagItem *) {
-    m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "marker access is not part of the B200 decode path");
+    m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "marker access is not part of the GPU decode path");
     return -1;
 }
 JPG_LONG JPEG::ReadMarker(void *, JPG_LONG, struct JPG_TagItem *) {
-    m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "marker access is not part of the B200 decode path");
+    m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "marker access is not part of the GPU decode path");
     return -1;
 }
 JPG_LONG JPEG::SkipMarker(JPG_LONG, struct JPG_TagItem *) {
-    m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "marker access is not part of the B200 decode path");
+    m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "marker access is not part of the GPU decode path");
     return -1;
 }
 JPG_LONG JPEG::WriteMarker(void *, JPG_LONG, struct JPG_TagItem *) {
-    m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "marker access is not part of the B200 decode path");
+    m_pImpl->fail(JPGERR_NOT_IMPLEMENTED, "marker access is not part of the GPU decode path");
     return -1;
 }

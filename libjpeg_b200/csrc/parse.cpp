@@ -277,7 +277,7 @@ int parse_codestream(const uint8_t *data, size_t len, ParsedFrame &out, std::str
             int nc = s[5];
             if (nc < 1) FAIL(B200JPG_ERR_MALFORMED_STREAM, "number of components must be between 1 and 255");
             if (seglen - 8 != 3 * nc) FAIL(B200JPG_ERR_MALFORMED_STREAM, "frame header marker size is invalid");
-            if (nc > B200JPG_MAX_COMPONENTS) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "more than four components are not supported by the B200 path");
+            if (nc > B200JPG_MAX_COMPONENTS) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "more than four components are not supported by the GPU path");
             fi.ncomp = (uint8_t)nc;
             for (int i = 0; i < nc; i++) {
                 fi.comp_id[i] = s[6 + 3 * i];
@@ -307,7 +307,7 @@ int parse_codestream(const uint8_t *data, size_t len, ParsedFrame &out, std::str
         }
         case 0xda: {
             if (!have_sof) FAIL(B200JPG_ERR_MALFORMED_STREAM, "found a start of scan before the frame header");
-            if (out.scans.size() >= B200JPG_MAX_SCANS) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "too many scans for the B200 path");
+            if (out.scans.size() >= B200JPG_MAX_SCANS) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "too many scans for the GPU path");
             if (seglen < 8) FAIL(B200JPG_ERR_MALFORMED_STREAM, "marker length of the SOS marker invalid, must be at least 8 bytes long");
             ScanInfo sc;
             sc.ns = s[0];
@@ -388,7 +388,7 @@ int parse_codestream(const uint8_t *data, size_t len, ParsedFrame &out, std::str
                 const uint64_t room = (len - (pos + (size_t)seglen)) / 2 + 2;
                 if (nint > room && nint > (1u << 16))
                     FAIL(B200JPG_ERR_MALFORMED_STREAM, "frame header promises more restart intervals than the stream can hold");
-                if (total > (1ull << 31)) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "frame too large for the B200 path");
+                if (total > (1ull << 31)) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "frame too large for the GPU path");
             }
             // A scan with restart markers that carries every component is the only scan of the frame: its entropy coded
             // segment runs up to the closing EOI, which is looked for from the end (bytes behind EOI are legal), and the
@@ -440,7 +440,7 @@ int parse_codestream(const uint8_t *data, size_t len, ParsedFrame &out, std::str
         }
         default:
             if (m == 0xc3 || (m >= 0xc5 && m <= 0xcf && m != 0xc8 && m != 0xcc))
-                FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "only baseline, extended sequential and progressive Huffman frames are supported by the B200 path");
+                FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "only baseline, extended sequential and progressive Huffman frames are supported by the GPU path");
             break;  // APPn, COM, JPG extensions: skipped by length (tables.cpp:1057-1072,1385-1399)
         }
         pos += (size_t)seglen;
@@ -470,7 +470,7 @@ parsed:
             p += lbox;
         }
         if (p != sp.size()) FAIL(B200JPG_ERR_MALFORMED_STREAM, "merging specification box is corrupt");
-        const char *nimpl = "JPEG XT profile outside the B200 path (covered: 8-bit base + 8-bit DCT residual, default tables, clamped output)";
+        const char *nimpl = "JPEG XT profile outside the GPU path (covered: 8-bit base + 8-bit DCT residual, default tables, clamped output)";
         if (xt_other || !xt_spec.seen || fi.precision != 8 || (fi.ncomp != 1 && fi.ncomp != 3)) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, nimpl);
         if (ocon != 0x02) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, nimpl);                  // clamping only: no lossless, float, lookup, extra range bits
         if (ctrf != -1 && ctrf != (1 << 4)) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, nimpl);  // C transformation: the identity
@@ -523,7 +523,7 @@ int build_table_set(const ScanInfo &scan, TableSet &out, std::string &err) {
         for (int i = 0; i < scan.ns; i++) used |= is_ac ? (scan.ta[i] == t - 4) : (scan.td[i] == t);
         if (!used) continue;
         size_t base = lut.size();
-        if (base > 0xf000) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "Huffman tables too large for the B200 decoder tables");
+        if (base > 0xf000) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "Huffman tables too large for the GPU decoder tables");
         lut_off[t] = (uint16_t)base;
         lut.resize(base + ((size_t)1 << L1), kUnused);
         std::vector<int> sub_of((size_t)1 << L1, 0);
@@ -562,7 +562,7 @@ int build_table_set(const ScanInfo &scan, TableSet &out, std::string &err) {
                         const uint32_t q = c16 >> L2;
                         if (!sub_of[q]) {
                             sub_of[q] = ++nsub;
-                            if (nsub > 255) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "Huffman tables too large for the B200 decoder tables");
+                            if (nsub > 255) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "Huffman tables too large for the GPU decoder tables");
                             lut.resize(base + ((size_t)1 << L1) + ((size_t)nsub << L2), kUnused);
                             lut[base + q] = (uint32_t)(sub_of[q] - 1) << 10;  // len field 0 -> second level
                         }
@@ -573,7 +573,7 @@ int build_table_set(const ScanInfo &scan, TableSet &out, std::string &err) {
             }
         }
     }
-    if (lut.size() > 0xffffu) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "Huffman tables too large for the B200 decoder tables");
+    if (lut.size() > 0xffffu) FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "Huffman tables too large for the GPU decoder tables");
     // quantisation + de-zigzag: per table kQzEntries (q, byte offset) pairs indexed by the zig-zag position k. 64..95 is
     // the "AC coefficient decoding out of sync" case of sequentialscan.cpp:764-766 (flagged); 96.. is where symbols that
     // end the block point (EOB, error entries): a zero parked in the pad slot, like the flagged ones
@@ -590,7 +590,7 @@ int build_table_set(const ScanInfo &scan, TableSet &out, std::string &err) {
             if (k < 64) {
                 uint32_t delta = scan.quant_defined[t] ? scan.quant[t][k] : 0;
                 if (((uint64_t)delta << scan.lowbit) >= (1u << 24))
-                    FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "quantisation step times point transform too large for the B200 path");
+                    FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "quantisation step times point transform too large for the GPU path");
                 q = delta << scan.lowbit;
                 off = 2u * kZigZagToRaster[k];
             } else {

@@ -1,4 +1,4 @@
-// progressive_sm100.cu -- SURVEY 8f2: progressive (SOF2) Huffman scans on sm_100a.
+// progressive_sm100.cu -- SURVEY 8f2: progressive (SOF2) Huffman scans on sm_90a.
 //
 // Replaces, for progressive frames, the reference's
 //   SequentialScan::DecodeBlock with m_bProgressive     codestream/sequentialscan.cpp:678-773 (DC / AC first passes:

@@ -91,8 +91,7 @@ __device__ __forceinline__ void unpack_row(const uint4 q, int (&v)[8]) {
 
 // ---- instruction-selection helpers ---------------------------------------------------------------------------------------
 // Both integer pipes of an SM sub-partition (ALU: IADD3 / SHF / LOP3 / LEA / PRMT; FMA-heavy: IMAD, IMAD.IADD, IMAD.MOV, VIADD)
-// take one warp instruction every other cycle (tools/opbench.cu, profiles/), so the kernel runs at the pace of the fuller one
-// -- r01: FMA-heavy 79 % busy, ALU 57 %. ptxas likes "x * 3 + y" as IMAD followed by VIADD for the rounding constant: two
+// take one warp instruction every other cycle (tools/opbench.cu), so the kernel runs at the pace of the fuller one. ptxas likes "x * 3 + y" as IMAD followed by VIADD for the rounding constant: two
 // FMA-heavy instructions per filter tap. Spelled as below it emits IADD3 (a + b + r) and one IMAD (b * 2 + t): one on each pipe.
 #ifndef B200JPG_FUSED_PLAIN
 __device__ __forceinline__ int add3(int a, int b, int c) {
@@ -1288,7 +1287,7 @@ static void launch_b2(const ReconLaunch &l, dim3 grid, const T *samples, cudaStr
 // seg_rows: chroma block rows per CTA of the fused kernel -- as long as possible (a segment recomputes one chroma block row
 // of its upper neighbour) while the grid still holds several waves of CTAs
 static uint32_t fused_seg_rows(const ReconLaunch &l, uint32_t strips, uint32_t rows_all) {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const uint64_t want = (uint64_t)sms * B200JPG_FUSED_CTAS * 6u;  // six waves
     uint32_t seg = 16;
@@ -1336,9 +1335,9 @@ int launch_recon(const ReconLaunch &l, void *stream, int *launches) {
     cudaStream_t s = (cudaStream_t)stream;
     int n = 0;
     if (l.generic) return launch_recon_generic(l, s, launches);
-    // B200JPG_FUSED=1 selects the single-kernel reconstruction of 4:2:0 frames (no sample planes: 51 instead of 66 MB of DRAM
-    // traffic per 4K frame and 25 MB less memory per frame, but 19 % more time: the stage is bound by instruction issue, not by
-    // HBM, and the fused kernel issues more -- profiles/README.md); the default is the two-kernel path through int16 planes.
+    // B200JPG_FUSED=1 selects the single-kernel reconstruction of 4:2:0 frames (no sample planes: less DRAM traffic and 25 MB
+    // less memory per 4K frame, but the stage is bound by instruction issue, not by HBM, and the fused kernel issues more); the
+    // default is the two-kernel path through int16 planes.
     const char *fused = getenv("B200JPG_FUSED");
     if (l.ncomp == 3 && l.subx == 2 && l.suby == 2 && fused && fused[0] == '1') return launch_recon_fused420(l, s, launches);
     const uint32_t cblocks = (l.max_bwc * l.max_bhc + kThreadsB - 1) / kThreadsB;

@@ -125,7 +125,7 @@ spec_sync_kernel(ScanClassParams p, const uint8_t *__restrict__ clean, const uin
 int launch_spec_sync(const EntropyLaunch &l, void *stream) {
     if (l.p.n_scans == 0) return 0;
     const size_t smem = (size_t)l.p.lut_words * 4;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const bool many = l.p.n_scans >= 2u * (uint32_t)sms;  // more CTAs than two per SM: occupancy counts more than the single path
     auto kernel = many ? spec_sync_kernel<3> : spec_sync_kernel<2>;

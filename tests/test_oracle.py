@@ -1,7 +1,9 @@
-"""CPU: pins the oracle (oracle/jpeg_oracle.c) -- against the committed golden vectors that the unmodified
-reference produced (tests/golden/make_golden.py) and, where the reference build is present, against the
-reference itself on fresh streams."""
+"""CPU: pins the oracle (oracle/jpeg_oracle.c) against what the unmodified reference produced: the committed golden
+vectors (tests/golden/make_golden.py ...) and, for streams the repo's generator writes here, the digests of the reference's
+output stored in tests/golden/reference (make_reference_checks.py)."""
 import glob
+import hashlib
+import json
 import os
 
 import numpy as np
@@ -32,34 +34,88 @@ def test_golden_covers_all_vectors(golden_pixels):
     assert sorted(golden_pixels.files) == NAMES and len(NAMES) >= 12
 
 
-@pytest.mark.skipif(not oracle_binding.have_reference(), reason="reference build (oracle/_ref) not present")
-@pytest.mark.parametrize("w,h,sub,z,q", [(72, 40, (2, 2), 3, 60), (31, 47, (2, 2), 0, 85), (64, 32, (1, 1), 8, 92),
-                                          (90, 33, (2, 1), 2, 70), (45, 90, (1, 2), 6, 70)])
-def test_oracle_matches_reference_on_synthetic_streams(oracle, built, tmp_path, w, h, sub, z, q):
-    """Streams from the repo's own generator, decoded by the real reference and by the oracle."""
+# streams of the repo's generator whose decode by the reference is stored as digests (tests/golden/make_reference_checks.py)
+REFERENCE = os.path.join(GOLDEN, "reference")
+SYNTHETIC = [(72, 40, (2, 2), 3, 60), (31, 47, (2, 2), 0, 85), (64, 32, (1, 1), 8, 92), (90, 33, (2, 1), 2, 70), (45, 90, (1, 2), 6, 70)]
+BEYOND_RANGE = [(96, 80, (2, 2), 3, 255), (200, 120, (2, 1), 0, 160), (64, 64, (1, 1), 4, 255), (130, 70, (1, 2), 2, 200)]
+OTHER_SUBSAMPLING = ["1x1,4x1,4x1", "1x1,3x2,3x2", "1x1,2x3,2x3", "1x1,1x4,1x4", "1x1,3x4,3x4", "1x1,4x3,4x3", "1x1,2x1,4x2"]
+STREAM_VARIANTS = [(1, 70, 50, (2, 2), 5), (1, 64, 48, (1, 1), 0), (2, 40, 40, (2, 2), 3), (6, 40, 40, (2, 1), 0), (7, 33, 47, (1, 2), 4)]
+FOUR_COMPONENT = [(64, 48, (1, 1), 4), (70, 50, (2, 2), 5), (100, 37, (2, 1), 0), (33, 90, (1, 2), 3)]
+NO_COLOR_TRANSFORM = ["c420_96x80_z6_q75", "c444_64x64_z16_q90", "c422_100x60_z5_q80"]
+
+
+def synthetic_stream(w, h, sub, z, q):
     from libjpeg_b200 import synth
-    data = synth.encode(synth.source_image(w, h, 7 * w + h), q, sub, z)
-    jpg = tmp_path / "s.jpg"
-    jpg.write_bytes(data.tobytes())
-    ref = oracle_binding.reference_decode(str(jpg), str(tmp_path / "s.raw"))
-    assert ref is not None
-    rc, px = oracle.decode(data.tobytes())
-    assert rc == 0 and np.array_equal(px, ref)
+    return synth.encode(synth.source_image(w, h, 7 * w + h), q, sub, z).tobytes()
 
 
-@pytest.mark.skipif(not oracle_binding.have_reference(), reason="reference build (oracle/_ref) not present")
-@pytest.mark.parametrize("w,h,sub,z,dcq", [(96, 80, (2, 2), 3, 255), (200, 120, (2, 1), 0, 160), (64, 64, (1, 1), 4, 255), (130, 70, (1, 2), 2, 200)])
-def test_oracle_matches_reference_beyond_the_usual_sample_range(oracle, built, tmp_path, w, h, sub, z, dcq):
+def beyond_range_stream(w, h, sub, z, dcq):
+    from libjpeg_b200 import synth
+    return oracle_binding.with_dc_quantiser(synth.encode(synth.source_image(w, h, 5), 75, sub, z), dcq)
+
+
+def damaged_stream(damage):
+    from libjpeg_b200 import synth
+    return oracle_binding.with_restart_damage(synth.encode(synth.source_image(200, 136, 3), 75, (2, 2), 2), damage)
+
+
+def variant_stream(flags, w, h, sub, z):
+    from libjpeg_b200 import synth
+    return synth.encode(synth.source_image(w, h, 5), 80, sub, z, flags).tobytes()
+
+
+def four_component_stream(w, h, sub, z):
+    from libjpeg_b200 import synth
+    return oracle_binding.with_fourth_component(synth.encode(synth.source_image(w, h, 5), 80, sub, z, 1))
+
+
+def other_subsampling_name(sub):
+    return "sub_" + sub.replace(",", "_")
+
+
+def reference_cases():
+    """(key, stream) of every generated stream the reference's verdict is stored for."""
+    for p in SYNTHETIC:
+        yield "synthetic%r" % (p,), synthetic_stream(*p)
+    for p in BEYOND_RANGE:
+        yield "beyond_range%r" % (p,), beyond_range_stream(*p)
+    for d in oracle_binding.RESTART_DAMAGES:
+        yield "restart_damage[%s]" % d, damaged_stream(d)
+    for p in STREAM_VARIANTS:
+        yield "stream_variant%r" % (p,), variant_stream(*p)
+    yield "zrl_overrun", oracle_binding.zrl_overrun_stream()
+    for p in FOUR_COMPONENT:
+        yield "four_component%r" % (p,), four_component_stream(*p)
+
+
+def check_reference(key, data, rc, px):
+    """The oracle's verdict (rc) and samples (px) for `data` against what the reference delivered for the same stream."""
+    want = json.load(open(os.path.join(REFERENCE, "reference_digests.json")))[key]
+    assert hashlib.sha256(bytes(data)).hexdigest() == want["input_sha256"], "%s: not the stream the reference decoded" % key
+    if want["shape"] is None:
+        assert rc != 0, "%s: the reference refused this stream" % key
+        return
+    assert rc == 0, key
+    px = np.ascontiguousarray(px)
+    assert px.size == int(np.prod(want["shape"])), key
+    assert hashlib.sha256(px.tobytes()).hexdigest() == want["sha256"], "%s: samples differ from the reference's" % key
+
+
+@pytest.mark.parametrize("w,h,sub,z,q", SYNTHETIC)
+def test_oracle_matches_reference_on_synthetic_streams(oracle, built, w, h, sub, z, q):
+    """Streams from the repo's own generator, decoded by the real reference and by the oracle."""
+    data = synthetic_stream(w, h, sub, z, q)
+    rc, px = oracle.decode(data)
+    check_reference("synthetic%r" % ((w, h, sub, z, q),), data, rc, px)
+
+
+@pytest.mark.parametrize("w,h,sub,z,dcq", BEYOND_RANGE)
+def test_oracle_matches_reference_beyond_the_usual_sample_range(oracle, built, w, h, sub, z, dcq):
     """DC quantiser patched to a large value: IDCT samples leave int16 and the 32-bit colour range (the reference
     computes the colour matrix in 64 bits); the oracle must follow the reference there too."""
-    from libjpeg_b200 import synth
-    data = oracle_binding.with_dc_quantiser(synth.encode(synth.source_image(w, h, 5), 75, sub, z), dcq)
-    jpg = tmp_path / "hot.jpg"
-    jpg.write_bytes(data)
-    ref = oracle_binding.reference_decode(str(jpg), str(tmp_path / "hot.raw"))
-    assert ref is not None
+    data = beyond_range_stream(w, h, sub, z, dcq)
     rc, px = oracle.decode(data)
-    assert rc == 0 and np.array_equal(px, ref)
+    check_reference("beyond_range%r" % ((w, h, sub, z, dcq),), data, rc, px)
 
 
 def test_oracle_idct_dc_only(oracle):
@@ -112,22 +168,13 @@ def test_oracle_matches_3x_4x_subsampling_golden(oracle, name):
     assert np.array_equal(px.reshape(want.shape), want)
 
 
-@pytest.mark.skipif(not oracle_binding.have_reference(), reason="reference build (oracle/_ref) not present")
-@pytest.mark.parametrize("sub", ["1x1,4x1,4x1", "1x1,3x2,3x2", "1x1,2x3,2x3", "1x1,1x4,1x4", "1x1,3x4,3x4", "1x1,4x3,4x3", "1x1,2x1,4x2"])
-def test_oracle_matches_reference_on_other_subsampling(oracle, tmp_path, sub):
-    """Fresh streams from the reference's encoder (its CLI takes the sampling factors), decoded by reference and oracle."""
-    import subprocess
-    from libjpeg_b200 import synth
-    w, h = 75, 61
-    ppm = tmp_path / "in.ppm"
-    ppm.write_bytes(b"P6\n%d %d\n255\n" % (w, h) + synth.source_image(w, h, 17).tobytes())
-    jpg = tmp_path / "s.jpg"
-    r = subprocess.run([oracle_binding.REF_CLI, "-q", "80", "-bl", "-s", sub, "-z", "3", str(ppm), str(jpg)],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    ref = oracle_binding.reference_decode(str(jpg), str(tmp_path / "s.raw"))
-    rc, px = oracle.decode(jpg.read_bytes())
-    assert rc == 0 and np.array_equal(px.reshape(ref.shape), ref)
+@pytest.mark.parametrize("sub", OTHER_SUBSAMPLING)
+def test_oracle_matches_reference_on_other_subsampling(oracle, sub):
+    """Streams of the reference's encoder (its CLI takes the sampling factors; tests/golden/reference), decoded by reference
+    and oracle."""
+    data = open(os.path.join(REFERENCE, other_subsampling_name(sub) + ".jpg"), "rb").read()
+    rc, px = oracle.decode(data)
+    check_reference("other_subsampling[%s]" % sub, data, rc, px)
 
 
 DAMAGED = os.path.join(GOLDEN, "damaged")
@@ -144,20 +191,12 @@ def test_oracle_matches_damaged_golden(oracle, name):
     assert np.array_equal(px.reshape(want.shape), want)
 
 
-@pytest.mark.skipif(not oracle_binding.have_reference(), reason="reference build (oracle/_ref) not present")
 @pytest.mark.parametrize("damage", oracle_binding.RESTART_DAMAGES)
-def test_oracle_resynchronises_like_the_reference(oracle, tmp_path, damage):
+def test_oracle_resynchronises_like_the_reference(oracle, built, damage):
     """Restart markers out of sequence, missing, duplicated, buried in garbage: same verdict and same pixels as the reference."""
-    from libjpeg_b200 import synth
-    b = oracle_binding.with_restart_damage(synth.encode(synth.source_image(200, 136, 3), 75, (2, 2), 2), damage)
-    jpg = tmp_path / "d.jpg"
-    jpg.write_bytes(bytes(b))
-    ref = oracle_binding.reference_decode(str(jpg), str(tmp_path / "d.raw"))
-    rc, px = oracle.decode(bytes(b))
-    if ref is None:
-        assert rc != 0
-    else:
-        assert rc == 0 and np.array_equal(px.reshape(ref.shape), ref)
+    data = damaged_stream(damage)
+    rc, px = oracle.decode(data)
+    check_reference("restart_damage[%s]" % damage, data, rc, px)
 
 
 DEEP12 = os.path.join(GOLDEN, "deep12")
@@ -187,19 +226,13 @@ def test_progressive_golden_is_complete():
     assert set(np.load(os.path.join(PROGRESSIVE, "progressive_pixels.npz")).files) == set(PNAMES)
 
 
-@pytest.mark.skipif(not oracle_binding.have_reference(), reason="reference build (oracle/_ref) not present")
-@pytest.mark.parametrize("flags,w,h,sub,z", [(1, 70, 50, (2, 2), 5), (1, 64, 48, (1, 1), 0), (2, 40, 40, (2, 2), 3), (6, 40, 40, (2, 1), 0),
-                                            (7, 33, 47, (1, 2), 4)])
-def test_oracle_matches_reference_on_stream_variants(oracle, built, tmp_path, flags, w, h, sub, z):
+@pytest.mark.parametrize("flags,w,h,sub,z", STREAM_VARIANTS)
+def test_oracle_matches_reference_on_stream_variants(oracle, built, flags, w, h, sub, z):
     """One scan per component (flag 1), SOF1 header (2), 16-bit DQT (4): accepted by the reference, same pixels."""
-    from libjpeg_b200 import synth
-    data = synth.encode(synth.source_image(w, h, 5), 80, sub, z, flags)
-    jpg = tmp_path / "v.jpg"
-    jpg.write_bytes(data.tobytes())
-    ref = oracle_binding.reference_decode(str(jpg), str(tmp_path / "v.raw"))
-    assert ref is not None
-    rc, px = oracle.decode(data.tobytes())
-    assert rc == 0 and np.array_equal(px, ref)
+    data = variant_stream(flags, w, h, sub, z)
+    rc, px = oracle.decode(data)
+    assert rc == 0
+    check_reference("stream_variant%r" % ((flags, w, h, sub, z),), data, rc, px)
 
 
 NOEOI = os.path.join(GOLDEN, "noeoi")
@@ -227,16 +260,12 @@ def test_noeoi_fixtures_cover_both_verdicts():
     assert sorted(status) == NENAMES and 0 in status.values() and -1025 in status.values()
 
 
-@pytest.mark.skipif(not oracle_binding.have_reference(), reason="reference build (oracle/_ref) not present")
-def test_zrl_that_steps_over_position_63_ends_the_block_silently(oracle, tmp_path):
+def test_zrl_that_steps_over_position_63_ends_the_block_silently(oracle):
     """sequentialscan.cpp:717-719: after a ZRL the reference re-tests k <= 63 and leaves the block without an error."""
     data = oracle_binding.zrl_overrun_stream()
-    jpg = tmp_path / "z.jpg"
-    jpg.write_bytes(data)
-    ref = oracle_binding.reference_decode(str(jpg), str(tmp_path / "z.raw"))
-    assert ref is not None
     rc, px = oracle.decode(data)
-    assert rc == 0 and np.array_equal(px.reshape(ref.shape), ref)
+    assert rc == 0
+    check_reference("zrl_overrun", data, rc, px)
 
 
 DNL = os.path.join(GOLDEN, "dnl")
@@ -254,34 +283,20 @@ def test_oracle_reads_the_height_from_the_dnl_marker(oracle, name):
     assert np.array_equal(got[:-1], px[name + "__ref_dnl"][:-1])
 
 
-@pytest.mark.skipif(not oracle_binding.have_reference(), reason="reference build (oracle/_ref) not present")
-@pytest.mark.parametrize("w,h,sub,z", [(64, 48, (1, 1), 4), (70, 50, (2, 2), 5), (100, 37, (2, 1), 0), (33, 90, (1, 2), 3)])
-def test_oracle_matches_reference_on_four_component_streams(oracle, built, tmp_path, w, h, sub, z):
-    from libjpeg_b200 import synth
-    data = oracle_binding.with_fourth_component(synth.encode(synth.source_image(w, h, 5), 80, sub, z, 1))
-    jpg = tmp_path / "f4.jpg"
-    jpg.write_bytes(data)
-    ref = oracle_binding.reference_decode(str(jpg), str(tmp_path / "f4.raw"))
-    assert ref is not None and ref.shape[2] == 4
+@pytest.mark.parametrize("w,h,sub,z", FOUR_COMPONENT)
+def test_oracle_matches_reference_on_four_component_streams(oracle, built, w, h, sub, z):
+    data = four_component_stream(w, h, sub, z)
     rc, px = oracle.decode(data)
-    assert rc == 0 and np.array_equal(px, ref)
+    assert rc == 0 and px.shape == (h, w, 4)
+    check_reference("four_component%r" % ((w, h, sub, z),), data, rc, px)
 
 
-@pytest.mark.skipif(not oracle_binding.have_reference(), reason="reference build (oracle/_ref) not present")
-@pytest.mark.parametrize("name", ["c420_96x80_z6_q75", "c444_64x64_z16_q90", "c422_100x60_z5_q80"])
-def test_oracle_without_color_transform_matches_reference_cli(oracle, tmp_path, name):
+@pytest.mark.parametrize("name", NO_COLOR_TRANSFORM)
+def test_oracle_without_color_transform_matches_reference_cli(oracle, name):
     """JPGTAG_MATRIX_LTRAFO = none (`jpeg -c` on decoding, cmd/main.cpp / reconstruct.cpp:336): Y, Cb, Cr upsampled, untransformed."""
-    import subprocess
-    src = os.path.join(GOLDEN, name + ".jpg")
-    ppm = tmp_path / "o.ppm"
-    r = subprocess.run([oracle_binding.REF_CLI, "-c", src, str(ppm)], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    raw = ppm.read_bytes()
-    magic, dims, maxv, rest = raw.split(b"\n", 3)
-    w, h = map(int, dims.split())
-    ref = np.frombuffer(rest, dtype=np.uint8).reshape(h, w, 3)
-    rc, px = oracle.decode_without_color_transform(open(src, "rb").read())
-    assert rc == 0 and np.array_equal(px, ref)
+    data = open(os.path.join(GOLDEN, name + ".jpg"), "rb").read()
+    rc, px = oracle.decode_without_color_transform(data)
+    check_reference("no_color_transform[%s]" % name, data, rc, px)
 
 
 def test_oracle_planes_match_reference_without_upsampling(oracle):

@@ -51,7 +51,7 @@ def main():
                    "upload_plus_kernels_ms_median": round(statistics.median(td[2:]), 3), "entropy_ms": round(e, 3), "reconstruction_ms": round(r, 3),
                    "codestream_bytes": len(data)}
         dec.close()
-    print(json.dumps({"what": "one frame per call, one B200; decode_to_host = b200jpg_decode_to_host wall clock (host parse + pack + H2D + "
+    print(json.dumps({"what": "one frame per call, one GPU; decode_to_host = b200jpg_decode_to_host wall clock (host parse + pack + H2D + "
                               "restart index + kernels + D2H into pinned memory + batch teardown)", "frames": res}))
 
 

@@ -1,6 +1,6 @@
 // opbench.cu -- per-opcode issue rates of the integer pipes on this GPU (one SMSP's warp-instructions per clock), and which
 // opcodes share a pipe with IMAD. Each kernel runs 8 independent register chains of one SASS opcode (checked with
-// cuobjdump -sass) per thread, unrolled; MIX kernels interleave two opcodes 1:1.  Build: nvcc -arch=sm_100a -O3 -o opbench opbench.cu
+// cuobjdump -sass) per thread, unrolled; MIX kernels interleave two opcodes 1:1.  Build: nvcc -arch=sm_90a -O3 -o opbench opbench.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>
