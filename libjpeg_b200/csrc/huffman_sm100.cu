@@ -1048,6 +1048,10 @@ static int launch_entropy_impl(const EntropyLaunch &l, void *stream) {
         entropy_decode_kernel<true, kIndexed><<<grid, kThreads, smem, s>>>(l.p, l.clean, l.clean_off, l.interval_len, l.scans, l.tables, l.coef,
                                                                             l.frame_status, l.overrun_list, l.spec_segments);
     } else {
+        // decoder tables too large for shared memory: read from global memory; the staging blocks and the ring alone are
+        // beyond the 48 KB a launch gets without opting in
+        e = cudaFuncSetAttribute(entropy_decode_kernel<false, kIndexed>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)base_smem);
+        if (e != cudaSuccess) return (int)e;
         entropy_decode_kernel<false, kIndexed><<<grid, kThreads, base_smem, s>>>(l.p, l.clean, l.clean_off, l.interval_len, l.scans, l.tables, l.coef,
                                                                                  l.frame_status, l.overrun_list, l.spec_segments);
     }

@@ -86,6 +86,9 @@ def reference_cases():
     yield "zrl_overrun", oracle_binding.zrl_overrun_stream()
     for p in FOUR_COMPONENT:
         yield "four_component%r" % (p,), four_component_stream(*p)
+    from tests import entropy_cases
+    for name in entropy_cases.NAMES:
+        yield "entropy_stress[%s]" % name, entropy_cases.case(name)[1]
 
 
 def check_reference(key, data, rc, px):
@@ -289,6 +292,22 @@ def test_oracle_matches_reference_on_four_component_streams(oracle, built, w, h,
     rc, px = oracle.decode(data)
     assert rc == 0 and px.shape == (h, w, 4)
     check_reference("four_component%r" % ((w, h, sub, z),), data, rc, px)
+
+
+def _entropy_case_names():
+    from tests import entropy_cases
+    return entropy_cases.NAMES
+
+
+@pytest.mark.parametrize("name", _entropy_case_names())
+def test_oracle_matches_reference_on_hand_built_entropy_streams(oracle, name):
+    """Streams of the test writer (tests/entropy_cases.py: long codes, decoder tables beyond shared memory, degenerate tables,
+    dense blocks, run edges, FF 00 stuffing, the int16 edge, EOBRUN 32767 ...): the reference's verdict and samples, also for
+    the frame whose coefficient +32768 the GPU refuses."""
+    from tests import entropy_cases
+    data = entropy_cases.case(name)[1]
+    rc, px = (oracle.decode16 if entropy_cases.case(name)[0].precision > 8 else oracle.decode)(data)
+    check_reference("entropy_stress[%s]" % name, data, rc, px)
 
 
 @pytest.mark.parametrize("name", NO_COLOR_TRANSFORM)
