@@ -944,13 +944,11 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
     b->sz_status = sizeof(uint32_t) * (5 * (size_t)n + 1);  // status words, wide flags, narrow flags, narrow list, index status
     b->d_input = (uint8_t *)ctx->get(1, b->input_bytes, &ce);
     if (ce == cudaSuccess && b->coef_elems) b->d_coef = (int16_t *)ctx->get(1, b->coef_elems * sizeof(int16_t), &ce);
-    // sample planes only for the reconstruction groups that go through them (with B200JPG_FUSED=1, 4:2:0 frames are reconstructed
-    // by the fused kernel: coefficients -> pixels, chroma samples live in shared memory)
+    // sample planes only for the reconstruction groups that go through them (4:2:0 frames go from coefficients to pixels in one
+    // kernel, their chroma samples live in shared memory)
     {
-        const char *fused = getenv("B200JPG_FUSED");
-        const bool use_fused = fused && fused[0] == '1';
         bool need_planes = false;
-        for (auto &g : b->groups) need_planes = need_planes || g.generic || (g.ncomp > 1 && !(use_fused && g.ncomp == 3 && g.subx == 2 && g.suby == 2));
+        for (auto &g : b->groups) need_planes = need_planes || g.generic || (g.ncomp > 1 && !(g.ncomp == 3 && g.subx == 2 && g.suby == 2));
         if (!need_planes) b->sample_elems = 0;
     }
     if (ce == cudaSuccess && b->sample_elems) b->d_samples = (int32_t *)ctx->get(1, b->sample_elems * sizeof(int32_t), &ce);

@@ -11,6 +11,8 @@
 //   YCbCrTrafo<UBYTE,3,ClampFlag,YCbCr,Zero>::YCbCr2RGB colortrafo/ycbcrtrafo.cpp:679-1008 (:842-850, :922-935)
 //
 // Mapping.  One thread owns one 8x8 block.
+//  4:2:0 frames: reconstruct420_kernel, one kernel from coefficients to pixels (chroma IDCT into a shared-memory window,
+//     then the luma rows exactly like b2); see its section below.  Every other 1..3 component format:
 //  b1 idct_planes_kernel: blocks of the non-luma components -> int32 sample planes (the whole-frame equivalent of
 //     the reference's upsampler line buffers); both 1-D passes in registers.
 //  b2 reconstruct_kernel: a warp owns 32 horizontally adjacent luma blocks (256 x 8 pixels), a CTA four such rows.
@@ -266,6 +268,69 @@ narrow_list_kernel(const FrameRecon *__restrict__ frames, uint32_t n_frames, con
         if (narrow_flags[frames[i].status_idx]) list[1 + atomicAdd(list, 1u)] = i;
 }
 
+// ---- the chroma window of reconstruct420_kernel -------------------------------------------------------------------------
+// A CTA of reconstruct420_kernel covers 32 luma block columns x kRows420 luma block rows, one warp per row (kRows420 = 4 is
+// b2's CTA). Its chroma window holds, per component, the kRows420 / 2 chroma block rows under the tile plus the line above and
+// the line below (kLines lines) and, per line, the 128 columns under the tile plus the column either side. Line l is chroma
+// line 4 kRows420 blockIdx.y - 1 + l, column i is chroma column 128 blockIdx.x - 4 + i: a lane's own four samples start at
+// i = 4 + 4 lane (an aligned 8- / 16-byte load), its left / right neighbour is i = 3 + 4 lane / 8 + 4 lane.
+#ifndef B200JPG_R420_ROWS
+#define B200JPG_R420_ROWS 4
+#endif
+constexpr int kRows420 = B200JPG_R420_ROWS;
+constexpr int kThreads420 = 32 * kRows420;
+static_assert(kRows420 % 2 == 0 && kRows420 >= 4 && kRows420 <= 8, "whole chroma block rows, enough warps for phase 1, at most 8 warps");
+
+template <typename T>
+struct Window420 {
+    static constexpr int kLines = 4 * kRows420 + 2;
+    static constexpr int kLineBytes = 136 * (int)sizeof(T);  // [3 unused][left][128][right][3 unused]
+    // + 4 samples: Cr lies two banks off Cb for the int16 stores of phase 1, and 16-byte aligned for the int32 loads
+    static constexpr int kCompBytes = kLines * kLineBytes + 4 * (int)sizeof(T);
+    static constexpr int kYsBytes = 64 * kThreads420 * 4;  // the luma tile `ys` in front of the window
+    static constexpr int kSmemBytes = kYsBytes + 2 * kCompBytes;
+};
+
+__device__ __forceinline__ uint32_t lds32(uint32_t a) {
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint2 lds64(uint32_t a) {
+    uint2 v;
+    asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint4 lds128(uint32_t a) {
+    uint4 v;
+    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a) : "memory");
+    return v;
+}
+__device__ __forceinline__ int lds_s16(uint32_t a) {
+    int v;
+    asm volatile("ld.shared.s16 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+    return v;
+}
+__device__ __forceinline__ void sts16(uint32_t a, int v) { asm volatile("st.shared.u16 [%0], %1;" ::"r"(a), "h"((short)v) : "memory"); }
+__device__ __forceinline__ void sts32(uint32_t a, int v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+
+// one window sample (T = short / int) at a shared-space byte address
+template <typename T>
+__device__ __forceinline__ int win_load(uint32_t a) {
+    return sizeof(T) == 2 ? lds_s16(a) : (int)lds32(a);
+}
+template <typename T>
+__device__ __forceinline__ void win_store(uint32_t a, int v) {
+    if (sizeof(T) == 2) sts16(a, v);
+    else sts32(a, v);
+}
+// two horizontally adjacent window samples, the first at an even column: one 32- / 64-bit store
+template <typename T>
+__device__ __forceinline__ void win_store2(uint32_t a, int v0, int v1) {
+    if (sizeof(T) == 2) sts32(a, (int)(((uint32_t)v0 & 0xffffu) | ((uint32_t)v1 << 16)));
+    else asm volatile("st.shared.v2.u32 [%0], {%1,%2};" ::"r"(a), "r"(v0), "r"(v1) : "memory");
+}
+
 // ---- b2 ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ int clampi(int v, int lo, int hi) { return v < lo ? lo : (v > hi ? hi : v); }
 
@@ -358,13 +423,17 @@ __device__ __forceinline__ void to_rgb(int y, int cbv, int crv, int &r, int &g, 
     }
 }
 
-template <int NC, int SX, int SY, typename T>
+// kWin: the chroma samples come from the window of reconstruct420_kernel at shared-space address `win` instead of the sample
+// planes. chroma_wide: a chroma sample the tile reads may leave the 32-bit colour range.
+template <int NC, int SX, int SY, typename T, bool kWin = false>
 __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, const int16_t *__restrict__ coef, const T *__restrict__ samples,
-                                                 const uint32_t *__restrict__ wide_flags, uint8_t *__restrict__ out) {
+                                                 uint32_t win, bool chroma_wide, uint8_t *__restrict__ out) {
+    static_assert(!kWin || (NC == 3 && SX == 2 && SY == 2), "the chroma window is 4:2:0 only");
+    constexpr uint32_t NT = kWin ? kThreads420 : kThreadsB;  // threads per CTA: the stride of the tile [coefficient][thread]
     const uint32_t W = f.width, H = f.height;
     const uint32_t vbw = (W + 7) >> 3, vbh = (H + 7) >> 3;  // blocks that carry visible pixels
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t bx0 = blockIdx.x * 32, bx = bx0 + lane, by = blockIdx.y * (kThreadsB / 32) + warp;
+    const uint32_t bx0 = blockIdx.x * 32, bx = bx0 + lane, by = blockIdx.y * (NT / 32) + warp;
     if (by >= vbh) return;  // whole warp
     const bool valid = bx < vbw;
     const int X = 8 * (int)bx, Y = 8 * (int)by;
@@ -375,7 +444,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
     // columns, 16-byte piece (block, row) at row segment 32 + 4*row + block/8, slot (block%8) ^ row: conflict-free for
     // these writes and for the per-lane reads below. The row pass overwrites a segment only after its piece was consumed.
     {
-        const uint32_t wseg = (uint32_t)__cvta_generic_to_shared(ys) + 128u * warp;  // bytes; row segment j at + 512*j
+        const uint32_t wseg = (uint32_t)__cvta_generic_to_shared(ys) + 128u * warp;  // bytes; row segment j at + 4*NT*j
         const uint4 *src = reinterpret_cast<const uint4 *>(coef + f.coef_base[0] + ((uint64_t)by * f.bw[0] + bx0) * 64u);
         const uint32_t prow = lane & 7u, sub = lane >> 3;
         uint4 pc[8];
@@ -387,17 +456,17 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
 #pragma unroll
         for (uint32_t i = 0; i < 8; i++) {
             const uint32_t blk = 4u * i + sub;
-            const uint32_t dst = wseg + 512u * (32u + 4u * prow + (blk >> 3)) + 16u * ((blk & 7u) ^ prow);
+            const uint32_t dst = wseg + 4u * NT * (32u + 4u * prow + (blk >> 3)) + 16u * ((blk & 7u) ^ prow);
             asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(dst), "r"(pc[i].x), "r"(pc[i].y), "r"(pc[i].z), "r"(pc[i].w) : "memory");
         }
         __syncwarp();
         // ---- row pass (dct/idct.cpp:237-287): the next row's piece is read before this row's results are written
-        const uint32_t mine = wseg + 512u * (32u + (lane >> 3));
+        const uint32_t mine = wseg + 4u * NT * (32u + (lane >> 3));
         auto piece = [&](int r) {
             uint4 q;
             asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];"
                          : "=r"(q.x), "=r"(q.y), "=r"(q.z), "=r"(q.w)
-                         : "r"(mine + 2048u * (uint32_t)r + 16u * ((lane & 7u) ^ (uint32_t)r))
+                         : "r"(mine + 16u * NT * (uint32_t)r + 16u * ((lane & 7u) ^ (uint32_t)r))
                          : "memory");
             return q;
         };
@@ -411,7 +480,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
             idct8t<16, 5>(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
             __syncwarp();
 #pragma unroll
-            for (int k = 0; k < 8; k++) my[(8 * r + k) * kThreadsB] = v[k];
+            for (int k = 0; k < 8; k++) my[(8 * r + k) * NT] = v[k];
             q = qn;
         }
     }
@@ -421,10 +490,10 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
     for (int k = 0; k < 8; k++) {
         int v[8];
 #pragma unroll
-        for (int r = 0; r < 8; r++) v[r] = my[(8 * r + k) * kThreadsB];
+        for (int r = 0; r < 8; r++) v[r] = my[(8 * r + k) * NT];
         idct8t<2048, 12>(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
 #pragma unroll
-        for (int r = 0; r < 8; r++) my[(8 * r + k) * kThreadsB] = v[r];
+        for (int r = 0; r < 8; r++) my[(8 * r + k) * NT] = v[r];
         mx = __vimax3_s32(__vimax3_s32(mx, v[0], v[1]), v[2], v[3]);
         mx = __vimax3_s32(__vimax3_s32(mx, v[4], v[5]), v[6], v[7]);
         mn = __vimin3_s32(__vimin3_s32(mn, v[0], v[1]), v[2], v[3]);
@@ -443,7 +512,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
             uint8_t *o = obase + (uint64_t)r * opitch;
             int px[8];
 #pragma unroll
-            for (int x = 0; x < 8; x++) px[x] = WADD(my[(8 * r + x) * kThreadsB], 8) >> 4;
+            for (int x = 0; x < 8; x++) px[x] = WADD(my[(8 * r + x) * NT], 8) >> 4;
             const uint32_t w0 = pack_sat4(px[0], px[1], px[2], px[3]), w1 = pack_sat4(px[4], px[5], px[6], px[7]);
             if (xmax == 7 && ((reinterpret_cast<uintptr_t>(o) & 7u) == 0)) {
                 *reinterpret_cast<uint2 *>(o) = make_uint2(w0, w1);
@@ -459,21 +528,51 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
     constexpr int NW = (SX == 2) ? 6 : 8;
     const int cw = (int)f.cw, ch = (int)f.ch;
     const uint32_t cpitch = 8u * f.bw[1];
-    const T *p1 = samples + f.sample_base[1];
-    const T *p2 = samples + f.sample_base[2];
+    const T *p1 = kWin ? nullptr : samples + f.sample_base[1];
+    const T *p2 = kWin ? nullptr : samples + f.sample_base[2];
     const int cx0 = X / SX - ((SX == 2) ? 1 : 0);  // window column 0 (upsampler.cpp:87,108-109)
     const int cy0 = Y / SY;
     const bool ycbcr = f.ycbcr != 0;
-    // int16 planes: chroma is inside the guarded range by construction, only this block's luma can leave it
-    const bool wide = (sizeof(T) == 4 && wide_flags[f.status_idx] != 0u) || mx > kWide || mn < -kWide;
+    // int16 samples: chroma is inside the guarded range by construction, only this block's luma can leave it
+    const bool wide = chroma_wide || mx > kWide || mn < -kWide;
     // the whole window lies inside the plane: no clamping needed
     const bool interior = valid && cx0 >= 0 && cx0 + NW <= cw && cy0 - 1 >= 0 && cy0 + ((SY == 2) ? 5 : 8) <= ch;
     // warp-uniform: every block of the warp is visible and every lane's own samples lie inside the plane
     constexpr int OWN = 8 / SX;
     const bool fast = (bx0 + 32 <= vbw) && ((int)((bx0 + 32) * OWN) <= cw);
     const int xl = (cx0 > 0) ? cx0 : 0, xr = (cx0 + NW - 1 < cw) ? cx0 + NW - 1 : cw - 1;
+    // chroma (line 0, column 0) of the shared-memory window (Window420)
+    const int wy0 = 4 * (int)(NT / 32) * (int)blockIdx.y - 1, wx0 = 128 * (int)blockIdx.x - 4;
     auto fetch = [&](int y, int (&d1)[NW], int (&d2)[NW]) {
-        if (fast) {
+        if (kWin) {
+            using Wn = Window420<T>;
+            const uint32_t line = win + (uint32_t)(clampi(y, 0, ch - 1) - wy0) * (uint32_t)Wn::kLineBytes;
+            constexpr uint32_t S = sizeof(T);
+            if (fast) {
+#pragma unroll
+                for (int c = 0; c < 2; c++) {
+                    int (&d)[NW] = c ? d2 : d1;
+                    const uint32_t a = line + (uint32_t)c * (uint32_t)Wn::kCompBytes;
+                    if (S == 2) {
+                        const uint2 o = lds64(a + (4u + 4u * lane) * S);
+                        d[1] = (int)(short)(o.x & 0xffffu), d[2] = (int)o.x >> 16, d[3] = (int)(short)(o.y & 0xffffu), d[4] = (int)o.y >> 16;
+                    } else {
+                        const uint4 o = lds128(a + (4u + 4u * lane) * S);
+                        d[1] = (int)o.x, d[2] = (int)o.y, d[3] = (int)o.z, d[4] = (int)o.w;
+                    }
+                    d[0] = win_load<T>(a + (uint32_t)(xl - wx0) * S);
+                    d[NW - 1] = win_load<T>(a + (uint32_t)(xr - wx0) * S);
+                }
+            } else if (valid) {
+                // at the frame edge: the clamped addressing below, always inside the window
+#pragma unroll
+                for (int j = 0; j < NW; j++) {
+                    const uint32_t a = line + (uint32_t)(clampi(cx0 + j, 0, cw - 1) - wx0) * S;
+                    d1[j] = win_load<T>(a);
+                    d2[j] = win_load<T>(a + (uint32_t)Wn::kCompBytes);
+                }
+            }
+        } else if (fast) {
             load_row_own<NW, SX, T>(p1, cpitch, y, ch, bx, xl, xr, d1);
             load_row_own<NW, SX, T>(p2, cpitch, y, ch, bx, xl, xr, d2);
         } else if (valid) {
@@ -533,7 +632,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                 }
 #pragma unroll
                 for (int x = 0; x < 8; x++) {
-                    const int yv = my[(8 * r + x) * kThreadsB];
+                    const int yv = my[(8 * r + x) * NT];
                     int R, G, B;
                     to_rgb<MODE>(yv, c1[x], c2[x], R, G, B);
                     px[3 * x] = R;
@@ -605,11 +704,13 @@ reconstruct_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restr
                    const uint32_t *__restrict__ wide_flags, const uint32_t *__restrict__ list, uint8_t *__restrict__ out) {
     __shared__ int ys[64 * kThreadsB];  // [coefficient][thread]; warps only ever touch their own 32 columns
     if (!kListed) {
-        reconstruct_tile<NC, SX, SY, T>(frames[blockIdx.z], ys, coef, samples, wide_flags, out);
+        const FrameRecon &f = frames[blockIdx.z];
+        reconstruct_tile<NC, SX, SY, T>(f, ys, coef, samples, 0u, sizeof(T) == 4 && wide_flags[f.status_idx] != 0u, out);
     } else {
         const uint32_t n = list[0];
         for (uint32_t k = blockIdx.z; k < n; k += gridDim.z) {
-            reconstruct_tile<NC, SX, SY, T>(frames[list[1 + k]], ys, coef, samples, wide_flags, out);
+            const FrameRecon &f = frames[list[1 + k]];
+            reconstruct_tile<NC, SX, SY, T>(f, ys, coef, samples, 0u, sizeof(T) == 4 && wide_flags[f.status_idx] != 0u, out);
             __syncwarp();
         }
     }
@@ -617,74 +718,27 @@ reconstruct_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restr
 
 
 // =====================================================================================================
-// fused reconstruction for 4:2:0 frames: chroma IDCT + luma IDCT + upsampling + colour + store in ONE kernel
+// 4:2:0 frames: chroma IDCT + luma IDCT + upsampling + colour + store in ONE kernel
 // =====================================================================================================
-// A CTA is one warp. It owns a strip of 32 luma block columns (256 pixels) and walks a segment of the frame top to bottom,
-// two luma block rows per chroma block row:
-//     [C(r0-1)]  C(r0)   L(2 r0)  C(r0+1)  L(2 r0 + 1)  L(2 r0 + 2)  C(r0+2)  L(2 r0 + 3) ...
-// C(k): the 16 Cb + 16 Cr blocks under the strip -- one per lane, the same two compact IDCT loops as a luma row -- go as
-// int16 samples into a two-slot ring in shared memory (slot k & 1: eight sample rows of 128 columns per component plus the
-// one column either side that the upsampling window of the strip's first / last luma block needs).  Those two halo columns
-// belong to the neighbouring strips' blocks; only that one column of them is computed: per (component, side) eight single
-// outputs of the row pass -- one dot product per lane, the row pass is linear before its rounding shift -- and one column
-// pass.  L(j): exactly the luma row of reconstruct_kernel, with the chroma window read from the ring instead of from planes
-// in HBM.  Nothing but coefficients is read from and nothing but pixels is written to HBM: the sample planes, the kernel that
-// wrote them and their 16.5 MB per 4K frame round trip are gone.  A segment recomputes one chroma block row of its upper
-// neighbour (1 / seg_rows of the chroma work); the host picks seg_rows so that the grid fills the chip.
-// Frames whose chroma samples do not fit int16 are flagged `narrow` and redone by the int32 instance (list-driven), as before.
-// ring: [slot 2][component 2][row 8][128 columns] of T, followed by the halo columns [slot][component][row][left, right]
-template <typename T>
-struct RingOf {
-    static constexpr int kRowBytes = 128 * (int)sizeof(T);
-    static constexpr int kCompBytes = 8 * kRowBytes;
-    static constexpr int kSlotBytes = 2 * kCompBytes;
-    static constexpr int kMainBytes = 2 * kSlotBytes;
-    static constexpr int kHaloRowBytes = 2 * (int)sizeof(T);
-    static constexpr int kHaloCompBytes = 8 * kHaloRowBytes;
-    static constexpr int kHaloSlotBytes = 2 * kHaloCompBytes;
-    static constexpr int kBytes = kMainBytes + 2 * kHaloSlotBytes;
-};
+// A CTA covers 32 luma block columns x kRows420 luma block rows, one warp per row. Phase 1 fills the chroma window
+// (Window420) with the int16 samples of both chroma components:
+//  - warps 0 .. kRows420/2 - 1: one chroma block row under the tile each, 16 Cb + 16 Cr blocks through the tile helpers;
+//  - the next two warps: the line above / below the tile, the row pass of the chroma block row above / below, then only output
+//    row 7 / 0 of the column pass;
+//  - every warp: the columns left and right of the tile (corners included), column 7 / 0 of the neighbouring blocks, eight
+//    lanes per block: one output of the row pass per coefficient row (a dot product), then one column pass.
+// Phase 2 is b2's reconstruct_tile<3, 2, 2> with the chroma window read from shared memory instead of the planes. HBM sees
+// coefficients in and pixels out only: b1's chroma planes (written once, read once: 16.6 MB per 4K frame) and the memory
+// they take are gone. Window positions outside the chroma plane are never read: phase 2 clamps its addressing to the true
+// subsampled size like b2 (upsamplerbase.cpp:322-323, upsampler.cpp:100-106), and the clamped positions lie in the window.
+// Range flags as in b1 + b2: a window sample outside int16 flags the frame `narrow`, and the int32 instance (list-driven)
+// redoes it; there a window sample beyond +-kWide selects the 64-bit colour mode for the CTA.
 
-__device__ __forceinline__ uint32_t lds32(uint32_t a) {
-    uint32_t v;
-    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
-    return v;
-}
-__device__ __forceinline__ uint2 lds64(uint32_t a) {
-    uint2 v;
-    asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(v.x), "=r"(v.y) : "r"(a) : "memory");
-    return v;
-}
-__device__ __forceinline__ uint4 lds128(uint32_t a) {
-    uint4 v;
-    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a) : "memory");
-    return v;
-}
-__device__ __forceinline__ int lds_s16(uint32_t a) {
-    int v;
-    asm volatile("ld.shared.s16 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
-    return v;
-}
-__device__ __forceinline__ void sts16(uint32_t a, int v) { asm volatile("st.shared.u16 [%0], %1;" ::"r"(a), "h"((short)v) : "memory"); }
-__device__ __forceinline__ void sts32(uint32_t a, int v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
-
-// one ring sample (T = short / int) at a shared-space byte address
-template <typename T>
-__device__ __forceinline__ int ring_load(uint32_t a) {
-    return sizeof(T) == 2 ? lds_s16(a) : (int)lds32(a);
-}
-template <typename T>
-__device__ __forceinline__ void ring_store(uint32_t a, int v) {
-    if (sizeof(T) == 2) sts16(a, v);
-    else sts32(a, v);
-}
-
-// The warp's 32 blocks of coefficients come in as 4 KB of 16-byte pieces, eight per lane (piece i * 32 + lane): a luma row is
-// one contiguous run, a chroma row two runs of 2 KB (Cb blocks 0..15, Cr blocks 16..31). tile_fetch only ISSUES the loads --
-// the strip walk calls it for the NEXT unit before it computes the current one, so HBM latency hides behind a whole unit of
-// arithmetic --, tile_idct parks the pieces in the upper half of the tile (piece (block, row) at row segment 32 + 4 row +
-// block / 8, slot (block % 8) ^ row: conflict-free both ways), hands every lane its own block and runs the row pass and the
-// column pass (dct/idct.cpp:237-334) as two compact loops over the tile [sample][lane].
+// The warp's 32 blocks of coefficients come in as 4 KB of 16-byte pieces, eight per lane (piece i * 32 + lane): a chroma row is
+// two runs of 2 KB (Cb blocks 0..15, Cr blocks 16..31). tile_stash parks the pieces in the upper half of the warp's tile (piece
+// (block, row) at row segment 32 + 4 row + block / 8, slot (block % 8) ^ row: conflict-free both ways), tile_idct hands every
+// lane its own block and runs the row pass and the column pass (dct/idct.cpp:237-334) as two compact loops over the tile
+// [sample][lane].
 template <typename Have>
 __device__ __forceinline__ void tile_fetch(uint4 (&pc)[8], const uint4 *__restrict__ src_a, const uint4 *__restrict__ src_b, Have have) {
     const uint32_t lane = threadIdx.x & 31, sub = lane >> 3;
@@ -707,10 +761,12 @@ __device__ __forceinline__ void tile_stash(int *ys, const uint4 (&pc)[8]) {
     __syncwarp();
 }
 
-// Returns this lane's block's min / max sample in mn / mx. `sink(k, v)` receives column k of the block (v[r] = sample of row r):
-// a luma row puts it back into the tile for the line loop, a chroma row sends it straight to the sample ring.
-template <typename Sink>
-__device__ __forceinline__ void tile_idct(int *ys, int &mn, int &mx, Sink sink) {
+// `sink(k, r, a, b)` receives the samples (row r, columns k and k + 1) of this lane's block, k even; only = -1: all 64 samples,
+// only = 0 / 7: row 0 / 7 alone. kRows: coefficient rows 0 .. kRows - 1 may be non-zero, the others are zero in every block of
+// the warp: their row pass would only yield zeros, so it is skipped and the column pass sees literal zeros (the same integer
+// arithmetic, folded by the compiler). Returns the min / max of what was sunk in mn / mx (both start at 0).
+template <int kRows, typename Sink>
+__device__ __forceinline__ void tile_idct_rows(int *ys, int only, int &mn, int &mx, Sink sink) {
     const uint32_t lane = threadIdx.x & 31;
     int *my = ys + lane;
     const uint32_t wseg = (uint32_t)__cvta_generic_to_shared(ys);
@@ -718,8 +774,8 @@ __device__ __forceinline__ void tile_idct(int *ys, int &mn, int &mx, Sink sink) 
     auto piece = [&](int r) { return lds128(mine + 512u * (uint32_t)r + 16u * ((lane & 7u) ^ (uint32_t)r)); };
     uint4 q = piece(0);
 #pragma unroll 1
-    for (int r = 0; r < 8; r++) {
-        const uint4 qn = piece((r < 7) ? r + 1 : r);
+    for (int r = 0; r < kRows; r++) {
+        const uint4 qn = piece((r < kRows - 1) ? r + 1 : r);
         int v[8];
         unpack_row_raw(q, v);
         if (r == 0) v[0] = WADD(v[0], 128 << 3);  // dcoffset << 3 (idct.cpp:233,244), the << 4 preshift left out like in the inputs
@@ -731,61 +787,96 @@ __device__ __forceinline__ void tile_idct(int *ys, int &mn, int &mx, Sink sink) 
     }
     mx = 0, mn = 0;
 #pragma unroll 1
-    for (int k = 0; k < 8; k++) {
-        int v[8];
+    for (int k = 0; k < 8; k += 2) {
+        int a[8], b[8];
 #pragma unroll
-        for (int r = 0; r < 8; r++) v[r] = my[(8 * r + k) * 32];
-        idct8t<2048, 12>(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-        sink(k, v);
-        mx = __vimax3_s32(__vimax3_s32(mx, v[0], v[1]), v[2], v[3]);
-        mx = __vimax3_s32(__vimax3_s32(mx, v[4], v[5]), v[6], v[7]);
-        mn = __vimin3_s32(__vimin3_s32(mn, v[0], v[1]), v[2], v[3]);
-        mn = __vimin3_s32(__vimin3_s32(mn, v[4], v[5]), v[6], v[7]);
+        for (int r = 0; r < 8; r++) {
+            a[r] = (r < kRows) ? my[(8 * r + k) * 32] : 0;
+            b[r] = (r < kRows) ? my[(8 * r + k + 1) * 32] : 0;
+        }
+        if (only < 0) {
+            idct8t<2048, 12>(a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7]);
+            idct8t<2048, 12>(b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7]);
+#pragma unroll
+            for (int r = 0; r < 8; r++) sink(k, r, a[r], b[r]);
+#pragma unroll
+            for (int r = 0; r < 8; r += 2) {
+                mx = __vimax3_s32(__vimax3_s32(mx, a[r], a[r + 1]), b[r], b[r + 1]);
+                mn = __vimin3_s32(__vimin3_s32(mn, a[r], a[r + 1]), b[r], b[r + 1]);
+            }
+        } else {
+            // output 0 / 7 of the column pass is one dot product: the butterfly of idct8t is linear in front of its rounding shift
+            //   out0 = 512 v0 + 710 v1 + 669 v2 + 602 v3 + 512 v4 + 402 v5 + 277 v6 + 141 v7,  out7 = the same with the odd terms negated
+            auto one = [&](const int (&v)[8]) {
+                const int even = WADD(WADD(WMUL(v[0], 512), WMUL(v[2], 669)), WADD(WMUL(v[4], 512), WMUL(v[6], 277)));
+                const int odd = WADD(WADD(WMUL(v[1], 710), WMUL(v[3], 602)), WADD(WMUL(v[5], 402), WMUL(v[7], 141)));
+                return WADD(only == 0 ? WADD(even, odd) : WSUB(even, odd), 2048) >> 12;
+            };
+            const int sa = one(a), sb = one(b);
+            sink(k, only, sa, sb);
+            mx = __vimax3_s32(mx, sa, sb);
+            mn = __vimin3_s32(mn, sa, sb);
+        }
     }
 }
 
-template <typename T, bool kListed>
-__device__ __forceinline__ void reconstruct420_strip(const FrameRecon &f, int *ys, uint32_t ring, const int16_t *__restrict__ coef,
-                                                     uint32_t *__restrict__ narrow_flags, uint8_t *__restrict__ out, uint32_t seg_rows) {
-    using R = RingOf<T>;
-    const uint32_t W = f.width, H = f.height;
-    const uint32_t vbw = (W + 7) >> 3, vbh = (H + 7) >> 3;  // luma blocks that carry visible pixels
-    const int cw = (int)f.cw, ch = (int)f.ch;
-    const uint32_t vch = ((uint32_t)ch + 7u) >> 3;          // chroma block rows that carry real lines
+// Chroma blocks of ordinary images rarely carry anything in coefficient rows 6 and 7 (4:2:0 q75 frames of the benchmark: in
+// about 98 % of the warps none of the 32 blocks does), so the warp checks once and takes the shorter instance when it can.
+template <typename Sink>
+__device__ __forceinline__ void tile_idct(int *ys, int only, int &mn, int &mx, Sink sink) {
     const uint32_t lane = threadIdx.x & 31;
-    const uint32_t sx = blockIdx.x, bx0 = sx * 32u, bx = bx0 + lane;
-    const uint32_t r0 = blockIdx.y * seg_rows;
-    const uint32_t rows_all = (vbh + 1u) >> 1;              // chroma block rows that have luma rows to serve
-    if (r0 >= rows_all || bx0 >= vbw) return;
-    const uint32_t r1 = (r0 + seg_rows < rows_all) ? r0 + seg_rows : rows_all;
-    const uint32_t bwc = f.bw[1];
-    int *my = ys + lane;
-    uint32_t wide_slot[2] = {0u, 0u};  // warp-uniform: a chroma sample of that ring slot lies outside the 32-bit colour range
+    const uint32_t mine = (uint32_t)__cvta_generic_to_shared(ys) + 128u * (32u + (lane >> 3));
+    const uint4 p6 = lds128(mine + 512u * 6u + 16u * ((lane & 7u) ^ 6u)), p7 = lds128(mine + 512u * 7u + 16u * ((lane & 7u) ^ 7u));
+    const bool high = ((p6.x | p6.y | p6.z | p6.w) | (p7.x | p7.y | p7.z | p7.w)) != 0u;
+    if (__any_sync(0xffffffffu, high)) tile_idct_rows<8>(ys, only, mn, mx, sink);
+    else tile_idct_rows<6>(ys, only, mn, mx, sink);
+}
 
-    // ---- C(k): chroma block row k -> ring slot k & 1
-    auto chroma_row = [&](uint32_t k) {
-        const uint32_t slot = k & 1u;
-        const uint32_t comp = lane >> 4, bl = lane & 15u;  // this lane's block: Cb / Cr, column 16 sx + bl
-        const uint32_t cbx0 = 16u * sx;
-        int mn, mx;
-        // samples -> ring, one column of the block per step of the column pass (two lanes share a bank: comp stride and the
-        // 16-byte block pitch put lanes bl and bl + 8 on the same one)
-        const uint32_t base = ring + slot * R::kSlotBytes + comp * R::kCompBytes + (8u * bl) * (uint32_t)sizeof(T);
-        tile_idct(ys, mn, mx, [&](int k, const int (&v)[8]) {
-#pragma unroll
-            for (int r = 0; r < 8; r++) ring_store<T>(base + (uint32_t)r * R::kRowBytes + (uint32_t)k * (uint32_t)sizeof(T), v[r]);
-        });
-        // ---- halo columns: lane (h, r) = (lane >> 3, lane & 7); h & 1 = side (0: column 7 of the block to the left, 1: column 0
-        // of the block to the right), h >> 1 = component. Output 0 / 7 of the row pass over coefficient row r is one dot
-        // product (the butterfly is linear in front of its rounding shift):
-        //   out0 = 512 v0 + 710 v1 + 669 v2 + 602 v3 + 512 v4 + 402 v5 + 277 v6 + 141 v7,  out7 = the same with the odd terms negated
-        {
-            const uint32_t h = lane >> 3, r = lane & 7u, side = h & 1u, hc = h >> 1;
-            const int nb = side ? (int)(cbx0 + 16u) : (int)cbx0 - 1;
-            const bool exists = nb >= 0 && nb < (int)bwc;
+template <typename T>
+__device__ __forceinline__ void reconstruct420_tile(const FrameRecon &f, int *ys, uint32_t win, const int16_t *__restrict__ coef,
+                                                    uint32_t *__restrict__ narrow_flags, uint8_t *__restrict__ out) {
+    using Wn = Window420<T>;
+    constexpr int kHalf = kRows420 / 2;  // chroma block rows under the tile
+    const uint32_t vbw = (f.width + 7) >> 3, vbh = (f.height + 7) >> 3;
+    if (blockIdx.x * 32u >= vbw || blockIdx.y * (uint32_t)kRows420 >= vbh) return;  // whole CTA
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int bwc = (int)f.bw[1], bhc = (int)f.bh[1];
+    const int cbx0 = 16 * (int)blockIdx.x, cby0 = kHalf * (int)blockIdx.y;
+    auto at = [&](uint32_t comp, int line, int col) {
+        return win + comp * (uint32_t)Wn::kCompBytes + (uint32_t)line * (uint32_t)Wn::kLineBytes + (uint32_t)col * (uint32_t)sizeof(T);
+    };
+    int mn = 0, mx = 0;
+
+    // ---- phase 1a: chroma block rows -> window; q = the block row relative to the tile (-1: the row above, kHalf: below)
+    if (warp < (uint32_t)kHalf + 2u) {
+        const int q = (warp < (uint32_t)kHalf) ? (int)warp : (warp == (uint32_t)kHalf ? -1 : kHalf);
+        const int cby = cby0 + q;
+        if (cby >= 0 && cby < bhc) {
+            int *yw = ys + warp * 2048u;  // this warp's 8 KB of the luma tile, free until phase 2
+            uint4 pc[8];
+            const uint4 *src_a = reinterpret_cast<const uint4 *>(coef + f.coef_base[1] + ((uint64_t)cby * (uint32_t)bwc + (uint32_t)cbx0) * 64u);
+            const uint4 *src_b = reinterpret_cast<const uint4 *>(coef + f.coef_base[2] + ((uint64_t)cby * (uint32_t)bwc + (uint32_t)cbx0) * 64u);
+            tile_fetch(pc, src_a, src_b, [&](uint32_t blk) { return cbx0 + (int)(blk & 15u) < bwc; });
+            tile_stash(yw, pc);
+            const uint32_t comp = lane >> 4;
+            const int col = 4 + 8 * (int)(lane & 15u), line0 = 1 + 8 * q;  // window line of the block's row 0
+            tile_idct(yw, q < 0 ? 7 : (q == kHalf ? 0 : -1), mn, mx,
+                      [&](int k, int r, int a, int b) { win_store2<T>(at(comp, line0 + r, col + k), a, b); });
+        }
+    }
+    // ---- phase 1b: the columns left / right of the tile. Eight lanes per (block row j, component, side); lane r&7 = coefficient
+    // row r, then = output row r of the column pass
+    {
+        const uint32_t job = threadIdx.x >> 3, r = lane & 7u;
+        if (job < 4u * (kHalf + 2)) {  // warp-uniform: four jobs per warp
+            const uint32_t side = job & 1u, hc = (job >> 1) & 1u;
+            const int j = (int)(job >> 2), cby = cby0 - 1 + j;
+            const int nb = side ? cbx0 + 16 : cbx0 - 1;
+            const bool exists = nb >= 0 && nb < bwc && cby >= 0 && cby < bhc;
             int v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-            if (exists) unpack_row_raw(__ldg(reinterpret_cast<const uint4 *>(coef + f.coef_base[1 + hc] + ((uint64_t)k * bwc + (uint32_t)nb) * 64u) + r), v);
+            if (exists) unpack_row_raw(__ldg(reinterpret_cast<const uint4 *>(coef + f.coef_base[1 + hc] + ((uint64_t)cby * (uint32_t)bwc + (uint32_t)nb) * 64u) + r), v);
             if (r == 0) v[0] = WADD(v[0], 128 << 3);
+            // output 0 (side 1) / 7 (side 0) of the row pass, the dot products of tile_idct
             const int even = WADD(WADD(WMUL(v[0], 512), WMUL(v[2], 669)), WADD(WMUL(v[4], 512), WMUL(v[6], 277)));
             const int odd = WADD(WADD(WMUL(v[1], 710), WMUL(v[3], 602)), WADD(WMUL(v[5], 402), WMUL(v[7], 141)));
             const int inter = WADD(side ? WADD(even, odd) : WSUB(even, odd), 16) >> 5;  // row pass without the << 4 preshift, see unpack_row_raw
@@ -793,246 +884,41 @@ __device__ __forceinline__ void reconstruct420_strip(const FrameRecon &f, int *y
 #pragma unroll
             for (int i = 0; i < 8; i++) c[i] = __shfl_sync(0xffffffffu, inter, (int)((lane & ~7u) + (uint32_t)i));
             idct8t<2048, 12>(c[0], c[1], c[2], c[3], c[4], c[5], c[6], c[7]);
-            int mine = c[0];
+            int s = c[0];
 #pragma unroll
-            for (int i = 1; i < 8; i++) mine = (r == (uint32_t)i) ? c[i] : mine;
-            ring_store<T>(ring + R::kMainBytes + slot * R::kHaloSlotBytes + hc * R::kHaloCompBytes + r * R::kHaloRowBytes + side * (uint32_t)sizeof(T), mine);
-            if (exists) {
-                mx = mine > mx ? mine : mx;
-                mn = mine < mn ? mine : mn;
+            for (int i = 1; i < 8; i++) s = (r == (uint32_t)i) ? c[i] : s;
+            const int line = 8 * j - 7 + (int)r;  // the row above contributes its row 7 only, the row below its row 0
+            if (exists && line >= 0 && line < Wn::kLines) {
+                win_store<T>(at(hc, line, side ? 132 : 3), s);
+                mx = s > mx ? s : mx;
+                mn = s < mn ? s : mn;
             }
         }
-        if (sizeof(T) == 2) {
-            if (mx > 32767 || mn < -32768) atomicOr(narrow_flags + f.status_idx, 1u);  // `narrow`: the frame needs the int32 ring
-        } else {
-            wide_slot[slot] = __any_sync(0xffffffffu, mx > kWide || mn < -kWide) ? 1u : 0u;
-        }
-        __syncwarp();
-    };
-
-    // ---- L(by): one row of 32 luma blocks -> pixels
-    const uint32_t opitch = W * 3u;
-    const bool valid = bx < vbw;
-    const int X = 8 * (int)bx;
-    const int xmax = (X + 7 < (int)W) ? 7 : (int)((W - 1) & 7);
-    const int cx0 = X / 2 - 1;
-    // this lane's six window columns lie inside the plane: own four by one 8-byte (int16) load, the neighbours by one load each
-    const bool fastx = valid && cx0 >= 0 && cx0 + 6 <= cw;
-    const uint32_t own_off = (4u * lane) * (uint32_t)sizeof(T);
-    const uint32_t left_off = (4u * lane - 1u) * (uint32_t)sizeof(T), right_off = (4u * lane + 4u) * (uint32_t)sizeof(T);
-    auto luma_row = [&](uint32_t by) {
-        const int Y = 8 * (int)by;
-        int mn, mx;
-        tile_idct(ys, mn, mx, [&](int k, const int (&v)[8]) {
-#pragma unroll
-            for (int r = 0; r < 8; r++) my[(8 * r + k) * 32] = v[r];
-        });
-        if (!valid) return;
-        const int ymax = (Y + 7 < (int)H) ? 7 : (int)((H - 1) & 7);
-        uint8_t *obase = out + f.out_base + (uint64_t)Y * opitch + (uint64_t)X * 3u;
-        const int cy0 = Y / 2;
-        const bool ycbcr = f.ycbcr != 0;
-        const bool wide = (sizeof(T) == 4 && (wide_slot[0] | wide_slot[1]) != 0u) || mx > kWide || mn < -kWide;
-        // chroma line y (clamped to the plane = the duplicated first / last line, upsampler.cpp:100-106) of both components
-        auto fetch = [&](int y, int (&d1)[6], int (&d2)[6]) {
-            const int yc = clampi(y, 0, ch - 1);
-            const uint32_t slot = ((uint32_t)yc >> 3) & 1u, rr = (uint32_t)yc & 7u;
-            const uint32_t rowa = ring + slot * R::kSlotBytes + rr * R::kRowBytes;
-            const uint32_t haloa = ring + R::kMainBytes + slot * R::kHaloSlotBytes + rr * R::kHaloRowBytes;  // {left, right} of the row
-            if (fastx) {
-#pragma unroll
-                for (int c = 0; c < 2; c++) {
-                    int (&d)[6] = c ? d2 : d1;
-                    const uint32_t a = rowa + (uint32_t)c * R::kCompBytes, ha = haloa + (uint32_t)c * R::kHaloCompBytes;
-                    if (sizeof(T) == 2) {
-                        const uint2 o = lds64(a + own_off);
-                        d[1] = (int)(short)(o.x & 0xffffu), d[2] = (int)o.x >> 16, d[3] = (int)(short)(o.y & 0xffffu), d[4] = (int)o.y >> 16;
-                    } else {
-                        const uint4 o = lds128(a + own_off);
-                        d[1] = (int)o.x, d[2] = (int)o.y, d[3] = (int)o.z, d[4] = (int)o.w;
-                    }
-                    d[0] = ring_load<T>(lane == 0 ? ha : a + left_off);
-                    d[5] = ring_load<T>(lane == 31 ? ha + (uint32_t)sizeof(T) : a + right_off);
-                }
-            } else {
-                // at the frame edge: dest[-1] = dest[0], dest[width] = dest[width-1] at the TRUE subsampled width
-                // (upsamplerbase.cpp:322-323) = clamped addressing; a clamped column is a strip column or one of its halos
-#pragma unroll
-                for (int j = 0; j < 6; j++) {
-                    const int local = clampi(cx0 + j, 0, cw - 1) - 128 * (int)sx;
-                    const bool in_halo = local < 0 || local > 127;
-                    const uint32_t a = in_halo ? haloa + (local < 0 ? 0u : (uint32_t)sizeof(T)) : rowa + (uint32_t)local * (uint32_t)sizeof(T);
-                    d1[j] = ring_load<T>(a);
-                    d2[j] = ring_load<T>(a + (in_halo ? R::kHaloCompBytes : R::kCompBytes));
-                }
-            }
-        };
-        // four chroma lines live at a time: output lines r, r+1 lean on (A, B, C) = (top, cur, bot), lines r+2, r+3 on (B, C, D)
-        // (upsampler.cpp:92-106,160-165); the loop below runs twice, so the line window is renamed once instead of rotated four times
-        int A1[6], B1[6], C1[6], D1[6], A2[6], B2[6], C2[6], D2[6];
-        fetch(cy0 - 1, A1, A2);
-        fetch(cy0, B1, B2);
-        fetch(cy0 + 1, C1, C2);
-        fetch(cy0 + 2, D1, D2);
-        auto lines = [&](auto mode_tag) {
-            constexpr int MODE = decltype(mode_tag)::value;
-            // one output line: `n` = the neighbour line it leans on (top for even lines, bot for odd ones), `c` = the current line
-            auto one_line = [&](int r, auto odd_tag, const int (&n1)[6], const int (&c1w)[6], const int (&n2)[6], const int (&c2w)[6]) {
-                constexpr bool odd = decltype(odd_tag)::value;
-                constexpr int ra = odd ? 1 : 2, rb = odd ? 2 : 1;  // rounding of even / odd window columns (upsampler.cpp:136-168)
-                int w1[6], w2[6];
-#pragma unroll
-                for (int j = 0; j < 6; j += 2) {
-                    w1[j] = tap<ra>(n1[j], c1w[j]), w1[j + 1] = tap<rb>(n1[j + 1], c1w[j + 1]);
-                    w2[j] = tap<ra>(n2[j], c2w[j]), w2[j + 1] = tap<rb>(n2[j + 1], c2w[j + 1]);
-                }
-                int c1[8], c2[8];
-                hfilter2t(w1, c1);
-                hfilter2t(w2, c2);
-                int px[24];
-#pragma unroll
-                for (int x = 0; x < 8; x++) {
-                    int Rr, G, B;
-                    to_rgb<MODE>(my[(8 * r + x) * 32], c1[x], c2[x], Rr, G, B);
-                    px[3 * x] = Rr, px[3 * x + 1] = G, px[3 * x + 2] = B;
-                }
-                uint32_t wd[6];
-#pragma unroll
-                for (int k = 0; k < 6; k++) wd[k] = pack_sat4(px[4 * k], px[4 * k + 1], px[4 * k + 2], px[4 * k + 3]);
-                uint8_t *o = obase + (uint64_t)r * opitch;
-                if (xmax == 7 && ((reinterpret_cast<uintptr_t>(o) & 7u) == 0)) {
-                    uint2 *o2 = reinterpret_cast<uint2 *>(o);
-#pragma unroll
-                    for (int k = 0; k < 3; k++) o2[k] = make_uint2(wd[2 * k], wd[2 * k + 1]);
-                } else {
-#pragma unroll
-                    for (int x = 0; x < 8; x++) {
-                        if (x <= xmax) {
-#pragma unroll
-                            for (int i = 3 * x; i < 3 * x + 3; i++) o[i] = (uint8_t)(wd[i >> 2] >> (8 * (i & 3)));
-                        }
-                    }
-                }
-            };
-#pragma unroll 1
-            for (int r = 0; r < 8; r += 4) {
-                if (r > ymax) break;
-                one_line(r, std::false_type(), A1, B1, A2, B2);
-                if (r + 1 <= ymax) one_line(r + 1, std::true_type(), C1, B1, C2, B2);
-                if (r + 2 <= ymax) one_line(r + 2, std::false_type(), B1, C1, B2, C2);
-                if (r + 3 <= ymax) one_line(r + 3, std::true_type(), D1, C1, D2, C2);
-                if (r == 0) {
-#pragma unroll
-                    for (int j = 0; j < 6; j++) {
-                        A1[j] = C1[j], B1[j] = D1[j];
-                        A2[j] = C2[j], B2[j] = D2[j];
-                    }
-                    fetch(cy0 + 3, C1, C2);
-                    fetch(cy0 + 4, D1, D2);
-                }
-            }
-        };
-        if (!ycbcr) lines(std::integral_constant<int, 2>());
-        else if (wide) lines(std::integral_constant<int, 1>());
-        else lines(std::integral_constant<int, 0>());
-    };
-
-    // ---- the walk: [C(r0-1)] C(r0) { L(2k) [C(k+1)] [L(2k+1)] } for k = r0 .. r1-1, the coefficients of unit n+1 in flight
-    // (32 registers per lane) while unit n is computed
-    uint32_t kk = r0;
-    int phase = 0;
-    auto next_unit = [&](int &kind, uint32_t &idx) {  // kind 0: none, 1: chroma block row idx, 2: luma block row idx
-        for (;;) {
-            switch (phase) {
-            case 0:
-                phase = 1;
-                if (r0 > 0) {
-                    kind = 1, idx = r0 - 1;
-                    return;
-                }
-                break;
-            case 1:
-                phase = 2;
-                kind = 1, idx = r0;
-                return;
-            case 2:
-                if (kk >= r1) {
-                    phase = 5;
-                    break;
-                }
-                phase = 3;
-                kind = 2, idx = 2u * kk;
-                return;
-            case 3:
-                phase = 4;
-                if (kk + 1u < vch) {
-                    kind = 1, idx = kk + 1u;
-                    return;
-                }
-                break;
-            case 4: {
-                const uint32_t odd = 2u * kk + 1u;
-                phase = 2;
-                kk++;
-                if (odd < vbh) {
-                    kind = 2, idx = odd;
-                    return;
-                }
-                break;
-            }
-            default:
-                kind = 0, idx = 0;
-                return;
-            }
-        }
-    };
-    uint4 pc[8];
-    auto fetch_unit = [&](int kind, uint32_t idx) {
-        if (kind == 1) {
-            const uint32_t cbx0 = 16u * sx;
-            const uint4 *src_a = reinterpret_cast<const uint4 *>(coef + f.coef_base[1] + ((uint64_t)idx * bwc + cbx0) * 64u);
-            const uint4 *src_b = reinterpret_cast<const uint4 *>(coef + f.coef_base[2] + ((uint64_t)idx * bwc + cbx0) * 64u);
-            tile_fetch(pc, src_a, src_b, [&](uint32_t blk) { return cbx0 + (blk & 15u) < bwc; });
-        } else if (kind == 2) {
-            const uint4 *src = reinterpret_cast<const uint4 *>(coef + f.coef_base[0] + ((uint64_t)idx * f.bw[0] + bx0) * 64u);
-            tile_fetch(pc, src, src + 128, [&](uint32_t blk) { return bx0 + blk < f.bw[0]; });
-        }
-    };
-    int kind, nkind;
-    uint32_t idx, nidx;
-    next_unit(kind, idx);
-    fetch_unit(kind, idx);
-    while (kind) {
-        next_unit(nkind, nidx);
-        __syncwarp();  // every lane is done with the tile (and, before a chroma unit, with the ring slot it replaces)
-        tile_stash(ys, pc);
-        fetch_unit(nkind, nidx);
-        if (kind == 1) chroma_row(idx);
-        else luma_row(idx);
-        kind = nkind, idx = nidx;
     }
+    const bool out_of_range = (sizeof(T) == 2) ? (mx > 32767 || mn < -32768) : (mx > kWide || mn < -kWide);
+    const bool flagged = __syncthreads_or(out_of_range) != 0;
+    if (sizeof(T) == 2 && flagged && threadIdx.x == 0) atomicOr(narrow_flags + f.status_idx, 1u);  // `narrow`: the int32 instance redoes the frame
+
+    // ---- phase 2: the luma rows
+    reconstruct_tile<3, 2, 2, T, true>(f, ys, coef, nullptr, win, sizeof(T) == 4 && flagged, out);
 }
 
-// twelve one-warp CTAs per SM: 168 registers hold the prefetched coefficients of the next unit and a four-line chroma window
-// without spilling (13 and 10 CTAs per SM run at the same speed: the kernel is bound by instruction issue, not by occupancy)
-#ifndef B200JPG_FUSED_CTAS
-#define B200JPG_FUSED_CTAS 12
-#endif
-// grid (strips of 32 luma block columns, segments of seg_rows chroma block rows, frames or kWideSlots); one warp per CTA
+// grid (luma block columns / 32, luma block rows / kRows420, frames or kWideSlots); dynamic shared memory Window420<T>::kSmemBytes.
+// At kRows420 = 4 five CTAs (20 warps) per SM, like b2; the int32 instance (rare frames) three, which keeps it free of spills.
 template <typename T, bool kListed>
-__global__ void __launch_bounds__(32, (sizeof(T) == 2) ? B200JPG_FUSED_CTAS : 8)
+__global__ void __launch_bounds__(kThreads420, ((sizeof(T) == 2) ? 20 : 12) / kRows420)
 reconstruct420_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, uint32_t *__restrict__ narrow_flags,
-                      const uint32_t *__restrict__ list, uint8_t *__restrict__ out, uint32_t seg_rows) {
-    __shared__ int ys[64 * 32];
-    __shared__ __align__(16) uint8_t ring_mem[RingOf<T>::kBytes];
-    const uint32_t ring = (uint32_t)__cvta_generic_to_shared(ring_mem);
+                      const uint32_t *__restrict__ list, uint8_t *__restrict__ out) {
+    extern __shared__ __align__(16) uint8_t smem420[];
+    int *ys = reinterpret_cast<int *>(smem420);  // phase 2: [coefficient][thread]; phase 1: 8 KB per warp
+    const uint32_t win = (uint32_t)__cvta_generic_to_shared(smem420) + (uint32_t)Window420<T>::kYsBytes;
     if (!kListed) {
-        reconstruct420_strip<T, kListed>(frames[blockIdx.z], ys, ring, coef, narrow_flags, out, seg_rows);
+        reconstruct420_tile<T>(frames[blockIdx.z], ys, win, coef, narrow_flags, out);
     } else {
         const uint32_t n = list[0];
         for (uint32_t k = blockIdx.z; k < n; k += gridDim.z) {
-            reconstruct420_strip<T, kListed>(frames[list[1 + k]], ys, ring, coef, narrow_flags, out, seg_rows);
-            __syncwarp();
+            reconstruct420_tile<T>(frames[list[1 + k]], ys, win, coef, narrow_flags, out);
+            __syncthreads();  // the next frame's phase 1 overwrites the tile and the window
         }
     }
 }
@@ -1273,8 +1159,6 @@ template <typename T, bool kListed>
 static void launch_b2(const ReconLaunch &l, dim3 grid, const T *samples, cudaStream_t s) {
     if (l.ncomp == 1) {
         reconstruct_kernel<1, 1, 1, T, kListed><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, l.out);
-    } else if (l.subx == 2 && l.suby == 2) {
-        reconstruct_kernel<3, 2, 2, T, kListed><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, l.out);
     } else if (l.subx == 2 && l.suby == 1) {
         reconstruct_kernel<3, 2, 1, T, kListed><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, l.out);
     } else if (l.subx == 1 && l.suby == 2) {
@@ -1284,25 +1168,17 @@ static void launch_b2(const ReconLaunch &l, dim3 grid, const T *samples, cudaStr
     }
 }
 
-// seg_rows: chroma block rows per CTA of the fused kernel -- as long as possible (a segment recomputes one chroma block row
-// of its upper neighbour) while the grid still holds several waves of CTAs
-static uint32_t fused_seg_rows(const ReconLaunch &l, uint32_t strips, uint32_t rows_all) {
-    int dev = 0, sms = 132;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const uint64_t want = (uint64_t)sms * B200JPG_FUSED_CTAS * 6u;  // six waves
-    uint32_t seg = 16;
-    while (seg > 1 && (uint64_t)strips * ((rows_all + seg - 1) / seg) * l.n_frames < want) seg >>= 1;
-    return seg;
-}
-
-static int launch_recon_fused420(const ReconLaunch &l, cudaStream_t s, int *launches) {
-    const uint32_t strips = (l.max_bw0 + 31) / 32, rows_all = (l.max_bh0 + 1) / 2;
-    const uint32_t seg = fused_seg_rows(l, strips, rows_all);
-    const uint32_t gy = (rows_all + seg - 1) / seg;
-    reconstruct420_kernel<int16_t, false><<<dim3(strips, gy, l.n_frames), 32, 0, s>>>(l.frames, l.coef, l.narrow_flags, nullptr, l.out, seg);
+static int launch_recon420(const ReconLaunch &l, cudaStream_t s, int *launches) {
+    const uint32_t gx = (l.max_bw0 + 31) / 32, gy = (l.max_bh0 + kRows420 - 1) / kRows420;
+    constexpr int smem16 = Window420<int16_t>::kSmemBytes, smem32 = Window420<int32_t>::kSmemBytes;
+    cudaError_t e = cudaFuncSetAttribute(reconstruct420_kernel<int16_t, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    if (e == cudaSuccess && smem16 > 48 * 1024) e = cudaFuncSetAttribute(reconstruct420_kernel<int16_t, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem16);
+    if (e == cudaSuccess && smem32 > 48 * 1024) e = cudaFuncSetAttribute(reconstruct420_kernel<int32_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem32);
+    if (e != cudaSuccess) return (int)e;
+    reconstruct420_kernel<int16_t, false><<<dim3(gx, gy, l.n_frames), kThreads420, smem16, s>>>(l.frames, l.coef, l.narrow_flags, nullptr, l.out);
     // the exact pass over the frames flagged `narrow` (none for real images: two near-empty launches)
     narrow_list_kernel<<<1, 256, 0, s>>>(l.frames, l.n_frames, l.narrow_flags, l.narrow_list);
-    reconstruct420_kernel<int32_t, true><<<dim3(strips, gy, kWideSlots), 32, 0, s>>>(l.frames, l.coef, l.narrow_flags, l.narrow_list, l.out, seg);
+    reconstruct420_kernel<int32_t, true><<<dim3(gx, gy, kWideSlots), kThreads420, smem32, s>>>(l.frames, l.coef, l.narrow_flags, l.narrow_list, l.out);
     if (launches) *launches = 3;
     return (int)cudaGetLastError();
 }
@@ -1335,11 +1211,7 @@ int launch_recon(const ReconLaunch &l, void *stream, int *launches) {
     cudaStream_t s = (cudaStream_t)stream;
     int n = 0;
     if (l.generic) return launch_recon_generic(l, s, launches);
-    // B200JPG_FUSED=1 selects the single-kernel reconstruction of 4:2:0 frames (no sample planes: less DRAM traffic and 25 MB
-    // less memory per 4K frame, but the stage is bound by instruction issue, not by HBM, and the fused kernel issues more); the
-    // default is the two-kernel path through int16 planes.
-    const char *fused = getenv("B200JPG_FUSED");
-    if (l.ncomp == 3 && l.subx == 2 && l.suby == 2 && fused && fused[0] == '1') return launch_recon_fused420(l, s, launches);
+    if (l.ncomp == 3 && l.subx == 2 && l.suby == 2) return launch_recon420(l, s, launches);
     const uint32_t cblocks = (l.max_bwc * l.max_bhc + kThreadsB - 1) / kThreadsB;
     const uint32_t gx = (l.max_bw0 + 31) / 32, gy = (l.max_bh0 + kThreadsB / 32 - 1) / (kThreadsB / 32);
     // every frame through the int16 planes, B200JPG_RECON_CHUNK frames at a time (0: all at once): in chunks the planes b1 writes
