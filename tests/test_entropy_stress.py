@@ -2,8 +2,7 @@
 dequantised coefficients must equal what the writer coded times the quantiser, its pixels the oracle's and its status the
 oracle's verdict -- except the one frame whose coefficient +32768 leaves the int16 store, which the GPU reports as
 MALFORMED_STREAM (DESIGN.md section 7) while the frames around it stay exact. The same cases run again through the host restart
-index, the single-work-item path for restart-less scans, the scan-by-scan progressive kernels and the fused 4:2:0
-reconstruction."""
+index, the single-work-item path for restart-less scans and the scan-by-scan progressive kernels."""
 import glob
 import os
 
@@ -17,7 +16,6 @@ pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 SEQUENTIAL = [n for n in ec.NAMES if not ec.case(n)[0].progressive]
 PROGRESSIVE = [n for n in ec.NAMES if ec.case(n)[0].progressive]
-SUB420 = [n for n in ec.NAMES if [(c.h, c.v) for c in ec.case(n)[0].components] == [(2, 2), (1, 1), (1, 1)]]
 
 
 def gpu_decode(built, frames):
@@ -78,8 +76,7 @@ def test_all_cases_in_one_batch_next_to_golden_frames(built, oracle):
 
 
 @pytest.mark.parametrize("env,names", [({"B200JPG_HOST_INDEX": "1", "B200JPG_NO_SPEC": "1"}, SEQUENTIAL),
-                                       ({"B200JPG_NO_PFUSE": "1"}, PROGRESSIVE),
-                                       ({"B200JPG_FUSED": "1"}, SUB420)], ids=["host_index_no_spec", "no_pfuse", "fused420"])
+                                       ({"B200JPG_NO_PFUSE": "1"}, PROGRESSIVE)], ids=["host_index_no_spec", "no_pfuse"])
 def test_cases_through_the_other_paths(built, oracle, monkeypatch, env, names):
     assert names
     for k, v in env.items():

@@ -104,9 +104,11 @@ def test_batch_of_identical_geometry_is_frame_independent(built, oracle):
 @pytest.mark.parametrize("w,h,sub,z,dcq,copies", [(96, 80, (2, 2), 3, 255, 1), (200, 120, (2, 1), 0, 160, 1), (64, 64, (1, 1), 4, 255, 1),
                                                    (130, 70, (1, 2), 2, 200, 1), (320, 176, (2, 2), 20, 255, 5), (640, 360, (2, 2), 40, 160, 3)])
 def test_samples_beyond_the_fast_ranges_match_oracle(built, oracle, w, h, sub, z, dcq, copies):
-    """DC quantiser 255 on a full-range image: chroma samples beyond int16 (narrow planes) and luma / chroma beyond
-    +-65535 (32-bit colour arithmetic) -- the exact paths (int32 planes, 64-bit colour) must give the reference's
-    pixels; ordinary frames in the same batch must be unaffected."""
+    """DC quantiser patched to 160 .. 255 on a full-range image: most of these frames have chroma samples beyond int16 and go
+    through the exact path (int32 planes or the int32 instance of reconstruct420_kernel), which must give the reference's
+    pixels; ordinary frames in the same batch must be unaffected. No sample reaches +-65535 here (the peaks are about 62,000
+    luma and 49,000 chroma, and 640 x 360 stays inside int16), so the 64-bit colour mode is not exercised: the wide cases of
+    tests/test_recon420_stress.py are."""
     from libjpeg_b200 import synth
     normal = synth.encode(synth.source_image(w, h, 5), 75, sub, z)
     from tests import oracle_binding
@@ -481,12 +483,11 @@ def test_dnl_streams_match_reference_fixtures(built):
         assert np.array_equal(got[:-1], px[n + "__ref_dnl"][:-1]), n
 
 
-def test_fused_420_reconstruction_matches_oracle(built, oracle, golden_pixels, monkeypatch):
-    """The single-kernel reconstruction of 4:2:0 frames (B200JPG_FUSED=1: chroma IDCT into a shared-memory ring, no sample
-    planes) on the 4:2:0 goldens, odd sizes, frames whose samples leave the int16 / 32-bit colour ranges, and benchmark frames."""
+def test_fused_420_reconstruction_matches_oracle(built, oracle, golden_pixels):
+    """The 4:2:0 reconstruction (reconstruct420_kernel: chroma IDCT into a shared-memory window, no sample planes) on the 4:2:0
+    goldens, odd sizes, frames whose chroma samples leave int16, and benchmark frames, all in one batch."""
     from libjpeg_b200 import synth
     from tests import oracle_binding
-    monkeypatch.setenv("B200JPG_FUSED", "1")
     names = [n for n in NAMES if n.startswith("c420")]
     frames = [open(os.path.join(GOLDEN, n + ".jpg"), "rb").read() for n in names]
     want = [golden_pixels[n] for n in names]

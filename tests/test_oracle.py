@@ -89,6 +89,9 @@ def reference_cases():
     from tests import entropy_cases
     for name in entropy_cases.NAMES:
         yield "entropy_stress[%s]" % name, entropy_cases.case(name)[1]
+    from tests import recon420_cases
+    for name in recon420_cases.NAMES:
+        yield "recon420[%s]" % name, recon420_cases.case(name)[1]
 
 
 def check_reference(key, data, rc, px):
@@ -308,6 +311,21 @@ def test_oracle_matches_reference_on_hand_built_entropy_streams(oracle, name):
     data = entropy_cases.case(name)[1]
     rc, px = (oracle.decode16 if entropy_cases.case(name)[0].precision > 8 else oracle.decode)(data)
     check_reference("entropy_stress[%s]" % name, data, rc, px)
+
+
+def _recon420_case_names():
+    from tests import recon420_cases
+    return recon420_cases.NAMES
+
+
+@pytest.mark.parametrize("name", _recon420_case_names())
+def test_oracle_matches_reference_on_hand_built_reconstruction_frames(oracle, name):
+    """Frames of the test writer aimed at the 4:2:0 reconstruction (tests/recon420_cases.py: dense blocks at the CTA seams, the
+    row-6/7 skip, samples at the int16 edge and beyond the 32-bit colour range): the reference's samples."""
+    from tests import recon420_cases
+    data = recon420_cases.case(name)[1]
+    rc, px = oracle.decode(data)
+    check_reference("recon420[%s]" % name, data, rc, px)
 
 
 @pytest.mark.parametrize("name", NO_COLOR_TRANSFORM)
