@@ -3,7 +3,8 @@
  *
  * This is the drop-in boundary beneath the reference's C++ interface (include/interface/jpeg.hpp restates
  * thorfdbg/libjpeg's interface/jpeg.hpp:79-250): plain pointers and sizes, no C++ and no torch types.
- * The C++ `class JPEG` shim (libjpeg_b200/csrc/jpeg_shim.cpp) calls exactly these entry points; the batch
+ * The C++ `class JPEG` shim (libjpeg_b200/csrc/jpeg_shim.cpp) calls these entry points (and, for device bitmaps, the
+ * library's internal rectangle-to-bitmap copy kernel); the batch
  * entry points are what the throughput benchmark and the Python host layer bind (ctypes).
  *
  * What each entry point replaces in the reference (file:line relative to the reference tree):
@@ -17,6 +18,7 @@
  *                            IDCT::InverseTransformBlock                dct/idct.cpp:226
  *                            Upsampler<sx,sy>::UpsampleRegion           upsampling/upsampler.cpp:83
  *                            YCbCrTrafo::YCbCr2RGB                      colortrafo/ycbcrtrafo.cpp:679
+ *   b200jpg_batch_decode_into  the same, into per-component ImageBitMaps interface/imagebitmap.hpp:104-109
  *   b200jpg_last_error       JPEG::LastError                            interface/jpeg.cpp:962
  *
  * Error codes are the reference's (interface/parameters.hpp:1156-1228).
@@ -138,6 +140,30 @@ B200JPG_API int b200jpg_batch_reindex(b200jpg_batch *batch, void *stream);
 /* The hot path: entropy decode kernel(s) then reconstruction kernel(s), asynchronous on `stream`.
  * `out_dev` is a DEVICE pointer to b200jpg_batch_out_bytes(batch,-1) bytes. */
 B200JPG_API int b200jpg_batch_decode(b200jpg_batch *batch, uint8_t *out_dev, void *stream);
+/* Where component c of a frame goes, the device-side ImageBitMap of interface/imagebitmap.hpp:104-109 (ibm_pData,
+ * ibm_cBytesPerPixel, ibm_lBytesPerRow): the sample at (x, y) is written at
+ *     data + x * bytes_per_pixel + y * bytes_per_row      (both strides signed: BGR order, padded rows, bottom-up images)
+ * Samples are bytes for 8-bit frames, native-endian 16-bit for 12-bit frames (as in the packed output). */
+typedef struct b200jpg_plane {
+    void *data;
+    int32_t bytes_per_pixel;
+    int32_t pad;
+    int64_t bytes_per_row;
+} b200jpg_plane;
+
+/* b200jpg_batch_decode with caller-described destinations, what the reference's BitMapHook hands out per component
+ * (interface/bitmaphook.cpp, BitmapCtrl::RequestUserData control/bitmapctrl.cpp:142): planes[4*i + c] for frame i (the caller's frame index; JPEG XT residual
+ * codestreams own no output), component c < ncomp.  Component geometry is what the batch was created with: width x height,
+ * or ceil(width/subx[c]) x ceil(height/suby[c]) with B200JPG_FLAG_NO_UPSAMPLE.
+ * For every frame the call writes exactly the samples b200jpg_batch_decode writes into that frame's slot (damaged frames
+ * under tolerate_bad included), rearranged, and nothing else: bytes between pixels and between rows keep their contents.
+ * A frame whose parse failed has no destination (its data may be NULL).  Overlap between components or frames is the
+ * caller's responsibility, as in the reference.  Returns B200JPG_ERR_INVALID_PARAMETER and launches nothing when a live
+ * frame has a NULL data, a pointer is not device (or managed) memory of the batch's device, |bytes_per_pixel| is below the
+ * sample size, |bytes_per_row| < width * |bytes_per_pixel| for a component more than one row high, or a 16-bit destination
+ * is not 2-byte aligned in data or in either stride.  `planes` may be reused as soon as the call returns; the call issues
+ * as many kernel launches as b200jpg_batch_decode. */
+B200JPG_API int b200jpg_batch_decode_into(b200jpg_batch *batch, const b200jpg_plane *planes, void *stream);
 /* Only one of the two stages (profiling / roofline measurements / parity of the intermediate). */
 B200JPG_API int b200jpg_batch_decode_entropy(b200jpg_batch *batch, void *stream);
 B200JPG_API int b200jpg_batch_reconstruct(b200jpg_batch *batch, uint8_t *out_dev, void *stream);
@@ -182,8 +208,9 @@ B200JPG_API int b200jpg_decode_to_host_ex(b200jpg_ctx *ctx, const uint8_t *const
 
 /* The same, but the pixels STAY ON THE DEVICE (consumers that work on the GPU skip the PCIe copy of 24.9 MB per 4K frame, SURVEY 5):
  * *out_dev receives a device buffer (frame i at the 256-byte aligned running offset, frame 0 at 0; *out_bytes its size), to be
- * released with b200jpg_device_free.  b200jpg_device_copy_rect copies a rectangle of rows between two device bitmaps (what the
- * JPEG::DisplayRectangle shim does for clients whose BitMapHook hands out device pointers, JPGTAG_B200_DEVICE_BITMAPS). */
+ * released with b200jpg_device_free.  b200jpg_device_copy_rect copies a rectangle of rows between two device bitmaps (for clients
+ * that keep an interleaved device canvas of their own; JPEG::DisplayRectangle with JPGTAG_B200_DEVICE_BITMAPS copies into the
+ * client's per-component bitmaps with a kernel of its own). */
 B200JPG_API int b200jpg_decode_to_device_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, unsigned flags,
                                 uint8_t **out_dev, uint64_t *out_bytes);
 B200JPG_API void b200jpg_device_free(b200jpg_ctx *ctx, uint8_t *p);

@@ -18,7 +18,7 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden",
           "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
-CUDA_SOURCES = ["huffman_sm100.cu", "specsync_sm100.cu", "progressive_sm100.cu", "progfused_sm100.cu", "recon_sm100.cu", "microbench_sm100.cu"]
+CUDA_SOURCES = ["huffman_sm100.cu", "specsync_sm100.cu", "progressive_sm100.cu", "progfused_sm100.cu", "recon_sm100.cu", "bitmap_sm100.cu", "microbench_sm100.cu"]
 HOST_SOURCES = ["abi.cpp", "parse.cpp", "jpeg_shim.cpp"]
 
 

@@ -212,6 +212,13 @@ struct b200jpg_batch {
 
     size_t sz_status = 0, sz_ilen = 0;
     cudaEvent_t ev_last = nullptr;  // recorded after the last work enqueued for this batch: destroy waits for it
+    // b200jpg_batch_decode_into: the descriptor table [4 * n], staged in a ring of kPlaneSlots pinned copies and copied on the
+    // call's stream; ev_planes[k] is recorded behind the copy out of slot k, which is rewritten only after it. With several
+    // slots the host may run that many calls ahead of the device.
+    static constexpr int kPlaneSlots = 3;
+    b200jpg_plane *h_planes = nullptr, *d_planes = nullptr;
+    cudaEvent_t ev_planes[kPlaneSlots] = {};
+    int plane_slot = 0;
     int last_launches = 0;
     bool timing = false;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // start, after a0, after a1, after b
@@ -397,6 +404,10 @@ void b200jpg_batch_destroy(b200jpg_batch *b) {
     if (b->d_spec) b->ctx->put(1, b->d_spec, b->sz_spec);
     if (b->d_dcplane) b->ctx->put(1, b->d_dcplane, b->coef_elems / 64 * sizeof(int16_t));
     b->ctx->put(1, b->d_status, b->sz_status);
+    b->ctx->put(0, b->h_planes, sizeof(b200jpg_plane) * 4 * (size_t)b->n * b200jpg_batch::kPlaneSlots);
+    b->ctx->put(1, b->d_planes, sizeof(b200jpg_plane) * 4 * (size_t)b->n);
+    for (auto &e : b->ev_planes)
+        if (e) cudaEventDestroy(e);
     for (auto &e : b->ev)
         if (e) cudaEventDestroy(e);
     delete b;
@@ -1184,7 +1195,10 @@ static int run_entropy(b200jpg_batch *b, void *stream) {
     return B200JPG_OK;
 }
 
-static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream) {
+// planes_dev: b200jpg_batch_decode_into's descriptor table (device), planar[i]: every component of frame i has
+// bytes_per_pixel == sample size
+static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b200jpg_plane *planes_dev = nullptr,
+                     const std::vector<char> *planar = nullptr) {
     NvtxRange nvtx("b200jpg reconstruction: IDCT + upsampling + colour");
     cudaError_t me = cudaMemsetAsync(b->d_status + b->n, 0, sizeof(uint32_t) * 2 * (size_t)b->n, (cudaStream_t)stream);
     if (me != cudaSuccess) return b->ctx->fail_cuda(me, "flag reset");
@@ -1208,6 +1222,10 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream) {
         l.narrow_flags = b->d_status + 2 * (size_t)b->n;
         l.narrow_list = b->d_status + 3 * (size_t)b->n;
         l.out = out_dev;
+        l.planes = planes_dev;
+        l.planar = planes_dev != nullptr;
+        if (planes_dev)
+            for (const FrameRecon &fr : g.frames) l.planar = l.planar && (*planar)[fr.status_idx];
         int launches = 0;
         // grid.y carries the frame index: at most 65535 frames per launch. A generic group that is cut runs the IDCT of ALL its
         // frames first: a JPEG XT frame reads the planes of its residual frame, which may sit in another part
@@ -1234,10 +1252,8 @@ static int ensure_events(b200jpg_batch *b) {
     return 0;
 }
 
-int b200jpg_batch_decode(b200jpg_batch *b, uint8_t *out_dev, void *stream) {
-    if (!b || !out_dev) return B200JPG_ERR_INVALID_PARAMETER;
-    if (!b->uploaded) return b->ctx->fail(B200JPG_ERR_OBJECT_DOESNT_EXIST, "batch has not been uploaded");
-    cudaSetDevice(b->ctx->device);
+static int run_decode(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b200jpg_plane *planes_dev = nullptr,
+                      const std::vector<char> *planar = nullptr) {
     b->last_launches = 0;
     b->status_fetched = false;
     if (b->timing) {
@@ -1247,10 +1263,82 @@ int b200jpg_batch_decode(b200jpg_batch *b, uint8_t *out_dev, void *stream) {
     int rc = run_entropy(b, stream);
     if (rc) return rc;
     if (b->timing) cudaEventRecord(b->ev[1], (cudaStream_t)stream);
-    rc = run_recon(b, out_dev, stream);
+    rc = run_recon(b, out_dev, stream, planes_dev, planar);
     if (rc) return rc;
     if (b->timing) cudaEventRecord(b->ev[2], (cudaStream_t)stream);
     return B200JPG_OK;
+}
+
+int b200jpg_batch_decode(b200jpg_batch *b, uint8_t *out_dev, void *stream) {
+    if (!b || !out_dev) return B200JPG_ERR_INVALID_PARAMETER;
+    if (!b->uploaded) return b->ctx->fail(B200JPG_ERR_OBJECT_DOESNT_EXIST, "batch has not been uploaded");
+    cudaSetDevice(b->ctx->device);
+    return run_decode(b, out_dev, stream);
+}
+
+static uint64_t magnitude(int64_t v) { return v < 0 ? 0 - (uint64_t)v : (uint64_t)v; }
+
+int b200jpg_batch_decode_into(b200jpg_batch *b, const b200jpg_plane *planes, void *stream) {
+    if (!b || !planes) return B200JPG_ERR_INVALID_PARAMETER;
+    if (!b->uploaded) return b->ctx->fail(B200JPG_ERR_OBJECT_DOESNT_EXIST, "batch has not been uploaded");
+    cudaSetDevice(b->ctx->device);
+    // every descriptor of every live frame is checked before anything is enqueued
+    const bool own_size = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
+    std::vector<char> planar((size_t)b->n, 1);
+    for (int i = 0; i < b->n_user; i++) {
+        if (b->parse_status[i] != 0) continue;
+        const b200jpg_frame_info &fi = b->frames[i].info;
+        const uint64_t size = fi.precision > 8 ? 2 : 1;
+        for (int c = 0; c < fi.ncomp; c++) {
+            const b200jpg_plane &p = planes[4 * i + c];
+            const uint64_t w = own_size ? (fi.width + fi.subx[c] - 1) / fi.subx[c] : fi.width;
+            const uint64_t h = own_size ? (fi.height + fi.suby[c] - 1) / fi.suby[c] : fi.height;
+            const uint64_t bpp = magnitude(p.bytes_per_pixel), bpr = magnitude(p.bytes_per_row);
+            const std::string at = "frame " + std::to_string(i) + " component " + std::to_string(c) + ": ";
+            if (!p.data) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "no destination");
+            if (bpp < size) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "|bytes_per_pixel| is smaller than the sample size");
+            if (h > 1 && bpr < w * bpp) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "rows overlap: |bytes_per_row| < width * |bytes_per_pixel|");
+            if (size == 2 && ((reinterpret_cast<uintptr_t>(p.data) | bpp | bpr) & 1u))
+                return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "16-bit samples need a 2-byte aligned address and strides");
+            cudaPointerAttributes a{};
+            const cudaError_t e = cudaPointerGetAttributes(&a, p.data);
+            if (e != cudaSuccess) cudaGetLastError();
+            if (e != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != b->ctx->device)
+                return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "not device memory of the batch's device");
+            if ((uint64_t)p.bytes_per_pixel != size) planar[(size_t)i] = 0;
+        }
+    }
+    const size_t bytes = sizeof(b200jpg_plane) * 4 * (size_t)b->n;
+    cudaError_t ce = cudaSuccess;
+    constexpr int kSlots = b200jpg_batch::kPlaneSlots;
+    if (!b->d_planes) {  // everything is allocated before any of it is kept: a failure leaves the batch as it was
+        b200jpg_plane *h = (b200jpg_plane *)b->ctx->get(0, bytes * kSlots, &ce), *d = nullptr;
+        cudaEvent_t ev[kSlots] = {};
+        if (ce == cudaSuccess) d = (b200jpg_plane *)b->ctx->get(1, bytes, &ce);
+        for (int k = 0; k < kSlots && ce == cudaSuccess; k++) ce = cudaEventCreateWithFlags(&ev[k], cudaEventDisableTiming);
+        if (ce != cudaSuccess) {
+            const std::string why = cudaGetErrorString(ce);
+            b->ctx->put(0, h, bytes * kSlots);
+            b->ctx->put(1, d, bytes);
+            for (auto &e : ev)
+                if (e) cudaEventDestroy(e);
+            return b->ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "descriptor table allocation failed: " + why);
+        }
+        b->h_planes = h, b->d_planes = d;
+        for (int k = 0; k < kSlots; k++) b->ev_planes[k] = ev[k];
+    }
+    const int slot = b->plane_slot;
+    ce = cudaEventSynchronize(b->ev_planes[slot]);  // the copy kSlots calls ago has read this slot (at once when never recorded)
+    if (ce != cudaSuccess) return b->ctx->fail_cuda(ce, "descriptor table");
+    b200jpg_plane *stage = b->h_planes + 4 * (size_t)b->n * slot;
+    memset(stage, 0, bytes);  // residual codestreams and failed frames: no destination
+    for (int i = 0; i < b->n_user; i++)
+        if (b->parse_status[i] == 0) memcpy(stage + 4 * (size_t)i, planes + 4 * (size_t)i, sizeof(b200jpg_plane) * b->frames[i].info.ncomp);
+    ce = cudaMemcpyAsync(b->d_planes, stage, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream);
+    if (ce == cudaSuccess) ce = cudaEventRecord(b->ev_planes[slot], (cudaStream_t)stream);
+    b->plane_slot = (slot + 1) % kSlots;
+    if (ce != cudaSuccess) return b->ctx->fail_cuda(ce, "descriptor table upload");
+    return run_decode(b, nullptr, stream, b->d_planes, &planar);
 }
 
 int b200jpg_batch_decode_entropy(b200jpg_batch *b, void *stream) {
@@ -1536,3 +1624,22 @@ int b200jpg_device_copy_rect(b200jpg_ctx *ctx, uint8_t *dst_dev, int64_t dst_pit
 }
 
 }  // extern "C"
+
+namespace b200jpg {
+int device_bitmap_copy(b200jpg_ctx *ctx, const BitmapRequest &r, const uint8_t *src) {
+    if (!ctx || !src) return B200JPG_ERR_INVALID_PARAMETER;
+    cudaSetDevice(ctx->device);
+    for (int k = 0; k < r.ncomp; k++) {
+        if (!r.comp[k].dst) continue;
+        cudaPointerAttributes a{};
+        const cudaError_t e = cudaPointerGetAttributes(&a, r.comp[k].dst);
+        if (e != cudaSuccess) cudaGetLastError();
+        if (e != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != ctx->device)
+            return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "device bitmaps: component " + std::to_string(k) + " is not device memory of the decoding device");
+    }
+    int rc = launch_bitmap_copy(r, src, nullptr);
+    cudaError_t e = rc ? (cudaError_t)rc : cudaStreamSynchronize(nullptr);
+    if (e != cudaSuccess) return ctx->fail_cuda(e, "device bitmap copy");
+    return B200JPG_OK;
+}
+}  // namespace b200jpg

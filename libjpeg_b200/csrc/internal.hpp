@@ -270,7 +270,39 @@ struct ReconLaunch {
     uint32_t *wide_flags;          // [frames in batch], zeroed per decode: a chroma sample leaves the 32-bit colour range
     uint32_t *narrow_list;         // [1 + frames in group] scratch: {count, group-local indices of the flagged frames}
     uint8_t *out;
+    // b200jpg_batch_decode_into: where every component goes, [4 * frames in batch] indexed 4 * status_idx + c (device);
+    // null: the packed slots of `out`
+    const b200jpg_plane *planes;
+    bool planar;                   // every plane of the group's frames has bytes_per_pixel == sample size
 };
+
+// How the reconstruction kernels store a block (the destination kind of the launch, chosen per group from the descriptors):
+// kStoreCanvas: the packed slot of `out` (b200jpg_batch_decode); kStorePlanar: one plane per component, samples adjacent;
+// kStoreStrided: any signed pixel and row stride, one store per sample.
+enum StoreKind : int { kStoreCanvas = 0, kStorePlanar = 1, kStoreStrided = 2 };
 int launch_recon(const ReconLaunch &l, void *stream, int *launches);
+
+// JPEG::DisplayRectangle into device bitmaps (bitmap_sm100.cu): the rectangle x0..x1, y0..y1 (inclusive, in the coordinates of
+// the decoded samples) of every requested component goes from the decoded frame to the client's bitmap. Sample (x, y) of
+// component k is src[comp[k].src_off + y * src_pitch + x * src_step] (samples of 1 or 2 bytes, `deep`) and lands at
+// dst + x * bytes_per_pixel + y * bytes_per_row, as a byte or (wide_out) a native-endian 16-bit value. A component with a null
+// dst, and the samples of a block whose origin (inside the rectangle) lies outside its bitmap's width x height, stay unwritten.
+struct BitmapCopy {
+    uint8_t *dst;
+    int64_t bytes_per_pixel, bytes_per_row;
+    uint32_t width, height;
+    uint64_t src_off;
+    uint32_t src_step, src_pitch;
+};
+struct BitmapRequest {
+    BitmapCopy comp[4];
+    int ncomp;
+    int x0, x1, y0, y1;
+    int deep, wide_out;
+};
+int launch_bitmap_copy(const BitmapRequest &r, const uint8_t *src, void *stream);
+// the same from the C++ shim on the context's device: checks that every destination is device memory of that device, waits for
+// the copy; returns 0 or an error code (message on the context)
+int device_bitmap_copy(b200jpg_ctx *ctx, const BitmapRequest &r, const uint8_t *src);
 
 }  // namespace b200jpg

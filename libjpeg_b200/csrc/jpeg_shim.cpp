@@ -9,7 +9,8 @@
 //                                   control/bitmapctrl.cpp:142-160, control/blockbitmaprequester.cpp:1229-1244
 //                                   (BIO_HEIGHT >> 3 block rows), interface/imagebitmap.cpp:58-125 (canvas anchoring)
 //   JPEG::LastError                 interface/jpeg.cpp:962
-// Pixels come from b200jpg_decode_to_host (CUDA); there is no CPU decode in here.
+// Pixels come from b200jpg_decode_to_host (CUDA), or stay on the device for device bitmaps (b200jpg_decode_to_device_ex +
+// the copy kernel of bitmap_sm100.cu); there is no CPU decode in here.
 #include <cstdlib>
 #include <cstring>
 #include <memory>
@@ -19,6 +20,7 @@
 #include <vector>
 
 #include "b200jpg.h"
+#include "internal.hpp"
 #include "interface/hooks.hpp"
 #include "interface/jpeg.hpp"
 #include "interface/parameters.hpp"
@@ -367,7 +369,6 @@ JPG_LONG JPEG::DisplayRectangle(struct JPG_TagItem *tags) {
     const unsigned want_flags = !upsample ? (B200JPG_FLAG_NO_UPSAMPLE | B200JPG_FLAG_NO_COLOR_TRANSFORM)
                                           : ((!colortrafo && s.info.ycbcr) ? B200JPG_FLAG_NO_COLOR_TRANSFORM : 0u);
     if (device_bitmaps) {
-        if (!upsample) return s.fail(JPGERR_NOT_IMPLEMENTED, "device bitmaps are filled with upsampled, interleaved pixels only");
         if (!s.d_pixels || s.d_flags != want_flags) {
             b200jpg_ctx *ctx = 0;
             std::string msg;
@@ -479,22 +480,31 @@ JPG_LONG JPEG::DisplayRectangle(struct JPG_TagItem *tags) {
     long long last_by = (long long)(cmaxy >> 3);
     if ((long long)max_block_row < last_by) last_by = (long long)max_block_row;
     if (device_bitmaps) {
-        // the client's bitmaps are device memory: one rectangle copy on the device. Only the usual layout -- one interleaved
-        // canvas, component c at base + c -- is offered; whole blocks whose origin lies outside the bitmap stay unwritten
-        // (imagebitmap.cpp:78-110), like in the loop below
-        const BitmapLayout &l = lay[0];
-        if (!interleaved && !(nc == 1 && l.mem && l.pixel_type && l.bytes_per_pixel == sample_bytes && deep == wide_out && firstc == 0 && lastc == 0))
-            return s.fail(JPGERR_INVALID_PARAMETER, "device bitmaps must be one interleaved canvas of the frame's sample type");
-        JPG_LONG xlast = cmaxx, ylast = cmaxy;
-        if (last_by * 8 + 7 < ylast) ylast = (JPG_LONG)(last_by * 8 + 7);
-        if (l.width > 0 && (JPG_LONG)((((l.width - 1) >> 3) << 3) + 7) < xlast) xlast = (JPG_LONG)((((l.width - 1) >> 3) << 3) + 7);
-        if (l.height > 0 && (JPG_LONG)((((l.height - 1) >> 3) << 3) + 7) < ylast) ylast = (JPG_LONG)((((l.height - 1) >> 3) << 3) + 7);
-        if (l.width > 0 && l.height > 0 && l.width > (JPG_ULONG)cminx && l.height > (JPG_ULONG)cminy && xlast >= cminx && ylast >= cminy) {
-            const size_t px = (size_t)nc * sample_bytes;
-            int rc = b200jpg_device_copy_rect(s.d_ctx, l.mem + (ptrdiff_t)cminx * l.bytes_per_pixel + (ptrdiff_t)cminy * l.bytes_per_row, l.bytes_per_row,
-                                              s.d_pixels + ((size_t)cminy * W + (size_t)cminx) * px, (int64_t)((size_t)W * px),
-                                              (uint64_t)(xlast - cminx + 1) * px, (uint64_t)(ylast - cminy + 1));
-            if (rc) return s.fail(rc, "device rectangle copy failed");
+        // the client's bitmaps are device memory: the rectangle goes from the frame kept on the device to every requested
+        // component's bitmap in one kernel, with the rules of the loop below (whole blocks whose origin lies outside a bitmap,
+        // a NULL base or pixel type 0 leave the component unwritten, imagebitmap.cpp:78-110), any pointer and strides
+        b200jpg::BitmapRequest r{};
+        r.x0 = (int)cminx, r.x1 = (int)cmaxx, r.y0 = (int)cminy, r.y1 = (int)cmaxy;
+        if (last_by * 8 + 7 < (long long)r.y1) r.y1 = (int)(last_by * 8 + 7);
+        r.deep = deep, r.wide_out = wide_out;
+        for (int c = (int)firstc; c <= (int)lastc; c++) {
+            const BitmapLayout &l = lay[c];
+            b200jpg::BitmapCopy &k = r.comp[r.ncomp++];
+            k.dst = (l.mem && l.pixel_type) ? l.mem : nullptr;
+            k.bytes_per_pixel = l.bytes_per_pixel, k.bytes_per_row = l.bytes_per_row;
+            k.width = l.width, k.height = l.height;
+            // sample (x, y) of component c: in the interleaved frame, or in the component's own plane (as in the loop below)
+            k.src_off = upsample ? (uint64_t)c : (uint64_t)plane_at[c];
+            k.src_step = upsample ? (uint32_t)nc : 1u;
+            k.src_pitch = upsample ? W * (uint32_t)nc : plane_w[c];
+        }
+        if (r.y1 >= r.y0) {
+            int rc = b200jpg::device_bitmap_copy(s.d_ctx, r, s.d_pixels);
+            if (rc) {
+                const char *m = 0;
+                b200jpg_last_error(0, &m);
+                return s.fail(rc, (m && *m) ? m : "device bitmap copy failed");
+            }
         }
         last_by = -1;  // nothing left for the host loop
     }

@@ -397,6 +397,37 @@ __device__ __forceinline__ uint32_t pack_sat4(int p0, int p1, int p2, int p3) {
     return w;
 }
 
+// ---- destinations (StoreKind): the canvas kind stores into the batch's output buffer, the described kinds read the
+// frame's four b200jpg_plane descriptors at 4 * status_idx of the table b200jpg_batch_decode_into uploads
+template <int K>
+using StoreDst = std::conditional_t<K == kStoreCanvas, uint8_t *, const b200jpg_plane *>;
+
+// the sample (x, y) of a described component, signed 64-bit addressing (ImageBitMap, interface/imagebitmap.hpp:104-109).
+// The descriptor is read again at every call (L1 hits): held in registers through the line loop of reconstruct_tile, three of
+// them push the 4:2:0 kernel over its 96-register budget.
+__device__ __forceinline__ uint8_t *plane_at(const b200jpg_plane *p, int x, int y) {
+    uint64_t data, bpr;
+    int bpp;
+    asm volatile("ld.global.nc.u64 %0, [%1];" : "=l"(data) : "l"(&p->data));
+    asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(bpp) : "l"(&p->bytes_per_pixel));
+    asm volatile("ld.global.nc.u64 %0, [%1];" : "=l"(bpr) : "l"(&p->bytes_per_row));
+    return reinterpret_cast<uint8_t *>(data + (uint64_t)((int64_t)x * bpp) + (uint64_t)((int64_t)y * (int64_t)bpr));
+}
+
+// the first xmax + 1 of eight 8-bit samples (w0 | w1, sample 0 in the low byte of w0) from o on: one 8-byte store for a whole
+// aligned planar row, else one store per sample
+template <int K>
+__device__ __forceinline__ void store_row8(const b200jpg_plane *p, uint8_t *o, uint32_t w0, uint32_t w1, int xmax) {
+    if (K == kStorePlanar && xmax == 7 && (reinterpret_cast<uintptr_t>(o) & 7u) == 0) {
+        *reinterpret_cast<uint2 *>(o) = make_uint2(w0, w1);
+        return;
+    }
+    const int64_t s = (K == kStorePlanar) ? 1 : p->bytes_per_pixel;
+#pragma unroll
+    for (int x = 0; x < 8; x++)
+        if (x <= xmax) o[x * s] = (uint8_t)(((x < 4) ? w0 : w1) >> (8 * (x & 3)));
+}
+
 // ycbcrtrafo.cpp:842-850 with the matrix of colortransformerfactory.cpp:136-138 (13 fractional bits) and
 // FIX_COLOR_TO_INT (tools/numerics.hpp:65).  The reference multiplies in 64 bits; 32 bits give the same result
 // while |y|, |cb|, |cr| <= 65535 -- blocks that violate that (damaged streams only) are flagged `wide`.
@@ -425,9 +456,10 @@ __device__ __forceinline__ void to_rgb(int y, int cbv, int crv, int &r, int &g, 
 
 // kWin: the chroma samples come from the window of reconstruct420_kernel at shared-space address `win` instead of the sample
 // planes. chroma_wide: a chroma sample the tile reads may leave the 32-bit colour range.
-template <int NC, int SX, int SY, typename T, bool kWin = false>
+// K: the destination kind (StoreKind).
+template <int NC, int SX, int SY, typename T, bool kWin = false, int K = kStoreCanvas>
 __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, const int16_t *__restrict__ coef, const T *__restrict__ samples,
-                                                 uint32_t win, bool chroma_wide, uint8_t *__restrict__ out) {
+                                                 uint32_t win, bool chroma_wide, StoreDst<K> __restrict__ out) {
     static_assert(!kWin || (NC == 3 && SX == 2 && SY == 2), "the chroma window is 4:2:0 only");
     constexpr uint32_t NT = kWin ? kThreads420 : kThreadsB;  // threads per CTA: the stride of the tile [coefficient][thread]
     const uint32_t W = f.width, H = f.height;
@@ -503,23 +535,30 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
     const int xmax = (X + 7 < (int)W) ? 7 : (int)((W - 1) & 7);
     const int ymax = (Y + 7 < (int)H) ? 7 : (int)((H - 1) & 7);
     const uint32_t opitch = W * NC;
-    uint8_t *obase = out + f.out_base + (uint64_t)Y * opitch + (uint64_t)X * NC;
+    uint8_t *obase = nullptr;
+    const b200jpg_plane *pl = nullptr;  // described kinds: the frame's component descriptors
+    if constexpr (K == kStoreCanvas) obase = out + f.out_base + (uint64_t)Y * opitch + (uint64_t)X * NC;
+    else pl = out + 4u * f.status_idx;
 
     if (NC == 1) {  // identity, COLOR_TO_INT (numerics.hpp:69) + clamp
         if (!valid) return;
 #pragma unroll 1
         for (int r = 0; r <= ymax; r++) {
-            uint8_t *o = obase + (uint64_t)r * opitch;
+            uint8_t *o = (K == kStoreCanvas) ? obase + (uint64_t)r * opitch : plane_at(pl, X, Y + r);
             int px[8];
 #pragma unroll
             for (int x = 0; x < 8; x++) px[x] = WADD(my[(8 * r + x) * NT], 8) >> 4;
             const uint32_t w0 = pack_sat4(px[0], px[1], px[2], px[3]), w1 = pack_sat4(px[4], px[5], px[6], px[7]);
-            if (xmax == 7 && ((reinterpret_cast<uintptr_t>(o) & 7u) == 0)) {
-                *reinterpret_cast<uint2 *>(o) = make_uint2(w0, w1);
-            } else {
+            if (K == kStoreCanvas) {
+                if (xmax == 7 && ((reinterpret_cast<uintptr_t>(o) & 7u) == 0)) {
+                    *reinterpret_cast<uint2 *>(o) = make_uint2(w0, w1);
+                } else {
 #pragma unroll
-                for (int x = 0; x < 8; x++)
-                    if (x <= xmax) o[x] = (uint8_t)(((x < 4) ? w0 : w1) >> (8 * (x & 3)));
+                    for (int x = 0; x < 8; x++)
+                        if (x <= xmax) o[x] = (uint8_t)(((x < 4) ? w0 : w1) >> (8 * (x & 3)));
+                }
+            } else {
+                store_row8<K>(pl, o, w0, w1, xmax);
             }
         }
         return;
@@ -639,10 +678,23 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                     px[3 * x + 1] = G;
                     px[3 * x + 2] = B;
                 }
+                if (K == kStoreCanvas) {
 #pragma unroll
-                for (int k = 0; k < 6; k++) wd[k] = pack_sat4(px[4 * k], px[4 * k + 1], px[4 * k + 2], px[4 * k + 3]);
+                    for (int k = 0; k < 6; k++) wd[k] = pack_sat4(px[4 * k], px[4 * k + 1], px[4 * k + 2], px[4 * k + 3]);
+                } else {  // component by component: wd[2 c], wd[2 c + 1] = the eight samples of component c
+#pragma unroll
+                    for (int c = 0; c < 3; c++) {
+                        wd[2 * c] = pack_sat4(px[c], px[3 + c], px[6 + c], px[9 + c]);
+                        wd[2 * c + 1] = pack_sat4(px[12 + c], px[15 + c], px[18 + c], px[21 + c]);
+                    }
+                }
             }
-            if (valid) {
+            if (K != kStoreCanvas) {
+                if (valid) {
+#pragma unroll
+                    for (int c = 0; c < 3; c++) store_row8<K>(pl + c, plane_at(pl + c, X, Y + r), wd[2 * c], wd[2 * c + 1], xmax);
+                }
+            } else if (valid) {
                 uint8_t *o = obase + (uint64_t)r * opitch;
                 if (xmax == 7 && ((reinterpret_cast<uintptr_t>(o) & 7u) == 0)) {
                     uint2 *o2 = reinterpret_cast<uint2 *>(o);
@@ -698,19 +750,19 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
 #ifndef B200JPG_B2_MINCTAS
 #define B200JPG_B2_MINCTAS 5
 #endif
-template <int NC, int SX, int SY, typename T, bool kListed>
+template <int NC, int SX, int SY, typename T, bool kListed, int K>
 __global__ void __launch_bounds__(kThreadsB, B200JPG_B2_MINCTAS)
 reconstruct_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, const T *__restrict__ samples,
-                   const uint32_t *__restrict__ wide_flags, const uint32_t *__restrict__ list, uint8_t *__restrict__ out) {
+                   const uint32_t *__restrict__ wide_flags, const uint32_t *__restrict__ list, StoreDst<K> __restrict__ out) {
     __shared__ int ys[64 * kThreadsB];  // [coefficient][thread]; warps only ever touch their own 32 columns
     if (!kListed) {
         const FrameRecon &f = frames[blockIdx.z];
-        reconstruct_tile<NC, SX, SY, T>(f, ys, coef, samples, 0u, sizeof(T) == 4 && wide_flags[f.status_idx] != 0u, out);
+        reconstruct_tile<NC, SX, SY, T, false, K>(f, ys, coef, samples, 0u, sizeof(T) == 4 && wide_flags[f.status_idx] != 0u, out);
     } else {
         const uint32_t n = list[0];
         for (uint32_t k = blockIdx.z; k < n; k += gridDim.z) {
             const FrameRecon &f = frames[list[1 + k]];
-            reconstruct_tile<NC, SX, SY, T>(f, ys, coef, samples, 0u, sizeof(T) == 4 && wide_flags[f.status_idx] != 0u, out);
+            reconstruct_tile<NC, SX, SY, T, false, K>(f, ys, coef, samples, 0u, sizeof(T) == 4 && wide_flags[f.status_idx] != 0u, out);
             __syncwarp();
         }
     }
@@ -832,9 +884,9 @@ __device__ __forceinline__ void tile_idct(int *ys, int only, int &mn, int &mx, S
     else tile_idct_rows<6>(ys, only, mn, mx, sink);
 }
 
-template <typename T>
+template <typename T, int K>
 __device__ __forceinline__ void reconstruct420_tile(const FrameRecon &f, int *ys, uint32_t win, const int16_t *__restrict__ coef,
-                                                    uint32_t *__restrict__ narrow_flags, uint8_t *__restrict__ out) {
+                                                    uint32_t *__restrict__ narrow_flags, StoreDst<K> __restrict__ out) {
     using Wn = Window420<T>;
     constexpr int kHalf = kRows420 / 2;  // chroma block rows under the tile
     const uint32_t vbw = (f.width + 7) >> 3, vbh = (f.height + 7) >> 3;
@@ -900,24 +952,24 @@ __device__ __forceinline__ void reconstruct420_tile(const FrameRecon &f, int *ys
     if (sizeof(T) == 2 && flagged && threadIdx.x == 0) atomicOr(narrow_flags + f.status_idx, 1u);  // `narrow`: the int32 instance redoes the frame
 
     // ---- phase 2: the luma rows
-    reconstruct_tile<3, 2, 2, T, true>(f, ys, coef, nullptr, win, sizeof(T) == 4 && flagged, out);
+    reconstruct_tile<3, 2, 2, T, true, K>(f, ys, coef, nullptr, win, sizeof(T) == 4 && flagged, out);
 }
 
 // grid (luma block columns / 32, luma block rows / kRows420, frames or kWideSlots); dynamic shared memory Window420<T>::kSmemBytes.
 // At kRows420 = 4 five CTAs (20 warps) per SM, like b2; the int32 instance (rare frames) three, which keeps it free of spills.
-template <typename T, bool kListed>
+template <typename T, bool kListed, int K>
 __global__ void __launch_bounds__(kThreads420, ((sizeof(T) == 2) ? 20 : 12) / kRows420)
 reconstruct420_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, uint32_t *__restrict__ narrow_flags,
-                      const uint32_t *__restrict__ list, uint8_t *__restrict__ out) {
+                      const uint32_t *__restrict__ list, StoreDst<K> __restrict__ out) {
     extern __shared__ __align__(16) uint8_t smem420[];
     int *ys = reinterpret_cast<int *>(smem420);  // phase 2: [coefficient][thread]; phase 1: 8 KB per warp
     const uint32_t win = (uint32_t)__cvta_generic_to_shared(smem420) + (uint32_t)Window420<T>::kYsBytes;
     if (!kListed) {
-        reconstruct420_tile<T>(frames[blockIdx.z], ys, win, coef, narrow_flags, out);
+        reconstruct420_tile<T, K>(frames[blockIdx.z], ys, win, coef, narrow_flags, out);
     } else {
         const uint32_t n = list[0];
         for (uint32_t k = blockIdx.z; k < n; k += gridDim.z) {
-            reconstruct420_tile<T>(frames[list[1 + k]], ys, win, coef, narrow_flags, out);
+            reconstruct420_tile<T, K>(frames[list[1 + k]], ys, win, coef, narrow_flags, out);
             __syncthreads();  // the next frame's phase 1 overwrites the tile and the window
         }
     }
@@ -1044,9 +1096,11 @@ __device__ void generic_upsample_block(const int32_t *__restrict__ plane, uint32
     }
 }
 
-// grid (output block columns / 64, output block rows, frames)
+// grid (output block columns / 64, output block rows, frames). K: kStoreCanvas, or kStoreStrided for every described
+// destination (this path stores one sample at a time anyway)
+template <int K>
 __global__ void __launch_bounds__(64)
-generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restrict__ samples, uint8_t *__restrict__ out) {
+generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restrict__ samples, StoreDst<K> __restrict__ out) {
     const FrameRecon &f = frames[blockIdx.z];
     const uint32_t W = f.width, H = f.height, nc = f.ncomp;
     const uint32_t bx = blockIdx.x * 64 + threadIdx.x, by = blockIdx.y;
@@ -1080,7 +1134,8 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
         auto res_at = [&](uint32_t c, int x, int y) -> int { return rdirect[c] ? rdirect[c][(uint64_t)y * (8u * f.res_bw[c]) + (uint32_t)x] : rbuf[c][8 * y + x]; };
         auto clamp_to = [](long long v, long long mx) { return v < 0 ? 0ll : (v > mx ? mx : v); };
         for (int y = 0; y <= ymax; y++) {
-            uint8_t *o = out + f.out_base + ((uint64_t)(Y + y) * W + (uint64_t)X) * nc;
+            uint8_t *o = nullptr;
+            if constexpr (K == kStoreCanvas) o = out + f.out_base + ((uint64_t)(Y + y) * W + (uint64_t)X) * nc;
             for (int x = 0; x <= xmax; x++) {
                 const int i = 8 * y + x;
                 long long res[3] = {128, 128, 128}, v[3] = {0, 0, 0};
@@ -1100,8 +1155,11 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
                 } else {
                     for (uint32_t c = 0; c < nc; c++) v[c] = ((long long)base_at(c, x, y) + 8) >> 4;
                 }
-                for (uint32_t c = 0; c < nc; c++)  // merge and clamp (:863-878, :935-947)
-                    o[nc * x + c] = (uint8_t)clamp_to(clamp_to(v[c], 255) + ((clamp_to(res[c], 4095) + 8) >> 4) - 128, 255);
+                for (uint32_t c = 0; c < nc; c++) {  // merge and clamp (:863-878, :935-947)
+                    const uint8_t m = (uint8_t)clamp_to(clamp_to(v[c], 255) + ((clamp_to(res[c], 4095) + 8) >> 4) - 128, 255);
+                    if constexpr (K == kStoreCanvas) o[nc * x + c] = m;
+                    else *plane_at(out + 4u * f.status_idx + c, X + x, Y + y) = m;
+                }
             }
         }
         return;
@@ -1112,8 +1170,12 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
     const long long maxval = (1ll << f.precision) - 1, coff = 16ll << (f.precision - 1u);
     for (int y = 0; y <= ymax; y++) {
         const uint64_t at = ((uint64_t)(Y + y) * W + (uint64_t)X) * nc;
-        uint8_t *o8 = out + f.out_base + at;
-        uint16_t *o16 = reinterpret_cast<uint16_t *>(out + f.out_base) + at;
+        uint8_t *o8 = nullptr;
+        uint16_t *o16 = nullptr;
+        if constexpr (K == kStoreCanvas) {
+            o8 = out + f.out_base + at;
+            o16 = reinterpret_cast<uint16_t *>(out + f.out_base) + at;
+        }
         for (int x = 0; x <= xmax; x++) {
             long long v[4];
             if (nc == 3 && f.ycbcr) {
@@ -1126,17 +1188,25 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
             }
             for (uint32_t c = 0; c < nc; c++) {
                 const long long w = v[c] < 0 ? 0 : (v[c] > maxval ? maxval : v[c]);
-                if (deep) o16[nc * x + c] = (uint16_t)w;
-                else o8[nc * x + c] = (uint8_t)w;
+                if constexpr (K == kStoreCanvas) {
+                    if (deep) o16[nc * x + c] = (uint16_t)w;
+                    else o8[nc * x + c] = (uint8_t)w;
+                } else {
+                    uint8_t *o = plane_at(out + 4u * f.status_idx + c, X + x, Y + y);
+                    if (deep) *reinterpret_cast<uint16_t *>(o) = (uint16_t)w;
+                    else *o = (uint8_t)w;
+                }
             }
         }
     }
 }
 
 // B200JPG_FLAG_NO_UPSAMPLE: component blockIdx.z of frame blockIdx.y, one thread per sample of its true (subsampled) size:
-// COLOR_TO_INT and the clamp of the identity transformation (tools/numerics.hpp:69), nothing else
+// COLOR_TO_INT and the clamp of the identity transformation (tools/numerics.hpp:69), nothing else. K as for
+// generic_reconstruct_kernel
+template <int K>
 __global__ void __launch_bounds__(256)
-planes_out_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restrict__ samples, uint8_t *__restrict__ out) {
+planes_out_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restrict__ samples, StoreDst<K> __restrict__ out) {
     const FrameRecon &f = frames[blockIdx.y];
     const uint32_t c = blockIdx.z;
     if (c >= f.ncomp) return;
@@ -1148,41 +1218,57 @@ planes_out_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restri
         const uint32_t x = (uint32_t)(i % w), y = (uint32_t)(i / w);
         int v = (samples[f.sample_base[c] + (uint64_t)y * (8u * f.bw[c]) + x] + 8) >> 4;
         v = v < 0 ? 0 : (v > maxval ? maxval : v);
-        if (f.precision > 8) reinterpret_cast<uint16_t *>(out + f.out_base)[before + i] = (uint16_t)v;
-        else out[f.out_base + before + i] = (uint8_t)v;
+        if constexpr (K == kStoreCanvas) {
+            if (f.precision > 8) reinterpret_cast<uint16_t *>(out + f.out_base)[before + i] = (uint16_t)v;
+            else out[f.out_base + before + i] = (uint8_t)v;
+        } else {
+            uint8_t *o = plane_at(out + 4u * f.status_idx + c, (int)x, (int)y);
+            if (f.precision > 8) *reinterpret_cast<uint16_t *>(o) = (uint16_t)v;
+            else *o = (uint8_t)v;
+        }
     }
 }
 
 }  // namespace
 
-template <typename T, bool kListed>
+// the destination argument of a launch of kind K
+template <int K>
+static StoreDst<K> dst_of(const ReconLaunch &l) {
+    if constexpr (K == kStoreCanvas) return l.out;
+    else return l.planes;
+}
+
+template <typename T, bool kListed, int K>
 static void launch_b2(const ReconLaunch &l, dim3 grid, const T *samples, cudaStream_t s) {
+    const StoreDst<K> out = dst_of<K>(l);
     if (l.ncomp == 1) {
-        reconstruct_kernel<1, 1, 1, T, kListed><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, l.out);
+        reconstruct_kernel<1, 1, 1, T, kListed, K><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, out);
     } else if (l.subx == 2 && l.suby == 1) {
-        reconstruct_kernel<3, 2, 1, T, kListed><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, l.out);
+        reconstruct_kernel<3, 2, 1, T, kListed, K><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, out);
     } else if (l.subx == 1 && l.suby == 2) {
-        reconstruct_kernel<3, 1, 2, T, kListed><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, l.out);
+        reconstruct_kernel<3, 1, 2, T, kListed, K><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, out);
     } else {
-        reconstruct_kernel<3, 1, 1, T, kListed><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, l.out);
+        reconstruct_kernel<3, 1, 1, T, kListed, K><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, out);
     }
 }
 
+template <int K>
 static int launch_recon420(const ReconLaunch &l, cudaStream_t s, int *launches) {
     const uint32_t gx = (l.max_bw0 + 31) / 32, gy = (l.max_bh0 + kRows420 - 1) / kRows420;
     constexpr int smem16 = Window420<int16_t>::kSmemBytes, smem32 = Window420<int32_t>::kSmemBytes;
-    cudaError_t e = cudaFuncSetAttribute(reconstruct420_kernel<int16_t, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    if (e == cudaSuccess && smem16 > 48 * 1024) e = cudaFuncSetAttribute(reconstruct420_kernel<int16_t, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem16);
-    if (e == cudaSuccess && smem32 > 48 * 1024) e = cudaFuncSetAttribute(reconstruct420_kernel<int32_t, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem32);
+    cudaError_t e = cudaFuncSetAttribute(reconstruct420_kernel<int16_t, false, K>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    if (e == cudaSuccess && smem16 > 48 * 1024) e = cudaFuncSetAttribute(reconstruct420_kernel<int16_t, false, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem16);
+    if (e == cudaSuccess && smem32 > 48 * 1024) e = cudaFuncSetAttribute(reconstruct420_kernel<int32_t, true, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem32);
     if (e != cudaSuccess) return (int)e;
-    reconstruct420_kernel<int16_t, false><<<dim3(gx, gy, l.n_frames), kThreads420, smem16, s>>>(l.frames, l.coef, l.narrow_flags, nullptr, l.out);
+    reconstruct420_kernel<int16_t, false, K><<<dim3(gx, gy, l.n_frames), kThreads420, smem16, s>>>(l.frames, l.coef, l.narrow_flags, nullptr, dst_of<K>(l));
     // the exact pass over the frames flagged `narrow` (none for real images: two near-empty launches)
     narrow_list_kernel<<<1, 256, 0, s>>>(l.frames, l.n_frames, l.narrow_flags, l.narrow_list);
-    reconstruct420_kernel<int32_t, true><<<dim3(gx, gy, kWideSlots), kThreads420, smem32, s>>>(l.frames, l.coef, l.narrow_flags, l.narrow_list, l.out);
+    reconstruct420_kernel<int32_t, true, K><<<dim3(gx, gy, kWideSlots), kThreads420, smem32, s>>>(l.frames, l.coef, l.narrow_flags, l.narrow_list, dst_of<K>(l));
     if (launches) *launches = 3;
     return (int)cudaGetLastError();
 }
 
+template <int K>
 static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launches) {
     uint32_t mb = 0;
     mb = l.max_bwc * l.max_bhc;  // the largest component block grid of the group (set by the host for generic groups)
@@ -1199,19 +1285,19 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
     n++;
     if (l.planes_out) {
         const uint32_t gx = std::min<uint32_t>((l.max_bw0 * l.max_bh0 * 64u + 255u) / 256u, 4096u);
-        planes_out_kernel<<<dim3(gx, l.n_frames, l.ncomp), 256, 0, s>>>(l.frames, l.samples32, l.out);
+        planes_out_kernel<K><<<dim3(gx, l.n_frames, l.ncomp), 256, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
     } else {
-        generic_reconstruct_kernel<<<dim3((l.max_bw0 + 63) / 64, l.max_bh0, l.n_frames), 64, 0, s>>>(l.frames, l.samples32, l.out);
+        generic_reconstruct_kernel<K><<<dim3((l.max_bw0 + 63) / 64, l.max_bh0, l.n_frames), 64, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
     }
     if (launches) *launches = n;
     return (int)cudaGetLastError();
 }
 
-int launch_recon(const ReconLaunch &l, void *stream, int *launches) {
-    cudaStream_t s = (cudaStream_t)stream;
+template <int K>
+static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches) {
     int n = 0;
-    if (l.generic) return launch_recon_generic(l, s, launches);
-    if (l.ncomp == 3 && l.subx == 2 && l.suby == 2) return launch_recon420(l, s, launches);
+    if (l.generic) return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : kStoreStrided>(l, s, launches);
+    if (l.ncomp == 3 && l.subx == 2 && l.suby == 2) return launch_recon420<K>(l, s, launches);
     const uint32_t cblocks = (l.max_bwc * l.max_bhc + kThreadsB - 1) / kThreadsB;
     const uint32_t gx = (l.max_bw0 + 31) / 32, gy = (l.max_bh0 + kThreadsB / 32 - 1) / (kThreadsB / 32);
     // every frame through the int16 planes, B200JPG_RECON_CHUNK frames at a time (0: all at once): in chunks the planes b1 writes
@@ -1229,18 +1315,26 @@ int launch_recon(const ReconLaunch &l, void *stream, int *launches) {
             idct_planes_kernel<int16_t, false><<<dim3(cblocks, nf, l.ncomp - 1), kThreadsB, 0, s>>>(c.frames, l.coef, l.samples16, l.narrow_flags, nullptr, 1);
             n++;
         }
-        launch_b2<int16_t, false>(c, dim3(gx, gy, nf), l.samples16, s);
+        launch_b2<int16_t, false, K>(c, dim3(gx, gy, nf), l.samples16, s);
         n++;
     }
     // the exact pass over the frames that were flagged `narrow` (none for real images: three near-empty launches)
     if (l.ncomp > 1) {
         narrow_list_kernel<<<1, 256, 0, s>>>(l.frames, l.n_frames, l.narrow_flags, l.narrow_list);
         idct_planes_kernel<int32_t, true><<<dim3(cblocks, kWideSlots, l.ncomp - 1), kThreadsB, 0, s>>>(l.frames, l.coef, l.samples32, l.wide_flags, l.narrow_list, 1);
-        launch_b2<int32_t, true>(l, dim3(gx, gy, kWideSlots), l.samples32, s);
+        launch_b2<int32_t, true, K>(l, dim3(gx, gy, kWideSlots), l.samples32, s);
         n += 3;
     }
     if (launches) *launches = n;
     return (int)cudaGetLastError();
+}
+
+// the destination kind is chosen per group from the descriptors (b200jpg_batch_decode_into), never by the caller
+int launch_recon(const ReconLaunch &l, void *stream, int *launches) {
+    cudaStream_t s = (cudaStream_t)stream;
+    if (!l.planes) return launch_recon_kind<kStoreCanvas>(l, s, launches);
+    if (l.planar) return launch_recon_kind<kStorePlanar>(l, s, launches);
+    return launch_recon_kind<kStoreStrided>(l, s, launches);
 }
 
 }  // namespace b200jpg

@@ -64,6 +64,84 @@ def parse(data):
     return FrameInfo.from_struct(s)
 
 
+def component_shapes(info, upsample=True):
+    """[(h, w)] of every component of a frame as the decoder writes it: the frame size, or without upsampling each
+    component's own ceil(H / suby) x ceil(W / subx)."""
+    if upsample:
+        return [(info.height, info.width)] * info.ncomp
+    return [((info.height + info.suby[c] - 1) // info.suby[c], (info.width + info.subx[c] - 1) // info.subx[c])
+            for c in range(info.ncomp)]
+
+
+def plane_table(geometry, dst, device_type="cuda"):
+    """The b200jpg_plane table of BatchDecoder.decode_into (4 entries per frame).
+
+    geometry[i] = (component shapes [(h, w)], deep) of frame i, or None for a frame that failed to parse. dst[i] is a
+    sequence of one 2-D tensor per component (a [C, H, W] tensor is one), uint8 for 8-bit and int16 for 12-bit (`deep`)
+    frames, or None where geometry[i] is None. Component c's sample (x, y) goes to t[y, x]: bytes_per_pixel =
+    stride(1) * itemsize, bytes_per_row = stride(0) * itemsize. Raises ValueError / TypeError on a wrong count, shape,
+    dtype or device; nothing has been launched then."""
+    import torch
+    n = len(geometry)
+    if len(dst) != n:
+        raise ValueError("decode_into: %d destinations for %d frames" % (len(dst), n))
+    if isinstance(dst, torch.Tensor) and dst.dim() == 4:
+        return _batch_tensor_table(geometry, dst, device_type)
+    table = (native.PlaneStruct * (4 * n))()
+    for i, (geo, entry) in enumerate(zip(geometry, dst)):
+        if geo is None:
+            if entry is not None:
+                raise ValueError("frame %d failed to parse: its destination must be None" % i)
+            continue
+        if entry is None:
+            raise ValueError("frame %d needs a destination" % i)
+        shapes, deep = geo
+        if len(entry) != len(shapes):
+            raise ValueError("frame %d has %d components, its destination %d" % (i, len(shapes), len(entry)))
+        dtype = torch.int16 if deep else torch.uint8
+        for c, t in enumerate(entry):
+            if not isinstance(t, torch.Tensor):
+                raise TypeError("frame %d component %d: expected a tensor, got %s" % (i, c, type(t).__name__))
+            if t.device.type != device_type:
+                raise ValueError("frame %d component %d: a %s tensor, expected %s" % (i, c, t.device.type, device_type))
+            if t.dtype != dtype:
+                raise TypeError("frame %d component %d: dtype %s, expected %s" % (i, c, t.dtype, dtype))
+            if tuple(t.shape) != tuple(shapes[c]):
+                raise ValueError("frame %d component %d: shape %s, expected %s" % (i, c, tuple(t.shape), tuple(shapes[c])))
+            e = table[4 * i + c]
+            e.data = t.data_ptr()
+            e.bytes_per_pixel = t.stride(1) * t.element_size()
+            e.bytes_per_row = t.stride(0) * t.element_size()
+    return table
+
+
+def _batch_tensor_table(geometry, t, device_type):
+    """plane_table for one [N, C, H, W] tensor, without a view per component (a batch of thousands of frames would spend
+    longer building views than the GPU spends decoding it)"""
+    import torch
+    live = [i for i, g in enumerate(geometry) if g is not None]
+    if not live:
+        return (native.PlaneStruct * (4 * len(geometry)))()
+    shapes, deep = geometry[live[0]]
+    if any(geometry[i] != (shapes, deep) for i in live) or len(set(shapes)) != 1:
+        raise ValueError("a [N, C, H, W] destination needs frames of one geometry")
+    want = (len(geometry), len(shapes)) + tuple(shapes[0])
+    if t.device.type != device_type:
+        raise ValueError("a %s tensor, expected %s" % (t.device.type, device_type))
+    if t.dtype != (torch.int16 if deep else torch.uint8):
+        raise TypeError("dtype %s, expected %s" % (t.dtype, torch.int16 if deep else torch.uint8))
+    if tuple(t.shape) != want:
+        raise ValueError("shape %s, expected %s" % (tuple(t.shape), want))
+    arr = np.zeros(4 * len(geometry), dtype=np.dtype([("data", "<u8"), ("bpp", "<i4"), ("pad", "<i4"), ("bpr", "<i8")]))
+    assert arr.itemsize == ctypes.sizeof(native.PlaneStruct)
+    isz, st, idx = t.element_size(), t.stride(), np.asarray(live, dtype=np.int64)
+    for c in range(len(shapes)):
+        arr["data"][4 * idx + c] = t.data_ptr() + (idx * st[0] + c * st[1]) * isz
+        arr["bpp"][4 * idx + c] = st[3] * isz
+        arr["bpr"][4 * idx + c] = st[2] * isz
+    return (native.PlaneStruct * (4 * len(geometry))).from_buffer_copy(arr.tobytes())
+
+
 class Context:
     def __init__(self, device=-1):
         self.handle = ctypes.c_void_p()
@@ -172,6 +250,27 @@ class BatchDecoder:
         assert out.is_cuda and out.numel() >= self.out_bytes
         native.check(lib.b200jpg_batch_decode(self.handle, out.data_ptr(), self._stream_ptr(stream)), self.ctx.handle)
         return out
+
+    def geometry(self):
+        """Per frame (component shapes [(h, w)], deep), or None for a frame that failed to parse: what decode_into expects."""
+        if getattr(self, "_geometry", None) is None:
+            geo = []
+            for i in range(self.n):
+                s = native.FrameInfoStruct()
+                rc = lib.b200jpg_batch_frame_info(self.handle, i, ctypes.byref(s))
+                fi = FrameInfo.from_struct(s)
+                geo.append(None if rc != 0 else (component_shapes(fi, self.upsample), fi.precision > 8))
+            self._geometry = geo
+        return self._geometry
+
+    def decode_into(self, dst, stream=None):
+        """decode() into caller-described tensors: dst[i] holds one 2-D CUDA tensor per component of frame i ([H, W], or
+        each component's own size with upsample=False), so a [N, C, H, W] batch tensor can be passed as it is, an NHWC
+        tensor t as t.permute(0, 3, 1, 2), BGR as [t[i, ..., 2], t[i, ..., 1], t[i, ..., 0]]. uint8 for 8-bit frames,
+        int16 for 12-bit frames; None for frames that failed to parse. Only the samples are written. Returns dst."""
+        table = plane_table(self.geometry(), dst)
+        native.check(lib.b200jpg_batch_decode_into(self.handle, table, self._stream_ptr(stream)), self.ctx.handle)
+        return dst
 
     def decode_entropy(self, stream=None):
         native.check(lib.b200jpg_batch_decode_entropy(self.handle, self._stream_ptr(stream)), self.ctx.handle)
