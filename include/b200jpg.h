@@ -19,6 +19,7 @@
  *                            Upsampler<sx,sy>::UpsampleRegion           upsampling/upsampler.cpp:83
  *                            YCbCrTrafo::YCbCr2RGB                      colortrafo/ycbcrtrafo.cpp:679
  *   b200jpg_batch_decode_into  the same, into per-component ImageBitMaps interface/imagebitmap.hpp:104-109
+ *   b200jpg_batch_decode_into_ex  the same, samples converted to float32 / float16 / bfloat16 on the way out (no counterpart)
  *   b200jpg_last_error       JPEG::LastError                            interface/jpeg.cpp:962
  *
  * Error codes are the reference's (interface/parameters.hpp:1156-1228).
@@ -164,6 +165,27 @@ typedef struct b200jpg_plane {
  * is not 2-byte aligned in data or in either stride.  `planes` may be reused as soon as the call returns; the call issues
  * as many kernel launches as b200jpg_batch_decode. */
 B200JPG_API int b200jpg_batch_decode_into(b200jpg_batch *batch, const b200jpg_plane *planes, void *stream);
+/* Float destinations: every sample v that b200jpg_batch_decode_into would write (0..255, or 0..4095 for 12-bit frames) is
+ * written as
+ *     y = fp32_round(fp32_round((float)v * scale[c]) + bias[c])      (two roundings, no fused multiply-add)
+ * stored as float32, or rounded to nearest even into float16 (overflow -> inf, subnormals kept) or bfloat16. c is the output
+ * component: R, G, B after the colour transformation, else the frame's component / plane index. One map per call, uniform
+ * over the batch's frames. */
+#define B200JPG_SAMPLE_F32 1
+#define B200JPG_SAMPLE_F16 2
+#define B200JPG_SAMPLE_BF16 3
+typedef struct b200jpg_convert {
+    int32_t type; /* B200JPG_SAMPLE_* */
+    float scale[B200JPG_MAX_COMPONENTS], bias[B200JPG_MAX_COMPONENTS];
+} b200jpg_convert;
+/* b200jpg_batch_decode_into with the samples converted by `convert` (NULL: exactly b200jpg_batch_decode_into). The
+ * descriptor rules are those above with the element size (4 bytes for float32, 2 for float16 / bfloat16) in place of the
+ * sample size: |bytes_per_pixel| >= element size, no overlapping rows, data and both strides aligned to the element size.
+ * Also B200JPG_ERR_INVALID_PARAMETER, with nothing launched: an unknown type, or a non-finite scale or bias of a component
+ * that a live frame of the batch has. The call writes the same positions as b200jpg_batch_decode_into and issues as many
+ * kernel launches. */
+B200JPG_API int b200jpg_batch_decode_into_ex(b200jpg_batch *batch, const b200jpg_plane *planes, const b200jpg_convert *convert,
+                                             void *stream);
 /* Only one of the two stages (profiling / roofline measurements / parity of the intermediate). */
 B200JPG_API int b200jpg_batch_decode_entropy(b200jpg_batch *batch, void *stream);
 B200JPG_API int b200jpg_batch_reconstruct(b200jpg_batch *batch, uint8_t *out_dev, void *stream);

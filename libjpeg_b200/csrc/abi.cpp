@@ -8,6 +8,7 @@
 
 #include <algorithm>
 #include <array>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -1196,9 +1197,9 @@ static int run_entropy(b200jpg_batch *b, void *stream) {
 }
 
 // planes_dev: b200jpg_batch_decode_into's descriptor table (device), planar[i]: every component of frame i has
-// bytes_per_pixel == sample size
+// bytes_per_pixel == sample size (element size with `convert`, the float map of b200jpg_batch_decode_into_ex)
 static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b200jpg_plane *planes_dev = nullptr,
-                     const std::vector<char> *planar = nullptr) {
+                     const std::vector<char> *planar = nullptr, const b200jpg_convert *convert = nullptr) {
     NvtxRange nvtx("b200jpg reconstruction: IDCT + upsampling + colour");
     cudaError_t me = cudaMemsetAsync(b->d_status + b->n, 0, sizeof(uint32_t) * 2 * (size_t)b->n, (cudaStream_t)stream);
     if (me != cudaSuccess) return b->ctx->fail_cuda(me, "flag reset");
@@ -1223,6 +1224,7 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.narrow_list = b->d_status + 3 * (size_t)b->n;
         l.out = out_dev;
         l.planes = planes_dev;
+        l.convert = convert;
         l.planar = planes_dev != nullptr;
         if (planes_dev)
             for (const FrameRecon &fr : g.frames) l.planar = l.planar && (*planar)[fr.status_idx];
@@ -1253,7 +1255,7 @@ static int ensure_events(b200jpg_batch *b) {
 }
 
 static int run_decode(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b200jpg_plane *planes_dev = nullptr,
-                      const std::vector<char> *planar = nullptr) {
+                      const std::vector<char> *planar = nullptr, const b200jpg_convert *convert = nullptr) {
     b->last_launches = 0;
     b->status_fetched = false;
     if (b->timing) {
@@ -1263,7 +1265,7 @@ static int run_decode(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b2
     int rc = run_entropy(b, stream);
     if (rc) return rc;
     if (b->timing) cudaEventRecord(b->ev[1], (cudaStream_t)stream);
-    rc = run_recon(b, out_dev, stream, planes_dev, planar);
+    rc = run_recon(b, out_dev, stream, planes_dev, planar, convert);
     if (rc) return rc;
     if (b->timing) cudaEventRecord(b->ev[2], (cudaStream_t)stream);
     return B200JPG_OK;
@@ -1279,16 +1281,32 @@ int b200jpg_batch_decode(b200jpg_batch *b, uint8_t *out_dev, void *stream) {
 static uint64_t magnitude(int64_t v) { return v < 0 ? 0 - (uint64_t)v : (uint64_t)v; }
 
 int b200jpg_batch_decode_into(b200jpg_batch *b, const b200jpg_plane *planes, void *stream) {
+    return b200jpg_batch_decode_into_ex(b, planes, nullptr, stream);
+}
+
+int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, const b200jpg_convert *convert, void *stream) {
     if (!b || !planes) return B200JPG_ERR_INVALID_PARAMETER;
     if (!b->uploaded) return b->ctx->fail(B200JPG_ERR_OBJECT_DOESNT_EXIST, "batch has not been uploaded");
     cudaSetDevice(b->ctx->device);
-    // every descriptor of every live frame is checked before anything is enqueued
+    // the map and every descriptor of every live frame are checked before anything is enqueued
+    uint64_t element = 0;  // float destinations: the element size replaces the sample size
+    if (convert) {
+        if (convert->type == B200JPG_SAMPLE_F32) element = 4;
+        else if (convert->type == B200JPG_SAMPLE_F16 || convert->type == B200JPG_SAMPLE_BF16) element = 2;
+        else return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "unknown sample type " + std::to_string(convert->type));
+        int ncomp = 0;  // the components some live frame has
+        for (int i = 0; i < b->n_user; i++)
+            if (b->parse_status[i] == 0) ncomp = std::max(ncomp, (int)b->frames[i].info.ncomp);
+        for (int c = 0; c < ncomp; c++)
+            if (!std::isfinite(convert->scale[c]) || !std::isfinite(convert->bias[c]))
+                return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "component " + std::to_string(c) + ": scale and bias must be finite");
+    }
     const bool own_size = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
     std::vector<char> planar((size_t)b->n, 1);
     for (int i = 0; i < b->n_user; i++) {
         if (b->parse_status[i] != 0) continue;
         const b200jpg_frame_info &fi = b->frames[i].info;
-        const uint64_t size = fi.precision > 8 ? 2 : 1;
+        const uint64_t size = convert ? element : (fi.precision > 8 ? 2 : 1);
         for (int c = 0; c < fi.ncomp; c++) {
             const b200jpg_plane &p = planes[4 * i + c];
             const uint64_t w = own_size ? (fi.width + fi.subx[c] - 1) / fi.subx[c] : fi.width;
@@ -1298,8 +1316,10 @@ int b200jpg_batch_decode_into(b200jpg_batch *b, const b200jpg_plane *planes, voi
             if (!p.data) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "no destination");
             if (bpp < size) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "|bytes_per_pixel| is smaller than the sample size");
             if (h > 1 && bpr < w * bpp) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "rows overlap: |bytes_per_row| < width * |bytes_per_pixel|");
-            if (size == 2 && ((reinterpret_cast<uintptr_t>(p.data) | bpp | bpr) & 1u))
-                return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "16-bit samples need a 2-byte aligned address and strides");
+            if (size > 1 && ((reinterpret_cast<uintptr_t>(p.data) | bpp | bpr) & (size - 1u)))
+                return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER,
+                                    at + (convert ? std::to_string(size) + "-byte elements need a " + std::to_string(size) + "-byte aligned address and strides"
+                                                  : std::string("16-bit samples need a 2-byte aligned address and strides")));
             cudaPointerAttributes a{};
             const cudaError_t e = cudaPointerGetAttributes(&a, p.data);
             if (e != cudaSuccess) cudaGetLastError();
@@ -1338,7 +1358,7 @@ int b200jpg_batch_decode_into(b200jpg_batch *b, const b200jpg_plane *planes, voi
     if (ce == cudaSuccess) ce = cudaEventRecord(b->ev_planes[slot], (cudaStream_t)stream);
     b->plane_slot = (slot + 1) % kSlots;
     if (ce != cudaSuccess) return b->ctx->fail_cuda(ce, "descriptor table upload");
-    return run_decode(b, nullptr, stream, b->d_planes, &planar);
+    return run_decode(b, nullptr, stream, b->d_planes, &planar, convert);
 }
 
 int b200jpg_batch_decode_entropy(b200jpg_batch *b, void *stream) {

@@ -273,13 +273,25 @@ struct ReconLaunch {
     // b200jpg_batch_decode_into: where every component goes, [4 * frames in batch] indexed 4 * status_idx + c (device);
     // null: the packed slots of `out`
     const b200jpg_plane *planes;
-    bool planar;                   // every plane of the group's frames has bytes_per_pixel == sample size
+    bool planar;                   // every plane of the group's frames has bytes_per_pixel == sample size (element size with `convert`)
+    // b200jpg_batch_decode_into_ex: the samples leave as float32 / float16 / bfloat16 through this map (host memory, passed to
+    // the kernels by value); null: as integers
+    const b200jpg_convert *convert;
 };
 
 // How the reconstruction kernels store a block (the destination kind of the launch, chosen per group from the descriptors):
 // kStoreCanvas: the packed slot of `out` (b200jpg_batch_decode); kStorePlanar: one plane per component, samples adjacent;
-// kStoreStrided: any signed pixel and row stride, one store per sample.
-enum StoreKind : int { kStoreCanvas = 0, kStorePlanar = 1, kStoreStrided = 2 };
+// kStoreStrided: any signed pixel and row stride, one store per sample. kStorePlanarF / kStoreStridedF: the same layouts with
+// float elements, every clamped integer sample v converted to fp32_round(fp32_round(v * scale[c]) + bias[c]) and rounded to
+// the element type (B200JPG_SAMPLE_*, a launch-uniform switch inside the kind).
+enum StoreKind : int { kStoreCanvas = 0, kStorePlanar = 1, kStoreStrided = 2, kStorePlanarF = 3, kStoreStridedF = 4 };
+
+// the destination argument of the float kinds: the descriptors plus the map, both in the kernel's parameter bank
+struct FloatDst {
+    const b200jpg_plane *planes;
+    int32_t type;
+    float scale[B200JPG_MAX_COMPONENTS], bias[B200JPG_MAX_COMPONENTS];
+};
 int launch_recon(const ReconLaunch &l, void *stream, int *launches);
 
 // JPEG::DisplayRectangle into device bitmaps (bitmap_sm100.cu): the rectangle x0..x1, y0..y1 (inclusive, in the coordinates of

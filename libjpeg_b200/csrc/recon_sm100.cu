@@ -24,6 +24,8 @@
 //     interleaved RGB per line.  The kernel is co-limited by instruction issue and by the L1 data pipe, so global
 //     accesses are shaped for few L1 wavefronts; small loop bodies keep it inside the instruction cache (the fully
 //     unrolled register-resident version stalled on instruction fetch).
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -398,9 +400,64 @@ __device__ __forceinline__ uint32_t pack_sat4(int p0, int p1, int p2, int p3) {
 }
 
 // ---- destinations (StoreKind): the canvas kind stores into the batch's output buffer, the described kinds read the
-// frame's four b200jpg_plane descriptors at 4 * status_idx of the table b200jpg_batch_decode_into uploads
+// frame's four b200jpg_plane descriptors at 4 * status_idx of the table b200jpg_batch_decode_into uploads; the float kinds
+// carry the conversion map next to the table pointer, as a launch argument
 template <int K>
-using StoreDst = std::conditional_t<K == kStoreCanvas, uint8_t *, const b200jpg_plane *>;
+using StoreDst = std::conditional_t<K == kStoreCanvas, uint8_t *, std::conditional_t<(K >= kStorePlanarF), FloatDst, const b200jpg_plane *>>;
+
+__device__ __forceinline__ const b200jpg_plane *planes_of(const b200jpg_plane *p) { return p; }
+__device__ __forceinline__ const b200jpg_plane *planes_of(const FloatDst &d) { return d.planes; }
+
+// ---- float elements. The samples arrive as clamped integers 0 <= v < 2^23: 0x4B000000 | v is the float 2^23 + v, so one
+// subtraction makes (float)v exactly -- a LOP3 (or the PRMT that takes the byte out of its packed word) and an FADD on the
+// otherwise idle FP32 pipe, where I2F would issue at a fraction of that rate. Then fp32_round(fp32_round(v * s) + b), never
+// fused.
+__device__ __forceinline__ float convert_bits(uint32_t bits, float s, float b) {
+    return __fadd_rn(__fmul_rn(__fsub_rn(__uint_as_float(bits), 8388608.f), s), b);
+}
+__device__ __forceinline__ float convert_int(int v, float s, float b) { return convert_bits(0x4B000000u | (uint32_t)v, s, b); }
+// byte k of a packed word of four 8-bit samples as 0x4B0000vv: bytes 4..7 of the permute are those of 0x4B000000
+__device__ __forceinline__ float convert_byte(uint32_t w, int k, float s, float b) {
+    return convert_bits(__byte_perm(w, 0x4B000000u, 0x7440u | (uint32_t)k), s, b);
+}
+// scale[c] / bias[c] of a component index known only at run time (a select chain: the parameter bank is not indexed)
+__device__ __forceinline__ float pick4(const float (&a)[B200JPG_MAX_COMPONENTS], uint32_t c) {
+    return c == 0 ? a[0] : (c == 1 ? a[1] : (c == 2 ? a[2] : a[3]));
+}
+__device__ __forceinline__ uint32_t pack2(int type, float lo, float hi) {
+    if (type == B200JPG_SAMPLE_F16) {
+        const __half2 h = __floats2half2_rn(lo, hi);
+        return *reinterpret_cast<const uint32_t *>(&h);
+    }
+    const __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
+    return *reinterpret_cast<const uint32_t *>(&h);
+}
+// one element at o, rounded to the destination type
+__device__ __forceinline__ void store_elem(int type, uint8_t *o, float y) {
+    if (type == B200JPG_SAMPLE_F32) *reinterpret_cast<float *>(o) = y;
+    else if (type == B200JPG_SAMPLE_F16) *reinterpret_cast<__half *>(o) = __float2half_rn(y);
+    else *reinterpret_cast<__nv_bfloat16 *>(o) = __float2bfloat16_rn(y);
+}
+// the first xmax + 1 of eight converted samples from o on: a whole 16-byte aligned planar row leaves as one 16-byte store
+// (fp16 / bf16) or two (fp32), else one store per element
+template <int K>
+__device__ __forceinline__ void store_row_f(int type, const b200jpg_plane *p, uint8_t *o, const float (&y)[8], int xmax) {
+    const bool f32 = type == B200JPG_SAMPLE_F32;
+    if (K == kStorePlanarF && xmax == 7 && (reinterpret_cast<uintptr_t>(o) & 15u) == 0) {
+        uint4 *o4 = reinterpret_cast<uint4 *>(o);
+        if (f32) {
+            o4[0] = make_uint4(__float_as_uint(y[0]), __float_as_uint(y[1]), __float_as_uint(y[2]), __float_as_uint(y[3]));
+            o4[1] = make_uint4(__float_as_uint(y[4]), __float_as_uint(y[5]), __float_as_uint(y[6]), __float_as_uint(y[7]));
+        } else {
+            o4[0] = make_uint4(pack2(type, y[0], y[1]), pack2(type, y[2], y[3]), pack2(type, y[4], y[5]), pack2(type, y[6], y[7]));
+        }
+        return;
+    }
+    const int64_t s = (K == kStorePlanarF) ? (f32 ? 4 : 2) : p->bytes_per_pixel;
+#pragma unroll
+    for (int x = 0; x < 8; x++)
+        if (x <= xmax) store_elem(type, o + x * s, y[x]);
+}
 
 // the sample (x, y) of a described component, signed 64-bit addressing (ImageBitMap, interface/imagebitmap.hpp:104-109).
 // The descriptor is read again at every call (L1 hits): held in registers through the line loop of reconstruct_tile, three of
@@ -426,6 +483,20 @@ __device__ __forceinline__ void store_row8(const b200jpg_plane *p, uint8_t *o, u
 #pragma unroll
     for (int x = 0; x < 8; x++)
         if (x <= xmax) o[x * s] = (uint8_t)(((x < 4) ? w0 : w1) >> (8 * (x & 3)));
+}
+
+// one block row of component c of a described destination, the eight clamped samples packed in w0 | w1: as bytes, or
+// converted for the float kinds
+template <int K, typename D>
+__device__ __forceinline__ void store_row(const D &out, int c, const b200jpg_plane *p, uint8_t *o, uint32_t w0, uint32_t w1, int xmax) {
+    if constexpr (K >= kStorePlanarF) {
+        float y[8];
+#pragma unroll
+        for (int x = 0; x < 8; x++) y[x] = convert_byte((x < 4) ? w0 : w1, x & 3, out.scale[c], out.bias[c]);
+        store_row_f<K>(out.type, p, o, y, xmax);
+    } else {
+        store_row8<K>(p, o, w0, w1, xmax);
+    }
 }
 
 // ycbcrtrafo.cpp:842-850 with the matrix of colortransformerfactory.cpp:136-138 (13 fractional bits) and
@@ -538,7 +609,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
     uint8_t *obase = nullptr;
     const b200jpg_plane *pl = nullptr;  // described kinds: the frame's component descriptors
     if constexpr (K == kStoreCanvas) obase = out + f.out_base + (uint64_t)Y * opitch + (uint64_t)X * NC;
-    else pl = out + 4u * f.status_idx;
+    else pl = planes_of(out) + 4u * f.status_idx;
 
     if (NC == 1) {  // identity, COLOR_TO_INT (numerics.hpp:69) + clamp
         if (!valid) return;
@@ -558,7 +629,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                         if (x <= xmax) o[x] = (uint8_t)(((x < 4) ? w0 : w1) >> (8 * (x & 3)));
                 }
             } else {
-                store_row8<K>(pl, o, w0, w1, xmax);
+                store_row<K>(out, 0, pl, o, w0, w1, xmax);
             }
         }
         return;
@@ -692,7 +763,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
             if (K != kStoreCanvas) {
                 if (valid) {
 #pragma unroll
-                    for (int c = 0; c < 3; c++) store_row8<K>(pl + c, plane_at(pl + c, X, Y + r), wd[2 * c], wd[2 * c + 1], xmax);
+                    for (int c = 0; c < 3; c++) store_row<K>(out, c, pl + c, plane_at(pl + c, X, Y + r), wd[2 * c], wd[2 * c + 1], xmax);
                 }
             } else if (valid) {
                 uint8_t *o = obase + (uint64_t)r * opitch;
@@ -1096,8 +1167,8 @@ __device__ void generic_upsample_block(const int32_t *__restrict__ plane, uint32
     }
 }
 
-// grid (output block columns / 64, output block rows, frames). K: kStoreCanvas, or kStoreStrided for every described
-// destination (this path stores one sample at a time anyway)
+// grid (output block columns / 64, output block rows, frames). K: kStoreCanvas, or kStoreStrided / kStoreStridedF for every
+// described destination (this path stores one sample at a time anyway)
 template <int K>
 __global__ void __launch_bounds__(64)
 generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restrict__ samples, StoreDst<K> __restrict__ out) {
@@ -1158,6 +1229,8 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
                 for (uint32_t c = 0; c < nc; c++) {  // merge and clamp (:863-878, :935-947)
                     const uint8_t m = (uint8_t)clamp_to(clamp_to(v[c], 255) + ((clamp_to(res[c], 4095) + 8) >> 4) - 128, 255);
                     if constexpr (K == kStoreCanvas) o[nc * x + c] = m;
+                    else if constexpr (K == kStoreStridedF)
+                        store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, X + x, Y + y), convert_int(m, pick4(out.scale, c), pick4(out.bias, c)));
                     else *plane_at(out + 4u * f.status_idx + c, X + x, Y + y) = m;
                 }
             }
@@ -1191,6 +1264,8 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
                 if constexpr (K == kStoreCanvas) {
                     if (deep) o16[nc * x + c] = (uint16_t)w;
                     else o8[nc * x + c] = (uint8_t)w;
+                } else if constexpr (K == kStoreStridedF) {
+                    store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, X + x, Y + y), convert_int((int)w, pick4(out.scale, c), pick4(out.bias, c)));
                 } else {
                     uint8_t *o = plane_at(out + 4u * f.status_idx + c, X + x, Y + y);
                     if (deep) *reinterpret_cast<uint16_t *>(o) = (uint16_t)w;
@@ -1221,6 +1296,8 @@ planes_out_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restri
         if constexpr (K == kStoreCanvas) {
             if (f.precision > 8) reinterpret_cast<uint16_t *>(out + f.out_base)[before + i] = (uint16_t)v;
             else out[f.out_base + before + i] = (uint8_t)v;
+        } else if constexpr (K == kStoreStridedF) {
+            store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, (int)x, (int)y), convert_int(v, pick4(out.scale, c), pick4(out.bias, c)));
         } else {
             uint8_t *o = plane_at(out + 4u * f.status_idx + c, (int)x, (int)y);
             if (f.precision > 8) *reinterpret_cast<uint16_t *>(o) = (uint16_t)v;
@@ -1234,8 +1311,17 @@ planes_out_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restri
 // the destination argument of a launch of kind K
 template <int K>
 static StoreDst<K> dst_of(const ReconLaunch &l) {
-    if constexpr (K == kStoreCanvas) return l.out;
-    else return l.planes;
+    if constexpr (K == kStoreCanvas) {
+        return l.out;
+    } else if constexpr (K >= kStorePlanarF) {
+        FloatDst d{};
+        d.planes = l.planes;
+        d.type = l.convert->type;
+        for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) d.scale[c] = l.convert->scale[c], d.bias[c] = l.convert->bias[c];
+        return d;
+    } else {
+        return l.planes;
+    }
 }
 
 template <typename T, bool kListed, int K>
@@ -1296,7 +1382,7 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
 template <int K>
 static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches) {
     int n = 0;
-    if (l.generic) return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : kStoreStrided>(l, s, launches);
+    if (l.generic) return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : (K >= kStorePlanarF ? kStoreStridedF : kStoreStrided)>(l, s, launches);
     if (l.ncomp == 3 && l.subx == 2 && l.suby == 2) return launch_recon420<K>(l, s, launches);
     const uint32_t cblocks = (l.max_bwc * l.max_bhc + kThreadsB - 1) / kThreadsB;
     const uint32_t gx = (l.max_bw0 + 31) / 32, gy = (l.max_bh0 + kThreadsB / 32 - 1) / (kThreadsB / 32);
@@ -1333,6 +1419,7 @@ static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches
 int launch_recon(const ReconLaunch &l, void *stream, int *launches) {
     cudaStream_t s = (cudaStream_t)stream;
     if (!l.planes) return launch_recon_kind<kStoreCanvas>(l, s, launches);
+    if (l.convert) return l.planar ? launch_recon_kind<kStorePlanarF>(l, s, launches) : launch_recon_kind<kStoreStridedF>(l, s, launches);
     if (l.planar) return launch_recon_kind<kStorePlanar>(l, s, launches);
     return launch_recon_kind<kStoreStrided>(l, s, launches);
 }

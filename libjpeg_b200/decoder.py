@@ -73,14 +73,73 @@ def component_shapes(info, upsample=True):
             for c in range(info.ncomp)]
 
 
+def _sample_types():
+    """torch float dtype -> B200JPG_SAMPLE_* of the float destinations"""
+    import torch
+    return {torch.float32: native.SAMPLE_F32, torch.float16: native.SAMPLE_F16, torch.bfloat16: native.SAMPLE_BF16}
+
+
+def _check_dtype(dtype, deep, first, where):
+    """integer destinations: uint8 for 8-bit, int16 for 12-bit frames; float destinations: any frame, one dtype per call
+    (`first` = the dtype of the call's first tensor)"""
+    import torch
+    floats = _sample_types()
+    if (dtype in floats or first in floats) and dtype != first:
+        raise TypeError("%sdtype %s, but the call's first destination is %s: one float dtype per call" % (where, dtype, first))
+    want = torch.int16 if deep else torch.uint8
+    if dtype not in floats and dtype != want:
+        raise TypeError("%sdtype %s, expected %s" % (where, dtype, want))
+
+
+def destination_dtype(dst):
+    """The dtype of the first tensor of a decode_into destination (None when it holds no tensor)."""
+    if hasattr(dst, "dtype"):
+        return dst.dtype
+    for entry in dst:
+        for t in entry or ():
+            return getattr(t, "dtype", None)
+    return None
+
+
+def convert_args(dtype, scale=None, bias=None, ncomp=4):
+    """The b200jpg_convert of a decode_into call into `dtype` tensors: None for uint8 / int16 destinations (scale and bias
+    must then be left out), else the element type and the map y = v * scale[c] + bias[c]. scale and bias are a scalar, which
+    applies to every component, or one value per component (ncomp of them); the defaults are 1 and 0. Both are rounded to
+    float32 and must be finite there. Raises ValueError / TypeError."""
+    import numbers
+    floats = _sample_types()
+    if dtype not in floats:
+        if scale is not None or bias is not None:
+            raise TypeError("scale and bias need a float32, float16 or bfloat16 destination, not %s" % dtype)
+        return None
+    c = native.ConvertStruct()
+    c.type = floats[dtype]
+    for name, v, default in (("scale", scale, 1.0), ("bias", bias, 0.0)):
+        if v is None:
+            vals = [default] * 4
+        elif isinstance(v, numbers.Real) or getattr(v, "ndim", None) == 0:
+            vals = [float(v)] * 4
+        else:
+            vals = [float(x) for x in v]
+            if len(vals) != ncomp:
+                raise ValueError("%s: %d values for %d components" % (name, len(vals), ncomp))
+            vals += [default] * (4 - ncomp)
+        with np.errstate(over="ignore"):
+            f32 = np.asarray(vals, dtype=np.float32)
+        if not np.isfinite(f32).all():
+            raise ValueError("%s must be finite in float32, got %s" % (name, vals[:ncomp]))
+        getattr(c, name)[:] = [float(x) for x in f32]
+    return c
+
+
 def plane_table(geometry, dst, device_type="cuda"):
     """The b200jpg_plane table of BatchDecoder.decode_into (4 entries per frame).
 
     geometry[i] = (component shapes [(h, w)], deep) of frame i, or None for a frame that failed to parse. dst[i] is a
     sequence of one 2-D tensor per component (a [C, H, W] tensor is one), uint8 for 8-bit and int16 for 12-bit (`deep`)
-    frames, or None where geometry[i] is None. Component c's sample (x, y) goes to t[y, x]: bytes_per_pixel =
-    stride(1) * itemsize, bytes_per_row = stride(0) * itemsize. Raises ValueError / TypeError on a wrong count, shape,
-    dtype or device; nothing has been launched then."""
+    frames, or float32 / float16 / bfloat16 for any frame (one of them for the whole call), or None where geometry[i] is
+    None. Component c's sample (x, y) goes to t[y, x]: bytes_per_pixel = stride(1) * itemsize, bytes_per_row = stride(0) *
+    itemsize. Raises ValueError / TypeError on a wrong count, shape, dtype or device; nothing has been launched then."""
     import torch
     n = len(geometry)
     if len(dst) != n:
@@ -88,6 +147,7 @@ def plane_table(geometry, dst, device_type="cuda"):
     if isinstance(dst, torch.Tensor) and dst.dim() == 4:
         return _batch_tensor_table(geometry, dst, device_type)
     table = (native.PlaneStruct * (4 * n))()
+    first = None
     for i, (geo, entry) in enumerate(zip(geometry, dst)):
         if geo is None:
             if entry is not None:
@@ -98,14 +158,13 @@ def plane_table(geometry, dst, device_type="cuda"):
         shapes, deep = geo
         if len(entry) != len(shapes):
             raise ValueError("frame %d has %d components, its destination %d" % (i, len(shapes), len(entry)))
-        dtype = torch.int16 if deep else torch.uint8
         for c, t in enumerate(entry):
             if not isinstance(t, torch.Tensor):
                 raise TypeError("frame %d component %d: expected a tensor, got %s" % (i, c, type(t).__name__))
             if t.device.type != device_type:
                 raise ValueError("frame %d component %d: a %s tensor, expected %s" % (i, c, t.device.type, device_type))
-            if t.dtype != dtype:
-                raise TypeError("frame %d component %d: dtype %s, expected %s" % (i, c, t.dtype, dtype))
+            first = t.dtype if first is None else first
+            _check_dtype(t.dtype, deep, first, "frame %d component %d: " % (i, c))
             if tuple(t.shape) != tuple(shapes[c]):
                 raise ValueError("frame %d component %d: shape %s, expected %s" % (i, c, tuple(t.shape), tuple(shapes[c])))
             e = table[4 * i + c]
@@ -123,13 +182,13 @@ def _batch_tensor_table(geometry, t, device_type):
     if not live:
         return (native.PlaneStruct * (4 * len(geometry)))()
     shapes, deep = geometry[live[0]]
-    if any(geometry[i] != (shapes, deep) for i in live) or len(set(shapes)) != 1:
+    same_depth = t.dtype not in _sample_types()  # a float tensor takes 8- and 12-bit frames alike
+    if any(geometry[i][0] != shapes or (same_depth and geometry[i][1] != deep) for i in live) or len(set(shapes)) != 1:
         raise ValueError("a [N, C, H, W] destination needs frames of one geometry")
     want = (len(geometry), len(shapes)) + tuple(shapes[0])
     if t.device.type != device_type:
         raise ValueError("a %s tensor, expected %s" % (t.device.type, device_type))
-    if t.dtype != (torch.int16 if deep else torch.uint8):
-        raise TypeError("dtype %s, expected %s" % (t.dtype, torch.int16 if deep else torch.uint8))
+    _check_dtype(t.dtype, deep, t.dtype, "")
     if tuple(t.shape) != want:
         raise ValueError("shape %s, expected %s" % (tuple(t.shape), want))
     arr = np.zeros(4 * len(geometry), dtype=np.dtype([("data", "<u8"), ("bpp", "<i4"), ("pad", "<i4"), ("bpr", "<i8")]))
@@ -263,13 +322,27 @@ class BatchDecoder:
             self._geometry = geo
         return self._geometry
 
-    def decode_into(self, dst, stream=None):
+    def decode_into(self, dst, stream=None, scale=None, bias=None):
         """decode() into caller-described tensors: dst[i] holds one 2-D CUDA tensor per component of frame i ([H, W], or
         each component's own size with upsample=False), so a [N, C, H, W] batch tensor can be passed as it is, an NHWC
         tensor t as t.permute(0, 3, 1, 2), BGR as [t[i, ..., 2], t[i, ..., 1], t[i, ..., 0]]. uint8 for 8-bit frames,
-        int16 for 12-bit frames; None for frames that failed to parse. Only the samples are written. Returns dst."""
-        table = plane_table(self.geometry(), dst)
-        native.check(lib.b200jpg_batch_decode_into(self.handle, table, self._stream_ptr(stream)), self.ctx.handle)
+        int16 for 12-bit frames; None for frames that failed to parse. Only the samples are written. Returns dst.
+
+        float32, float16 or bfloat16 destinations (one dtype per call, any frame) receive every integer sample v (0..255,
+        or 0..4095 for 12-bit frames) converted in the reconstruction kernels' store, with no extra pass:
+            y = float32(float32(v * scale[c]) + bias[c]), then rounded to nearest even into float16 / bfloat16
+        which is what t.float() * scale + bias followed by .half() / .bfloat16() gives. c is the output component (R, G, B
+        after the colour transformation). scale and bias are a scalar or one value per component (defaults 1 and 0),
+        rounded to float32. ImageNet-style normalisation (x / 255 - mean) / std is scale = 1 / (255 * std),
+        bias = -mean / std."""
+        geo = self.geometry()
+        table = plane_table(geo, dst)
+        ncomp = max([len(g[0]) for g in geo if g is not None] or [1])
+        conv = convert_args(destination_dtype(dst), scale, bias, ncomp)
+        if conv is None:
+            native.check(lib.b200jpg_batch_decode_into(self.handle, table, self._stream_ptr(stream)), self.ctx.handle)
+        else:
+            native.check(lib.b200jpg_batch_decode_into_ex(self.handle, table, ctypes.byref(conv), self._stream_ptr(stream)), self.ctx.handle)
         return dst
 
     def decode_entropy(self, stream=None):

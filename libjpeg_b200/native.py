@@ -31,6 +31,14 @@ class PlaneStruct(ctypes.Structure):
     _fields_ = [("data", ctypes.c_void_p), ("bytes_per_pixel", ctypes.c_int32), ("pad", ctypes.c_int32), ("bytes_per_row", ctypes.c_int64)]
 
 
+class ConvertStruct(ctypes.Structure):
+    """b200jpg_convert: element type (SAMPLE_*) and the per-component map y = v * scale[c] + bias[c] of a float destination."""
+    _fields_ = [("type", ctypes.c_int32), ("scale", ctypes.c_float * 4), ("bias", ctypes.c_float * 4)]
+
+
+SAMPLE_F32, SAMPLE_F16, SAMPLE_BF16 = 1, 2, 3
+
+
 def library_path():
     return _LIB_PATH
 
@@ -64,6 +72,7 @@ def _load():
         "b200jpg_batch_reindex": (i32, [vp, vp]),
         "b200jpg_batch_decode": (i32, [vp, vp, vp]),
         "b200jpg_batch_decode_into": (i32, [vp, ctypes.POINTER(PlaneStruct), vp]),
+        "b200jpg_batch_decode_into_ex": (i32, [vp, ctypes.POINTER(PlaneStruct), ctypes.POINTER(ConvertStruct), vp]),
         "b200jpg_batch_decode_entropy": (i32, [vp, vp]),
         "b200jpg_batch_reconstruct": (i32, [vp, vp, vp]),
         "b200jpg_batch_frame_status": (i32, [vp, i32]),
@@ -93,7 +102,8 @@ ABI_SYMBOLS = [
     "b200jpg_parse", "b200jpg_build_tables", "b200jpg_create", "b200jpg_destroy", "b200jpg_trim", "b200jpg_last_error", "b200jpg_batch_create", "b200jpg_batch_create_ex",
     "b200jpg_batch_destroy", "b200jpg_batch_frame_info", "b200jpg_batch_out_offset", "b200jpg_batch_out_bytes",
     "b200jpg_batch_ecs_bytes", "b200jpg_batch_stored_blocks", "b200jpg_batch_h2d_bytes", "b200jpg_batch_export_tables",
-    "b200jpg_batch_import_tables", "b200jpg_batch_upload", "b200jpg_batch_reindex", "b200jpg_batch_decode", "b200jpg_batch_decode_into", "b200jpg_batch_decode_entropy",
+    "b200jpg_batch_import_tables", "b200jpg_batch_upload", "b200jpg_batch_reindex", "b200jpg_batch_decode", "b200jpg_batch_decode_into", "b200jpg_batch_decode_into_ex",
+    "b200jpg_batch_decode_entropy",
     "b200jpg_batch_reconstruct", "b200jpg_batch_frame_status", "b200jpg_batch_read_coefficients",
     "b200jpg_batch_last_launch_count", "b200jpg_batch_enable_timing", "b200jpg_batch_last_timing", "b200jpg_batch_last_unstuff_ms", "b200jpg_decode_to_host", "b200jpg_decode_to_host_ex", "b200jpg_decode_to_device_ex",
     "b200jpg_device_free", "b200jpg_device_copy_rect", "b200jpg_selftest_restartless", "b200jpg_selftest_table_cache",
