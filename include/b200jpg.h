@@ -215,6 +215,11 @@ B200JPG_API int b200jpg_microbench_int32(int device, float *imad_gops, float *al
  * device kernel for scan 0 of one codestream on the host and checks the resulting work items against a front-to-back walk.
  * Returns B200JPG_OK, a parser error, or -1..-4 for an inconsistent partition. */
 B200JPG_API int b200jpg_selftest_restartless(const uint8_t *data, size_t len, uint32_t *rounds, uint32_t *n_segments);
+/* The work items of the same host replay (tests only, no device), seven int32 per item: start bit in the unstuffed scan, first
+ * block, block count and the DC predictors of the four scan components. *n_items receives the count; with fewer than that in
+ * `cap` nothing is written and the call returns B200JPG_ERR_INVALID_PARAMETER. */
+B200JPG_API int b200jpg_selftest_restartless_items(const uint8_t *data, size_t len, int32_t *items, uint32_t cap, uint32_t *n_items,
+                                                   uint32_t *rounds);
 /* Host-only self-test of the decoder-table cache of b200jpg_batch_create (frames of one source share their tables; the tables of a
  * scan are built once per distinct set of Huffman specifications, quantisation tables and scan parameters): every scan of the
  * given codestreams through the cache, twice, against a fresh HuffmanTemplate::BuildDecoder-equivalent build

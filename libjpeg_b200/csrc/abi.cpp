@@ -1438,17 +1438,23 @@ int b200jpg_batch_last_timing(b200jpg_batch *b, float *entropy_ms, float *recons
     return B200JPG_OK;
 }
 
-// Host replay of the synchronisation rounds of spec_sync_kernel on scan 0 of one codestream, checked against a plain
-// front-to-back walk of the same stream (tests only: it validates the round logic, prefix sums and clipping that the device
-// kernel shares through specsync.hpp; nothing in the decode path calls it).
-int b200jpg_selftest_restartless(const uint8_t *data, size_t len, uint32_t *rounds, uint32_t *n_segments) {
+// Scan 0 of a restart-less codestream as the host replay of spec_sync_kernel takes it (tests only)
+struct ReplayScan {
+    TableSet ts;
+    SpecScan ss{};
+    std::vector<uint32_t> words;
+    uint32_t len_bytes = 0, total_mcus = 0;
+    int ns = 0;
+};
+
+static int replay_scan0(const uint8_t *data, size_t len, ReplayScan &rs) {
     ParsedFrame pf;
     std::string err;
     int rc = parse_codestream(data, len, pf, err);
     if (rc) return rc;
     const ScanInfo &sc = pf.scans[0];
     if (sc.progressive || sc.interval_off.size() != 1) return B200JPG_ERR_INVALID_PARAMETER;
-    TableSet ts;
+    TableSet &ts = rs.ts;
     rc = build_table_set(sc, ts, err);
     if (rc) return rc;
     // unstuff (io/bitstream.cpp:56-118) into big-endian words
@@ -1464,13 +1470,14 @@ int b200jpg_selftest_restartless(const uint8_t *data, size_t len, uint32_t *roun
         }
         bytes.push_back(data[i]);
     }
-    const uint32_t len_bytes = (uint32_t)bytes.size();
+    rs.len_bytes = (uint32_t)bytes.size();
     bytes.resize((bytes.size() + 3) / 4 * 4 + 64, 0);
-    std::vector<uint32_t> words(bytes.size() / 4);
+    std::vector<uint32_t> &words = rs.words;
+    words.resize(bytes.size() / 4);
     for (size_t i = 0; i < words.size(); i++)
         words[i] = ((uint32_t)bytes[4 * i] << 24) | ((uint32_t)bytes[4 * i + 1] << 16) | ((uint32_t)bytes[4 * i + 2] << 8) | bytes[4 * i + 3];
     const uint16_t *lut_off = reinterpret_cast<const uint16_t *>(ts.blob.data() + 16);
-    SpecScan ss{};
+    SpecScan &ss = rs.ss;
     ss.lut = reinterpret_cast<const uint32_t *>(ts.blob.data() + kTableHeaderBytes);
     const b200jpg_frame_info &fi = pf.info;
     for (int c = 0; c < sc.ns; c++) {
@@ -1479,13 +1486,38 @@ int b200jpg_selftest_restartless(const uint8_t *data, size_t len, uint32_t *roun
         const int nb = sc.ns > 1 ? fi.hs[sc.comp[c]] * fi.vs[sc.comp[c]] : 1;
         for (int k = 0; k < nb; k++) ss.comp_of_block[ss.blocks_per_mcu++] = (uint8_t)c;
     }
-    const uint32_t total_mcus = sc.mcu_cols * sc.mcu_rows;
-    std::vector<SpecSegment> segs;
-    extern unsigned long long g_spec_replay_bits;
+    ss.blk_period = ss.blocks_per_mcu;  // exact positions for the walks of the self-test; the replay finds its own period
+    rs.total_mcus = sc.mcu_cols * sc.mcu_rows;
+    rs.ns = sc.ns;
+    return B200JPG_OK;
+}
+
+static int replay_rounds(const ReplayScan &rs, std::vector<SpecSegment> &segs) {
+    extern unsigned long long g_spec_replay_bits, g_spec_replay_merges[kSpecMarks];
     g_spec_replay_bits = 0;
-    const int r = spec_sync_host_replay(ss, words.data(), len_bytes, total_mcus, segs);
-    if (getenv("B200JPG_SPEC_STATS"))
-        fprintf(stderr, "restart-less replay: %u rounds, %.2f x the stream walked\n", (unsigned)r, (double)g_spec_replay_bits / (8.0 * len_bytes + 1));
+    for (auto &m : g_spec_replay_merges) m = 0;
+    const int r = spec_sync_host_replay(rs.ss, rs.words.data(), rs.len_bytes, rs.total_mcus, segs);
+    if (getenv("B200JPG_SPEC_STATS")) {
+        fprintf(stderr, "restart-less replay: %u rounds, %.2f x the stream walked, merges at marks", (unsigned)r,
+                (double)g_spec_replay_bits / (8.0 * rs.len_bytes + 1));
+        for (int m = 0; m < kSpecMarks; m++) fprintf(stderr, " %llu", g_spec_replay_merges[m]);
+        fprintf(stderr, "\n");
+    }
+    return r;
+}
+
+// Host replay of the synchronisation rounds of spec_sync_kernel on scan 0 of one codestream, checked against a plain
+// front-to-back walk of the same stream (tests only: it validates the round logic, prefix sums and clipping that the device
+// kernel shares through specsync.hpp; nothing in the decode path calls it).
+int b200jpg_selftest_restartless(const uint8_t *data, size_t len, uint32_t *rounds, uint32_t *n_segments) {
+    ReplayScan rs;
+    const int rc = replay_scan0(data, len, rs);
+    if (rc) return rc;
+    const SpecScan &ss = rs.ss;
+    const std::vector<uint32_t> &words = rs.words;
+    const uint32_t len_bytes = rs.len_bytes, total_mcus = rs.total_mcus;
+    std::vector<SpecSegment> segs;
+    const int r = replay_rounds(rs, segs);
     if (rounds) *rounds = (uint32_t)r;
     if (n_segments) *n_segments = (uint32_t)segs.size();
     // the truth: one walk from the first bit, block by block
@@ -1508,12 +1540,31 @@ int b200jpg_selftest_restartless(const uint8_t *data, size_t len, uint32_t *roun
         if (g.first_block != covered) return -1;                       // the segments tile the blocks in order
         if (g.first_block < walked) {
             if (g.bit != start_bit[g.first_block]) return -2;          // and start where their first block starts
-            for (int c = 0; c < sc.ns; c++)
+            for (int c = 0; c < rs.ns; c++)
                 if (g.pred[c] != pred_at[(size_t)g.first_block * 4 + c]) return -3;  // with the predictors of that place
         }
         covered += g.n_blocks;
     }
     if (covered != total_blocks) return -4;
+    return B200JPG_OK;
+}
+
+// The same replay's work items themselves (tests only), seven int32 each: start bit, first block, block count and the four
+// DC predictors, for tests that hold them against what the encoder recorded rather than against another walk of the decoder.
+int b200jpg_selftest_restartless_items(const uint8_t *data, size_t len, int32_t *items, uint32_t cap, uint32_t *n_items, uint32_t *rounds) {
+    ReplayScan rs;
+    const int rc = replay_scan0(data, len, rs);
+    if (rc) return rc;
+    std::vector<SpecSegment> segs;
+    const int r = replay_rounds(rs, segs);
+    if (rounds) *rounds = (uint32_t)r;
+    if (n_items) *n_items = (uint32_t)segs.size();
+    if (!items || segs.size() > cap) return B200JPG_ERR_INVALID_PARAMETER;
+    for (size_t i = 0; i < segs.size(); i++) {
+        int32_t *o = items + 7 * i;
+        o[0] = (int32_t)segs[i].bit, o[1] = (int32_t)segs[i].first_block, o[2] = (int32_t)segs[i].n_blocks;
+        for (int c = 0; c < 4; c++) o[3 + c] = segs[i].pred[c];
+    }
     return B200JPG_OK;
 }
 

@@ -43,8 +43,29 @@ struct SpecScan {               // what the length-only decoder needs to know ab
     const uint32_t *lut;        // two-level tables of the scan's table set (internal.hpp), word offsets below
     uint32_t dc_tab[4], ac_tab[4];   // word offset of the DC / AC table of scan component c
     uint32_t blocks_per_mcu;
+    uint32_t blk_period;        // SpecState::blk counts modulo this (spec_table_period, or blocks_per_mcu for the exact position)
     uint8_t comp_of_block[kSpecMaxBlocksPerMcu];  // scan component of block b of an MCU (sequentialscan.cpp:387-424 order)
 };
+
+// The smallest p (a divisor of blocks_per_mcu) for which block b and block b + p of the MCU decode with the same DC and AC
+// tables. Decoding a stream determines a block's position in the MCU only modulo p: two paths that start on the same bit
+// with positions that differ by a multiple of p walk the same bits forever. So the rounds compare and log states with blk
+// counted modulo p -- 1 when every component uses the same tables (the reference encoder without colour transformation),
+// blocks_per_mcu when the tables tell every position apart -- and the DC differences, which do depend on the exact
+// position, are summed by a second walk from the true first block once the entries are known (spec_sync_kernel).
+B200JPG_HD uint32_t spec_table_period(const SpecScan &sc) {
+    const uint32_t bpm = sc.blocks_per_mcu;
+    for (uint32_t p = 1; p < bpm; p++) {
+        if (bpm % p) continue;
+        bool same = true;
+        for (uint32_t b = p; b < bpm && same; b++) {
+            const uint32_t c = sc.comp_of_block[b], d = sc.comp_of_block[b - p];
+            same = sc.dc_tab[c] == sc.dc_tab[d] && sc.ac_tab[c] == sc.ac_tab[d];
+        }
+        if (same) return p;
+    }
+    return bpm;
+}
 
 struct SpecState {  // a block boundary on some decoding path
     uint32_t bit;   // position in the unstuffed stream
@@ -96,19 +117,22 @@ struct SpecLog {
 // Decodes whole blocks from `from` until a block boundary at or behind `limit_bit` (or behind the end of the data).
 // ONE flat loop, one symbol per iteration (the DC symbol of a block when k == 0, else an AC symbol): the threads of a warp
 // run the same few instructions whatever their blocks look like, and only diverge where they finish.
+// Block positions advance modulo sc.blk_period: with a period below blocks_per_mcu the states are canonical (blk < period)
+// and the DC sums are attributed to the components of those canonical positions, i.e. meaningless; only the block counts
+// and the states are used then.
 // With a log: `log` holds the marks of this subsequence's previous path (states ~0 before the first round) and receives
-// those of the new one; `merged` tells that the walk ended on an old mark (the exit of the previous round stands) and the
-// returned counts already include the logged rest.
+// those of the new one; `merged_at` receives the old mark the walk ended on (the exit of the previous round stands and the
+// returned counts already include the logged rest), or -1.
 // With a run-up (count_from > from.bit): the walk starts somewhere IN FRONT of the subsequence, on a guess; blocks that start in
 // front of `count_from` are decoded but not counted, and `*entered` receives the first block boundary at or behind count_from
 // -- the subsequence's entry state as this path sees it. A path that has fallen into step during the run-up reports the true
 // entry, and its counts and its exit are the true ones without a second walk.
 B200JPG_HD SpecResult spec_decode(const SpecScan &sc, const uint32_t *w, uint32_t nwords, uint32_t total_bits, SpecState from, uint32_t limit_bit,
-                                  SpecLog *log = nullptr, uint32_t first_mark_bit = 0, bool *merged = nullptr, uint32_t count_from = 0,
+                                  SpecLog *log = nullptr, uint32_t first_mark_bit = 0, int *merged_at = nullptr, uint32_t count_from = 0,
                                   SpecState *entered = nullptr) {
     uint32_t comp_bits = 0;  // two bits per block of an MCU: no indexed local array in the loop
     for (uint32_t b = 0; b < sc.blocks_per_mcu; b++) comp_bits |= (uint32_t)sc.comp_of_block[b] << (2u * b);
-    const uint32_t bpm = sc.blocks_per_mcu;
+    const uint32_t wrap = sc.blk_period;
     // everything the loop needs from the scan description in registers (the struct itself may sit in local memory)
     const uint32_t *const lut = sc.lut;
     const uint32_t dc0 = sc.dc_tab[0], dc1 = sc.dc_tab[1], dc2 = sc.dc_tab[2], dc3 = sc.dc_tab[3];
@@ -124,7 +148,7 @@ B200JPG_HD SpecResult spec_decode(const SpecScan &sc, const uint32_t *w, uint32_
     int32_t s0 = 0, s1 = 0, s2 = 0, s3 = 0;
     int mark = 0, merge_at = -1;   // next mark to pass; the mark the path merged at
     uint32_t next_mark = first_mark_bit;
-    if (merged) *merged = false;
+    if (merged_at) *merged_at = -1;
     if (log) {  // a path that starts behind marks leaves them unreached
         while (mark < kSpecMarks && bit > next_mark) {
             log->state[mark] = ~0ull;
@@ -179,7 +203,7 @@ B200JPG_HD SpecResult spec_decode(const SpecScan &sc, const uint32_t *w, uint32_
         if (k > 63) {
             k = 0;
             n++;
-            blk = blk + 1 == bpm ? 0 : blk + 1;
+            blk = blk + 1 == wrap ? 0 : blk + 1;
             cur = (comp_bits >> (2u * blk)) & 3u;
             dct = cur == 0 ? dc0 : (cur == 1 ? dc1 : (cur == 2 ? dc2 : dc3));
             act = cur == 0 ? ac0 : (cur == 1 ? ac1 : (cur == 2 ? ac2 : ac3));
@@ -199,7 +223,7 @@ B200JPG_HD SpecResult spec_decode(const SpecScan &sc, const uint32_t *w, uint32_
         if (merge_at >= 0) {  // the rest of the way is the logged one
             n += log->n_after[merge_at];
             s0 += log->dc_after[merge_at][0], s1 += log->dc_after[merge_at][1], s2 += log->dc_after[merge_at][2], s3 += log->dc_after[merge_at][3];
-            if (merged) *merged = true;
+            if (merged_at) *merged_at = merge_at;
         } else {  // marks behind the exit were not reached on this path
             for (int m = mark; m < kSpecMarks; m++) log->state[m] = ~0ull;
         }

@@ -43,6 +43,7 @@ spec_sync_kernel(ScanClassParams p, const uint8_t *__restrict__ clean, const uin
         sc.ac_tab[c] = lut_off[4 + p.ac_slot[c]];
         for (int b = 0; b < p.mw[c] * p.mh[c]; b++) sc.comp_of_block[sc.blocks_per_mcu++] = (uint8_t)c;
     }
+    sc.blk_period = spec_table_period(sc);
     const uint32_t len_bytes = interval_len[j] & kIntervalLenMask;
     const uint32_t total_bits = len_bytes * 8u, nwords = (len_bytes + 3u) / 4u;
     const uint32_t *w = reinterpret_cast<const uint32_t *>(clean + clean_off[j]);
@@ -76,14 +77,14 @@ spec_sync_kernel(ScanClassParams p, const uint8_t *__restrict__ clean, const uin
             SpecState from, entered;
             from.bit = (uint32_t)entry;
             from.blk = (uint32_t)(entry >> 32);
-            bool merged;
-            const SpecResult r = spec_decode(sc, w, nwords, total_bits, from, (i + 1u) * kSpecSeqBits, lg + i, i * kSpecSeqBits + kSpecMarkBits, &merged,
+            int merged_at;
+            const SpecResult r = spec_decode(sc, w, nwords, total_bits, from, (i + 1u) * kSpecSeqBits, lg + i, i * kSpecSeqBits + kSpecMarkBits, &merged_at,
                                              run_up ? i * kSpecSeqBits : 0u, run_up ? &entered : nullptr);
             // the entry this walk really had: after a run-up, the first block boundary inside the subsequence as the walk found it
             en[i] = run_up ? ((unsigned long long)entered.bit | ((unsigned long long)entered.blk << 32)) : entry;
             cnt[i] = r.n_blocks;
             ds[4 * i + 0] = r.dc_sum[0], ds[4 * i + 1] = r.dc_sum[1], ds[4 * i + 2] = r.dc_sum[2], ds[4 * i + 3] = r.dc_sum[3];
-            if (merged) continue;  // the path joined the previous round's: its exit stands
+            if (merged_at >= 0) continue;  // the path joined the previous round's: its exit stands
             const unsigned long long out = (unsigned long long)r.exit.bit | ((unsigned long long)r.exit.blk << 32);
             if (out != ex[i]) {
                 *reinterpret_cast<volatile unsigned long long *>(ex + i) = out;
@@ -93,10 +94,34 @@ spec_sync_kernel(ScanClassParams p, const uint8_t *__restrict__ clean, const uin
         if (changed) s_changed = 1;
         __syncthreads();
     }
+    const uint32_t total_blocks = p.total_mcus * sc.blocks_per_mcu;
+    if (sc.blk_period != sc.blocks_per_mcu) {
+        // the rounds knew block positions modulo the table period only, so their DC sums went to the wrong components.
+        // The first block of every subsequence (prefix sums of the counts, into the exits, which are done with) gives its
+        // true position; one more walk from there sums the DC differences per component.
+        if (tid == 0) {
+            uint32_t first = 0;
+            for (uint32_t i = 0; i < nseq; i++) {
+                ex[i] = first < total_blocks ? first : ~0ull;
+                if (first < total_blocks) first += cnt[i] < total_blocks - first ? cnt[i] : total_blocks - first;
+            }
+        }
+        __syncthreads();
+        sc.blk_period = sc.blocks_per_mcu;
+        for (uint32_t i = tid; i < nseq; i += kSyncThreads) {
+            const unsigned long long first = ex[i];
+            if (first == ~0ull) continue;
+            SpecState from;
+            from.bit = (uint32_t)en[i];
+            from.blk = (uint32_t)first % sc.blocks_per_mcu;
+            const SpecResult r = spec_decode(sc, w, nwords, total_bits, from, (i + 1u) * kSpecSeqBits);
+            ds[4 * i + 0] = r.dc_sum[0], ds[4 * i + 1] = r.dc_sum[1], ds[4 * i + 2] = r.dc_sum[2], ds[4 * i + 3] = r.dc_sum[3];
+        }
+        __syncthreads();
+    }
     // prefix sums over the subsequences: first block index and DC predictors. Sequential in one thread: a few thousand
     // additions per scan next to megabits of Huffman decoding.
     if (tid == 0) {
-        const uint32_t total_blocks = p.total_mcus * sc.blocks_per_mcu;
         uint32_t first = 0, last_used = 0;
         int32_t pred[4] = {0, 0, 0, 0};
         for (uint32_t i = 0; i < cap; i++) {
@@ -140,10 +165,13 @@ int launch_spec_sync(const EntropyLaunch &l, void *stream) {
 
 }  // namespace b200jpg
 unsigned long long g_spec_replay_bits = 0;
-namespace b200jpg {  // host replay only: bits walked (a merged walk counts up to the merge)
+unsigned long long g_spec_replay_merges[b200jpg::kSpecMarks] = {};
+namespace b200jpg {  // host replay only: bits walked (a merged walk counts up to the merge), walks that merged at each mark
 
 // Host replay of the same rounds (tests only): fills `segs` for one scan given its unstuffed words; returns the rounds used.
-int spec_sync_host_replay(const SpecScan &sc, const uint32_t *w, uint32_t len_bytes, uint32_t total_mcus, std::vector<SpecSegment> &segs) {
+int spec_sync_host_replay(const SpecScan &scan, const uint32_t *w, uint32_t len_bytes, uint32_t total_mcus, std::vector<SpecSegment> &segs) {
+    SpecScan sc = scan;
+    sc.blk_period = spec_table_period(sc);
     const uint32_t total_bits = len_bytes * 8u, nwords = (len_bytes + 3u) / 4u;
     const uint32_t nseq = (total_bits + kSpecSeqBits - 1u) / kSpecSeqBits;
     std::vector<unsigned long long> ex(nseq, ~0ull), en(nseq, ~0ull);
@@ -162,19 +190,34 @@ int spec_sync_host_replay(const SpecScan &sc, const uint32_t *w, uint32_t len_by
             if (!run_up && (entry == en[i] || entry == ~0ull)) continue;
             SpecState from, entered;
             from.bit = (uint32_t)entry, from.blk = (uint32_t)(entry >> 32);
-            bool merged;
-            const SpecResult r = spec_decode(sc, w, nwords, total_bits, from, (i + 1u) * kSpecSeqBits, &logs[i], i * kSpecSeqBits + kSpecMarkBits, &merged,
+            int merged_at;
+            const SpecResult r = spec_decode(sc, w, nwords, total_bits, from, (i + 1u) * kSpecSeqBits, &logs[i], i * kSpecSeqBits + kSpecMarkBits, &merged_at,
                                              run_up ? i * kSpecSeqBits : 0u, run_up ? &entered : nullptr);
             en[i] = run_up ? ((unsigned long long)entered.bit | ((unsigned long long)entered.blk << 32)) : entry;
             ::g_spec_replay_bits += r.exit.bit > from.bit ? r.exit.bit - from.bit : 0;
             cnt[i] = r.n_blocks;
             for (int c = 0; c < 4; c++) ds[4 * i + c] = r.dc_sum[c];
-            if (merged) continue;
+            if (merged_at >= 0) {
+                ::g_spec_replay_merges[merged_at]++;
+                continue;
+            }
             const unsigned long long out = (unsigned long long)r.exit.bit | ((unsigned long long)r.exit.blk << 32);
             if (out != ex[i]) ex[i] = out, changed = true;
         }
     }
     const uint32_t total_blocks = total_mcus * sc.blocks_per_mcu;
+    if (sc.blk_period != sc.blocks_per_mcu) {  // the DC sums again from every subsequence's true first block (spec_sync_kernel)
+        uint32_t first = 0;
+        SpecScan exact = sc;
+        exact.blk_period = sc.blocks_per_mcu;
+        for (uint32_t i = 0; i < nseq && first < total_blocks; i++) {
+            const SpecState from{(uint32_t)en[i], first % sc.blocks_per_mcu};
+            const SpecResult r = spec_decode(exact, w, nwords, total_bits, from, (i + 1u) * kSpecSeqBits);
+            ::g_spec_replay_bits += r.exit.bit > from.bit ? r.exit.bit - from.bit : 0;
+            for (int c = 0; c < 4; c++) ds[4 * i + c] = r.dc_sum[c];
+            first += cnt[i] < total_blocks - first ? cnt[i] : total_blocks - first;
+        }
+    }
     segs.assign(nseq, SpecSegment{});
     uint32_t first = 0, last_used = 0;
     int32_t pred[4] = {0, 0, 0, 0};

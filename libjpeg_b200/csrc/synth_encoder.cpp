@@ -142,7 +142,8 @@ void put16(std::vector<uint8_t> &o, int v) {
 
 }  // namespace
 
-// flags: 1 = one scan per component (non-interleaved), 2 = SOF1 (extended sequential) frame header, 4 = 16-bit DQT entries
+// flags: 1 = one scan per component (non-interleaved), 2 = SOF1 (extended sequential) frame header, 4 = 16-bit DQT entries,
+//        8 = every component on Huffman table 0 (the layout of the reference encoder without colour transformation)
 extern "C" __attribute__((visibility("default"))) long b200jpg_synth_encode_ex(const uint8_t *pix, int w, int h, int ncomp, int hs, int vs,
                                                                                  int quality, int dri, int flags, uint8_t *dst, long cap);
 extern "C" __attribute__((visibility("default"))) long b200jpg_synth_encode(const uint8_t *pix, int w, int h, int ncomp, int hs, int vs,
@@ -270,7 +271,8 @@ extern "C" __attribute__((visibility("default"))) long b200jpg_synth_encode_ex(c
         int qc[64];
         const uint8_t *qt = q[c ? 1 : 0];
         for (int i = 0; i < 64; i++) qc[i] = (int)std::lrintf(co[i] / qt[i]);
-        const HuffEnc &dc = c ? dcc : dcl, &ac = c ? acc_ : acl;
+        const bool chroma_tables = c && !(flags & 8);
+        const HuffEnc &dc = chroma_tables ? dcc : dcl, &ac = chroma_tables ? acc_ : acl;
         int diff = qc[0] - pred[c];
         pred[c] = qc[0];
         int s = bitsize(diff);
@@ -314,7 +316,7 @@ extern "C" __attribute__((visibility("default"))) long b200jpg_synth_encode_ex(c
         o.push_back((uint8_t)count);
         for (int c = first; c < first + count; c++) {
             o.push_back((uint8_t)c);
-            o.push_back(c == 0 ? 0x00 : 0x11);
+            o.push_back(c == 0 || (flags & 8) ? 0x00 : 0x11);
         }
         o.push_back(0), o.push_back(63), o.push_back(0);
         pred[0] = pred[1] = pred[2] = 0;

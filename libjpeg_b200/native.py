@@ -82,6 +82,8 @@ def _load():
         "b200jpg_batch_last_timing": (i32, [vp, ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float)]),
         "b200jpg_batch_last_unstuff_ms": (ctypes.c_float, [vp]),
         "b200jpg_selftest_restartless": (i32, [vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint32)]),
+        "b200jpg_selftest_restartless_items": (i32, [vp, ctypes.c_size_t, vp, ctypes.c_uint32, ctypes.POINTER(ctypes.c_uint32),
+                                                     ctypes.POINTER(ctypes.c_uint32)]),
         "b200jpg_selftest_table_cache": (i32, [ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32]),
         "b200jpg_decode_to_host": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, vp, u64]),
         "b200jpg_decode_to_host_ex": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, vp, u64, ctypes.c_uint]),
@@ -106,8 +108,8 @@ ABI_SYMBOLS = [
     "b200jpg_batch_decode_entropy",
     "b200jpg_batch_reconstruct", "b200jpg_batch_frame_status", "b200jpg_batch_read_coefficients",
     "b200jpg_batch_last_launch_count", "b200jpg_batch_enable_timing", "b200jpg_batch_last_timing", "b200jpg_batch_last_unstuff_ms", "b200jpg_decode_to_host", "b200jpg_decode_to_host_ex", "b200jpg_decode_to_device_ex",
-    "b200jpg_device_free", "b200jpg_device_copy_rect", "b200jpg_selftest_restartless", "b200jpg_selftest_table_cache",
-    "b200jpg_microbench_int32",
+    "b200jpg_device_free", "b200jpg_device_copy_rect", "b200jpg_selftest_restartless", "b200jpg_selftest_restartless_items",
+    "b200jpg_selftest_table_cache", "b200jpg_microbench_int32",
 ]
 
 

@@ -38,12 +38,13 @@ def source_image(w, h, seed):
     return np.clip(img, 0, 255).astype(np.uint8)
 
 
-NON_INTERLEAVED, SOF1, DQT16 = 1, 2, 4
+NON_INTERLEAVED, SOF1, DQT16, SHARED_TABLES = 1, 2, 4, 8
 
 
 def encode(pixels, quality=75, subsampling=(2, 2), restart_interval=0, flags=0):
     """Baseline JPEG bytes for an [H,W,3] or [H,W] uint8 image. subsampling = (hs, vs) of the luma component.
-    flags: NON_INTERLEAVED (one scan per component), SOF1 (extended sequential header), DQT16 (16-bit table entries)."""
+    flags: NON_INTERLEAVED (one scan per component), SOF1 (extended sequential header), DQT16 (16-bit table entries),
+    SHARED_TABLES (every component on Huffman tables 0)."""
     lib = _load()
     px = np.ascontiguousarray(pixels, dtype=np.uint8)
     h, w = px.shape[:2]

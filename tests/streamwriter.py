@@ -119,6 +119,7 @@ class BitWriter:
         self.n = 0
         self.bit = 0          # bits written in the current interval
         self.symbols = []     # (start bit within the interval, code length + value bits)
+        self.blocks = []      # start bit within the interval of every block of a sequential scan, in coding order
         self.intervals = []   # unstuffed bytes of every finished interval
 
     def put(self, value, n):
@@ -355,6 +356,7 @@ class _ScanCoder:
     def block(self, k, blk):
         s = self.s
         if not self.f.progressive:
+            self.w.blocks.append(self.w.bit)
             self.sequential(k, blk)
         elif s.ss == 0:
             dc = int(blk[0, 0])
@@ -381,7 +383,8 @@ def _check_scan(frame, scan):
 
 
 def encode(frame):
-    """-> the codestream (bytes). frame.stats receives, per scan, the coded symbols and the unstuffed interval lengths."""
+    """-> the codestream (bytes). frame.stats receives, per scan, the coded symbols, the unstuffed interval lengths and the start
+    bits of the blocks of a sequential scan."""
     if frame.precision not in (8, 12):
         raise ValueError("precision is 8 or 12")
     hmax, vmax, mcx, mcy, own = geometry(frame)
@@ -408,7 +411,7 @@ def encode(frame):
     if frame.restart_interval:
         out += _segment(0xDD, list(frame.restart_interval.to_bytes(2, "big")))
     current = dict(frame.tables)
-    frame.stats = {"symbols": [], "intervals": []}
+    frame.stats = {"symbols": [], "intervals": [], "blocks": []}
     for scan in frame.scans:
         _check_scan(frame, scan)
         out += _dht(scan.tables)
@@ -444,5 +447,6 @@ def encode(frame):
         out += w.out
         frame.stats["symbols"].append(w.symbols)
         frame.stats["intervals"].append(w.intervals)
+        frame.stats["blocks"].append(w.blocks)
     out += b"\xff\xd9"
     return bytes(out)
