@@ -17,6 +17,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "internal.hpp"
@@ -132,7 +133,7 @@ struct ScanClass {
 
 struct ReconGroup {
     uint32_t ncomp = 0, subx = 1, suby = 1;
-    bool generic = false;
+    ReconPath path = ReconPath::Tiled;
     std::vector<FrameRecon> frames;
     uint32_t max_bw0 = 0, max_bh0 = 0, max_bwc = 0, max_bhc = 0;
     uint64_t dev_frames = 0;
@@ -145,20 +146,34 @@ struct PfGroupHost {
     int comp_of_ac[4] = {0, 0, 0, 0};
 };
 
-// the tuned reconstruction kernels cover grey frames and three-component frames whose first component is not subsampled and
-// whose two other components share factors of 1 or 2; everything else (SURVEY 8f4) goes through the generic kernels
-static bool frame_is_generic(const b200jpg_frame_info &fi, unsigned flags = 0) {
-    if (flags & B200JPG_FLAG_NO_UPSAMPLE) return true;  // planes of every component, then one sample -> one output value
-    if (fi.precision != 8) return true;  // 12-bit frames: int32 planes, 16-bit samples out
-    if (fi.ncomp == 1) return fi.subx[0] != 1 || fi.suby[0] != 1;
-    if (fi.ncomp != 3) return true;
-    return fi.subx[0] != 1 || fi.suby[0] != 1 || fi.subx[1] != fi.subx[2] || fi.suby[1] != fi.suby[2] || fi.subx[1] > 2 || fi.suby[1] > 2;
+// scans share a launch class when their launch parameters and their table set are equal, compared bytewise
+struct ClassKey {
+    ScanClassParams p;
+    int table_set;
+    bool operator<(const ClassKey &o) const { return memcmp(this, &o, sizeof(ClassKey)) < 0; }
+};
+static_assert(std::has_unique_object_representations_v<ClassKey>, "ClassKey is compared bytewise: ScanClassParams must have no padding");
+
+struct Extent {
+    uint64_t w, h;
+};
+// component c as it leaves the decoder: the frame size, or without upsampling its own ceil(W / subx) x ceil(H / suby)
+Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags) {
+    if (!(flags & B200JPG_FLAG_NO_UPSAMPLE)) return {fi.width, fi.height};
+    return {(fi.width + fi.subx[c] - 1) / fi.subx[c], (fi.height + fi.suby[c] - 1) / fi.suby[c]};
 }
 
-struct ClassKey {
-    int v[40];
-    bool operator<(const ClassKey &o) const { return memcmp(v, o.v, sizeof(v)) < 0; }
-};
+// body(i) for every frame i < n, on at most max_threads host threads
+template <class Body>
+void for_frames(int n, unsigned max_threads, const Body &body) {
+    const unsigned nt = std::min({std::max(1u, std::thread::hardware_concurrency()), max_threads, (unsigned)n});
+    std::vector<std::thread> pool;
+    for (unsigned t = 0; t < nt; t++)
+        pool.emplace_back([&, t]() {
+            for (int i = (int)t; i < n; i += (int)nt) body(i);
+        });
+    for (auto &th : pool) th.join();
+}
 
 }  // namespace
 
@@ -172,6 +187,7 @@ struct b200jpg_batch {
     std::vector<int> xt_child, xt_parent;  // [n_user] index of a frame's residual frame or -1; [n] the reverse
     std::vector<uint64_t> out_off, out_bytes;
     uint64_t out_total = 0;
+    std::vector<std::array<uint64_t, 4>> coef_base;  // [n] int16 element offset of every component's coefficient plane (live frames)
     std::vector<TableSet> table_sets;
     std::vector<uint64_t> dev_tables;  // offset of each table blob inside the input buffer
     std::vector<ScanClass> classes;
@@ -414,115 +430,82 @@ void b200jpg_batch_destroy(b200jpg_batch *b) {
     delete b;
 }
 
-static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
-                             b200jpg_batch **out);
+// ---- batch planning: the steps of batch_create_impl, in the order they run
 
-int b200jpg_batch_create(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
-                         b200jpg_batch **out) {
-    return b200jpg_batch_create_ex(ctx, frames, lens, n, tolerate_bad, 0u, out);
+// the caller's codestreams, then the residual codestreams of its JPEG XT frames, and why each frame failed
+struct Codestreams {
+    std::vector<const uint8_t *> data;
+    std::vector<size_t> len;
+    std::vector<std::string> err;
+};
+
+static void parse_frames(b200jpg_batch &b, Codestreams &cs, bool device_index) {
+    b.frames.resize(b.n);
+    b.parse_status.assign(b.n, 0);
+    for_frames(b.n, 16, [&](int i) {
+        try {  // an exception must not leave the thread (std::terminate): it fails this frame only
+            b.parse_status[i] = parse_codestream(cs.data[i], cs.len[i], b.frames[i], cs.err[i], device_index);
+        } catch (const std::bad_alloc &) {
+            b.parse_status[i] = B200JPG_ERR_OUT_OF_MEMORY;
+            cs.err[i] = "out of memory while parsing the codestream";
+        } catch (...) {
+            b.parse_status[i] = B200JPG_ERR_MALFORMED_STREAM;
+            cs.err[i] = "codestream could not be parsed";
+        }
+    });
 }
 
-int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
-                            b200jpg_batch **out) {
-    if (!ctx) return B200JPG_ERR_INVALID_PARAMETER;
-    try {  // no exception crosses the C ABI
-        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, out);
-    } catch (const std::bad_alloc &) {
-        if (out) *out = nullptr;
-        return ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "out of host memory while preparing the batch");
-    } catch (...) {
-        if (out) *out = nullptr;
-        return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "unexpected failure while preparing the batch");
-    }
-}
-
-static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
-                             b200jpg_batch **out) {
-    NvtxRange nvtx("b200jpg batch_create: parse + pack");
-    if (!out || !frames || !lens || n <= 0) return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "invalid batch arguments");
-    *out = nullptr;
-    cudaError_t ce = cudaSetDevice(ctx->device);
-    if (ce != cudaSuccess) return ctx->fail_cuda(ce, "cudaSetDevice");
-
-    std::unique_ptr<b200jpg_batch, void (*)(b200jpg_batch *)> bp(new b200jpg_batch(), b200jpg_batch_destroy);
-    b200jpg_batch *b = bp.get();
-    b->ctx = ctx;
-    b->n = b->n_user = n;
-    b->flags = flags;
-    b->frames.resize(n);
-    b->parse_status.assign(n, 0);
-    std::vector<std::string> errs(n);
-    std::vector<const uint8_t *> fp(frames, frames + n);  // codestreams of the batch: the caller's, then the residual
-    std::vector<size_t> fl(lens, lens + n);               // codestreams of JPEG XT frames (internal frames behind them)
-
-    // ---- parse (host threads). Interleaved scans with restart markers get their restart index on the device (8f1);
-    // B200JPG_HOST_INDEX=1 keeps the memchr pass over every entropy coded byte on the host for all of them.
-    const bool device_index = getenv("B200JPG_HOST_INDEX") == nullptr;
-    {
-        unsigned nt = std::min<unsigned>(std::max(1u, std::thread::hardware_concurrency()), 16u);
-        nt = std::min<unsigned>(nt, (unsigned)n);
-        std::vector<std::thread> pool;
-        for (unsigned t = 0; t < nt; t++)
-            pool.emplace_back([&, t]() {
-                for (int i = (int)t; i < n; i += (int)nt) {
-                    try {  // an exception must not leave the thread (std::terminate): it fails this frame only
-                        b->parse_status[i] = parse_codestream(fp[i], fl[i], b->frames[i], errs[i], device_index);
-                    } catch (const std::bad_alloc &) {
-                        b->parse_status[i] = B200JPG_ERR_OUT_OF_MEMORY;
-                        errs[i] = "out of memory while parsing the codestream";
-                    } catch (...) {
-                        b->parse_status[i] = B200JPG_ERR_MALFORMED_STREAM;
-                        errs[i] = "codestream could not be parsed";
-                    }
-                }
-            });
-        for (auto &th : pool) th.join();
-    }
-    // ---- JPEG XT (SURVEY 8f3): the residual codestream of a frame is one more frame of the batch -- same entropy kernels, same
-    // IDCT -- that owns no output; the parent's reconstruction merges the two (generic_reconstruct_kernel)
-    const int n_user = n;
-    b->xt_child.assign(n_user, -1);
+// JPEG XT (SURVEY 8f3): the residual codestream of a frame is one more frame of the batch -- same entropy kernels, same
+// IDCT -- that owns no output; the parent's reconstruction merges the two (generic_reconstruct_kernel)
+static void attach_residuals(b200jpg_batch &b, Codestreams &cs, bool device_index) {
+    const int n_user = b.n_user;
+    b.xt_child.assign(n_user, -1);
     for (int i = 0; i < n_user; i++) {
-        if (b->parse_status[i] != 0 || !b->frames[i].xt.present) continue;
-        if (flags & (B200JPG_FLAG_NO_COLOR_TRANSFORM | B200JPG_FLAG_NO_UPSAMPLE)) {
-            b->parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;
-            errs[i] = "JPEG XT frames are only reconstructed with upsampling and colour transformation";
+        if (b.parse_status[i] != 0 || !b.frames[i].xt.present) continue;
+        if (b.flags & (B200JPG_FLAG_NO_COLOR_TRANSFORM | B200JPG_FLAG_NO_UPSAMPLE)) {
+            b.parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;
+            cs.err[i] = "JPEG XT frames are only reconstructed with upsampling and colour transformation";
             continue;
         }
         ParsedFrame rf;
         std::string rerr;
-        const int rst = parse_residual(b->frames[i], rf, rerr, device_index);
+        const int rst = parse_residual(b.frames[i], rf, rerr, device_index);
         if (rst != 0) {
-            b->parse_status[i] = rst;
-            errs[i] = rerr;
+            b.parse_status[i] = rst;
+            cs.err[i] = rerr;
             continue;
         }
-        b->xt_child[i] = (int)b->frames.size();
-        fp.push_back(b->frames[i].xt.resi.data());  // (the vectors' buffers stay where they are when b->frames grows: moved, not copied)
-        fl.push_back(b->frames[i].xt.resi.size());
-        b->frames.push_back(std::move(rf));
-        b->parse_status.push_back(0);
-        errs.emplace_back();
+        b.xt_child[i] = (int)b.frames.size();
+        cs.data.push_back(b.frames[i].xt.resi.data());  // (the vectors' buffers stay where they are when b.frames grows: moved, not copied)
+        cs.len.push_back(b.frames[i].xt.resi.size());
+        b.frames.push_back(std::move(rf));
+        b.parse_status.push_back(0);
+        cs.err.emplace_back();
     }
     for (int i = 0; i < n_user; i++)  // push_back may have moved the frames: take the addresses again
-        if (b->xt_child[i] >= 0) fp[b->xt_child[i]] = b->frames[i].xt.resi.data();
-    n = (int)b->frames.size();
-    b->n = n;
-    b->xt_parent.assign(n, -1);
+        if (b.xt_child[i] >= 0) cs.data[b.xt_child[i]] = b.frames[i].xt.resi.data();
+    b.n = (int)b.frames.size();
+    b.xt_parent.assign(b.n, -1);
     for (int i = 0; i < n_user; i++)
-        if (b->xt_child[i] >= 0) b->xt_parent[b->xt_child[i]] = i;
-    std::vector<std::vector<TableSet>> frame_tables(n);
+        if (b.xt_child[i] >= 0) b.xt_parent[b.xt_child[i]] = i;
+}
+
+// What the kernels cover, and the decoder tables of every scan of the frames that pass. A frame that fails here fails the batch
+// unless tolerate_bad: returns 0 or the status the batch fails with.
+static int admit_frames(b200jpg_batch &b, Codestreams &cs, bool tolerate_bad, std::vector<std::vector<TableSet>> &frame_tables) {
+    const int n = b.n;
+    frame_tables.assign(n, {});
     TableCache table_cache;
     for (int i = 0; i < n; i++) {
-        ParsedFrame &pf = b->frames[i];
-        int &st = b->parse_status[i];
-        if (st == 0) {  // what the kernels cover
+        ParsedFrame &pf = b.frames[i];
+        int &st = b.parse_status[i];
+        if (st == 0) {
             const b200jpg_frame_info &fi = pf.info;
             bool factors_ok = fi.ncomp >= 1 && fi.ncomp <= 4;
             for (int c = 0; c < fi.ncomp; c++) factors_ok = factors_ok && fi.subx[c] >= 1 && fi.subx[c] <= 4 && fi.suby[c] >= 1 && fi.suby[c] <= 4;
             if (!factors_ok) {  // the reference's upsampler cores exist for factors 1..4 (upsampling/upsamplerbase.cpp:CreateUpsampler)
                 st = B200JPG_ERR_NOT_IMPLEMENTED;
-                errs[i] = "only frames of one to four components with subsampling factors of one to four are supported";
+                cs.err[i] = "only frames of one to four components with subsampling factors of one to four are supported";
             } else {
                 // A sequential frame codes a component at most once. A component no scan codes (the stream ends early: the
                 // reference just stops at the EOI / the end of the data, Frame::ParseTrailer marker/frame.cpp:1062-1092)
@@ -533,9 +516,9 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
                 for (int c = 0; c < fi.ncomp; c++) {
                     if (fi.frame_type != 2 && seen[c] > 1) {
                         st = B200JPG_ERR_NOT_IMPLEMENTED;
-                        errs[i] = "sequential frame codes a component more than once, not supported by the GPU path";
+                        cs.err[i] = "sequential frame codes a component more than once, not supported by the GPU path";
                     }
-                    if (seen[c] == 0) b->clear_coef = true;
+                    if (seen[c] == 0) b.clear_coef = true;
                 }
             }
         }
@@ -545,71 +528,100 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
             frame_tables[i].resize(pf.scans.size());
             for (size_t si = 0; si < pf.scans.size() && st == 0; si++) {
                 try {
-                    st = build_table_set_cached(pf.scans[si], frame_tables[i][si], errs[i], table_cache);
+                    st = build_table_set_cached(pf.scans[si], frame_tables[i][si], cs.err[i], table_cache);
                 } catch (const std::bad_alloc &) {
                     st = B200JPG_ERR_OUT_OF_MEMORY;
-                    errs[i] = "out of memory while building the decoder tables";
+                    cs.err[i] = "out of memory while building the decoder tables";
                 }
             }
         }
-        if (st != 0 && b->xt_parent[i] >= 0) {  // a residual codestream the kernels do not cover fails its frame
-            const int par = b->xt_parent[i];
-            if (b->parse_status[par] == 0) b->parse_status[par] = st, errs[par] = "residual codestream: " + errs[i];
-            b->xt_child[par] = -1;
-            if (!tolerate_bad) return ctx->fail(st, "frame " + std::to_string(par) + ": " + errs[par]);
+        if (st != 0 && b.xt_parent[i] >= 0) {  // a residual codestream the kernels do not cover fails its frame
+            const int par = b.xt_parent[i];
+            if (b.parse_status[par] == 0) b.parse_status[par] = st, cs.err[par] = "residual codestream: " + cs.err[i];
+            b.xt_child[par] = -1;
+            if (!tolerate_bad) return b.ctx->fail(st, "frame " + std::to_string(par) + ": " + cs.err[par]);
         }
-        if (st != 0 && !tolerate_bad) return ctx->fail(st, "frame " + std::to_string(i) + ": " + errs[i]);
+        if (st != 0 && !tolerate_bad) return b.ctx->fail(st, "frame " + std::to_string(i) + ": " + cs.err[i]);
     }
     for (int i = 0; i < n; i++)  // ... and a frame that failed takes its residual codestream with it
-        if (b->xt_parent[i] >= 0 && b->parse_status[b->xt_parent[i]] != 0 && b->parse_status[i] == 0) b->parse_status[i] = b->parse_status[b->xt_parent[i]];
+        if (b.xt_parent[i] >= 0 && b.parse_status[b.xt_parent[i]] != 0 && b.parse_status[i] == 0) b.parse_status[i] = b.parse_status[b.xt_parent[i]];
+    return B200JPG_OK;
+}
 
-    // ---- layout of the packed input buffer: [codestreams][table blobs][per class: scans, intervals][per group: frames]
-    std::vector<uint64_t> byte_off(n, 0);
+// layout of the packed input buffer: [codestreams][table blobs][per class: scans, intervals][per group: frames]. Here the first
+// region: returns the offset of every frame's codestream.
+static std::vector<uint64_t> lay_out_codestreams(b200jpg_batch &b, const std::vector<size_t> &len) {
+    std::vector<uint64_t> byte_off(b.n, 0);
     uint64_t cur = 0;
-    for (int i = 0; i < n; i++) {
+    for (int i = 0; i < b.n; i++) {
         byte_off[i] = cur;
-        if (b->parse_status[i] == 0) cur = align_up(cur + fl[i] + 32, 16);
+        if (b.parse_status[i] == 0) cur = align_up(cur + len[i] + 32, 16);
     }
-    b->bytes_region = align_up(cur + 64, 256);
+    b.bytes_region = align_up(cur + 64, 256);
+    return byte_off;
+}
 
-    // coefficient / sample / output layout
-    b->out_off.assign(n, 0);
-    b->out_bytes.assign(n, 0);
-    std::vector<std::array<uint64_t, 4>> coef_base(n), sample_base(n);
+// How live frame i is reconstructed. The tuned kernels cover 8-bit grey frames and three-component frames whose first component
+// is not subsampled and whose two other components share factors of 1 or 2; everything else (SURVEY 8f4), planes without
+// upsampling and both codestreams of a JPEG XT frame go through the generic kernels.
+static ReconPath recon_path(const b200jpg_batch &b, int i) {
+    const b200jpg_frame_info &fi = b.frames[i].info;
+    if (b.xt_parent[i] >= 0 || (i < b.n_user && b.xt_child[i] >= 0)) return ReconPath::Generic;
+    if (b.flags & B200JPG_FLAG_NO_UPSAMPLE) return ReconPath::Generic;  // planes of every component, then one sample -> one output value
+    if (fi.precision != 8) return ReconPath::Generic;  // 12-bit frames: int32 planes, 16-bit samples out
+    if (fi.ncomp == 1) return (fi.subx[0] != 1 || fi.suby[0] != 1) ? ReconPath::Generic : ReconPath::Tiled;
+    if (fi.ncomp != 3 || fi.subx[0] != 1 || fi.suby[0] != 1 || fi.subx[1] != fi.subx[2] || fi.suby[1] != fi.suby[2] || fi.subx[1] > 2 || fi.suby[1] > 2)
+        return ReconPath::Generic;
+    return (fi.subx[1] == 2 && fi.suby[1] == 2) ? ReconPath::Fused420 : ReconPath::Tiled;
+}
+
+// Coefficient, sample and output layout of the live frames; returns the sample plane offsets. The sample planes a frame gets
+// follow its reconstruction path: Generic one per component, Tiled one per component from 1 on, Fused420 none (its chroma samples
+// live in shared memory).
+static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
+    const int n = b.n;
+    b.coef_base.assign(n, {});
+    b.out_off.assign(n, 0);
+    b.out_bytes.assign(n, 0);
+    std::vector<std::array<uint64_t, 4>> sample_base(n);
     uint64_t coef_cur = 0, sample_cur = 0, out_cur = 0;
     for (int i = 0; i < n; i++) {
-        if (b->parse_status[i] != 0) continue;
-        const b200jpg_frame_info &fi = b->frames[i].info;
+        if (b.parse_status[i] != 0) continue;
+        const b200jpg_frame_info &fi = b.frames[i].info;
+        const ReconPath path = recon_path(b, i);
+        const int first_plane = path == ReconPath::Generic ? 0 : (path == ReconPath::Tiled ? 1 : fi.ncomp);
+        uint64_t samples = 0;
         for (int c = 0; c < fi.ncomp; c++) {
-            coef_base[i][c] = coef_cur;
-            coef_cur += (uint64_t)fi.blocks_w[c] * fi.blocks_h[c] * 64;
-            if (c > 0 || frame_is_generic(fi, flags) || b->xt_parent[i] >= 0 || (i < n_user && b->xt_child[i] >= 0)) {  // generic reconstruction keeps a sample plane of every component
+            const uint64_t elems = (uint64_t)fi.blocks_w[c] * fi.blocks_h[c] * 64;
+            b.coef_base[i][c] = coef_cur;
+            coef_cur += elems;
+            if (c >= first_plane) {
                 sample_base[i][c] = sample_cur;
-                sample_cur += (uint64_t)fi.blocks_w[c] * fi.blocks_h[c] * 64;
+                sample_cur += elems;
             }
+            const Extent e = out_extent(fi, c, b.flags);  // the components one after the other
+            samples += e.w * e.h;
         }
-        b->out_off[i] = out_cur;
-        uint64_t samples = (uint64_t)fi.width * fi.height * fi.ncomp;
-        if (flags & B200JPG_FLAG_NO_UPSAMPLE) {  // plane after plane, every component at its own resolution
-            samples = 0;
-            for (int c = 0; c < fi.ncomp; c++)
-                samples += (uint64_t)((fi.width + fi.subx[c] - 1) / fi.subx[c]) * ((fi.height + fi.suby[c] - 1) / fi.suby[c]);
-        }
-        b->out_bytes[i] = (b->xt_parent[i] >= 0) ? 0 : samples * (fi.precision > 8 ? 2u : 1u);  // a residual codestream has no pixels of its own
-        out_cur = align_up(out_cur + b->out_bytes[i], 256);
-        b->ecs_bytes += fi.ecs_bytes;
-        b->stored_blocks += fi.stored_blocks;
+        b.out_off[i] = out_cur;
+        b.out_bytes[i] = (b.xt_parent[i] >= 0) ? 0 : samples * (fi.precision > 8 ? 2u : 1u);  // a residual codestream has no pixels of its own
+        out_cur = align_up(out_cur + b.out_bytes[i], 256);
+        b.ecs_bytes += fi.ecs_bytes;
+        b.stored_blocks += fi.stored_blocks;
     }
-    b->out_total = out_cur;
-    b->coef_elems = coef_cur;
-    b->sample_elems = sample_cur;
+    b.out_total = out_cur;
+    b.coef_elems = coef_cur;
+    b.sample_elems = sample_cur;
+    return sample_base;
+}
 
-    // ---- table sets (deduplicated by content) and scan classes
+// table sets (deduplicated by content) and scan classes, launched in the order they are formed here except that the scans of a
+// progressive frame build on each other: launch order = scan order (sequential classes: ordinal 0)
+static void form_scan_classes(b200jpg_batch &b, std::vector<std::vector<TableSet>> &frame_tables, const std::vector<uint64_t> &byte_off) {
     std::map<std::vector<uint8_t>, int> table_index;
     std::map<ClassKey, int> class_index;
-    for (int i = 0; i < n; i++) {
-        if (b->parse_status[i] != 0) continue;
-        ParsedFrame &pf = b->frames[i];
+    for (int i = 0; i < b.n; i++) {
+        if (b.parse_status[i] != 0) continue;
+        ParsedFrame &pf = b.frames[i];
         const b200jpg_frame_info &fi = pf.info;
         for (size_t si = 0; si < pf.scans.size(); si++) {
             auto &sc = pf.scans[si];
@@ -617,9 +629,9 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
             int ti;
             auto it = table_index.find(ts.blob);
             if (it == table_index.end()) {
-                ti = (int)b->table_sets.size();
+                ti = (int)b.table_sets.size();
                 table_index.emplace(ts.blob, ti);
-                b->table_sets.push_back(std::move(ts));
+                b.table_sets.push_back(std::move(ts));
             } else {
                 ti = it->second;
             }
@@ -638,7 +650,7 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
             p.total_mcus = sc.mcu_cols * sc.mcu_rows;
             p.dri = sc.dri ? sc.dri : p.total_mcus;
             p.intervals_per_scan = (uint32_t)sc.interval_off.size();
-            p.lut_words = b->table_sets[ti].lut_words();
+            p.lut_words = b.table_sets[ti].lut_words();
             p.progressive = sc.progressive ? 1 : 0;
             p.ss = sc.ss;
             p.se = sc.se;
@@ -646,45 +658,23 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
             p.al = sc.lowbit;
             p.ordinal = sc.progressive ? (int)si : 0;
             p.indexed = sc.spec ? 1 : 0;
-            ClassKey key{};
-            int kk = 0;
-            key.v[kk++] = p.ns;
-            for (int k = 0; k < 4; k++) {
-                key.v[kk++] = p.mw[k];
-                key.v[kk++] = p.mh[k];
-                key.v[kk++] = p.bw[k];
-                key.v[kk++] = p.dc_slot[k];
-                key.v[kk++] = p.ac_slot[k];
-                key.v[kk++] = p.q_slot[k];
-            }
-            key.v[kk++] = (int)p.mcu_cols;
-            key.v[kk++] = (int)p.total_mcus;
-            key.v[kk++] = (int)p.dri;
-            key.v[kk++] = (int)p.intervals_per_scan;
-            key.v[kk++] = ti;
-            key.v[kk++] = p.progressive;
-            key.v[kk++] = p.ss;
-            key.v[kk++] = p.se;
-            key.v[kk++] = p.ah;
-            key.v[kk++] = p.al;
-            key.v[kk++] = p.ordinal;
-            key.v[kk++] = p.indexed;
+            const ClassKey key{p, ti};  // n_scans and segs_per_scan are still 0 here
             int cidx;
             auto cit = class_index.find(key);
             if (cit == class_index.end()) {
-                cidx = (int)b->classes.size();
+                cidx = (int)b.classes.size();
                 class_index.emplace(key, cidx);
                 ScanClass cl;
                 cl.p = p;
                 cl.table_set = ti;
-                b->classes.push_back(std::move(cl));
+                b.classes.push_back(std::move(cl));
             } else {
                 cidx = cit->second;
             }
-            ScanClass &cl = b->classes[cidx];
+            ScanClass &cl = b.classes[cidx];
             cl.frame_comp0 = sc.comp[0];
             ClassScan cs{};
-            for (int k = 0; k < sc.ns; k++) cs.coef_base[k] = coef_base[i][sc.comp[k]];
+            for (int k = 0; k < sc.ns; k++) cs.coef_base[k] = b.coef_base[i][sc.comp[k]];
             cs.frame = (uint32_t)i;
             cl.scans.push_back(cs);
             cl.scan_on_device.push_back(sc.device_index ? 1 : 0);
@@ -704,15 +694,18 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
             }
         }
     }
-    // the scans of a progressive frame build on each other: launch order = scan order (sequential classes: ordinal 0)
-    std::stable_sort(b->classes.begin(), b->classes.end(), [](const ScanClass &x, const ScanClass &y) { return x.p.ordinal < y.p.ordinal; });
-    // ---- component-fused progressive groups: classes that hold exactly the same frames in the same order and whose scans are
-    // either interleaved DC scans of all components or single-component AC scans with equal restart intervals per group
-    std::vector<uint8_t> frame_fused(n, 0);
+    std::stable_sort(b.classes.begin(), b.classes.end(), [](const ScanClass &x, const ScanClass &y) { return x.p.ordinal < y.p.ordinal; });
+}
+
+// Component-fused progressive groups: classes that hold exactly the same frames in the same order and whose scans are either
+// interleaved DC scans of all components or single-component AC scans with equal restart intervals per group. The other
+// progressive frames go scan by scan and are dequantised after their last scan.
+static void form_progressive_groups(b200jpg_batch &b) {
+    std::vector<uint8_t> frame_fused(b.n, 0);
     if (getenv("B200JPG_NO_PFUSE") == nullptr) {
         std::map<std::vector<uint32_t>, std::vector<int>> by_frames;
-        for (size_t ci = 0; ci < b->classes.size(); ci++) {
-            const ScanClass &cl = b->classes[ci];
+        for (size_t ci = 0; ci < b.classes.size(); ci++) {
+            const ScanClass &cl = b.classes[ci];
             if (!cl.p.progressive) continue;
             std::vector<uint32_t> ids;
             for (auto &cs : cl.scans) ids.push_back(cs.frame);
@@ -722,24 +715,24 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
             const std::vector<uint32_t> &ids = kv.first;
             std::vector<int> cls = kv.second;  // ascending ordinal (the classes are sorted)
             bool ok = !ids.empty();
-            for (uint32_t id : ids) ok = ok && b->frames[id].scans.size() == cls.size();
+            for (uint32_t id : ids) ok = ok && b.frames[id].scans.size() == cls.size();
             PfGroupHost grp;
-            const b200jpg_frame_info &fi0 = b->frames[ids[0]].info;
+            const b200jpg_frame_info &fi0 = b.frames[ids[0]].info;
             for (int ci : cls) {
-                const ScanClassParams &p = b->classes[(size_t)ci].p;
+                const ScanClassParams &p = b.classes[(size_t)ci].p;
                 if (!ok) break;
                 if (p.ss == 0) {
                     ok = p.ns == (int)fi0.ncomp && (grp.dc.empty() ? p.ah == 0 : p.ah != 0);
                     if (ok && !grp.dc.empty()) {
-                        const ScanClassParams &q = b->classes[(size_t)grp.dc[0]].p;
+                        const ScanClassParams &q = b.classes[(size_t)grp.dc[0]].p;
                         ok = q.dri == p.dri && q.intervals_per_scan == p.intervals_per_scan && q.total_mcus == p.total_mcus;
                     }
                     grp.dc.push_back(ci);
                 } else {
-                    const int c = b->classes[(size_t)ci].frame_comp0;
+                    const int c = b.classes[(size_t)ci].frame_comp0;
                     ok = p.ns == 1 && c < 4;
                     if (ok && !grp.ac[c].empty()) {
-                        const ScanClassParams &q = b->classes[(size_t)grp.ac[c][0]].p;
+                        const ScanClassParams &q = b.classes[(size_t)grp.ac[c][0]].p;
                         ok = q.dri == p.dri && q.intervals_per_scan == p.intervals_per_scan && q.total_mcus == p.total_mcus && q.mcu_cols == p.mcu_cols;
                     }
                     if (ok) grp.ac[c].push_back(ci);
@@ -748,106 +741,108 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
             ok = ok && !grp.dc.empty() && grp.dc.size() <= (size_t)kPfMaxScans;
             for (int c = 0; c < 4; c++) ok = ok && grp.ac[c].size() <= (size_t)kPfMaxScans;
             if (!ok) continue;
-            for (int ci : cls) b->classes[(size_t)ci].fused = true;
+            for (int ci : cls) b.classes[(size_t)ci].fused = true;
             for (uint32_t id : ids) frame_fused[id] = 1;
-            const ParsedFrame &pf0 = b->frames[ids[0]];
+            const ParsedFrame &pf0 = b.frames[ids[0]];
             for (int c = 0; c < 4; c++)
-                b->pf_dc_quant.push_back(c < fi0.ncomp && pf0.scans[0].quant_defined[fi0.tq[c]] ? pf0.scans[0].quant[fi0.tq[c]][0] : 0);
-            b->pf_groups.push_back(std::move(grp));
+                b.pf_dc_quant.push_back(c < fi0.ncomp && pf0.scans[0].quant_defined[fi0.tq[c]] ? pf0.scans[0].quant[fi0.tq[c]][0] : 0);
+            b.pf_groups.push_back(std::move(grp));
         }
     }
-    for (int i = 0; i < n; i++) {
-        if (b->parse_status[i] != 0 || b->frames[i].info.frame_type != 2 || frame_fused[i]) continue;
-        const ParsedFrame &pf = b->frames[i];
+    for (int i = 0; i < b.n; i++) {
+        if (b.parse_status[i] != 0 || b.frames[i].info.frame_type != 2 || frame_fused[i]) continue;
+        const ParsedFrame &pf = b.frames[i];
         ProgFrame f{};
         f.frame = (uint32_t)i;
         for (int c = 0; c < pf.info.ncomp; c++) {
-            f.coef_base[c] = coef_base[i][c];
+            f.coef_base[c] = b.coef_base[i][c];
             f.n_blocks[c] = pf.info.blocks_w[c] * pf.info.blocks_h[c];
-            b->prog_max_blocks = std::max(b->prog_max_blocks, f.n_blocks[c]);
+            b.prog_max_blocks = std::max(b.prog_max_blocks, f.n_blocks[c]);
             const ScanInfo &last = pf.scans.back();  // quantisers in effect at the end of the frame
             for (int k = 0; k < 64; k++) f.q_raster[c][kZigZagToRaster[k]] = last.quant_defined[pf.info.tq[c]] ? last.quant[pf.info.tq[c]][k] : 0;
         }
-        b->prog_frames.push_back(f);
+        b.prog_frames.push_back(f);
     }
+}
 
-    // unstuffed-buffer layout. Host-indexed scans: every interval gets its source length rounded up to 16 bytes + 48 bytes
-    // of zero tail. Device-indexed scans: one region of ECS length + kCleanSlackPerInterval per interval, inside which the
-    // index kernel places interval k at (its source offset) + kCleanSlackPerInterval * k -- no lengths are known here.
-    {
-        uint64_t ccur = 0, ibase = 0;
-        for (size_t ci = 0; ci < b->classes.size(); ci++) {
-            auto &cl = b->classes[ci];
-            cl.p.n_scans = (uint32_t)cl.scans.size();
-            cl.interval_base = ibase;
-            cl.clean_off.resize(cl.interval_off.size());
-            const size_t nint = cl.p.intervals_per_scan;
-            for (size_t j = 0; j < cl.scans.size(); j++) {
-                if (cl.scan_on_device[j]) {
-                    IndexScan is{};
-                    is.ecs_off = cl.scan_ecs_off[j];
-                    is.ecs_end = cl.scan_ecs_end[j];
-                    is.off_arr = (uint64_t)ci;  // class index for now: becomes the array offset once the layout is known
-                    is.end_arr = (uint64_t)(j * nint);
-                    is.clean_base = ccur;
-                    is.n_intervals = (uint32_t)nint;
-                    is.frame = cl.scans[j].frame;
-                    b->index_scans.push_back(is);
-                    for (size_t k = 0; k < nint; k++) cl.clean_off[j * nint + k] = ccur;
-                    ccur += align_up((is.ecs_end - is.ecs_off) + (uint64_t)kCleanSlackPerInterval * nint + 64, 16);
-                } else {
-                    for (size_t k = j * nint; k < (j + 1) * nint; k++) {
-                        cl.clean_off[k] = ccur;
-                        uint64_t len = cl.interval_off[k] == ~0ull ? 0 : (cl.interval_end[k] & ~kIntervalEofFlag) - cl.interval_off[k];
-                        ccur += align_up(len, 16) + 48;
-                    }
+// Unstuffed-buffer layout. Host-indexed scans: every interval gets its source length rounded up to 16 bytes + 48 bytes of zero
+// tail. Device-indexed scans: one region of ECS length + kCleanSlackPerInterval per interval, inside which the index kernel places
+// interval k at (its source offset) + kCleanSlackPerInterval * k -- no lengths are known here.
+static void lay_out_unstuffed(b200jpg_batch &b) {
+    uint64_t ccur = 0, ibase = 0;
+    for (size_t ci = 0; ci < b.classes.size(); ci++) {
+        auto &cl = b.classes[ci];
+        cl.p.n_scans = (uint32_t)cl.scans.size();
+        cl.interval_base = ibase;
+        cl.clean_off.resize(cl.interval_off.size());
+        const size_t nint = cl.p.intervals_per_scan;
+        for (size_t j = 0; j < cl.scans.size(); j++) {
+            if (cl.scan_on_device[j]) {
+                IndexScan is{};
+                is.ecs_off = cl.scan_ecs_off[j];
+                is.ecs_end = cl.scan_ecs_end[j];
+                is.off_arr = (uint64_t)ci;  // class index for now: becomes the array offset once the layout is known
+                is.end_arr = (uint64_t)(j * nint);
+                is.clean_base = ccur;
+                is.n_intervals = (uint32_t)nint;
+                is.frame = cl.scans[j].frame;
+                b.index_scans.push_back(is);
+                for (size_t k = 0; k < nint; k++) cl.clean_off[j * nint + k] = ccur;
+                ccur += align_up((is.ecs_end - is.ecs_off) + (uint64_t)kCleanSlackPerInterval * nint + 64, 16);
+            } else {
+                for (size_t k = j * nint; k < (j + 1) * nint; k++) {
+                    cl.clean_off[k] = ccur;
+                    uint64_t len = cl.interval_off[k] == ~0ull ? 0 : (cl.interval_end[k] & ~kIntervalEofFlag) - cl.interval_off[k];
+                    ccur += align_up(len, 16) + 48;
                 }
             }
-            ibase += cl.interval_off.size();
-            if (cl.p.indexed) {
-                cl.spec_base = b->n_spec;
-                b->n_spec += (uint64_t)cl.scans.size() * cl.p.segs_per_scan;
-            }
         }
-        b->clean_bytes = ccur + 512;  // slack: the ring prefetch runs up to 64 bytes ahead of the reader
-        b->n_intervals = ibase;
+        ibase += cl.interval_off.size();
+        if (cl.p.indexed) {
+            cl.spec_base = b.n_spec;
+            b.n_spec += (uint64_t)cl.scans.size() * cl.p.segs_per_scan;
+        }
     }
+    b.clean_bytes = ccur + 512;  // slack: the ring prefetch runs up to 64 bytes ahead of the reader
+    b.n_intervals = ibase;
+}
 
-    // ---- reconstruction groups
-    for (int i = 0; i < n; i++) {
-        if (b->parse_status[i] != 0) continue;
-        const b200jpg_frame_info &fi = b->frames[i].info;
-        const int xt_res = (i < n_user) ? b->xt_child[i] : -1;  // JPEG XT: this frame's residual frame
-        const bool generic = frame_is_generic(fi, flags) || xt_res >= 0 || b->xt_parent[i] >= 0;
+// Reconstruction groups: frames of one component count, chroma factors and reconstruction path share the launches
+static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uint64_t, 4>> &sample_base) {
+    for (int i = 0; i < b.n; i++) {
+        if (b.parse_status[i] != 0) continue;
+        const b200jpg_frame_info &fi = b.frames[i].info;
+        const int xt_res = (i < b.n_user) ? b.xt_child[i] : -1;  // JPEG XT: this frame's residual frame
+        const ReconPath path = recon_path(b, i);
         uint32_t sx = fi.ncomp > 1 ? fi.subx[1] : 1, sy = fi.ncomp > 1 ? fi.suby[1] : 1;
-        if (generic) sx = sy = 0;  // one group per component count: the generic kernels read the factors per frame
+        if (path == ReconPath::Generic) sx = sy = 0;  // one group per component count: the generic kernels read the factors per frame
         ReconGroup *g = nullptr;
-        for (auto &gg : b->groups)
-            if (gg.ncomp == fi.ncomp && gg.subx == sx && gg.suby == sy && gg.generic == generic) g = &gg;
+        for (auto &gg : b.groups)
+            if (gg.ncomp == fi.ncomp && gg.subx == sx && gg.suby == sy && gg.path == path) g = &gg;
         if (!g) {
-            b->groups.emplace_back();
-            g = &b->groups.back();
+            b.groups.emplace_back();
+            g = &b.groups.back();
             g->ncomp = fi.ncomp;
             g->subx = sx;
             g->suby = sy;
-            g->generic = generic;
+            g->path = path;
         }
         FrameRecon fr{};
         for (int c = 0; c < fi.ncomp; c++) {
-            fr.coef_base[c] = coef_base[i][c];
+            fr.coef_base[c] = b.coef_base[i][c];
             fr.sample_base[c] = sample_base[i][c];
             fr.bw[c] = fi.blocks_w[c];
             fr.bh[c] = fi.blocks_h[c];
             fr.csx[c] = fi.subx[c];
             fr.csy[c] = fi.suby[c];
         }
-        fr.out_base = b->out_off[i];
+        fr.out_base = b.out_off[i];
         fr.width = fi.width;
         fr.height = fi.height;
-        if (b->xt_parent[i] >= 0) fr.width = fr.height = 0;  // a residual codestream: planes only, its frame's reconstruction reads them
+        if (b.xt_parent[i] >= 0) fr.width = fr.height = 0;  // a residual codestream: planes only, its frame's reconstruction reads them
         if (xt_res >= 0) {
-            const b200jpg_frame_info &ri = b->frames[xt_res].info;
-            fr.xt = 1u | (b->frames[i].xt.l_ycbcr ? 2u : 0u) | (b->frames[i].xt.r_ycbcr ? 4u : 0u);
+            const b200jpg_frame_info &ri = b.frames[xt_res].info;
+            fr.xt = 1u | (b.frames[i].xt.l_ycbcr ? 2u : 0u) | (b.frames[i].xt.r_ycbcr ? 4u : 0u);
             for (int c = 0; c < ri.ncomp; c++) {
                 fr.res_sample_base[c] = sample_base[xt_res][c];
                 fr.res_bw[c] = ri.blocks_w[c];
@@ -856,7 +851,7 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
             }
         }
         fr.ncomp = fi.ncomp;
-        fr.ycbcr = (flags & B200JPG_FLAG_NO_COLOR_TRANSFORM) ? 0 : fi.ycbcr;  // JPGTAG_MATRIX_LTRAFO = ..._NONE (rectanglerequest.cpp:150-152)
+        fr.ycbcr = (b.flags & B200JPG_FLAG_NO_COLOR_TRANSFORM) ? 0 : fi.ycbcr;  // JPGTAG_MATRIX_LTRAFO = ..._NONE (rectanglerequest.cpp:150-152)
         fr.subx = sx;
         fr.suby = sy;
         fr.cw = sx ? (fi.width + sx - 1) / sx : fi.width;  // (generic groups carry the factors per component: csx / csy)
@@ -866,7 +861,7 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
         g->frames.push_back(fr);
         g->max_bw0 = std::max(g->max_bw0, (fi.width + 7) / 8);
         g->max_bh0 = std::max(g->max_bh0, (fi.height + 7) / 8);
-        if (generic) {  // the largest block grid of any component: the extent of the generic IDCT launch
+        if (path == ReconPath::Generic) {  // the largest block grid of any component: the extent of the generic IDCT launch
             for (int c = 0; c < fi.ncomp; c++)
                 if ((uint64_t)fi.blocks_w[c] * fi.blocks_h[c] > (uint64_t)g->max_bwc * g->max_bhc) g->max_bwc = fi.blocks_w[c], g->max_bhc = fi.blocks_h[c];
         } else if (fi.ncomp > 1) {
@@ -874,15 +869,17 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
             g->max_bhc = std::max(g->max_bhc, fi.blocks_h[1]);
         }
     }
+}
 
-    // ---- descriptor region
-    cur = b->bytes_region;
-    b->dev_tables.resize(b->table_sets.size());
-    for (size_t t = 0; t < b->table_sets.size(); t++) {
-        b->dev_tables[t] = cur;
-        cur = align_up(cur + b->table_sets[t].blob.size(), 256);
+// descriptor region of the input buffer, behind the codestreams
+static void lay_out_descriptors(b200jpg_batch &b) {
+    uint64_t cur = b.bytes_region;
+    b.dev_tables.resize(b.table_sets.size());
+    for (size_t t = 0; t < b.table_sets.size(); t++) {
+        b.dev_tables[t] = cur;
+        cur = align_up(cur + b.table_sets[t].blob.size(), 256);
     }
-    for (auto &cl : b->classes) {
+    for (auto &cl : b.classes) {
         cl.dev_scans = cur;
         cur = align_up(cur + cl.scans.size() * sizeof(ClassScan), 256);
         cl.dev_intervals = cur;
@@ -892,94 +889,136 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
         cl.dev_clean_off = cur;
         cur = align_up(cur + cl.clean_off.size() * sizeof(uint64_t), 256);
     }
-    for (auto &g : b->groups) {
+    for (auto &g : b.groups) {
         g.dev_frames = cur;
         cur = align_up(cur + g.frames.size() * sizeof(FrameRecon), 256);
     }
-    b->dev_prog_frames = cur;
-    cur = align_up(cur + b->prog_frames.size() * sizeof(ProgFrame), 256);
-    b->dev_index_scans = cur;
-    cur = align_up(cur + b->index_scans.size() * sizeof(IndexScan), 256);
-    for (auto &is : b->index_scans) {  // class index + first interval -> offsets of the scan's slices
-        const ScanClass &cl = b->classes[(size_t)is.off_arr];
+    b.dev_prog_frames = cur;
+    cur = align_up(cur + b.prog_frames.size() * sizeof(ProgFrame), 256);
+    b.dev_index_scans = cur;
+    cur = align_up(cur + b.index_scans.size() * sizeof(IndexScan), 256);
+    for (auto &is : b.index_scans) {  // class index + first interval -> offsets of the scan's slices
+        const ScanClass &cl = b.classes[(size_t)is.off_arr];
         const uint64_t first = is.end_arr * sizeof(uint64_t);
         is.off_arr = cl.dev_intervals + first;
         is.end_arr = cl.dev_interval_end + first;
         is.clean_arr = cl.dev_clean_off + first;
     }
-    b->input_bytes = cur;
+    b.input_bytes = cur;
+}
 
-    // ---- pinned staging + device memory
-    b->h_input = (uint8_t *)ctx->get(0, b->input_bytes, &ce);
+// pinned staging of the input buffer + device memory; returns 0 or the status the batch fails with
+static int stage_and_allocate(b200jpg_batch &b, const Codestreams &cs, const std::vector<uint64_t> &byte_off) {
+    b200jpg_ctx *ctx = b.ctx;
+    cudaError_t ce;
+    b.h_input = (uint8_t *)ctx->get(0, b.input_bytes, &ce);
     if (ce != cudaSuccess) return ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, std::string("pinned staging allocation failed: ") + cudaGetErrorString(ce));
-    {
-        unsigned nt = std::min<unsigned>(std::max(1u, std::thread::hardware_concurrency()), 8u);
-        nt = std::min<unsigned>(nt, (unsigned)n);
-        std::vector<std::thread> pool;
-        for (unsigned t = 0; t < nt; t++)
-            pool.emplace_back([&, t]() {
-                for (int i = (int)t; i < n; i += (int)nt) {
-                    if (b->parse_status[i] != 0) continue;
-                    uint8_t *dst = b->h_input + byte_off[i];
-                    memcpy(dst, fp[i], fl[i]);
-                    // sentinel: a damaged segment must still meet a marker before it leaves its codestream
-                    uint64_t pad_end = align_up(byte_off[i] + fl[i] + 32, 16);
-                    memset(dst + fl[i], 0, pad_end - (byte_off[i] + fl[i]));
-                    dst[fl[i]] = 0xff;
-                    dst[fl[i] + 1] = 0xd9;
-                }
-            });
-        for (auto &th : pool) th.join();
-    }
+    for_frames(b.n, 8, [&](int i) {
+        if (b.parse_status[i] != 0) return;
+        uint8_t *dst = b.h_input + byte_off[i];
+        memcpy(dst, cs.data[i], cs.len[i]);
+        // sentinel: a damaged segment must still meet a marker before it leaves its codestream
+        uint64_t pad_end = align_up(byte_off[i] + cs.len[i] + 32, 16);
+        memset(dst + cs.len[i], 0, pad_end - (byte_off[i] + cs.len[i]));
+        dst[cs.len[i]] = 0xff;
+        dst[cs.len[i] + 1] = 0xd9;
+    });
     // tail of the codestream region (after the last frame) is zero + a final sentinel
     {
         uint64_t last_end = 0;
-        for (int i = 0; i < n; i++)
-            if (b->parse_status[i] == 0) last_end = align_up(byte_off[i] + fl[i] + 32, 16);
-        memset(b->h_input + last_end, 0, b->bytes_region - last_end);
-        b->h_input[last_end] = 0xff;
-        b->h_input[last_end + 1] = 0xd9;
+        for (int i = 0; i < b.n; i++)
+            if (b.parse_status[i] == 0) last_end = align_up(byte_off[i] + cs.len[i] + 32, 16);
+        memset(b.h_input + last_end, 0, b.bytes_region - last_end);
+        b.h_input[last_end] = 0xff;
+        b.h_input[last_end + 1] = 0xd9;
     }
-    for (size_t t = 0; t < b->table_sets.size(); t++)
-        memcpy(b->h_input + b->dev_tables[t], b->table_sets[t].blob.data(), b->table_sets[t].blob.size());
-    for (auto &cl : b->classes) {
-        memcpy(b->h_input + cl.dev_scans, cl.scans.data(), cl.scans.size() * sizeof(ClassScan));
-        memcpy(b->h_input + cl.dev_intervals, cl.interval_off.data(), cl.interval_off.size() * sizeof(uint64_t));
-        memcpy(b->h_input + cl.dev_interval_end, cl.interval_end.data(), cl.interval_end.size() * sizeof(uint64_t));
-        memcpy(b->h_input + cl.dev_clean_off, cl.clean_off.data(), cl.clean_off.size() * sizeof(uint64_t));
+    for (size_t t = 0; t < b.table_sets.size(); t++)
+        memcpy(b.h_input + b.dev_tables[t], b.table_sets[t].blob.data(), b.table_sets[t].blob.size());
+    for (auto &cl : b.classes) {
+        memcpy(b.h_input + cl.dev_scans, cl.scans.data(), cl.scans.size() * sizeof(ClassScan));
+        memcpy(b.h_input + cl.dev_intervals, cl.interval_off.data(), cl.interval_off.size() * sizeof(uint64_t));
+        memcpy(b.h_input + cl.dev_interval_end, cl.interval_end.data(), cl.interval_end.size() * sizeof(uint64_t));
+        memcpy(b.h_input + cl.dev_clean_off, cl.clean_off.data(), cl.clean_off.size() * sizeof(uint64_t));
     }
-    for (auto &g : b->groups) memcpy(b->h_input + g.dev_frames, g.frames.data(), g.frames.size() * sizeof(FrameRecon));
-    if (!b->index_scans.empty()) memcpy(b->h_input + b->dev_index_scans, b->index_scans.data(), b->index_scans.size() * sizeof(IndexScan));
-    if (!b->prog_frames.empty()) memcpy(b->h_input + b->dev_prog_frames, b->prog_frames.data(), b->prog_frames.size() * sizeof(ProgFrame));
+    for (auto &g : b.groups) memcpy(b.h_input + g.dev_frames, g.frames.data(), g.frames.size() * sizeof(FrameRecon));
+    if (!b.index_scans.empty()) memcpy(b.h_input + b.dev_index_scans, b.index_scans.data(), b.index_scans.size() * sizeof(IndexScan));
+    if (!b.prog_frames.empty()) memcpy(b.h_input + b.dev_prog_frames, b.prog_frames.data(), b.prog_frames.size() * sizeof(ProgFrame));
 
-    b->sz_ilen = sizeof(uint32_t) * (size_t)std::max<uint64_t>(b->n_intervals, 1);
-    b->sz_status = sizeof(uint32_t) * (5 * (size_t)n + 1);  // status words, wide flags, narrow flags, narrow list, index status
-    b->d_input = (uint8_t *)ctx->get(1, b->input_bytes, &ce);
-    if (ce == cudaSuccess && b->coef_elems) b->d_coef = (int16_t *)ctx->get(1, b->coef_elems * sizeof(int16_t), &ce);
-    // sample planes only for the reconstruction groups that go through them (4:2:0 frames go from coefficients to pixels in one
-    // kernel, their chroma samples live in shared memory)
-    {
-        bool need_planes = false;
-        for (auto &g : b->groups) need_planes = need_planes || g.generic || (g.ncomp > 1 && !(g.ncomp == 3 && g.subx == 2 && g.suby == 2));
-        if (!need_planes) b->sample_elems = 0;
+    b.sz_ilen = sizeof(uint32_t) * (size_t)std::max<uint64_t>(b.n_intervals, 1);
+    b.sz_status = sizeof(uint32_t) * (5 * (size_t)b.n + 1);  // status words, wide flags, narrow flags, narrow list, index status
+    b.d_input = (uint8_t *)ctx->get(1, b.input_bytes, &ce);
+    if (ce == cudaSuccess && b.coef_elems) b.d_coef = (int16_t *)ctx->get(1, b.coef_elems * sizeof(int16_t), &ce);
+    if (ce == cudaSuccess && b.sample_elems) b.d_samples = (int32_t *)ctx->get(1, b.sample_elems * sizeof(int32_t), &ce);
+    if (ce == cudaSuccess && b.sample_elems) b.d_samples16 = (int16_t *)ctx->get(1, b.sample_elems * sizeof(int16_t), &ce);
+    if (ce == cudaSuccess) b.d_clean = (uint8_t *)ctx->get(1, b.clean_bytes, &ce);
+    if (ce == cudaSuccess) b.d_interval_len = (uint32_t *)ctx->get(1, b.sz_ilen, &ce);
+    b.sz_overrun = sizeof(uint32_t) * (size_t)(b.n_intervals + b.classes.size() + 1);
+    if (ce == cudaSuccess) b.d_overrun = (uint32_t *)ctx->get(1, b.sz_overrun, &ce);
+    if (ce == cudaSuccess) b.d_status = (uint32_t *)ctx->get(1, b.sz_status, &ce);
+    if (ce == cudaSuccess && !b.pf_groups.empty()) b.d_dcplane = (int16_t *)ctx->get(1, b.coef_elems / 64 * sizeof(int16_t), &ce);
+    if (ce == cudaSuccess && b.n_spec) {
+        b.sz_spec = (size_t)align_up(b.n_spec, 4) * (sizeof(SpecSegment) + 8 + 8 + 4 + 16 + sizeof(SpecLog)) + 256;
+        b.d_spec = (uint8_t *)ctx->get(1, b.sz_spec, &ce);
     }
-    if (ce == cudaSuccess && b->sample_elems) b->d_samples = (int32_t *)ctx->get(1, b->sample_elems * sizeof(int32_t), &ce);
-    if (ce == cudaSuccess && b->sample_elems) b->d_samples16 = (int16_t *)ctx->get(1, b->sample_elems * sizeof(int16_t), &ce);
-    if (ce == cudaSuccess) b->d_clean = (uint8_t *)ctx->get(1, b->clean_bytes, &ce);
-    if (ce == cudaSuccess) b->d_interval_len = (uint32_t *)ctx->get(1, b->sz_ilen, &ce);
-    b->sz_overrun = sizeof(uint32_t) * (size_t)(b->n_intervals + b->classes.size() + 1);
-    if (ce == cudaSuccess) b->d_overrun = (uint32_t *)ctx->get(1, b->sz_overrun, &ce);
-    if (ce == cudaSuccess) b->d_status = (uint32_t *)ctx->get(1, b->sz_status, &ce);
-    if (ce == cudaSuccess && !b->pf_groups.empty()) b->d_dcplane = (int16_t *)ctx->get(1, b->coef_elems / 64 * sizeof(int16_t), &ce);
-    if (ce == cudaSuccess && b->n_spec) {
-        b->sz_spec = (size_t)align_up(b->n_spec, 4) * (sizeof(SpecSegment) + 8 + 8 + 4 + 16 + sizeof(SpecLog)) + 256;
-        b->d_spec = (uint8_t *)ctx->get(1, b->sz_spec, &ce);
-    }
-    if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&b->ev_last, cudaEventDisableTiming);
+    if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&b.ev_last, cudaEventDisableTiming);
     if (ce != cudaSuccess) return ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, std::string("device allocation failed: ") + cudaGetErrorString(ce));
-    b->h_status.assign(n, 0);
+    b.h_status.assign(b.n, 0);
+    return B200JPG_OK;
+}
+
+static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
+                             b200jpg_batch **out) {
+    NvtxRange nvtx("b200jpg batch_create: parse + pack");
+    if (!out || !frames || !lens || n <= 0) return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "invalid batch arguments");
+    *out = nullptr;
+    cudaError_t ce = cudaSetDevice(ctx->device);
+    if (ce != cudaSuccess) return ctx->fail_cuda(ce, "cudaSetDevice");
+
+    std::unique_ptr<b200jpg_batch, void (*)(b200jpg_batch *)> bp(new b200jpg_batch(), b200jpg_batch_destroy);  // a failed plan frees what it holds
+    b200jpg_batch &b = *bp;
+    b.ctx = ctx;
+    b.n = b.n_user = n;
+    b.flags = flags;
+    Codestreams cs;
+    cs.data.assign(frames, frames + n);
+    cs.len.assign(lens, lens + n);
+    cs.err.resize(n);
+    // Interleaved scans with restart markers get their restart index on the device (8f1); B200JPG_HOST_INDEX=1 keeps the memchr
+    // pass over every entropy coded byte on the host for all of them.
+    const bool device_index = getenv("B200JPG_HOST_INDEX") == nullptr;
+    parse_frames(b, cs, device_index);
+    attach_residuals(b, cs, device_index);
+    std::vector<std::vector<TableSet>> frame_tables;
+    if (int rc = admit_frames(b, cs, tolerate_bad != 0, frame_tables)) return rc;
+    const std::vector<uint64_t> byte_off = lay_out_codestreams(b, cs.len);
+    const std::vector<std::array<uint64_t, 4>> sample_base = lay_out_planes(b);
+    form_scan_classes(b, frame_tables, byte_off);
+    form_progressive_groups(b);
+    lay_out_unstuffed(b);
+    form_recon_groups(b, sample_base);
+    lay_out_descriptors(b);
+    if (int rc = stage_and_allocate(b, cs, byte_off)) return rc;
     *out = bp.release();
     return B200JPG_OK;
+}
+
+int b200jpg_batch_create(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
+                         b200jpg_batch **out) {
+    return b200jpg_batch_create_ex(ctx, frames, lens, n, tolerate_bad, 0u, out);
+}
+
+int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
+                            b200jpg_batch **out) {
+    if (!ctx) return B200JPG_ERR_INVALID_PARAMETER;
+    try {  // no exception crosses the C ABI
+        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, out);
+    } catch (const std::bad_alloc &) {
+        if (out) *out = nullptr;
+        return ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "out of host memory while preparing the batch");
+    } catch (...) {
+        if (out) *out = nullptr;
+        return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "unexpected failure while preparing the batch");
+    }
 }
 
 int b200jpg_batch_frame_info(const b200jpg_batch *b, int i, b200jpg_frame_info *info) {
@@ -1214,7 +1253,7 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.ncomp = g.ncomp;
         l.subx = g.subx;
         l.suby = g.suby;
-        l.generic = g.generic;
+        l.path = g.path;
         l.planes_out = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
         l.coef = b->d_coef;
         l.samples16 = b->d_samples16;
@@ -1231,8 +1270,8 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         int launches = 0;
         // grid.y carries the frame index: at most 65535 frames per launch. A generic group that is cut runs the IDCT of ALL its
         // frames first: a JPEG XT frame reads the planes of its residual frame, which may sit in another part
-        const bool cut = l.n_frames > 65535u;
-        for (int phase = (l.generic && cut) ? 1 : 0; phase <= ((l.generic && cut) ? 2 : 0); phase++) {
+        const bool cut = l.path == ReconPath::Generic && l.n_frames > 65535u;
+        for (int phase = cut ? 1 : 0; phase <= (cut ? 2 : 0); phase++) {
             for (uint32_t first = 0; first < l.n_frames; first += 65535u) {
                 ReconLaunch part = l;
                 part.frames = l.frames + first;
@@ -1301,7 +1340,6 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
             if (!std::isfinite(convert->scale[c]) || !std::isfinite(convert->bias[c]))
                 return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "component " + std::to_string(c) + ": scale and bias must be finite");
     }
-    const bool own_size = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
     std::vector<char> planar((size_t)b->n, 1);
     for (int i = 0; i < b->n_user; i++) {
         if (b->parse_status[i] != 0) continue;
@@ -1309,8 +1347,7 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
         const uint64_t size = convert ? element : (fi.precision > 8 ? 2 : 1);
         for (int c = 0; c < fi.ncomp; c++) {
             const b200jpg_plane &p = planes[4 * i + c];
-            const uint64_t w = own_size ? (fi.width + fi.subx[c] - 1) / fi.subx[c] : fi.width;
-            const uint64_t h = own_size ? (fi.height + fi.suby[c] - 1) / fi.suby[c] : fi.height;
+            const auto [w, h] = out_extent(fi, c, b->flags);
             const uint64_t bpp = magnitude(p.bytes_per_pixel), bpr = magnitude(p.bytes_per_row);
             const std::string at = "frame " + std::to_string(i) + " component " + std::to_string(c) + ": ";
             if (!p.data) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "no destination");
@@ -1398,19 +1435,8 @@ int b200jpg_batch_read_coefficients(b200jpg_batch *b, int i, int c, int16_t *dst
     if (c < 0 || c >= fi.ncomp) return B200JPG_ERR_INVALID_PARAMETER;
     uint64_t elems = (uint64_t)fi.blocks_w[c] * fi.blocks_h[c] * 64;
     if (capacity < elems) return B200JPG_ERR_INVALID_PARAMETER;
-    // recompute the plane base exactly as batch_create did
-    uint64_t base = 0;
-    for (int k = 0; k < b->n; k++) {
-        if (b->parse_status[k] != 0) continue;
-        const b200jpg_frame_info &fk = b->frames[k].info;
-        for (int cc = 0; cc < fk.ncomp; cc++) {
-            if (k == i && cc == c) goto found;
-            base += (uint64_t)fk.blocks_w[cc] * fk.blocks_h[cc] * 64;
-        }
-    }
-found:
     cudaSetDevice(b->ctx->device);
-    cudaError_t e = cudaMemcpy(dst, b->d_coef + base, elems * sizeof(int16_t), cudaMemcpyDeviceToHost);
+    cudaError_t e = cudaMemcpy(dst, b->d_coef + b->coef_base[i][c], elems * sizeof(int16_t), cudaMemcpyDeviceToHost);
     if (e != cudaSuccess) return b->ctx->fail_cuda(e, "coefficient download");
     return B200JPG_OK;
 }
@@ -1594,88 +1620,54 @@ int b200jpg_decode_to_host(b200jpg_ctx *ctx, const uint8_t *const *frames, const
     return b200jpg_decode_to_host_ex(ctx, frames, lens, n, out_host, out_capacity, 0u);
 }
 
-int b200jpg_decode_to_host_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, uint8_t *out_host,
-                              uint64_t out_capacity, unsigned flags) {
-    if (!ctx) return B200JPG_ERR_INVALID_PARAMETER;
+// One-shot decode of n frames into a fresh device buffer: handed to the caller through out_dev / out_bytes, or without out_dev
+// copied to out_host (its capacity checked first) and freed.
+static int decode_once(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, unsigned flags, uint8_t *out_host,
+                       uint64_t out_capacity, uint8_t **out_dev, uint64_t *out_bytes) {
+    const bool to_host = out_dev == nullptr;
     b200jpg_batch *b = nullptr;
     int rc = b200jpg_batch_create_ex(ctx, frames, lens, n, 0, flags, &b);
     if (rc) return rc;
     uint8_t *d_out = nullptr;
     cudaStream_t s = nullptr;
     cudaError_t e = cudaSuccess;
-    if (out_capacity < b->out_total) {
-        rc = ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "output buffer too small");
-        goto done;
-    }
-    e = cudaMalloc((void **)&d_out, b->out_total);
-    if (e != cudaSuccess) {
+    if (to_host && out_capacity < b->out_total) rc = ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "output buffer too small");
+    if (!rc && cudaMalloc((void **)&d_out, b->out_total ? b->out_total : 1) != cudaSuccess)
         rc = ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "device allocation of the output failed");
-        goto done;
-    }
-    e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
-    if (e != cudaSuccess) {
-        rc = ctx->fail_cuda(e, "cudaStreamCreate");
-        goto done;
-    }
-    rc = b200jpg_batch_upload(b, s);
+    if (!rc && (e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)) != cudaSuccess) rc = ctx->fail_cuda(e, "cudaStreamCreate");
+    if (!rc) rc = b200jpg_batch_upload(b, s);
     if (!rc) rc = b200jpg_batch_decode(b, d_out, s);
     if (!rc) {
-        e = cudaMemcpyAsync(out_host, d_out, b->out_total, cudaMemcpyDeviceToHost, s);
+        if (to_host) e = cudaMemcpyAsync(out_host, d_out, b->out_total, cudaMemcpyDeviceToHost, s);
         if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) rc = ctx->fail_cuda(e, "download");
+        if (e != cudaSuccess) rc = ctx->fail_cuda(e, to_host ? "download" : "decode");
     }
-    if (!rc) {
-        for (int i = 0; i < n && !rc; i++) {
-            int st = b200jpg_batch_frame_status(b, i);
-            if (st) rc = ctx->fail(st, "frame " + std::to_string(i) + ": invalid stream, found invalid huffman code in entropy coded segment");
-        }
+    for (int i = 0; i < n && !rc; i++) {
+        int st = b200jpg_batch_frame_status(b, i);
+        if (st) rc = ctx->fail(st, "frame " + std::to_string(i) + ": invalid stream, found invalid huffman code in entropy coded segment");
     }
-done:
+    if (!rc && !to_host) {
+        if (out_bytes) *out_bytes = b->out_total;
+        *out_dev = d_out;
+        d_out = nullptr;
+    }
     if (s) cudaStreamDestroy(s);
     if (d_out) cudaFree(d_out);
     b200jpg_batch_destroy(b);
     return rc;
 }
 
+int b200jpg_decode_to_host_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, uint8_t *out_host,
+                              uint64_t out_capacity, unsigned flags) {
+    if (!ctx) return B200JPG_ERR_INVALID_PARAMETER;
+    return decode_once(ctx, frames, lens, n, flags, out_host, out_capacity, nullptr, nullptr);
+}
+
 int b200jpg_decode_to_device_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, unsigned flags, uint8_t **out_dev,
                                 uint64_t *out_bytes) {
     if (!ctx || !out_dev) return B200JPG_ERR_INVALID_PARAMETER;
     *out_dev = nullptr;
-    b200jpg_batch *b = nullptr;
-    int rc = b200jpg_batch_create_ex(ctx, frames, lens, n, 0, flags, &b);
-    if (rc) return rc;
-    uint8_t *d_out = nullptr;
-    cudaStream_t s = nullptr;
-    cudaError_t e = cudaMalloc((void **)&d_out, b->out_total ? b->out_total : 1);
-    if (e != cudaSuccess) {
-        rc = ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "device allocation of the output failed");
-        goto done;
-    }
-    e = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
-    if (e != cudaSuccess) {
-        rc = ctx->fail_cuda(e, "cudaStreamCreate");
-        goto done;
-    }
-    rc = b200jpg_batch_upload(b, s);
-    if (!rc) rc = b200jpg_batch_decode(b, d_out, s);
-    if (!rc) {
-        e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) rc = ctx->fail_cuda(e, "decode");
-    }
-    for (int i = 0; i < n && !rc; i++) {
-        int st = b200jpg_batch_frame_status(b, i);
-        if (st) rc = ctx->fail(st, "frame " + std::to_string(i) + ": invalid stream, found invalid huffman code in entropy coded segment");
-    }
-    if (!rc) {
-        if (out_bytes) *out_bytes = b->out_total;
-        *out_dev = d_out;
-        d_out = nullptr;
-    }
-done:
-    if (s) cudaStreamDestroy(s);
-    if (d_out) cudaFree(d_out);
-    b200jpg_batch_destroy(b);
-    return rc;
+    return decode_once(ctx, frames, lens, n, flags, nullptr, 0, out_dev, out_bytes);
 }
 
 void b200jpg_device_free(b200jpg_ctx *ctx, uint8_t *p) {

@@ -254,13 +254,16 @@ int launch_progressive_scan(const EntropyLaunch &l, void *stream);
 int launch_progressive_dequant(const ProgFrame *frames_dev, uint32_t n_frames, uint32_t max_blocks, int16_t *coef, uint32_t *frame_status,
                                void *stream);
 
+// How a frame goes from coefficients to pixels (abi.cpp: recon_path). Tiled: b1 planes of components 1.. + b2 (grey, 4:4:4,
+// 4:2:2, 4:4:0); Fused420: reconstruct420_kernel, no planes; Generic: int32 planes of every component + the generic kernels
+enum class ReconPath : int { Tiled, Fused420, Generic };
 struct ReconLaunch {
     const FrameRecon *frames;  // device
     uint32_t n_frames;
     uint32_t max_bw0, max_bh0;     // largest luma block grid in the group
     uint32_t max_bwc, max_bhc;     // largest chroma block grid in the group
     uint32_t ncomp, subx, suby;    // uniform over the group
-    bool generic;                  // formats outside the tuned kernels: any component count / factors, per-frame parameters
+    ReconPath path;                // uniform over the group
     bool planes_out;               // B200JPG_FLAG_NO_UPSAMPLE: the components leave as planes at their own resolution
     int generic_phase;             // generic groups: 0 = IDCT then reconstruction, 1 = IDCT only, 2 = reconstruction only
     const int16_t *coef;

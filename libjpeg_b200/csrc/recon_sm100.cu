@@ -1381,9 +1381,9 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
 
 template <int K>
 static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches) {
-    int n = 0;
-    if (l.generic) return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : (K >= kStorePlanarF ? kStoreStridedF : kStoreStrided)>(l, s, launches);
-    if (l.ncomp == 3 && l.subx == 2 && l.suby == 2) return launch_recon420<K>(l, s, launches);
+    if (l.path == ReconPath::Generic) return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : (K >= kStorePlanarF ? kStoreStridedF : kStoreStrided)>(l, s, launches);
+    if (l.path == ReconPath::Fused420) return launch_recon420<K>(l, s, launches);
+    int n = 0;  // ReconPath::Tiled
     const uint32_t cblocks = (l.max_bwc * l.max_bhc + kThreadsB - 1) / kThreadsB;
     const uint32_t gx = (l.max_bw0 + 31) / 32, gy = (l.max_bh0 + kThreadsB / 32 - 1) / (kThreadsB / 32);
     // every frame through the int16 planes, B200JPG_RECON_CHUNK frames at a time (0: all at once): in chunks the planes b1 writes

@@ -694,6 +694,37 @@ def test_xt_profiles_outside_the_path_are_refused(built, name):
     assert dec.status(1) == -1034 and dec.status(0) == 0
 
 
+def test_mixed_batch_with_a_failed_frame_keeps_every_frames_planes(built, oracle, golden_pixels):
+    """One tolerant batch of 4:2:0, 4:4:4, JPEG XT and 12-bit frames around a frame that does not parse: every live frame's
+    coefficients == the oracle's, its pixels == the fixtures. The failed frame takes no coefficient plane, the XT frame's
+    residual codestream takes planes behind all of the caller's frames, and the reconstruction paths mix."""
+    from libjpeg_b200 import NativeError
+    bad = b"\xff\xd8\xff\xdb\x00\x43not a codestream"
+    with pytest.raises(NativeError) as parse_error:
+        built.parse(bad)
+    xt_name, d12_name = "xt_420_96x80_z6_q75_Q90", D12NAMES[0]
+    wants = [golden_pixels["c420_96x80_z6_q75"], None, golden_pixels["c444_64x64_z16_q90"],
+             np.load(os.path.join(XT, "xt_pixels.npz"))[xt_name], np.load(os.path.join(DEEP12, "deep12_pixels.npz"))[d12_name],
+             golden_pixels["c420_130x70_z9_q98"]]
+    paths = [os.path.join(GOLDEN, "c420_96x80_z6_q75.jpg"), None, os.path.join(GOLDEN, "c444_64x64_z16_q90.jpg"),
+             os.path.join(XT, xt_name + ".jpg"), os.path.join(DEEP12, d12_name + ".jpg"), os.path.join(GOLDEN, "c420_130x70_z9_q98.jpg")]
+    datas = [open(p, "rb").read() if p else bad for p in paths]
+    dec, out = gpu_decode(built, datas, tolerate_bad=True)
+    assert dec.status(1) == parse_error.value.code
+    for i, (data, want) in enumerate(zip(datas, wants)):
+        if want is None:
+            continue
+        assert dec.status(i) == 0, i
+        got = dec.frame_view(out, i).cpu().numpy()
+        got = got.view(np.uint16) if dec.info(i).precision > 8 else got
+        assert np.array_equal(got.reshape(want.shape), want), i
+        rc, s, planes = oracle.coefficients(data)
+        assert rc == 0 and s.ncomp == dec.info(i).ncomp, i
+        for c in range(s.ncomp):
+            q = np.array(s.quant[s.tq[c]], dtype=np.int32).reshape(8, 8)
+            assert np.array_equal(dec.coefficients(i, c).astype(np.int32), planes[c] * q), (i, c)
+
+
 def test_reference_cli_decodes_xt_through_the_b200_library(built, tmp_path):
     import subprocess
     exe = os.path.join(ROOT, "oracle", "_ref", "jpeg_b200")
