@@ -111,6 +111,18 @@ B200JPG_API int b200jpg_batch_create(b200jpg_ctx *ctx, const uint8_t *const *fra
  * refuses one without the other); frame i is written as plane after plane, component c holding ceil(width / subx[c]) x
  * ceil(height / suby[c]) samples, rows tightly packed.  Samples are bytes, or native-endian 16-bit for 12-bit frames. */
 #define B200JPG_FLAG_NO_UPSAMPLE 2u
+/* B200JPG_FLAG_DOWNSCALE_k (a two-bit field, B200JPG_FLAG_DOWNSCALE_MASK; no counterpart in the reference): every frame comes
+ * out at W' = ceil(width / k) x H' = ceil(height / k). Each 8x8 block goes through a reduced inverse transform to
+ * (8/k) x (8/k) samples -- the k x k box average of its exact IDCT, in fixed point as DESIGN §10 specifies -- and the result is
+ * reconstructed like the IDCT output of a W' x H' frame with the same sampling factors: upsampling, colour transformation, clamp
+ * and sample types as without the flag, B200JPG_FLAG_NO_COLOR_TRANSFORM and B200JPG_FLAG_NO_UPSAMPLE included (component c is
+ * then ceil(W' / subx[c]) x ceil(H' / suby[c])). A frame's status is its status at full size; a JPEG XT frame with a residual
+ * layer is B200JPG_ERR_NOT_IMPLEMENTED. Accepted by b200jpg_batch_create_ex, b200jpg_decode_to_host_ex and
+ * b200jpg_decode_to_device_ex; these bits were ignored before they were defined. b200jpg_batch_output_extent gives the size. */
+#define B200JPG_FLAG_DOWNSCALE_2 0x4u
+#define B200JPG_FLAG_DOWNSCALE_4 0x8u
+#define B200JPG_FLAG_DOWNSCALE_8 0xCu
+#define B200JPG_FLAG_DOWNSCALE_MASK 0xCu
 B200JPG_API int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
                             unsigned flags, b200jpg_batch **batch);
 /* Waits for the work last enqueued for this batch (its buffers return to the context's pool for reuse by the
@@ -118,6 +130,11 @@ B200JPG_API int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *
 B200JPG_API void b200jpg_batch_destroy(b200jpg_batch *batch);
 
 B200JPG_API int b200jpg_batch_frame_info(const b200jpg_batch *batch, int i, b200jpg_frame_info *info);
+/* Width and height of component c of frame i as the decode entry points write it: the frame size (reduced by
+ * B200JPG_FLAG_DOWNSCALE_k), or the component's own size with B200JPG_FLAG_NO_UPSAMPLE. Returns B200JPG_OK, the frame's parse
+ * status for a frame that failed (nothing written), or B200JPG_ERR_INVALID_PARAMETER. b200jpg_batch_frame_info keeps the
+ * codestream's geometry. */
+B200JPG_API int b200jpg_batch_output_extent(const b200jpg_batch *batch, int i, int c, uint32_t *width, uint32_t *height);
 /* Byte offset / size of frame i inside the batch output buffer; total size with i = -1. */
 B200JPG_API uint64_t b200jpg_batch_out_offset(const b200jpg_batch *batch, int i);
 B200JPG_API uint64_t b200jpg_batch_out_bytes(const b200jpg_batch *batch, int i);
@@ -155,7 +172,8 @@ typedef struct b200jpg_plane {
 /* b200jpg_batch_decode with caller-described destinations, what the reference's BitMapHook hands out per component
  * (interface/bitmaphook.cpp, BitmapCtrl::RequestUserData control/bitmapctrl.cpp:142): planes[4*i + c] for frame i (the caller's frame index; JPEG XT residual
  * codestreams own no output), component c < ncomp.  Component geometry is what the batch was created with: width x height,
- * or ceil(width/subx[c]) x ceil(height/suby[c]) with B200JPG_FLAG_NO_UPSAMPLE.
+ * or ceil(width/subx[c]) x ceil(height/suby[c]) with B200JPG_FLAG_NO_UPSAMPLE, each reduced with B200JPG_FLAG_DOWNSCALE_k
+ * (b200jpg_batch_output_extent).
  * For every frame the call writes exactly the samples b200jpg_batch_decode writes into that frame's slot (damaged frames
  * under tolerate_bad included), rearranged, and nothing else: bytes between pixels and between rows keep their contents.
  * A frame whose parse failed has no destination (its data may be NULL).  Overlap between components or frames is the

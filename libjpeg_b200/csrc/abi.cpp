@@ -157,10 +157,15 @@ static_assert(std::has_unique_object_representations_v<ClassKey>, "ClassKey is c
 struct Extent {
     uint64_t w, h;
 };
-// component c as it leaves the decoder: the frame size, or without upsampling its own ceil(W / subx) x ceil(H / suby)
+// the factor k of B200JPG_FLAG_DOWNSCALE_k: 1, 2, 4 or 8
+uint32_t downscale_of(unsigned flags) { return 1u << ((flags & B200JPG_FLAG_DOWNSCALE_MASK) >> 2); }
+
+// component c as it leaves the decoder: the frame size W' x H' = ceil(W / k) x ceil(H / k), or without upsampling its own
+// ceil(W' / subx) x ceil(H' / suby)
 Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags) {
-    if (!(flags & B200JPG_FLAG_NO_UPSAMPLE)) return {fi.width, fi.height};
-    return {(fi.width + fi.subx[c] - 1) / fi.subx[c], (fi.height + fi.suby[c] - 1) / fi.suby[c]};
+    const uint64_t k = downscale_of(flags), w = (fi.width + k - 1) / k, h = (fi.height + k - 1) / k;
+    if (!(flags & B200JPG_FLAG_NO_UPSAMPLE)) return {w, h};
+    return {(w + fi.subx[c] - 1) / fi.subx[c], (h + fi.suby[c] - 1) / fi.suby[c]};
 }
 
 // body(i) for every frame i < n, on at most max_threads host threads
@@ -467,6 +472,11 @@ static void attach_residuals(b200jpg_batch &b, Codestreams &cs, bool device_inde
             cs.err[i] = "JPEG XT frames are only reconstructed with upsampling and colour transformation";
             continue;
         }
+        if (downscale_of(b.flags) > 1) {  // never decoded base-only: the merge at reduced size is not defined here
+            b.parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;
+            cs.err[i] = "JPEG XT frames are only reconstructed at full size";
+            continue;
+        }
         ParsedFrame rf;
         std::string rerr;
         const int rst = parse_residual(b.frames[i], rf, rerr, device_index);
@@ -563,21 +573,25 @@ static std::vector<uint64_t> lay_out_codestreams(b200jpg_batch &b, const std::ve
 
 // How live frame i is reconstructed. The tuned kernels cover 8-bit grey frames and three-component frames whose first component
 // is not subsampled and whose two other components share factors of 1 or 2; everything else (SURVEY 8f4), planes without
-// upsampling and both codestreams of a JPEG XT frame go through the generic kernels.
+// upsampling and both codestreams of a JPEG XT frame go through the generic kernels. Downscaled frames: 8-bit 4:2:0 frames with
+// upsampling take reconstruct420_scaled_kernel, every other one the scaled IDCT into int32 planes and then the generic kernels (a
+// JPEG XT frame never gets here downscaled: attach_residuals refuses it).
 static ReconPath recon_path(const b200jpg_batch &b, int i) {
     const b200jpg_frame_info &fi = b.frames[i].info;
+    const bool scaled = downscale_of(b.flags) > 1;
     if (b.xt_parent[i] >= 0 || (i < b.n_user && b.xt_child[i] >= 0)) return ReconPath::Generic;
-    if (b.flags & B200JPG_FLAG_NO_UPSAMPLE) return ReconPath::Generic;  // planes of every component, then one sample -> one output value
-    if (fi.precision != 8) return ReconPath::Generic;  // 12-bit frames: int32 planes, 16-bit samples out
-    if (fi.ncomp == 1) return (fi.subx[0] != 1 || fi.suby[0] != 1) ? ReconPath::Generic : ReconPath::Tiled;
+    if (b.flags & B200JPG_FLAG_NO_UPSAMPLE) return scaled ? ReconPath::Scaled : ReconPath::Generic;  // planes of every component, then one sample -> one output value
+    if (fi.precision != 8) return scaled ? ReconPath::Scaled : ReconPath::Generic;  // 12-bit frames: int32 planes, 16-bit samples out
+    if (fi.ncomp == 1) return scaled ? ReconPath::Scaled : ((fi.subx[0] != 1 || fi.suby[0] != 1) ? ReconPath::Generic : ReconPath::Tiled);
     if (fi.ncomp != 3 || fi.subx[0] != 1 || fi.suby[0] != 1 || fi.subx[1] != fi.subx[2] || fi.suby[1] != fi.suby[2] || fi.subx[1] > 2 || fi.suby[1] > 2)
-        return ReconPath::Generic;
-    return (fi.subx[1] == 2 && fi.suby[1] == 2) ? ReconPath::Fused420 : ReconPath::Tiled;
+        return scaled ? ReconPath::Scaled : ReconPath::Generic;
+    if (fi.subx[1] == 2 && fi.suby[1] == 2) return scaled ? ReconPath::Scaled420 : ReconPath::Fused420;
+    return scaled ? ReconPath::Scaled : ReconPath::Tiled;
 }
 
 // Coefficient, sample and output layout of the live frames; returns the sample plane offsets. The sample planes a frame gets
 // follow its reconstruction path: Generic one per component, Tiled one per component from 1 on, Fused420 none (its chroma samples
-// live in shared memory).
+// live in shared memory), Scaled one per component of 8 ceil(blocks_w / k) x 8 ceil(blocks_h / k) samples, Scaled420 none.
 static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
     const int n = b.n;
     b.coef_base.assign(n, {});
@@ -589,7 +603,8 @@ static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
         if (b.parse_status[i] != 0) continue;
         const b200jpg_frame_info &fi = b.frames[i].info;
         const ReconPath path = recon_path(b, i);
-        const int first_plane = path == ReconPath::Generic ? 0 : (path == ReconPath::Tiled ? 1 : fi.ncomp);
+        const int first_plane = (path == ReconPath::Generic || path == ReconPath::Scaled) ? 0 : (path == ReconPath::Tiled ? 1 : fi.ncomp);
+        const uint32_t k = downscale_of(b.flags);
         uint64_t samples = 0;
         for (int c = 0; c < fi.ncomp; c++) {
             const uint64_t elems = (uint64_t)fi.blocks_w[c] * fi.blocks_h[c] * 64;
@@ -597,7 +612,7 @@ static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
             coef_cur += elems;
             if (c >= first_plane) {
                 sample_base[i][c] = sample_cur;
-                sample_cur += elems;
+                sample_cur += path == ReconPath::Scaled ? 64ull * ((fi.blocks_w[c] + k - 1) / k) * ((fi.blocks_h[c] + k - 1) / k) : elems;
             }
             const Extent e = out_extent(fi, c, b.flags);  // the components one after the other
             samples += e.w * e.h;
@@ -814,8 +829,9 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         const b200jpg_frame_info &fi = b.frames[i].info;
         const int xt_res = (i < b.n_user) ? b.xt_child[i] : -1;  // JPEG XT: this frame's residual frame
         const ReconPath path = recon_path(b, i);
+        const bool generic = path == ReconPath::Generic || path == ReconPath::Scaled;
         uint32_t sx = fi.ncomp > 1 ? fi.subx[1] : 1, sy = fi.ncomp > 1 ? fi.suby[1] : 1;
-        if (path == ReconPath::Generic) sx = sy = 0;  // one group per component count: the generic kernels read the factors per frame
+        if (generic) sx = sy = 0;  // one group per component count: the generic kernels read the factors per frame
         ReconGroup *g = nullptr;
         for (auto &gg : b.groups)
             if (gg.ncomp == fi.ncomp && gg.subx == sx && gg.suby == sy && gg.path == path) g = &gg;
@@ -828,17 +844,25 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
             g->path = path;
         }
         FrameRecon fr{};
+        const uint32_t k = downscale_of(b.flags);
         for (int c = 0; c < fi.ncomp; c++) {
             fr.coef_base[c] = b.coef_base[i][c];
             fr.sample_base[c] = sample_base[i][c];
             fr.bw[c] = fi.blocks_w[c];
             fr.bh[c] = fi.blocks_h[c];
+            if (k > 1) {  // the grid of the reduced planes; the coefficient grid moves to coef_bw / coef_bh
+                fr.coef_bw[c] = fi.blocks_w[c];
+                fr.coef_bh[c] = fi.blocks_h[c];
+                fr.bw[c] = (fi.blocks_w[c] + k - 1) / k;
+                fr.bh[c] = (fi.blocks_h[c] + k - 1) / k;
+            }
             fr.csx[c] = fi.subx[c];
             fr.csy[c] = fi.suby[c];
         }
         fr.out_base = b.out_off[i];
-        fr.width = fi.width;
-        fr.height = fi.height;
+        const Extent reduced = out_extent(fi, 0, b.flags & ~B200JPG_FLAG_NO_UPSAMPLE);  // W' x H' (the full size without downscaling)
+        fr.width = (uint32_t)reduced.w;
+        fr.height = (uint32_t)reduced.h;
         if (b.xt_parent[i] >= 0) fr.width = fr.height = 0;  // a residual codestream: planes only, its frame's reconstruction reads them
         if (xt_res >= 0) {
             const b200jpg_frame_info &ri = b.frames[xt_res].info;
@@ -854,14 +878,14 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         fr.ycbcr = (b.flags & B200JPG_FLAG_NO_COLOR_TRANSFORM) ? 0 : fi.ycbcr;  // JPGTAG_MATRIX_LTRAFO = ..._NONE (rectanglerequest.cpp:150-152)
         fr.subx = sx;
         fr.suby = sy;
-        fr.cw = sx ? (fi.width + sx - 1) / sx : fi.width;  // (generic groups carry the factors per component: csx / csy)
-        fr.ch = sy ? (fi.height + sy - 1) / sy : fi.height;
+        fr.cw = (uint32_t)(sx ? (reduced.w + sx - 1) / sx : reduced.w);  // (generic groups carry the factors per component: csx / csy)
+        fr.ch = (uint32_t)(sy ? (reduced.h + sy - 1) / sy : reduced.h);
         fr.status_idx = (uint32_t)i;
         fr.precision = fi.precision;
         g->frames.push_back(fr);
-        g->max_bw0 = std::max(g->max_bw0, (fi.width + 7) / 8);
-        g->max_bh0 = std::max(g->max_bh0, (fi.height + 7) / 8);
-        if (path == ReconPath::Generic) {  // the largest block grid of any component: the extent of the generic IDCT launch
+        g->max_bw0 = std::max(g->max_bw0, (uint32_t)(reduced.w + 7) / 8);
+        g->max_bh0 = std::max(g->max_bh0, (uint32_t)(reduced.h + 7) / 8);
+        if (generic) {  // the largest block grid of any component: the extent of the generic (or scaled) IDCT launch
             for (int c = 0; c < fi.ncomp; c++)
                 if ((uint64_t)fi.blocks_w[c] * fi.blocks_h[c] > (uint64_t)g->max_bwc * g->max_bhc) g->max_bwc = fi.blocks_w[c], g->max_bhc = fi.blocks_h[c];
         } else if (fi.ncomp > 1) {
@@ -949,7 +973,8 @@ static int stage_and_allocate(b200jpg_batch &b, const Codestreams &cs, const std
     b.d_input = (uint8_t *)ctx->get(1, b.input_bytes, &ce);
     if (ce == cudaSuccess && b.coef_elems) b.d_coef = (int16_t *)ctx->get(1, b.coef_elems * sizeof(int16_t), &ce);
     if (ce == cudaSuccess && b.sample_elems) b.d_samples = (int32_t *)ctx->get(1, b.sample_elems * sizeof(int32_t), &ce);
-    if (ce == cudaSuccess && b.sample_elems) b.d_samples16 = (int16_t *)ctx->get(1, b.sample_elems * sizeof(int16_t), &ce);
+    // the int16 planes serve the Tiled path only, which downscaled batches never take
+    if (ce == cudaSuccess && b.sample_elems && downscale_of(b.flags) == 1) b.d_samples16 = (int16_t *)ctx->get(1, b.sample_elems * sizeof(int16_t), &ce);
     if (ce == cudaSuccess) b.d_clean = (uint8_t *)ctx->get(1, b.clean_bytes, &ce);
     if (ce == cudaSuccess) b.d_interval_len = (uint32_t *)ctx->get(1, b.sz_ilen, &ce);
     b.sz_overrun = sizeof(uint32_t) * (size_t)(b.n_intervals + b.classes.size() + 1);
@@ -1025,6 +1050,17 @@ int b200jpg_batch_frame_info(const b200jpg_batch *b, int i, b200jpg_frame_info *
     if (!b || i < 0 || i >= b->n_user || !info) return B200JPG_ERR_INVALID_PARAMETER;
     *info = b->frames[i].info;
     return b->parse_status[i];
+}
+
+int b200jpg_batch_output_extent(const b200jpg_batch *b, int i, int c, uint32_t *width, uint32_t *height) {
+    if (!b || i < 0 || i >= b->n_user || !width || !height) return B200JPG_ERR_INVALID_PARAMETER;
+    if (b->parse_status[i] != 0) return b->parse_status[i];
+    const b200jpg_frame_info &fi = b->frames[i].info;
+    if (c < 0 || c >= fi.ncomp) return B200JPG_ERR_INVALID_PARAMETER;
+    const Extent e = out_extent(fi, c, b->flags);
+    *width = (uint32_t)e.w;
+    *height = (uint32_t)e.h;
+    return B200JPG_OK;
 }
 
 uint64_t b200jpg_batch_out_offset(const b200jpg_batch *b, int i) { return (b && i >= 0 && i < b->n_user) ? b->out_off[i] : 0; }
@@ -1254,6 +1290,7 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.subx = g.subx;
         l.suby = g.suby;
         l.path = g.path;
+        l.downscale = (int)downscale_of(b->flags);
         l.planes_out = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
         l.coef = b->d_coef;
         l.samples16 = b->d_samples16;

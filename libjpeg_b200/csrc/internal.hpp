@@ -219,6 +219,9 @@ struct FrameRecon {       // per frame, for the reconstruction kernels
     uint64_t res_sample_base[4];
     uint32_t res_bw[4];
     uint8_t res_csx[4], res_csy[4];
+    // downscaled frames (ReconPath::Scaled / Scaled420): the coefficient block grid; bw / bh are then the grid of the reduced
+    // sample planes, ceil(coef_bw / k) x ceil(coef_bh / k), and width / height the reduced frame
+    uint32_t coef_bw[4], coef_bh[4];
 };
 
 // kernel launchers (huffman_sm100.cu, recon_sm100.cu). All asynchronous on `stream`.
@@ -256,7 +259,10 @@ int launch_progressive_dequant(const ProgFrame *frames_dev, uint32_t n_frames, u
 
 // How a frame goes from coefficients to pixels (abi.cpp: recon_path). Tiled: b1 planes of components 1.. + b2 (grey, 4:4:4,
 // 4:2:2, 4:4:0); Fused420: reconstruct420_kernel, no planes; Generic: int32 planes of every component + the generic kernels
-enum class ReconPath : int { Tiled, Fused420, Generic };
+// Scaled (B200JPG_FLAG_DOWNSCALE_*): idct_scaled_planes_kernel into int32 planes laid out as the IDCT output of the reduced frame,
+// then the generic kernels on a FrameRecon of the reduced width and height; Scaled420 (downscaled 8-bit 4:2:0 frames with
+// upsampling): reconstruct420_scaled_kernel, no planes
+enum class ReconPath : int { Tiled, Fused420, Generic, Scaled, Scaled420 };
 struct ReconLaunch {
     const FrameRecon *frames;  // device
     uint32_t n_frames;
@@ -266,6 +272,7 @@ struct ReconLaunch {
     ReconPath path;                // uniform over the group
     bool planes_out;               // B200JPG_FLAG_NO_UPSAMPLE: the components leave as planes at their own resolution
     int generic_phase;             // generic groups: 0 = IDCT then reconstruction, 1 = IDCT only, 2 = reconstruction only
+    int downscale;                 // Scaled groups: the factor k (2, 4 or 8) of B200JPG_FLAG_DOWNSCALE_k
     const int16_t *coef;
     int16_t *samples16;            // chroma sample planes every frame goes through
     int32_t *samples32;            // the same planes for the exact pass over frames flagged `narrow`

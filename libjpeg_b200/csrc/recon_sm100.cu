@@ -261,6 +261,86 @@ idct_planes_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restr
     }
 }
 
+// ---- downscaled decoding (B200JPG_FLAG_DOWNSCALE_k): blocks -> (8/k) x (8/k) int32 samples -------------------------------
+// The k x k box average of the exact 8-point IDCT is, per dimension, the (8/k) x 8 matrix
+//     A_k(m, u) = 1/k sum_{j<k} C(u)/2 cos((2 (k m + j) + 1) u pi / 16),   C(0) = 1/sqrt(2), else 1
+// (for k = 2 the 4-point IDCT of the folded coefficients; DESIGN §10). With a_k = round(2^20 A_k) and F the dequantised
+// coefficients in raster order (row r = vertical frequency), the samples -- 4 fractional bits, level shifted, like the
+// planes of idct_planes_kernel -- are, with every sum in int64 (|F| <= 2^15 and sum_u |A_k(m, u)| < 1.69: nothing wraps)
+//     row pass     P[r][m] = (sum_u a_k[m][u] F[r][u] + 2^7) >> 8                        |P| < 2^28
+//     column pass  s[n][m] = ((sum_r a_k[n][r] P[r][m] + 2^27) >> 28) + (8 << precision)
+// and for k = 8, where only the DC term is left, exactly s = 2 F[0][0] + (8 << precision).
+__constant__ int kScaledBasis2[4][8] = {{370728, 475072, 342508, 166823, 0, -111468, -141871, -94498},
+                                        {370728, 196781, -342508, -402746, 0, 269107, 141871, -39142},
+                                        {370728, -196781, -342508, 402746, 0, -269107, 141871, 39142},
+                                        {370728, -475072, 342508, -166823, 0, 111468, -141871, 94498}};
+__constant__ int kScaledBasis4[2][8] = {{370728, 335926, 0, -117962, 0, 78819, 0, -66820}, {370728, -335926, 0, 117962, 0, -78819, 0, 66820}};
+
+template <int KS>
+__device__ __forceinline__ int scaled_basis(int m, int u) {
+    return KS == 2 ? kScaledBasis2[m][u] : kScaledBasis4[m][u];
+}
+
+// the (8/k) x (8/k) samples of one block (k = 2, 4, 8), level shifted by `level` = 8 << precision; for k = 8 only the block's DC
+// word is read
+template <int KS>
+__device__ __forceinline__ void scaled_idct_block(const int16_t *__restrict__ blk, int level, int (&s)[8 / KS][8 / KS]) {
+    constexpr int N = 8 / KS;
+    if constexpr (KS == 8) {
+        s[0][0] = 2 * (int)__ldg(blk) + level;
+    } else {
+        const uint4 *src = reinterpret_cast<const uint4 *>(blk);
+        int p[8][N];
+#pragma unroll
+        for (int r = 0; r < 8; r++) {
+            int v[8];
+            unpack_row_raw(__ldg(src + r), v);
+#pragma unroll
+            for (int m = 0; m < N; m++) {
+                long long acc = 1ll << 7;
+#pragma unroll
+                for (int u = 0; u < 8; u++) acc += (long long)scaled_basis<KS>(m, u) * v[u];
+                p[r][m] = (int)(acc >> 8);
+            }
+        }
+#pragma unroll
+        for (int n = 0; n < N; n++) {
+#pragma unroll
+            for (int m = 0; m < N; m++) {
+                long long acc = 1ll << 27;
+#pragma unroll
+                for (int r = 0; r < 8; r++) acc += (long long)scaled_basis<KS>(n, r) * p[r][m];
+                s[n][m] = (int)(acc >> 28) + level;
+            }
+        }
+    }
+}
+
+// grid (coefficient blocks / 128, frames, components). Block (bx, by) of the coefficient grid coef_bw x coef_bh lands at
+// ((8/k) bx, (8/k) by) of a plane whose FrameRecon grid bw x bh = ceil(coef_bw / k) x ceil(coef_bh / k) makes the pitch
+// 8 bw >= (8/k) coef_bw: the generic kernels address the planes of the reduced frame like any other
+template <int KS>
+__global__ void __launch_bounds__(kThreadsB)
+idct_scaled_planes_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, int32_t *__restrict__ samples) {
+    constexpr int N = 8 / KS;
+    const FrameRecon &f = frames[blockIdx.y];
+    const uint32_t c = blockIdx.z;
+    if (c >= f.ncomp) return;
+    const uint32_t cbw = f.coef_bw[c], t = blockIdx.x * kThreadsB + threadIdx.x;
+    if (t >= cbw * f.coef_bh[c]) return;
+    const uint32_t bx = t % cbw, by = t / cbw, pitch = 8u * f.bw[c];
+    int s[N][N];
+    scaled_idct_block<KS>(coef + f.coef_base[c] + (uint64_t)t * 64u, (int)(8u << f.precision), s);
+    int32_t *dst = samples + f.sample_base[c] + (uint64_t)(N * by) * pitch + N * bx;
+#pragma unroll
+    for (int n = 0; n < N; n++) {
+        int32_t *row = dst + (uint64_t)n * pitch;
+        if (N == 4) *reinterpret_cast<int4 *>(row) = make_int4(s[n][0], s[n][N > 1 ? 1 : 0], s[n][N > 2 ? 2 : 0], s[n][N > 3 ? 3 : 0]);
+        else if (N == 2) *reinterpret_cast<int2 *>(row) = make_int2(s[n][0], s[n][N > 1 ? 1 : 0]);
+        else row[0] = s[n][0];
+    }
+}
+
 // the frames of a group whose `narrow` flag is set -> list = {count, group-local indices}
 __global__ void __launch_bounds__(256)
 narrow_list_kernel(const FrameRecon *__restrict__ frames, uint32_t n_frames, const uint32_t *__restrict__ narrow_flags, uint32_t *__restrict__ list) {
@@ -527,8 +607,9 @@ __device__ __forceinline__ void to_rgb(int y, int cbv, int crv, int &r, int &g, 
 
 // kWin: the chroma samples come from the window of reconstruct420_kernel at shared-space address `win` instead of the sample
 // planes. chroma_wide: a chroma sample the tile reads may leave the 32-bit colour range.
-// K: the destination kind (StoreKind).
-template <int NC, int SX, int SY, typename T, bool kWin = false, int K = kStoreCanvas>
+// K: the destination kind (StoreKind). KS > 1: the frame is downscaled by KS (B200JPG_FLAG_DOWNSCALE_k) -- the luma of an output
+// block comes from the KS x KS coefficient blocks under it through scaled_idct_block instead of the 8x8 IDCT of one block.
+template <int NC, int SX, int SY, typename T, bool kWin = false, int K = kStoreCanvas, int KS = 1>
 __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, const int16_t *__restrict__ coef, const T *__restrict__ samples,
                                                  uint32_t win, bool chroma_wide, StoreDst<K> __restrict__ out) {
     static_assert(!kWin || (NC == 3 && SX == 2 && SY == 2), "the chroma window is 4:2:0 only");
@@ -542,65 +623,94 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
     const int X = 8 * (int)bx, Y = 8 * (int)by;
     int *my = ys + threadIdx.x;
 
-    // ---- luma coefficients: the warp's 32 blocks are 4 KB of contiguous HBM. Eight coalesced 16-byte loads per lane
-    // (four full lines per warp instruction instead of 32 partial ones) park them in the upper half of the warp's tile
-    // columns, 16-byte piece (block, row) at row segment 32 + 4*row + block/8, slot (block%8) ^ row: conflict-free for
-    // these writes and for the per-lane reads below. The row pass overwrites a segment only after its piece was consumed.
-    {
-        const uint32_t wseg = (uint32_t)__cvta_generic_to_shared(ys) + 128u * warp;  // bytes; row segment j at + 4*NT*j
-        const uint4 *src = reinterpret_cast<const uint4 *>(coef + f.coef_base[0] + ((uint64_t)by * f.bw[0] + bx0) * 64u);
-        const uint32_t prow = lane & 7u, sub = lane >> 3;
-        uint4 pc[8];
-#pragma unroll
-        for (uint32_t i = 0; i < 8; i++) {
-            const bool have = bx0 + 4u * i + sub < f.bw[0];  // past the end of the block row: nothing (those lanes store nothing)
-            pc[i] = have ? __ldg(src + i * 32u + lane) : make_uint4(0u, 0u, 0u, 0u);
-        }
-#pragma unroll
-        for (uint32_t i = 0; i < 8; i++) {
-            const uint32_t blk = 4u * i + sub;
-            const uint32_t dst = wseg + 4u * NT * (32u + 4u * prow + (blk >> 3)) + 16u * ((blk & 7u) ^ prow);
-            asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(dst), "r"(pc[i].x), "r"(pc[i].y), "r"(pc[i].z), "r"(pc[i].w) : "memory");
-        }
-        __syncwarp();
-        // ---- row pass (dct/idct.cpp:237-287): the next row's piece is read before this row's results are written
-        const uint32_t mine = wseg + 4u * NT * (32u + (lane >> 3));
-        auto piece = [&](int r) {
-            uint4 q;
-            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];"
-                         : "=r"(q.x), "=r"(q.y), "=r"(q.z), "=r"(q.w)
-                         : "r"(mine + 16u * NT * (uint32_t)r + 16u * ((lane & 7u) ^ (uint32_t)r))
-                         : "memory");
-            return q;
-        };
-        uint4 q = piece(0);
-#pragma unroll 1
-        for (int r = 0; r < 8; r++) {
-            const uint4 qn = piece((r < 7) ? r + 1 : r);
-            int v[8];
-            unpack_row_raw(q, v);
-            if (r == 0) v[0] = WADD(v[0], 128 << 3);  // dcoffset << 3 (idct.cpp:233,244), preshift folded into the rounding (unpack_row_raw)
-            idct8t<16, 5>(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-            __syncwarp();
-#pragma unroll
-            for (int k = 0; k < 8; k++) my[(8 * r + k) * NT] = v[k];
-            q = qn;
-        }
-    }
-    // ---- column pass (:291-334) + range guard for the 32-bit colour arithmetic
     int mx = 0, mn = 0;
+    if constexpr (KS > 1) {
+        // ---- downscaled: output block (bx, by) holds the (8/KS) x (8/KS) samples of coefficient blocks (KS bx + i, KS by + j)
+        constexpr int N = 8 / KS;
 #pragma unroll 1
-    for (int k = 0; k < 8; k++) {
-        int v[8];
+        for (int j = 0; j < KS; j++) {
+#pragma unroll 1
+            for (int i = 0; i < KS; i++) {
+                const uint32_t cx = KS * bx + i, cy = KS * by + j;
+                int sm[N][N];
+                if (cx < f.coef_bw[0] && cy < f.coef_bh[0]) {
+                    scaled_idct_block<KS>(coef + f.coef_base[0] + ((uint64_t)cy * f.coef_bw[0] + cx) * 64u, 128 << 4, sm);
+                } else {
 #pragma unroll
-        for (int r = 0; r < 8; r++) v[r] = my[(8 * r + k) * NT];
-        idct8t<2048, 12>(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+                    for (int n = 0; n < N; n++)
 #pragma unroll
-        for (int r = 0; r < 8; r++) my[(8 * r + k) * NT] = v[r];
-        mx = __vimax3_s32(__vimax3_s32(mx, v[0], v[1]), v[2], v[3]);
-        mx = __vimax3_s32(__vimax3_s32(mx, v[4], v[5]), v[6], v[7]);
-        mn = __vimin3_s32(__vimin3_s32(mn, v[0], v[1]), v[2], v[3]);
-        mn = __vimin3_s32(__vimin3_s32(mn, v[4], v[5]), v[6], v[7]);
+                        for (int m = 0; m < N; m++) sm[n][m] = 0;  // beyond the coefficient grid: never visible
+                }
+#pragma unroll
+                for (int n = 0; n < N; n++)
+#pragma unroll
+                    for (int m = 0; m < N; m++) {
+                        my[(8 * (N * j + n) + N * i + m) * NT] = sm[n][m];
+                        mx = max(mx, sm[n][m]);
+                        mn = min(mn, sm[n][m]);
+                    }
+            }
+        }
+    } else {
+        // ---- luma coefficients: the warp's 32 blocks are 4 KB of contiguous HBM. Eight coalesced 16-byte loads per lane
+        // (four full lines per warp instruction instead of 32 partial ones) park them in the upper half of the warp's tile
+        // columns, 16-byte piece (block, row) at row segment 32 + 4*row + block/8, slot (block%8) ^ row: conflict-free for
+        // these writes and for the per-lane reads below. The row pass overwrites a segment only after its piece was consumed.
+        {
+            const uint32_t wseg = (uint32_t)__cvta_generic_to_shared(ys) + 128u * warp;  // bytes; row segment j at + 4*NT*j
+            const uint4 *src = reinterpret_cast<const uint4 *>(coef + f.coef_base[0] + ((uint64_t)by * f.bw[0] + bx0) * 64u);
+            const uint32_t prow = lane & 7u, sub = lane >> 3;
+            uint4 pc[8];
+    #pragma unroll
+            for (uint32_t i = 0; i < 8; i++) {
+                const bool have = bx0 + 4u * i + sub < f.bw[0];  // past the end of the block row: nothing (those lanes store nothing)
+                pc[i] = have ? __ldg(src + i * 32u + lane) : make_uint4(0u, 0u, 0u, 0u);
+            }
+    #pragma unroll
+            for (uint32_t i = 0; i < 8; i++) {
+                const uint32_t blk = 4u * i + sub;
+                const uint32_t dst = wseg + 4u * NT * (32u + 4u * prow + (blk >> 3)) + 16u * ((blk & 7u) ^ prow);
+                asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(dst), "r"(pc[i].x), "r"(pc[i].y), "r"(pc[i].z), "r"(pc[i].w) : "memory");
+            }
+            __syncwarp();
+            // ---- row pass (dct/idct.cpp:237-287): the next row's piece is read before this row's results are written
+            const uint32_t mine = wseg + 4u * NT * (32u + (lane >> 3));
+            auto piece = [&](int r) {
+                uint4 q;
+                asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];"
+                             : "=r"(q.x), "=r"(q.y), "=r"(q.z), "=r"(q.w)
+                             : "r"(mine + 16u * NT * (uint32_t)r + 16u * ((lane & 7u) ^ (uint32_t)r))
+                             : "memory");
+                return q;
+            };
+            uint4 q = piece(0);
+    #pragma unroll 1
+            for (int r = 0; r < 8; r++) {
+                const uint4 qn = piece((r < 7) ? r + 1 : r);
+                int v[8];
+                unpack_row_raw(q, v);
+                if (r == 0) v[0] = WADD(v[0], 128 << 3);  // dcoffset << 3 (idct.cpp:233,244), preshift folded into the rounding (unpack_row_raw)
+                idct8t<16, 5>(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+                __syncwarp();
+    #pragma unroll
+                for (int k = 0; k < 8; k++) my[(8 * r + k) * NT] = v[k];
+                q = qn;
+            }
+        }
+        // ---- column pass (:291-334) + range guard for the 32-bit colour arithmetic
+    #pragma unroll 1
+        for (int k = 0; k < 8; k++) {
+            int v[8];
+    #pragma unroll
+            for (int r = 0; r < 8; r++) v[r] = my[(8 * r + k) * NT];
+            idct8t<2048, 12>(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+    #pragma unroll
+            for (int r = 0; r < 8; r++) my[(8 * r + k) * NT] = v[r];
+            mx = __vimax3_s32(__vimax3_s32(mx, v[0], v[1]), v[2], v[3]);
+            mx = __vimax3_s32(__vimax3_s32(mx, v[4], v[5]), v[6], v[7]);
+            mn = __vimin3_s32(__vimin3_s32(mn, v[0], v[1]), v[2], v[3]);
+            mn = __vimin3_s32(__vimin3_s32(mn, v[4], v[5]), v[6], v[7]);
+        }
     }
 
     const int xmax = (X + 7 < (int)W) ? 7 : (int)((W - 1) & 7);
@@ -1047,6 +1157,57 @@ reconstruct420_kernel(const FrameRecon *__restrict__ frames, const int16_t *__re
 }
 
 
+// ---- 8-bit 4:2:0 frames downscaled by KS (B200JPG_FLAG_DOWNSCALE_k): reconstruct420_kernel's tile on the reduced frame ------
+// The CTA covers 32 x kRows420 blocks of the REDUCED frame (f.width x f.height). Phase 1 fills the int32 chroma window (the same
+// Window420 lines and columns, now of the reduced chroma planes) straight from the chroma coefficients: every coefficient block
+// whose (8/KS) x (8/KS) samples meet the window goes through scaled_idct_block once, and the samples that lie in the window and in
+// the plane (f.cw x f.ch) are stored. Phase 2 is reconstruct_tile<3, 2, 2, int32_t, true, K, KS>: luma from the KS x KS
+// coefficient blocks under each output block, then the same upsampling, colour transformation and stores as every other 4:2:0
+// frame. No sample planes; a window sample beyond +-kWide selects the 64-bit colour mode for the CTA, as in the int32 instance
+// of reconstruct420_kernel.
+template <int KS, int K>
+__global__ void __launch_bounds__(kThreads420, 12 / kRows420)
+reconstruct420_scaled_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, StoreDst<K> __restrict__ out) {
+    using Wn = Window420<int32_t>;
+    constexpr int N = 8 / KS;
+    extern __shared__ __align__(16) uint8_t smem420s[];
+    int *ys = reinterpret_cast<int *>(smem420s);
+    const uint32_t win = (uint32_t)__cvta_generic_to_shared(smem420s) + (uint32_t)Wn::kYsBytes;
+    const FrameRecon &f = frames[blockIdx.z];
+    const uint32_t vbw = (f.width + 7) >> 3, vbh = (f.height + 7) >> 3;
+    if (blockIdx.x * 32u >= vbw || blockIdx.y * (uint32_t)kRows420 >= vbh) return;  // whole CTA
+    const int cw = (int)f.cw, ch = (int)f.ch;
+    const int wy0 = 4 * kRows420 * (int)blockIdx.y - 1, wx0 = 128 * (int)blockIdx.x - 4;  // window line 0 / column 0
+    // the window positions that lie in the plane: lines y0..y1, columns x0..x1 (columns 3..132 of the window)
+    const int y0 = max(wy0, 0), y1 = min(wy0 + Wn::kLines - 1, ch - 1), x0 = max(wx0 + 3, 0), x1 = min(wx0 + 132, cw - 1);
+    int mn = 0, mx = 0;
+    if (y0 <= y1 && x0 <= x1) {
+        const int by0 = y0 / N, bx0 = x0 / N, nby = y1 / N - by0 + 1, nbx = x1 / N - bx0 + 1;
+        const uint32_t bwc = f.coef_bw[1];
+        for (int job = (int)threadIdx.x; job < 2 * nby * nbx; job += kThreads420) {
+            const int comp = job / (nby * nbx), rest = job - comp * nby * nbx;
+            const int cy = by0 + rest / nbx, cx = bx0 + rest % nbx;
+            int sm[N][N];
+            scaled_idct_block<KS>(coef + f.coef_base[1 + comp] + ((uint64_t)cy * bwc + (uint32_t)cx) * 64u, 128 << 4, sm);
+#pragma unroll
+            for (int n = 0; n < N; n++) {
+#pragma unroll
+                for (int m = 0; m < N; m++) {
+                    const int y = N * cy + n, x = N * cx + m;
+                    if (y >= y0 && y <= y1 && x >= x0 && x <= x1) {
+                        sts32(win + (uint32_t)comp * (uint32_t)Wn::kCompBytes + (uint32_t)(y - wy0) * (uint32_t)Wn::kLineBytes + (uint32_t)(x - wx0) * 4u,
+                              sm[n][m]);
+                        mx = max(mx, sm[n][m]);
+                        mn = min(mn, sm[n][m]);
+                    }
+                }
+            }
+        }
+    }
+    const bool wide = __syncthreads_or(mx > kWide || mn < -kWide) != 0;
+    reconstruct_tile<3, 2, 2, int32_t, true, K, KS>(f, ys, coef, nullptr, win, wide, out);
+}
+
 // =====================================================================================================
 // generic reconstruction: any number of components (1..4), any subsampling factors (1..4, per component)
 // =====================================================================================================
@@ -1354,6 +1515,26 @@ static int launch_recon420(const ReconLaunch &l, cudaStream_t s, int *launches) 
     return (int)cudaGetLastError();
 }
 
+// 8-bit 4:2:0 frames downscaled by l.downscale: one launch of reconstruct420_scaled_kernel
+template <int K, int KS>
+static int launch_recon420_scaled_k(const ReconLaunch &l, cudaStream_t s, int *launches) {
+    const uint32_t gx = (l.max_bw0 + 31) / 32, gy = (l.max_bh0 + kRows420 - 1) / kRows420;
+    constexpr int smem = Window420<int32_t>::kSmemBytes;
+    cudaError_t e = cudaFuncSetAttribute(reconstruct420_scaled_kernel<KS, K>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    if (e == cudaSuccess && smem > 48 * 1024) e = cudaFuncSetAttribute(reconstruct420_scaled_kernel<KS, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return (int)e;
+    reconstruct420_scaled_kernel<KS, K><<<dim3(gx, gy, l.n_frames), kThreads420, smem, s>>>(l.frames, l.coef, dst_of<K>(l));
+    if (launches) *launches = 1;
+    return (int)cudaGetLastError();
+}
+
+template <int K>
+static int launch_recon420_scaled(const ReconLaunch &l, cudaStream_t s, int *launches) {
+    if (l.downscale == 2) return launch_recon420_scaled_k<K, 2>(l, s, launches);
+    if (l.downscale == 4) return launch_recon420_scaled_k<K, 4>(l, s, launches);
+    return launch_recon420_scaled_k<K, 8>(l, s, launches);
+}
+
 template <int K>
 static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launches) {
     uint32_t mb = 0;
@@ -1361,7 +1542,11 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
     const uint32_t cblocks = (mb + kThreadsB - 1) / kThreadsB;
     int n = 0;
     if (l.generic_phase != 2) {
-        idct_planes_kernel<int32_t, false><<<dim3(cblocks, l.n_frames, l.ncomp), kThreadsB, 0, s>>>(l.frames, l.coef, l.samples32, l.wide_flags, nullptr, 0);
+        const dim3 grid(cblocks, l.n_frames, l.ncomp);
+        if (l.path == ReconPath::Generic) idct_planes_kernel<int32_t, false><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, l.samples32, l.wide_flags, nullptr, 0);
+        else if (l.downscale == 2) idct_scaled_planes_kernel<2><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, l.samples32);
+        else if (l.downscale == 4) idct_scaled_planes_kernel<4><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, l.samples32);
+        else idct_scaled_planes_kernel<8><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, l.samples32);
         n++;
     }
     if (l.generic_phase == 1) {
@@ -1381,8 +1566,9 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
 
 template <int K>
 static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches) {
-    if (l.path == ReconPath::Generic) return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : (K >= kStorePlanarF ? kStoreStridedF : kStoreStrided)>(l, s, launches);
+    if (l.path == ReconPath::Generic || l.path == ReconPath::Scaled) return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : (K >= kStorePlanarF ? kStoreStridedF : kStoreStrided)>(l, s, launches);
     if (l.path == ReconPath::Fused420) return launch_recon420<K>(l, s, launches);
+    if (l.path == ReconPath::Scaled420) return launch_recon420_scaled<K>(l, s, launches);
     int n = 0;  // ReconPath::Tiled
     const uint32_t cblocks = (l.max_bwc * l.max_bhc + kThreadsB - 1) / kThreadsB;
     const uint32_t gx = (l.max_bw0 + 31) / 32, gy = (l.max_bh0 + kThreadsB / 32 - 1) / (kThreadsB / 32);

@@ -224,7 +224,13 @@ class Context:
 class BatchDecoder:
     """One batch of codestreams: parse + pack on construction, then upload() / decode() on a CUDA stream."""
 
-    def __init__(self, frames, device=-1, tolerate_bad=False, ctx=None, color_transform=True, upsample=True):
+    def __init__(self, frames, device=-1, tolerate_bad=False, ctx=None, color_transform=True, upsample=True, downscale=1):
+        """downscale = 2, 4 or 8 decodes every frame at ceil(W / k) x ceil(H / k) (B200JPG_FLAG_DOWNSCALE_k): each 8x8 block is
+        inverse transformed straight to (8/k) x (8/k) samples, the k x k box average of its IDCT, and the rest of the
+        reconstruction runs on the smaller frame. geometry(), frame_view() and plane_views() give the reduced sizes. Not to be
+        confused with the `scale` of decode_into, which maps sample values."""
+        if isinstance(downscale, bool) or not isinstance(downscale, int) or downscale not in native.DOWNSCALE_FLAGS:
+            raise ValueError("downscale must be 1, 2, 4 or 8, got %r" % (downscale,))
         self.ctx = ctx or Context(device)
         self._keep = []
         n = len(frames)
@@ -240,6 +246,8 @@ class BatchDecoder:
         if not upsample:
             flags = 3  # B200JPG_FLAG_NO_UPSAMPLE (JPGTAG_DECODER_UPSAMPLE = false): planes, no colour transformation
         self.upsample = bool(upsample)
+        self.downscale = downscale
+        flags |= native.DOWNSCALE_FLAGS[downscale]
         rc = lib.b200jpg_batch_create_ex(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, ctypes.byref(self.handle))
         native.check(rc, self.ctx.handle)
         self._keep = []  # the batch holds its own pinned copy
@@ -251,6 +259,21 @@ class BatchDecoder:
         s = native.FrameInfoStruct()
         lib.b200jpg_batch_frame_info(self.handle, i, ctypes.byref(s))
         return FrameInfo.from_struct(s)
+
+    def output_shape(self, i, c):
+        """(h, w) of component c of frame i as decode() / decode_into() write it: the frame size divided by `downscale`
+        (rounded up), or without upsampling the component's own size. Raises NativeError for a frame that failed."""
+        w, h = ctypes.c_uint32(), ctypes.c_uint32()
+        native.check(lib.b200jpg_batch_output_extent(self.handle, i, c, ctypes.byref(w), ctypes.byref(h)), self.ctx.handle)
+        return h.value, w.value
+
+    def _shape(self, i, c, fi):
+        """output_shape, or for a frame that failed the shape its partial frame info gives (such a frame has no samples)"""
+        w, h = ctypes.c_uint32(), ctypes.c_uint32()
+        if lib.b200jpg_batch_output_extent(self.handle, i, c, ctypes.byref(w), ctypes.byref(h)) != 0:
+            shapes = component_shapes(fi, self.upsample)
+            return shapes[c] if c < len(shapes) else (fi.height, fi.width)
+        return h.value, w.value
 
     def out_offset(self, i):
         return lib.b200jpg_batch_out_offset(self.handle, i)
@@ -318,7 +341,7 @@ class BatchDecoder:
                 s = native.FrameInfoStruct()
                 rc = lib.b200jpg_batch_frame_info(self.handle, i, ctypes.byref(s))
                 fi = FrameInfo.from_struct(s)
-                geo.append(None if rc != 0 else (component_shapes(fi, self.upsample), fi.precision > 8))
+                geo.append(None if rc != 0 else ([self.output_shape(i, c) for c in range(fi.ncomp)], fi.precision > 8))
             self._geometry = geo
         return self._geometry
 
@@ -378,23 +401,25 @@ class BatchDecoder:
         return lib.b200jpg_batch_last_unstuff_ms(self.handle)
 
     def frame_view(self, out, i):
-        """Frame i of a decoded output tensor as [H, W, C]."""
+        """Frame i of a decoded output tensor as [H, W, C] (H x W reduced by `downscale`)."""
         fi = self.info(i)
         off = self.out_offset(i)
-        n = fi.width * fi.height * fi.ncomp
+        h, w = self._shape(i, 0, fi)
+        n = w * h * fi.ncomp
         if fi.precision > 8:  # 12-bit frames: native-endian 16-bit samples
             import torch
-            return out[off:off + 2 * n].view(torch.int16).view(fi.height, fi.width, fi.ncomp)
-        return out[off:off + n].view(fi.height, fi.width, fi.ncomp)
+            return out[off:off + 2 * n].view(torch.int16).view(h, w, fi.ncomp)
+        return out[off:off + n].view(h, w, fi.ncomp)
 
     def plane_views(self, out, i):
-        """upsample=False: the components of frame i as planes [ceil(H/suby), ceil(W/subx)] at their own resolution."""
+        """upsample=False: the components of frame i as planes [ceil(H/suby), ceil(W/subx)] at their own resolution (H x W
+        reduced by `downscale`)."""
         import torch
         assert not self.upsample
         fi = self.info(i)
         off, deep, planes = self.out_offset(i), fi.precision > 8, []
         for c in range(fi.ncomp):
-            h, w = (fi.height + fi.suby[c] - 1) // fi.suby[c], (fi.width + fi.subx[c] - 1) // fi.subx[c]
+            h, w = self._shape(i, c, fi)
             n = h * w * (2 if deep else 1)
             p = out[off:off + n]
             planes.append(p.view(torch.int16).view(h, w) if deep else p.view(h, w))

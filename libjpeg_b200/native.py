@@ -37,6 +37,8 @@ class ConvertStruct(ctypes.Structure):
 
 
 SAMPLE_F32, SAMPLE_F16, SAMPLE_BF16 = 1, 2, 3
+FLAG_NO_COLOR_TRANSFORM, FLAG_NO_UPSAMPLE = 1, 2
+DOWNSCALE_FLAGS = {1: 0x0, 2: 0x4, 4: 0x8, 8: 0xC}  # B200JPG_FLAG_DOWNSCALE_k
 
 
 def library_path():
@@ -61,6 +63,7 @@ def _load():
         "b200jpg_batch_create_ex": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.c_uint, ctypes.POINTER(vp)]),
         "b200jpg_batch_destroy": (None, [vp]),
         "b200jpg_batch_frame_info": (i32, [vp, i32, ctypes.POINTER(FrameInfoStruct)]),
+        "b200jpg_batch_output_extent": (i32, [vp, i32, i32, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint32)]),
         "b200jpg_batch_out_offset": (u64, [vp, i32]),
         "b200jpg_batch_out_bytes": (u64, [vp, i32]),
         "b200jpg_batch_ecs_bytes": (u64, [vp]),
@@ -102,7 +105,7 @@ def _load():
 lib = _load()
 ABI_SYMBOLS = [
     "b200jpg_parse", "b200jpg_build_tables", "b200jpg_create", "b200jpg_destroy", "b200jpg_trim", "b200jpg_last_error", "b200jpg_batch_create", "b200jpg_batch_create_ex",
-    "b200jpg_batch_destroy", "b200jpg_batch_frame_info", "b200jpg_batch_out_offset", "b200jpg_batch_out_bytes",
+    "b200jpg_batch_destroy", "b200jpg_batch_frame_info", "b200jpg_batch_output_extent", "b200jpg_batch_out_offset", "b200jpg_batch_out_bytes",
     "b200jpg_batch_ecs_bytes", "b200jpg_batch_stored_blocks", "b200jpg_batch_h2d_bytes", "b200jpg_batch_export_tables",
     "b200jpg_batch_import_tables", "b200jpg_batch_upload", "b200jpg_batch_reindex", "b200jpg_batch_decode", "b200jpg_batch_decode_into", "b200jpg_batch_decode_into_ex",
     "b200jpg_batch_decode_entropy",
