@@ -73,6 +73,9 @@ typedef struct b200jpg_frame_info {
 /* --- host-side parse, no device ------------------------------------------------------------------ */
 /* Parses the marker segments of one codestream. Returns B200JPG_OK or a negative error code. */
 B200JPG_API int b200jpg_parse(const uint8_t *data, size_t len, b200jpg_frame_info *info);
+/* The Exif orientation 1..8 that B200JPG_FLAG_EXIF_ORIENTATION applies to this codestream (1 without a valid Exif orientation),
+ * or the negative error code b200jpg_parse returns for it. Host only, no device. */
+B200JPG_API int b200jpg_exif_orientation(const uint8_t *data, size_t len);
 
 /* Builds the device-independent Huffman / quantisation table blob of scan `scan` of one codestream on the host
  * (replaces HuffmanTemplate::BuildDecoder coding/huffmantemplate.cpp:802-874 and IDCT::DefineQuant dct/idct.cpp:98-108).
@@ -123,6 +126,21 @@ B200JPG_API int b200jpg_batch_create(b200jpg_ctx *ctx, const uint8_t *const *fra
 #define B200JPG_FLAG_DOWNSCALE_4 0x8u
 #define B200JPG_FLAG_DOWNSCALE_8 0xCu
 #define B200JPG_FLAG_DOWNSCALE_MASK 0xCu
+/* B200JPG_FLAG_EXIF_ORIENTATION (no counterpart in the reference, which skips the Exif segment): every frame leaves the decoder
+ * as its oriented image. D is the image as it is written without the flag ([H, W, ...], after downscaling, colour transformation
+ * and clamp; with B200JPG_FLAG_NO_UPSAMPLE each plane at its own extent), O what is written with it:
+ *     1  D                       2  D mirrored left-right     3  D rotated by 180 deg     4  D mirrored top-bottom
+ *     5  D transposed            6  D rotated 90 deg clockwise  7  D transposed about the anti-diagonal  8  D rotated 90 deg ccw
+ * (PIL's ImageOps.exif_transpose). Width and height are swapped for 5..8: b200jpg_batch_output_extent, out_bytes / out_offset
+ * and the descriptors of b200jpg_batch_decode_into(_ex) describe the oriented image. The orientation is tag 0x0112 of IFD0 of the
+ * first APP1 segment in front of the first scan whose payload starts with "Exif\0\0" (b200jpg_exif_orientation); a malformed
+ * segment means orientation 1 and never changes a frame's status or a sample. Accepted by b200jpg_batch_create_ex,
+ * b200jpg_decode_to_host_ex and b200jpg_decode_to_device_ex. b200jpg_batch_decode_into(_ex) also refuses a frame of orientation 5..8
+ * whose |bytes_per_row| exceeds INT32_MAX (it becomes that frame's pixel stride). b200jpg_batch_decode / b200jpg_batch_reconstruct
+ * of a batch with oriented frames describe those frames' slots in a descriptor table like b200jpg_batch_decode_into's: each call
+ * copies it to the device on the stream (one small H2D copy), and the host may wait for the copy issued three such calls earlier
+ * before it reuses its pinned staging slot. Without oriented frames these calls stay as before: no copy, no host wait. */
+#define B200JPG_FLAG_EXIF_ORIENTATION 0x10u
 B200JPG_API int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
                             unsigned flags, b200jpg_batch **batch);
 /* Waits for the work last enqueued for this batch (its buffers return to the context's pool for reuse by the
@@ -135,6 +153,9 @@ B200JPG_API int b200jpg_batch_frame_info(const b200jpg_batch *batch, int i, b200
  * status for a frame that failed (nothing written), or B200JPG_ERR_INVALID_PARAMETER. b200jpg_batch_frame_info keeps the
  * codestream's geometry. */
 B200JPG_API int b200jpg_batch_output_extent(const b200jpg_batch *batch, int i, int c, uint32_t *width, uint32_t *height);
+/* Frame i's Exif orientation 1..8, whether or not the batch applies it (B200JPG_FLAG_EXIF_ORIENTATION); the frame's status for a
+ * frame that failed, B200JPG_ERR_INVALID_PARAMETER for a bad index. */
+B200JPG_API int b200jpg_batch_frame_orientation(const b200jpg_batch *batch, int i);
 /* Byte offset / size of frame i inside the batch output buffer; total size with i = -1. */
 B200JPG_API uint64_t b200jpg_batch_out_offset(const b200jpg_batch *batch, int i);
 B200JPG_API uint64_t b200jpg_batch_out_bytes(const b200jpg_batch *batch, int i);

@@ -12,6 +12,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -134,6 +135,7 @@ struct ScanClass {
 struct ReconGroup {
     uint32_t ncomp = 0, subx = 1, suby = 1;
     ReconPath path = ReconPath::Tiled;
+    int orientation = 1;  // B200JPG_FLAG_EXIF_ORIENTATION: the frames' orientation; 2..8 store through rewritten descriptors
     std::vector<FrameRecon> frames;
     uint32_t max_bw0 = 0, max_bh0 = 0, max_bwc = 0, max_bhc = 0;
     uint64_t dev_frames = 0;
@@ -161,11 +163,37 @@ struct Extent {
 uint32_t downscale_of(unsigned flags) { return 1u << ((flags & B200JPG_FLAG_DOWNSCALE_MASK) >> 2); }
 
 // component c as it leaves the decoder: the frame size W' x H' = ceil(W / k) x ceil(H / k), or without upsampling its own
-// ceil(W' / subx) x ceil(H' / suby)
-Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags) {
-    const uint64_t k = downscale_of(flags), w = (fi.width + k - 1) / k, h = (fi.height + k - 1) / k;
-    if (!(flags & B200JPG_FLAG_NO_UPSAMPLE)) return {w, h};
-    return {(w + fi.subx[c] - 1) / fi.subx[c], (h + fi.suby[c] - 1) / fi.suby[c]};
+// ceil(W' / subx) x ceil(H' / suby); width and height swapped for the Exif orientations 5..8 (`orientation`: the one the frame
+// leaves with, 1 for the extent the kernels decode)
+Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags, int orientation) {
+    const uint64_t k = downscale_of(flags);
+    uint64_t w = (fi.width + k - 1) / k, h = (fi.height + k - 1) / k;
+    if (flags & B200JPG_FLAG_NO_UPSAMPLE) w = (w + fi.subx[c] - 1) / fi.subx[c], h = (h + fi.suby[c] - 1) / fi.suby[c];
+    if (orientation >= 5) return {h, w};
+    return {w, h};
+}
+
+// A destination described in output coordinates (data d, pixel stride p, row stride r) as seen from the decoded coordinates
+// (x, y) of a component of decoded extent w x h under Exif orientation o (DESIGN §11): the kernels walk (x, y) and store
+// through the rewritten descriptor. Returns false when the new pixel stride does not fit its int32 field.
+bool orient_plane(b200jpg_plane &pl, int o, uint64_t w, uint64_t h) {
+    const int64_t p = pl.bytes_per_pixel, r = pl.bytes_per_row, W = (int64_t)w - 1, H = (int64_t)h - 1;
+    int64_t off, np, nr;
+    switch (o) {
+    case 2: off = W * p, np = -p, nr = r; break;
+    case 3: off = W * p + H * r, np = -p, nr = -r; break;
+    case 4: off = H * r, np = p, nr = -r; break;
+    case 5: off = 0, np = r, nr = p; break;
+    case 6: off = H * p, np = r, nr = -p; break;
+    case 7: off = H * p + W * r, np = -r, nr = -p; break;
+    case 8: off = W * r, np = -r, nr = p; break;
+    default: return true;
+    }
+    if (np < INT32_MIN || np > INT32_MAX) return false;
+    pl.data = static_cast<uint8_t *>(pl.data) + off;
+    pl.bytes_per_pixel = (int32_t)np;
+    pl.bytes_per_row = nr;
+    return true;
 }
 
 // body(i) for every frame i < n, on at most max_threads host threads
@@ -241,10 +269,18 @@ struct b200jpg_batch {
     b200jpg_plane *h_planes = nullptr, *d_planes = nullptr;
     cudaEvent_t ev_planes[kPlaneSlots] = {};
     int plane_slot = 0;
+    bool oriented = false;  // some live frame leaves with an Exif orientation other than 1: its group stores through descriptors
     int last_launches = 0;
     bool timing = false;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // start, after a0, after a1, after b
 };
+
+// the Exif orientation frame i leaves the decoder with: its own (a JPEG XT residual codestream: its frame's, so that the two stay
+// in one reconstruction group) with B200JPG_FLAG_EXIF_ORIENTATION, else 1
+static int applied_orientation(const b200jpg_batch &b, int i) {
+    if (!(b.flags & B200JPG_FLAG_EXIF_ORIENTATION)) return 1;
+    return b.frames[b.xt_parent[i] >= 0 ? b.xt_parent[i] : i].orientation;
+}
 
 extern "C" {
 
@@ -311,8 +347,8 @@ static int parse_residual(const ParsedFrame &base, ParsedFrame &rf, std::string 
     return rst;
 }
 
-int b200jpg_parse(const uint8_t *data, size_t len, b200jpg_frame_info *info) {
-    ParsedFrame pf;
+// b200jpg_parse and b200jpg_exif_orientation: one parse, the residual codestream of a JPEG XT frame included
+static int parse_one(const uint8_t *data, size_t len, ParsedFrame &pf) {
     std::string err;
     int rc;
     try {
@@ -327,8 +363,20 @@ int b200jpg_parse(const uint8_t *data, size_t len, b200jpg_frame_info *info) {
     }
     g_tls_code = rc;
     g_tls_error = err;
+    return rc;
+}
+
+int b200jpg_parse(const uint8_t *data, size_t len, b200jpg_frame_info *info) {
+    ParsedFrame pf;
+    const int rc = parse_one(data, len, pf);
     if (info) *info = pf.info;
     return rc;
+}
+
+int b200jpg_exif_orientation(const uint8_t *data, size_t len) {
+    ParsedFrame pf;
+    const int rc = parse_one(data, len, pf);
+    return rc != 0 ? rc : pf.orientation;
 }
 
 uint64_t b200jpg_build_tables(const uint8_t *data, size_t len, int scan, uint8_t *dst, uint64_t capacity) {
@@ -614,7 +662,7 @@ static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
                 sample_base[i][c] = sample_cur;
                 sample_cur += path == ReconPath::Scaled ? 64ull * ((fi.blocks_w[c] + k - 1) / k) * ((fi.blocks_h[c] + k - 1) / k) : elems;
             }
-            const Extent e = out_extent(fi, c, b.flags);  // the components one after the other
+            const Extent e = out_extent(fi, c, b.flags, 1);  // the components one after the other (w * h: any orientation)
             samples += e.w * e.h;
         }
         b.out_off[i] = out_cur;
@@ -832,9 +880,13 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         const bool generic = path == ReconPath::Generic || path == ReconPath::Scaled;
         uint32_t sx = fi.ncomp > 1 ? fi.subx[1] : 1, sy = fi.ncomp > 1 ? fi.suby[1] : 1;
         if (generic) sx = sy = 0;  // one group per component count: the generic kernels read the factors per frame
+        // oriented frames (B200JPG_FLAG_EXIF_ORIENTATION, 2..8) form groups of their own, one per orientation: their destinations
+        // are rewritten descriptors, whose store kind is chosen per group
+        const int orientation = applied_orientation(b, i);
+        if (orientation != 1) b.oriented = true;
         ReconGroup *g = nullptr;
         for (auto &gg : b.groups)
-            if (gg.ncomp == fi.ncomp && gg.subx == sx && gg.suby == sy && gg.path == path) g = &gg;
+            if (gg.ncomp == fi.ncomp && gg.subx == sx && gg.suby == sy && gg.path == path && gg.orientation == orientation) g = &gg;
         if (!g) {
             b.groups.emplace_back();
             g = &b.groups.back();
@@ -842,6 +894,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
             g->subx = sx;
             g->suby = sy;
             g->path = path;
+            g->orientation = orientation;
         }
         FrameRecon fr{};
         const uint32_t k = downscale_of(b.flags);
@@ -860,7 +913,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
             fr.csy[c] = fi.suby[c];
         }
         fr.out_base = b.out_off[i];
-        const Extent reduced = out_extent(fi, 0, b.flags & ~B200JPG_FLAG_NO_UPSAMPLE);  // W' x H' (the full size without downscaling)
+        const Extent reduced = out_extent(fi, 0, b.flags & ~B200JPG_FLAG_NO_UPSAMPLE, 1);  // W' x H' (the full size without downscaling)
         fr.width = (uint32_t)reduced.w;
         fr.height = (uint32_t)reduced.h;
         if (b.xt_parent[i] >= 0) fr.width = fr.height = 0;  // a residual codestream: planes only, its frame's reconstruction reads them
@@ -1057,10 +1110,15 @@ int b200jpg_batch_output_extent(const b200jpg_batch *b, int i, int c, uint32_t *
     if (b->parse_status[i] != 0) return b->parse_status[i];
     const b200jpg_frame_info &fi = b->frames[i].info;
     if (c < 0 || c >= fi.ncomp) return B200JPG_ERR_INVALID_PARAMETER;
-    const Extent e = out_extent(fi, c, b->flags);
+    const Extent e = out_extent(fi, c, b->flags, applied_orientation(*b, i));
     *width = (uint32_t)e.w;
     *height = (uint32_t)e.h;
     return B200JPG_OK;
+}
+
+int b200jpg_batch_frame_orientation(const b200jpg_batch *b, int i) {
+    if (!b || i < 0 || i >= b->n_user) return B200JPG_ERR_INVALID_PARAMETER;
+    return b->parse_status[i] != 0 ? b->parse_status[i] : b->frames[i].orientation;
 }
 
 uint64_t b200jpg_batch_out_offset(const b200jpg_batch *b, int i) { return (b && i >= 0 && i < b->n_user) ? b->out_off[i] : 0; }
@@ -1271,11 +1329,92 @@ static int run_entropy(b200jpg_batch *b, void *stream) {
     return B200JPG_OK;
 }
 
+// The descriptor table [4 * n] that fill(table) writes (on zeros: residual codestreams and failed frames have no destination) to
+// b->d_planes on `stream`, staged in the next slot of the pinned ring (b200jpg_batch::kPlaneSlots)
+static int stage_planes(b200jpg_batch *b, void *stream, const std::function<void(b200jpg_plane *)> &fill) {
+    const size_t bytes = sizeof(b200jpg_plane) * 4 * (size_t)b->n;
+    cudaError_t ce = cudaSuccess;
+    constexpr int kSlots = b200jpg_batch::kPlaneSlots;
+    if (!b->d_planes) {  // everything is allocated before any of it is kept: a failure leaves the batch as it was
+        b200jpg_plane *h = (b200jpg_plane *)b->ctx->get(0, bytes * kSlots, &ce), *d = nullptr;
+        cudaEvent_t ev[kSlots] = {};
+        if (ce == cudaSuccess) d = (b200jpg_plane *)b->ctx->get(1, bytes, &ce);
+        for (int k = 0; k < kSlots && ce == cudaSuccess; k++) ce = cudaEventCreateWithFlags(&ev[k], cudaEventDisableTiming);
+        if (ce != cudaSuccess) {
+            const std::string why = cudaGetErrorString(ce);
+            b->ctx->put(0, h, bytes * kSlots);
+            b->ctx->put(1, d, bytes);
+            for (auto &e : ev)
+                if (e) cudaEventDestroy(e);
+            return b->ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "descriptor table allocation failed: " + why);
+        }
+        b->h_planes = h, b->d_planes = d;
+        for (int k = 0; k < kSlots; k++) b->ev_planes[k] = ev[k];
+    }
+    const int slot = b->plane_slot;
+    ce = cudaEventSynchronize(b->ev_planes[slot]);  // the copy kSlots calls ago has read this slot (at once when never recorded)
+    if (ce != cudaSuccess) return b->ctx->fail_cuda(ce, "descriptor table");
+    b200jpg_plane *stage = b->h_planes + 4 * (size_t)b->n * slot;
+    memset(stage, 0, bytes);
+    fill(stage);
+    ce = cudaMemcpyAsync(b->d_planes, stage, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream);
+    if (ce == cudaSuccess) ce = cudaEventRecord(b->ev_planes[slot], (cudaStream_t)stream);
+    b->plane_slot = (slot + 1) % kSlots;
+    if (ce != cudaSuccess) return b->ctx->fail_cuda(ce, "descriptor table upload");
+    return B200JPG_OK;
+}
+
+// Frame i's destinations rewritten for its Exif orientation (orient_plane), in place; planar[i] cleared unless every component
+// then has bytes_per_pixel == size. Returns false when a pixel stride does not fit (only a caller's descriptor can do that).
+static bool orient_frame(const b200jpg_batch *b, int i, b200jpg_plane *pl, uint64_t size, std::vector<char> &planar) {
+    const b200jpg_frame_info &fi = b->frames[i].info;
+    const int o = applied_orientation(*b, i);
+    for (int c = 0; c < fi.ncomp; c++) {
+        const Extent d = out_extent(fi, c, b->flags, 1);
+        if (!orient_plane(pl[c], o, d.w, d.h)) return false;
+        if ((uint64_t)pl[c].bytes_per_pixel != size) planar[(size_t)i] = 0;
+    }
+    return true;
+}
+
+// b200jpg_batch_decode of a batch with oriented frames: each such frame's packed slot in out_dev, seen as an interleaved bitmap of
+// the oriented extent (B200JPG_FLAG_NO_UPSAMPLE: plane after plane), rewritten for its orientation and staged like the table of
+// b200jpg_batch_decode_into. planar[i] as for that table.
+static int stage_slot_planes(b200jpg_batch *b, uint8_t *out_dev, void *stream, std::vector<char> &planar) {
+    return stage_planes(b, stream, [&](b200jpg_plane *table) {
+        for (int i = 0; i < b->n_user; i++) {
+            if (b->parse_status[i] != 0 || applied_orientation(*b, i) == 1) continue;
+            const b200jpg_frame_info &fi = b->frames[i].info;
+            const int o = applied_orientation(*b, i);
+            const int64_t size = fi.precision > 8 ? 2 : 1;
+            const bool planes = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
+            uint64_t before = 0;
+            b200jpg_plane *pl = table + 4 * (size_t)i;
+            for (int c = 0; c < fi.ncomp; c++) {
+                const Extent e = out_extent(fi, c, b->flags, o);
+                pl[c].data = out_dev + b->out_off[i] + (planes ? before : (uint64_t)c) * size;
+                pl[c].bytes_per_pixel = (int32_t)(planes ? size : fi.ncomp * size);
+                pl[c].bytes_per_row = (int64_t)e.w * pl[c].bytes_per_pixel;
+                before += e.w * e.h;
+            }
+            orient_frame(b, i, pl, (uint64_t)size, planar);  // a slot's row stride always fits the pixel stride
+        }
+    });
+}
+
 // planes_dev: b200jpg_batch_decode_into's descriptor table (device), planar[i]: every component of frame i has
 // bytes_per_pixel == sample size (element size with `convert`, the float map of b200jpg_batch_decode_into_ex)
 static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b200jpg_plane *planes_dev = nullptr,
                      const std::vector<char> *planar = nullptr, const b200jpg_convert *convert = nullptr) {
     NvtxRange nvtx("b200jpg reconstruction: IDCT + upsampling + colour");
+    // into the packed slots with oriented frames: those frames' slots as rewritten descriptors, built for this call's out_dev
+    std::vector<char> slot_planar;
+    const b200jpg_plane *slot_planes = nullptr;
+    if (!planes_dev && b->oriented) {
+        slot_planar.assign((size_t)b->n, 1);
+        if (int rc = stage_slot_planes(b, out_dev, stream, slot_planar)) return rc;
+        slot_planes = b->d_planes;
+    }
     cudaError_t me = cudaMemsetAsync(b->d_status + b->n, 0, sizeof(uint32_t) * 2 * (size_t)b->n, (cudaStream_t)stream);
     if (me != cudaSuccess) return b->ctx->fail_cuda(me, "flag reset");
     for (auto &g : b->groups) {
@@ -1301,9 +1440,13 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.out = out_dev;
         l.planes = planes_dev;
         l.convert = convert;
-        l.planar = planes_dev != nullptr;
-        if (planes_dev)
-            for (const FrameRecon &fr : g.frames) l.planar = l.planar && (*planar)[fr.status_idx];
+        const std::vector<char> *group_planar = planar;
+        if (slot_planes && g.orientation != 1) l.planes = slot_planes, group_planar = &slot_planar;
+        l.planar = l.planes != nullptr;
+        if (l.planes)
+            for (const FrameRecon &fr : g.frames) l.planar = l.planar && (*group_planar)[fr.status_idx];
+        // oriented frames into anything but planar destinations: the staged store kinds, runs of eight samples along x or y
+        l.runs = g.orientation != 1 && l.planes && !l.planar;
         int launches = 0;
         // grid.y carries the frame index: at most 65535 frames per launch. A generic group that is cut runs the IDCT of ALL its
         // frames first: a JPEG XT frame reads the planes of its residual frame, which may sit in another part
@@ -1378,13 +1521,16 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
                 return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "component " + std::to_string(c) + ": scale and bias must be finite");
     }
     std::vector<char> planar((size_t)b->n, 1);
+    // a batch with oriented frames: the table as staged, those frames' descriptors rewritten once here (orient_plane)
+    std::vector<b200jpg_plane> oriented(b->oriented ? 4 * (size_t)b->n_user : 0);
     for (int i = 0; i < b->n_user; i++) {
         if (b->parse_status[i] != 0) continue;
         const b200jpg_frame_info &fi = b->frames[i].info;
         const uint64_t size = convert ? element : (fi.precision > 8 ? 2 : 1);
+        const int orientation = applied_orientation(*b, i);
         for (int c = 0; c < fi.ncomp; c++) {
             const b200jpg_plane &p = planes[4 * i + c];
-            const auto [w, h] = out_extent(fi, c, b->flags);
+            const auto [w, h] = out_extent(fi, c, b->flags, orientation);  // the rules hold in output coordinates
             const uint64_t bpp = magnitude(p.bytes_per_pixel), bpr = magnitude(p.bytes_per_row);
             const std::string at = "frame " + std::to_string(i) + " component " + std::to_string(c) + ": ";
             if (!p.data) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "no destination");
@@ -1401,37 +1547,23 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
                 return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "not device memory of the batch's device");
             if ((uint64_t)p.bytes_per_pixel != size) planar[(size_t)i] = 0;
         }
-    }
-    const size_t bytes = sizeof(b200jpg_plane) * 4 * (size_t)b->n;
-    cudaError_t ce = cudaSuccess;
-    constexpr int kSlots = b200jpg_batch::kPlaneSlots;
-    if (!b->d_planes) {  // everything is allocated before any of it is kept: a failure leaves the batch as it was
-        b200jpg_plane *h = (b200jpg_plane *)b->ctx->get(0, bytes * kSlots, &ce), *d = nullptr;
-        cudaEvent_t ev[kSlots] = {};
-        if (ce == cudaSuccess) d = (b200jpg_plane *)b->ctx->get(1, bytes, &ce);
-        for (int k = 0; k < kSlots && ce == cudaSuccess; k++) ce = cudaEventCreateWithFlags(&ev[k], cudaEventDisableTiming);
-        if (ce != cudaSuccess) {
-            const std::string why = cudaGetErrorString(ce);
-            b->ctx->put(0, h, bytes * kSlots);
-            b->ctx->put(1, d, bytes);
-            for (auto &e : ev)
-                if (e) cudaEventDestroy(e);
-            return b->ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "descriptor table allocation failed: " + why);
+        if (b->oriented) {
+            b200jpg_plane *q = oriented.data() + 4 * (size_t)i;
+            memcpy(q, planes + 4 * (size_t)i, sizeof(b200jpg_plane) * fi.ncomp);
+            if (orientation != 1) {  // the kernels store through the rewritten descriptors: planar is decided on those
+                planar[(size_t)i] = 1;
+                if (!orient_frame(b, i, q, size, planar))
+                    return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) +
+                                                                           ": |bytes_per_row| does not fit the pixel stride of the transposed frame");
+            }
         }
-        b->h_planes = h, b->d_planes = d;
-        for (int k = 0; k < kSlots; k++) b->ev_planes[k] = ev[k];
     }
-    const int slot = b->plane_slot;
-    ce = cudaEventSynchronize(b->ev_planes[slot]);  // the copy kSlots calls ago has read this slot (at once when never recorded)
-    if (ce != cudaSuccess) return b->ctx->fail_cuda(ce, "descriptor table");
-    b200jpg_plane *stage = b->h_planes + 4 * (size_t)b->n * slot;
-    memset(stage, 0, bytes);  // residual codestreams and failed frames: no destination
-    for (int i = 0; i < b->n_user; i++)
-        if (b->parse_status[i] == 0) memcpy(stage + 4 * (size_t)i, planes + 4 * (size_t)i, sizeof(b200jpg_plane) * b->frames[i].info.ncomp);
-    ce = cudaMemcpyAsync(b->d_planes, stage, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream);
-    if (ce == cudaSuccess) ce = cudaEventRecord(b->ev_planes[slot], (cudaStream_t)stream);
-    b->plane_slot = (slot + 1) % kSlots;
-    if (ce != cudaSuccess) return b->ctx->fail_cuda(ce, "descriptor table upload");
+    const b200jpg_plane *src = b->oriented ? oriented.data() : planes;
+    const int rc = stage_planes(b, stream, [&](b200jpg_plane *table) {
+        for (int i = 0; i < b->n_user; i++)
+            if (b->parse_status[i] == 0) memcpy(table + 4 * (size_t)i, src + 4 * (size_t)i, sizeof(b200jpg_plane) * b->frames[i].info.ncomp);
+    });
+    if (rc) return rc;
     return run_decode(b, nullptr, stream, b->d_planes, &planar, convert);
 }
 

@@ -77,7 +77,14 @@ struct ParsedFrame {
     b200jpg_frame_info info{};
     std::vector<ScanInfo> scans;
     XtLayer xt;
+    // Exif orientation (tag 0x0112 of IFD0 in the first APP1 "Exif\0\0" segment in front of the first scan), 1..8; 1 when there
+    // is none or it is malformed. Applied only with B200JPG_FLAG_EXIF_ORIENTATION; never changes the parse status
+    int orientation = 1;
 };
+
+// The orientation an APP1 payload (the bytes behind the length field) gives: 0 when it is not an Exif segment, else 1..8
+// (1 for anything malformed)
+int exif_orientation_of(const uint8_t *s, size_t rem);
 
 // Returns 0 or a negative reference error code; `err` receives a message. With `device_index` a scan that carries all
 // components of the frame and uses restart markers is not walked on the host (ScanInfo::device_index).
@@ -284,6 +291,7 @@ struct ReconLaunch {
     // null: the packed slots of `out`
     const b200jpg_plane *planes;
     bool planar;                   // every plane of the group's frames has bytes_per_pixel == sample size (element size with `convert`)
+    bool runs;                     // a group of Exif-oriented frames that is not planar: kStoreRuns / kStoreRunsF
     // b200jpg_batch_decode_into_ex: the samples leave as float32 / float16 / bfloat16 through this map (host memory, passed to
     // the kernels by value); null: as integers
     const b200jpg_convert *convert;
@@ -294,7 +302,12 @@ struct ReconLaunch {
 // kStoreStrided: any signed pixel and row stride, one store per sample. kStorePlanarF / kStoreStridedF: the same layouts with
 // float elements, every clamped integer sample v converted to fp32_round(fp32_round(v * scale[c]) + bias[c]) and rounded to
 // the element type (B200JPG_SAMPLE_*, a launch-uniform switch inside the kind).
-enum StoreKind : int { kStoreCanvas = 0, kStorePlanar = 1, kStoreStrided = 2, kStorePlanarF = 3, kStoreStridedF = 4 };
+// kStoreRuns / kStoreRunsF (groups of Exif-oriented frames on the tiled 8-bit paths): the block is staged in the kernel's luma tile
+// and leaves as runs of eight contiguous samples along x (mirrored rows) or along y (transposed), in either direction, a packed
+// interleaved slot as 24-byte runs of pixels; whatever has no contiguous axis, one store per sample.
+enum StoreKind : int { kStoreCanvas = 0, kStorePlanar = 1, kStoreStrided = 2, kStorePlanarF = 3, kStoreStridedF = 4, kStoreRuns = 5, kStoreRunsF = 6 };
+template <int k>
+constexpr bool kFloatKind = k == kStorePlanarF || k == kStoreStridedF || k == kStoreRunsF;
 
 // the destination argument of the float kinds: the descriptors plus the map, both in the kernel's parameter bank
 struct FloatDst {

@@ -115,15 +115,42 @@ int resolve_restart_sequence(const std::vector<size_t> &rst_at, const std::vecto
     return 0;
 }
 
-namespace {
-
-}  // namespace
+// Exif (CIPA DC-008): "Exif\0\0", a TIFF header ("II*\0" little endian or "MM\0*" big endian, then the uint32 offset of IFD0
+// from the header), IFD0 = a 2-byte entry count and 12-byte entries {tag, type, count, value or offset}. Orientation is tag
+// 0x0112, type 3 (SHORT), count 1, its value in the first two bytes of the value field. Only what lies inside the segment is
+// read; IFD1, XMP and every other tag are ignored.
+int exif_orientation_of(const uint8_t *s, size_t rem) {
+    if (rem < 6 || memcmp(s, "Exif\0\0", 6) != 0) return 0;
+    const uint8_t *t = s + 6;
+    const uint64_t tlen = rem - 6;
+    if (tlen < 8) return 1;
+    bool le;
+    if (memcmp(t, "II*\0", 4) == 0) le = true;
+    else if (memcmp(t, "MM\0*", 4) == 0) le = false;
+    else return 1;
+    auto u16 = [&](uint64_t p) -> uint32_t { return le ? (t[p] | (t[p + 1] << 8)) : ((t[p] << 8) | t[p + 1]); };
+    auto u32 = [&](uint64_t p) -> uint32_t { return le ? (u16(p) | (u16(p + 2) << 16)) : ((u16(p) << 16) | u16(p + 2)); };
+    const uint64_t ifd = u32(4);
+    if (ifd + 2 > tlen) return 1;
+    const uint32_t count = u16(ifd);
+    for (uint64_t k = 0; k < count; k++) {
+        const uint64_t e = ifd + 2 + 12 * k;
+        if (e + 12 > tlen) return 1;
+        if (u16(e) != 0x0112) continue;
+        if (u16(e + 2) != 3 || u32(e + 4) != 1) return 1;
+        const uint32_t v = u16(e + 8);
+        return (v >= 1 && v <= 8) ? (int)v : 1;
+    }
+    return 1;
+}
 
 int parse_codestream(const uint8_t *data, size_t len, ParsedFrame &out, std::string &err, bool device_index) {
     Cursor c{data, len};
     b200jpg_frame_info &fi = out.info;
     memset(&fi, 0, sizeof(fi));
     out.scans.clear();
+    out.orientation = 1;
+    bool exif_seen = false;  // the first Exif segment decides
     if (!data || len < 4) FAIL(B200JPG_ERR_UNEXPECTED_EOF, "stream is too short to be a JPEG codestream");
     if (c.u16(0) != 0xffd8) FAIL(B200JPG_ERR_MALFORMED_STREAM, "stream does not start with SOI, not a JPEG codestream");
 
@@ -211,6 +238,12 @@ int parse_codestream(const uint8_t *data, size_t len, ParsedFrame &out, std::str
             break;
         case 0xee:  // APP14: Adobe colour information (tables.cpp:2023-2025)
             if (rem >= 12 && memcmp(s, "Adobe", 5) == 0) adobe_none = (s[11] == 0);
+            break;
+        case 0xe1:  // APP1: Exif orientation, read in front of the first scan only (the reference skips the segment)
+            if (out.scans.empty() && !exif_seen) {
+                const int o = exif_orientation_of(s, (size_t)rem);
+                if (o != 0) exif_seen = true, out.orientation = o;
+            }
             break;
         case 0xeb:  // APP11: a piece of a JPEG XT box -- 'JP', enumerator, sequence number, LBox, TBox, payload (boxes/box.cpp:95-205)
             if (out.scans.empty() && rem >= 2 + 2 + 4 + 4 + 4 && s[0] == 'J' && s[1] == 'P') {

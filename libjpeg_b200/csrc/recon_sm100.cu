@@ -483,7 +483,7 @@ __device__ __forceinline__ uint32_t pack_sat4(int p0, int p1, int p2, int p3) {
 // frame's four b200jpg_plane descriptors at 4 * status_idx of the table b200jpg_batch_decode_into uploads; the float kinds
 // carry the conversion map next to the table pointer, as a launch argument
 template <int K>
-using StoreDst = std::conditional_t<K == kStoreCanvas, uint8_t *, std::conditional_t<(K >= kStorePlanarF), FloatDst, const b200jpg_plane *>>;
+using StoreDst = std::conditional_t<K == kStoreCanvas, uint8_t *, std::conditional_t<kFloatKind<K>, FloatDst, const b200jpg_plane *>>;
 
 __device__ __forceinline__ const b200jpg_plane *planes_of(const b200jpg_plane *p) { return p; }
 __device__ __forceinline__ const b200jpg_plane *planes_of(const FloatDst &d) { return d.planes; }
@@ -569,13 +569,169 @@ __device__ __forceinline__ void store_row8(const b200jpg_plane *p, uint8_t *o, u
 // converted for the float kinds
 template <int K, typename D>
 __device__ __forceinline__ void store_row(const D &out, int c, const b200jpg_plane *p, uint8_t *o, uint32_t w0, uint32_t w1, int xmax) {
-    if constexpr (K >= kStorePlanarF) {
+    if constexpr (kFloatKind<K>) {
         float y[8];
 #pragma unroll
         for (int x = 0; x < 8; x++) y[x] = convert_byte((x < 4) ? w0 : w1, x & 3, out.scale[c], out.bias[c]);
         store_row_f<K>(out.type, p, o, y, xmax);
     } else {
         store_row8<K>(p, o, w0, w1, xmax);
+    }
+}
+
+// ---- kStoreRuns / kStoreRunsF: the lane's block has been staged in its luma tile column -- line y of component c in the words
+// st[(8 y + 2 c) NT] and st[(8 y + 2 c + 1) NT], eight clamped 8-bit samples, sample 0 in the low byte -- and leaves here. Exif
+// orientations make the rewritten descriptors of a [N, C, H, W] tensor or of the packed slot contiguous along x in descending
+// order (mirrored rows) or along y in either order (transposed): such runs of eight samples leave as one vector store each.
+__device__ __forceinline__ uint32_t byte_of(uint32_t w, int k) { return (w >> (8 * k)) & 0xffu; }
+__device__ __forceinline__ uint32_t rev4(uint32_t w) { return __byte_perm(w, 0u, 0x0123u); }
+
+// eight samples in memory order (w0 | w1) at o, stride e: one 8-byte store when aligned
+__device__ __forceinline__ void put_run8(uint8_t *o, uint32_t w0, uint32_t w1) {
+    if ((reinterpret_cast<uintptr_t>(o) & 7u) == 0) {
+        *reinterpret_cast<uint2 *>(o) = make_uint2(w0, w1);
+        return;
+    }
+#pragma unroll
+    for (int k = 0; k < 8; k++) o[k] = (uint8_t)byte_of(k < 4 ? w0 : w1, k & 3);
+}
+// the same converted to float elements of `type`: 16-byte stores when aligned
+__device__ __forceinline__ void put_run_f(int type, uint8_t *o, uint32_t w0, uint32_t w1, float s, float b) {
+    float y[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) y[k] = convert_byte(k < 4 ? w0 : w1, k & 3, s, b);
+    const bool f32 = type == B200JPG_SAMPLE_F32;
+    if ((reinterpret_cast<uintptr_t>(o) & 15u) == 0) {
+        uint4 *o4 = reinterpret_cast<uint4 *>(o);
+        if (f32) {
+            o4[0] = make_uint4(__float_as_uint(y[0]), __float_as_uint(y[1]), __float_as_uint(y[2]), __float_as_uint(y[3]));
+            o4[1] = make_uint4(__float_as_uint(y[4]), __float_as_uint(y[5]), __float_as_uint(y[6]), __float_as_uint(y[7]));
+        } else {
+            o4[0] = make_uint4(pack2(type, y[0], y[1]), pack2(type, y[2], y[3]), pack2(type, y[4], y[5]), pack2(type, y[6], y[7]));
+        }
+        return;
+    }
+    const int e = f32 ? 4 : 2;
+#pragma unroll
+    for (int k = 0; k < 8; k++) store_elem(type, o + k * e, y[k]);
+}
+
+template <int K, typename D>
+__device__ __forceinline__ void put_run(const D &out, int c, uint8_t *o, uint32_t w0, uint32_t w1) {
+    if constexpr (K == kStoreRunsF) put_run_f(out.type, o, w0, w1, pick4(out.scale, c), pick4(out.bias, c));
+    else put_run8(o, w0, w1);
+}
+
+struct PlaneDesc {
+    uint64_t data;
+    int64_t bpp, bpr;
+};
+__device__ __forceinline__ PlaneDesc desc_of(const b200jpg_plane *p) {
+    PlaneDesc d;
+    int bpp;
+    asm volatile("ld.global.nc.u64 %0, [%1];" : "=l"(d.data) : "l"(&p->data));
+    asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(bpp) : "l"(&p->bytes_per_pixel));
+    asm volatile("ld.global.nc.u64 %0, [%1];" : "=l"(d.bpr) : "l"(&p->bytes_per_row));
+    d.bpp = bpp;
+    return d;
+}
+
+// column x (0..7) of component c, rows 0..3 and 4..7 of the staged block, row 0 in the low byte
+template <uint32_t NT>
+__device__ __forceinline__ void staged_column(const int *st, int c, int x, uint32_t &lo, uint32_t &hi) {
+    uint32_t w[8];
+#pragma unroll
+    for (int y = 0; y < 8; y++) w[y] = (uint32_t)st[(8 * y + 2 * c + (x >> 2)) * NT];
+    const uint32_t k = (uint32_t)(x & 3), sel = k | ((4u + k) << 4);  // bytes k of two words -> bytes 0, 1
+    lo = __byte_perm(__byte_perm(w[0], w[1], sel), __byte_perm(w[2], w[3], sel), 0x5410u);
+    hi = __byte_perm(__byte_perm(w[4], w[5], sel), __byte_perm(w[6], w[7], sel), 0x5410u);
+}
+
+// The store phase of kStoreRuns / kStoreRunsF for the valid lane's block at (X, Y), samples x <= xmax, y <= ymax
+template <int K, int NC, uint32_t NT, typename D>
+__device__ __forceinline__ void store_staged(const D &out, const b200jpg_plane *pl, const int *st, int X, int Y, int xmax, int ymax) {
+    int64_t e = 1;  // element size
+    if constexpr (K == kStoreRunsF) e = out.type == B200JPG_SAMPLE_F32 ? 4 : 2;
+    if constexpr (K == kStoreRuns && NC == 3) {
+        // the packed slot seen as an interleaved bitmap: three components one byte apart with one pair of strides
+        const PlaneDesc d0 = desc_of(pl), d1 = desc_of(pl + 1), d2 = desc_of(pl + 2);
+        const bool inter = d1.data == d0.data + 1 && d2.data == d0.data + 2 && d1.bpp == d0.bpp && d2.bpp == d0.bpp && d1.bpr == d0.bpr &&
+                           d2.bpr == d0.bpr;
+        const bool along_x = inter && (d0.bpp == 3 || d0.bpp == -3) && xmax == 7, along_y = inter && (d0.bpr == 3 || d0.bpr == -3) && ymax == 7;
+        if (along_x || along_y) {
+            // run j: line y = j (along x) or column x = j (along y); 24 bytes of eight pixels in memory order from the lowest one
+            const int64_t step = along_x ? d0.bpp : d0.bpr;
+            const int jmax = along_x ? ymax : xmax;
+#pragma unroll 1
+            for (int j = 0; j <= jmax; j++) {
+                uint32_t cl[3], ch[3];  // component c's eight samples of the run, in run order (k = 0 first)
+#pragma unroll
+                for (int c = 0; c < 3; c++) {
+                    if (along_x) cl[c] = (uint32_t)st[(8 * j + 2 * c) * NT], ch[c] = (uint32_t)st[(8 * j + 2 * c + 1) * NT];
+                    else staged_column<NT>(st, c, j, cl[c], ch[c]);
+                    if (step < 0) {
+                        const uint32_t t = rev4(cl[c]);
+                        cl[c] = rev4(ch[c]);
+                        ch[c] = t;
+                    }
+                }
+                uint32_t wd[6];
+#pragma unroll
+                for (int q = 0; q < 6; q++) {
+                    uint32_t v = 0;
+#pragma unroll
+                    for (int b = 0; b < 4; b++) {
+                        const int i = 4 * q + b, p = i / 3, c = i % 3;
+                        v |= byte_of(p < 4 ? cl[c] : ch[c], p & 3) << (8 * b);
+                    }
+                    wd[q] = v;
+                }
+                const int x = along_x ? (step < 0 ? 7 : 0) : j, y = along_x ? j : (step < 0 ? 7 : 0);
+                uint8_t *o = reinterpret_cast<uint8_t *>(d0.data + (uint64_t)((int64_t)(X + x) * d0.bpp) + (uint64_t)((int64_t)(Y + y) * d0.bpr));
+                if ((reinterpret_cast<uintptr_t>(o) & 7u) == 0) {
+                    uint2 *o2 = reinterpret_cast<uint2 *>(o);
+#pragma unroll
+                    for (int q = 0; q < 3; q++) o2[q] = make_uint2(wd[2 * q], wd[2 * q + 1]);
+                } else if ((reinterpret_cast<uintptr_t>(o) & 3u) == 0) {
+#pragma unroll
+                    for (int q = 0; q < 6; q++) reinterpret_cast<uint32_t *>(o)[q] = wd[q];
+                } else {
+#pragma unroll
+                    for (int i = 0; i < 24; i++) o[i] = (uint8_t)byte_of(wd[i >> 2], i & 3);
+                }
+            }
+            return;
+        }
+    }
+#pragma unroll 1
+    for (int c = 0; c < NC; c++) {
+        const PlaneDesc d = desc_of(pl + c);
+        auto at = [&](int x, int y) { return reinterpret_cast<uint8_t *>(d.data + (uint64_t)((int64_t)(X + x) * d.bpp) + (uint64_t)((int64_t)(Y + y) * d.bpr)); };
+        if ((d.bpp == e || d.bpp == -e) && xmax == 7) {  // rows are runs (mirrored: descending)
+#pragma unroll 1
+            for (int y = 0; y <= ymax; y++) {
+                const uint32_t w0 = (uint32_t)st[(8 * y + 2 * c) * NT], w1 = (uint32_t)st[(8 * y + 2 * c + 1) * NT];
+                if (d.bpp > 0) put_run<K>(out, c, at(0, y), w0, w1);
+                else put_run<K>(out, c, at(7, y), rev4(w1), rev4(w0));
+            }
+        } else if ((d.bpr == e || d.bpr == -e) && ymax == 7) {  // columns are runs (transposed)
+#pragma unroll 1
+            for (int x = 0; x <= xmax; x++) {
+                uint32_t lo, hi;
+                staged_column<NT>(st, c, x, lo, hi);
+                if (d.bpr > 0) put_run<K>(out, c, at(x, 0), lo, hi);
+                else put_run<K>(out, c, at(x, 7), rev4(hi), rev4(lo));
+            }
+        } else {  // partial blocks at the frame edge, or a layout without a contiguous axis: one store per sample
+#pragma unroll 1
+            for (int y = 0; y <= ymax; y++)
+#pragma unroll 1
+                for (int x = 0; x <= xmax; x++) {
+                    const uint32_t v = byte_of((uint32_t)st[(8 * y + 2 * c + (x >> 2)) * NT], x & 3);
+                    if constexpr (K == kStoreRunsF) store_elem(out.type, at(x, y), convert_bits(0x4B000000u | v, pick4(out.scale, c), pick4(out.bias, c)));
+                    else *at(x, y) = (uint8_t)v;
+                }
+        }
     }
 }
 
@@ -725,11 +881,16 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
         if (!valid) return;
 #pragma unroll 1
         for (int r = 0; r <= ymax; r++) {
-            uint8_t *o = (K == kStoreCanvas) ? obase + (uint64_t)r * opitch : plane_at(pl, X, Y + r);
+            uint8_t *o = (K == kStoreCanvas) ? obase + (uint64_t)r * opitch : ((K == kStoreRuns || K == kStoreRunsF) ? nullptr : plane_at(pl, X, Y + r));
             int px[8];
 #pragma unroll
             for (int x = 0; x < 8; x++) px[x] = WADD(my[(8 * r + x) * NT], 8) >> 4;
             const uint32_t w0 = pack_sat4(px[0], px[1], px[2], px[3]), w1 = pack_sat4(px[4], px[5], px[6], px[7]);
+            if constexpr (K == kStoreRuns || K == kStoreRunsF) {  // staged in the line's luma slots, which are consumed
+                my[(8 * r) * NT] = (int)w0;
+                my[(8 * r + 1) * NT] = (int)w1;
+                continue;
+            }
             if (K == kStoreCanvas) {
                 if (xmax == 7 && ((reinterpret_cast<uintptr_t>(o) & 7u) == 0)) {
                     *reinterpret_cast<uint2 *>(o) = make_uint2(w0, w1);
@@ -742,6 +903,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                 store_row<K>(out, 0, pl, o, w0, w1, xmax);
             }
         }
+        if constexpr (K == kStoreRuns || K == kStoreRunsF) store_staged<K, 1, NT>(out, pl, my, X, Y, xmax, ymax);
         return;
     }
 
@@ -870,7 +1032,12 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                     }
                 }
             }
-            if (K != kStoreCanvas) {
+            if constexpr (K == kStoreRuns || K == kStoreRunsF) {  // staged in the line's luma slots, which are consumed
+                if (valid) {
+#pragma unroll
+                    for (int k = 0; k < 6; k++) my[(8 * r + k) * NT] = (int)wd[k];
+                }
+            } else if (K != kStoreCanvas) {
                 if (valid) {
 #pragma unroll
                     for (int c = 0; c < 3; c++) store_row<K>(out, c, pl + c, plane_at(pl + c, X, Y + r), wd[2 * c], wd[2 * c + 1], xmax);
@@ -923,6 +1090,9 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
     if (!ycbcr) lines(std::integral_constant<int, 2>());
     else if (wide) lines(std::integral_constant<int, 1>());
     else lines(std::integral_constant<int, 0>());
+    if constexpr (K == kStoreRuns || K == kStoreRunsF) {
+        if (valid) store_staged<K, 3, NT>(out, pl, my, X, Y, xmax, ymax);
+    }
 }
 
 // grid (luma block columns / 32, luma block rows / 4, frames or kWideSlots)
@@ -1474,7 +1644,7 @@ template <int K>
 static StoreDst<K> dst_of(const ReconLaunch &l) {
     if constexpr (K == kStoreCanvas) {
         return l.out;
-    } else if constexpr (K >= kStorePlanarF) {
+    } else if constexpr (kFloatKind<K>) {
         FloatDst d{};
         d.planes = l.planes;
         d.type = l.convert->type;
@@ -1566,7 +1736,7 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
 
 template <int K>
 static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches) {
-    if (l.path == ReconPath::Generic || l.path == ReconPath::Scaled) return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : (K >= kStorePlanarF ? kStoreStridedF : kStoreStrided)>(l, s, launches);
+    if (l.path == ReconPath::Generic || l.path == ReconPath::Scaled) return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : (kFloatKind<K> ? kStoreStridedF : kStoreStrided)>(l, s, launches);
     if (l.path == ReconPath::Fused420) return launch_recon420<K>(l, s, launches);
     if (l.path == ReconPath::Scaled420) return launch_recon420_scaled<K>(l, s, launches);
     int n = 0;  // ReconPath::Tiled
@@ -1605,6 +1775,7 @@ static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches
 int launch_recon(const ReconLaunch &l, void *stream, int *launches) {
     cudaStream_t s = (cudaStream_t)stream;
     if (!l.planes) return launch_recon_kind<kStoreCanvas>(l, s, launches);
+    if (l.runs) return l.convert ? launch_recon_kind<kStoreRunsF>(l, s, launches) : launch_recon_kind<kStoreRuns>(l, s, launches);
     if (l.convert) return l.planar ? launch_recon_kind<kStorePlanarF>(l, s, launches) : launch_recon_kind<kStoreStridedF>(l, s, launches);
     if (l.planar) return launch_recon_kind<kStorePlanar>(l, s, launches);
     return launch_recon_kind<kStoreStrided>(l, s, launches);

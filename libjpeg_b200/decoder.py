@@ -64,6 +64,17 @@ def parse(data):
     return FrameInfo.from_struct(s)
 
 
+def exif_orientation(data):
+    """The Exif orientation 1..8 of one codestream (1 without a valid one), the value BatchDecoder(exif_orientation=True)
+    applies; host only, no GPU. Raises NativeError where parse() does."""
+    addr, n, keep = _as_buffer(data)
+    rc = lib.b200jpg_exif_orientation(addr, n)
+    del keep
+    if rc < 0:
+        native.check(rc)
+    return rc
+
+
 def component_shapes(info, upsample=True):
     """[(h, w)] of every component of a frame as the decoder writes it: the frame size, or without upsampling each
     component's own ceil(H / suby) x ceil(W / subx)."""
@@ -224,11 +235,17 @@ class Context:
 class BatchDecoder:
     """One batch of codestreams: parse + pack on construction, then upload() / decode() on a CUDA stream."""
 
-    def __init__(self, frames, device=-1, tolerate_bad=False, ctx=None, color_transform=True, upsample=True, downscale=1):
+    def __init__(self, frames, device=-1, tolerate_bad=False, ctx=None, color_transform=True, upsample=True, downscale=1,
+                 exif_orientation=False):
         """downscale = 2, 4 or 8 decodes every frame at ceil(W / k) x ceil(H / k) (B200JPG_FLAG_DOWNSCALE_k): each 8x8 block is
         inverse transformed straight to (8/k) x (8/k) samples, the k x k box average of its IDCT, and the rest of the
         reconstruction runs on the smaller frame. geometry(), frame_view() and plane_views() give the reduced sizes. Not to be
-        confused with the `scale` of decode_into, which maps sample values."""
+        confused with the `scale` of decode_into, which maps sample values.
+
+        exif_orientation=True (B200JPG_FLAG_EXIF_ORIENTATION) writes every frame as its Exif-oriented image, what PIL's
+        ImageOps.exif_transpose gives: mirrored and rotated in the reconstruction's store, width and height swapped for the
+        orientations 5..8. output_shape(), geometry(), frame_view(), plane_views() and the destinations of decode_into() are
+        then in oriented shapes. orientation(i) gives a frame's Exif value either way."""
         if isinstance(downscale, bool) or not isinstance(downscale, int) or downscale not in native.DOWNSCALE_FLAGS:
             raise ValueError("downscale must be 1, 2, 4 or 8, got %r" % (downscale,))
         self.ctx = ctx or Context(device)
@@ -248,6 +265,9 @@ class BatchDecoder:
         self.upsample = bool(upsample)
         self.downscale = downscale
         flags |= native.DOWNSCALE_FLAGS[downscale]
+        self.exif_orientation = bool(exif_orientation)
+        if exif_orientation:
+            flags |= native.FLAG_EXIF_ORIENTATION
         rc = lib.b200jpg_batch_create_ex(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, ctypes.byref(self.handle))
         native.check(rc, self.ctx.handle)
         self._keep = []  # the batch holds its own pinned copy
@@ -266,6 +286,10 @@ class BatchDecoder:
         w, h = ctypes.c_uint32(), ctypes.c_uint32()
         native.check(lib.b200jpg_batch_output_extent(self.handle, i, c, ctypes.byref(w), ctypes.byref(h)), self.ctx.handle)
         return h.value, w.value
+
+    def orientation(self, i):
+        """Frame i's Exif orientation 1..8, whether or not the batch applies it; the (negative) status of a frame that failed."""
+        return lib.b200jpg_batch_frame_orientation(self.handle, i)
 
     def _shape(self, i, c, fi):
         """output_shape, or for a frame that failed the shape its partial frame info gives (such a frame has no samples)"""
@@ -401,7 +425,8 @@ class BatchDecoder:
         return lib.b200jpg_batch_last_unstuff_ms(self.handle)
 
     def frame_view(self, out, i):
-        """Frame i of a decoded output tensor as [H, W, C] (H x W reduced by `downscale`)."""
+        """Frame i of a decoded output tensor as [H, W, C] (H x W reduced by `downscale`, swapped by an applied Exif orientation
+        5..8)."""
         fi = self.info(i)
         off = self.out_offset(i)
         h, w = self._shape(i, 0, fi)

@@ -39,6 +39,7 @@ class ConvertStruct(ctypes.Structure):
 SAMPLE_F32, SAMPLE_F16, SAMPLE_BF16 = 1, 2, 3
 FLAG_NO_COLOR_TRANSFORM, FLAG_NO_UPSAMPLE = 1, 2
 DOWNSCALE_FLAGS = {1: 0x0, 2: 0x4, 4: 0x8, 8: 0xC}  # B200JPG_FLAG_DOWNSCALE_k
+FLAG_EXIF_ORIENTATION = 0x10
 
 
 def library_path():
@@ -54,6 +55,7 @@ def _load():
     vp, u8p, u64, i32 = ctypes.c_void_p, ctypes.POINTER(ctypes.c_uint8), ctypes.c_uint64, ctypes.c_int
     sig = {
         "b200jpg_parse": (i32, [vp, ctypes.c_size_t, ctypes.POINTER(FrameInfoStruct)]),
+        "b200jpg_exif_orientation": (i32, [vp, ctypes.c_size_t]),
         "b200jpg_build_tables": (u64, [vp, ctypes.c_size_t, i32, vp, u64]),
         "b200jpg_create": (i32, [i32, ctypes.POINTER(vp)]),
         "b200jpg_destroy": (None, [vp]),
@@ -64,6 +66,7 @@ def _load():
         "b200jpg_batch_destroy": (None, [vp]),
         "b200jpg_batch_frame_info": (i32, [vp, i32, ctypes.POINTER(FrameInfoStruct)]),
         "b200jpg_batch_output_extent": (i32, [vp, i32, i32, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint32)]),
+        "b200jpg_batch_frame_orientation": (i32, [vp, i32]),
         "b200jpg_batch_out_offset": (u64, [vp, i32]),
         "b200jpg_batch_out_bytes": (u64, [vp, i32]),
         "b200jpg_batch_ecs_bytes": (u64, [vp]),
@@ -112,7 +115,7 @@ ABI_SYMBOLS = [
     "b200jpg_batch_reconstruct", "b200jpg_batch_frame_status", "b200jpg_batch_read_coefficients",
     "b200jpg_batch_last_launch_count", "b200jpg_batch_enable_timing", "b200jpg_batch_last_timing", "b200jpg_batch_last_unstuff_ms", "b200jpg_decode_to_host", "b200jpg_decode_to_host_ex", "b200jpg_decode_to_device_ex",
     "b200jpg_device_free", "b200jpg_device_copy_rect", "b200jpg_selftest_restartless", "b200jpg_selftest_restartless_items",
-    "b200jpg_selftest_table_cache", "b200jpg_microbench_int32",
+    "b200jpg_selftest_table_cache", "b200jpg_microbench_int32", "b200jpg_exif_orientation", "b200jpg_batch_frame_orientation",
 ]
 
 
