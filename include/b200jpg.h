@@ -139,10 +139,36 @@ B200JPG_API int b200jpg_batch_create(b200jpg_ctx *ctx, const uint8_t *const *fra
  * whose |bytes_per_row| exceeds INT32_MAX (it becomes that frame's pixel stride). b200jpg_batch_decode / b200jpg_batch_reconstruct
  * of a batch with oriented frames describe those frames' slots in a descriptor table like b200jpg_batch_decode_into's: each call
  * copies it to the device on the stream (one small H2D copy), and the host may wait for the copy issued three such calls earlier
- * before it reuses its pinned staging slot. Without oriented frames these calls stay as before: no copy, no host wait. */
+ * before it reuses its pinned staging slot. Without oriented (or cropped, b200jpg_batch_create_crop) frames these calls stay as
+ * before: no copy, no host wait. */
 #define B200JPG_FLAG_EXIF_ORIENTATION 0x10u
 B200JPG_API int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
                             unsigned flags, b200jpg_batch **batch);
+/* A rectangle of a frame's output: columns x .. x + width - 1, rows y .. y + height - 1. {0, 0, 0, 0} is the whole frame. */
+typedef struct b200jpg_rect {
+    uint32_t x, y, width, height;
+} b200jpg_rect;
+/* b200jpg_batch_create_ex with a crop per frame (no counterpart in the reference). Let O be what the batch writes for the caller's
+ * frame i without a crop, [H_o, W_o, C] after downscaling, colour transformation, clamp, Exif orientation and any float conversion
+ * (b200jpg_batch_output_extent of the batch without rects). With rects[i] = (x, y, width, height), given in those output coordinates
+ * (the composition is downscale -> orientation -> crop), frame i is written as exactly O[y : y + height, x : x + width], bit for
+ * bit, for every destination kind, and nothing outside that rectangle's destination is written. b200jpg_batch_output_extent,
+ * out_bytes / out_offset (the slot of a cropped frame holds width x height x C samples) and the descriptor rules of
+ * b200jpg_batch_decode_into(_ex) then describe the cropped image. Every scan of every frame is still decoded in full, and a frame's
+ * status is its status without the crop. The reconstruction runs only the tiles that cover the rectangle.
+ * rects == NULL, or every entry {0, 0, 0, 0}: exactly b200jpg_batch_create_ex. Otherwise, for every frame that parses (the rectangle of
+ * a frame that failed is ignored), a rectangle other than {0, 0, 0, 0} needs width >= 1, height >= 1, x + width <= W_o and
+ * y + height <= H_o (in 64 bits); one that breaks this fails the call with B200JPG_ERR_INVALID_PARAMETER, tolerate_bad or not, and
+ * the message names the frame. A rectangle together with B200JPG_FLAG_NO_UPSAMPLE is B200JPG_ERR_NOT_IMPLEMENTED for the call.
+ * b200jpg_batch_decode / b200jpg_batch_reconstruct of a batch with cropped frames describe those frames' slots like those of oriented
+ * frames: one small H2D copy per call (see B200JPG_FLAG_EXIF_ORIENTATION). */
+B200JPG_API int b200jpg_batch_create_crop(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
+                                          unsigned flags, const b200jpg_rect *rects, b200jpg_batch **batch);
+/* The uncropped output size W_o x H_o of one codestream under `flags` (B200JPG_FLAG_DOWNSCALE_k, and width and height swapped for
+ * the Exif orientations 5..8 with B200JPG_FLAG_EXIF_ORIENTATION; the frame size, B200JPG_FLAG_NO_UPSAMPLE or not): what the crop
+ * rectangles of b200jpg_batch_create_crop are checked against. Returns B200JPG_OK or the error code b200jpg_parse returns for it
+ * (B200JPG_ERR_INVALID_PARAMETER for a NULL width or height). Host only, no device. */
+B200JPG_API int b200jpg_output_size(const uint8_t *data, size_t len, unsigned flags, uint32_t *width, uint32_t *height);
 /* Waits for the work last enqueued for this batch (its buffers return to the context's pool for reuse by the
  * next batch; b200jpg_destroy frees the pool). The caller must have consumed `out_dev` before reusing it. */
 B200JPG_API void b200jpg_batch_destroy(b200jpg_batch *batch);

@@ -136,6 +136,7 @@ struct ReconGroup {
     uint32_t ncomp = 0, subx = 1, suby = 1;
     ReconPath path = ReconPath::Tiled;
     int orientation = 1;  // B200JPG_FLAG_EXIF_ORIENTATION: the frames' orientation; 2..8 store through rewritten descriptors
+    bool cropped = false; // b200jpg_batch_create_crop: the frames' tiles cover their rectangles, clipped stores (FrameRecon::clip_*)
     std::vector<FrameRecon> frames;
     uint32_t max_bw0 = 0, max_bh0 = 0, max_bwc = 0, max_bhc = 0;
     uint64_t dev_frames = 0;
@@ -162,10 +163,14 @@ struct Extent {
 // the factor k of B200JPG_FLAG_DOWNSCALE_k: 1, 2, 4 or 8
 uint32_t downscale_of(unsigned flags) { return 1u << ((flags & B200JPG_FLAG_DOWNSCALE_MASK) >> 2); }
 
+bool rect_empty(const b200jpg_rect &r) { return r.x == 0 && r.y == 0 && r.width == 0 && r.height == 0; }
+
 // component c as it leaves the decoder: the frame size W' x H' = ceil(W / k) x ceil(H / k), or without upsampling its own
 // ceil(W' / subx) x ceil(H' / suby); width and height swapped for the Exif orientations 5..8 (`orientation`: the one the frame
-// leaves with, 1 for the extent the kernels decode)
-Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags, int orientation) {
+// leaves with, 1 for the extent the kernels decode); the rectangle's size for a frame with a crop (`crop`, given in those output
+// coordinates and checked against them; never together with B200JPG_FLAG_NO_UPSAMPLE)
+Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags, int orientation, const b200jpg_rect *crop = nullptr) {
+    if (crop) return {crop->width, crop->height};
     const uint64_t k = downscale_of(flags);
     uint64_t w = (fi.width + k - 1) / k, h = (fi.height + k - 1) / k;
     if (flags & B200JPG_FLAG_NO_UPSAMPLE) w = (w + fi.subx[c] - 1) / fi.subx[c], h = (h + fi.suby[c] - 1) / fi.suby[c];
@@ -194,6 +199,35 @@ bool orient_plane(b200jpg_plane &pl, int o, uint64_t w, uint64_t h) {
     pl.bytes_per_pixel = (int32_t)np;
     pl.bytes_per_row = nr;
     return true;
+}
+
+// A destination of a cropped image (the rectangle r of the output) as the destination of the uncropped output: d - x p - y r, in
+// 64-bit integer arithmetic on the address. The kernels store only inside the clip rectangle (crop_to_decoded), so nothing is ever
+// written through it outside the caller's bitmap.
+void translate_plane(b200jpg_plane &pl, const b200jpg_rect &r) {
+    const uint64_t a = reinterpret_cast<uintptr_t>(pl.data) - (uint64_t)((int64_t)r.x * pl.bytes_per_pixel) - (uint64_t)((int64_t)r.y * pl.bytes_per_row);
+    pl.data = reinterpret_cast<void *>((uintptr_t)a);
+}
+
+// [x0, x1) x [y0, y1) in the decoded coordinates the kernels walk
+struct Clip {
+    uint32_t x0, y0, x1, y1;
+};
+// The rectangle r of the output image of orientation o as a rectangle of the decoded (downscaled, upright) image of extent w x h:
+// the inverse of the mapping orient_plane applies (output (u, v) = decoded (w-1-x, y) for 2, (y, x) for 5, ...)
+Clip crop_to_decoded(int o, const b200jpg_rect &r, uint64_t w, uint64_t h) {
+    const uint32_t W = (uint32_t)w, H = (uint32_t)h;
+    const uint32_t u0 = r.x, u1 = r.x + r.width, v0 = r.y, v1 = r.y + r.height;  // output columns / rows
+    switch (o) {
+    case 2: return {W - u1, v0, W - u0, v1};
+    case 3: return {W - u1, H - v1, W - u0, H - v0};
+    case 4: return {u0, H - v1, u1, H - v0};
+    case 5: return {v0, u0, v1, u1};
+    case 6: return {v0, H - u1, v1, H - u0};
+    case 7: return {W - v1, H - u1, W - v0, H - u0};
+    case 8: return {W - v1, u0, W - v0, u1};
+    default: return {u0, v0, u1, v1};
+    }
 }
 
 // body(i) for every frame i < n, on at most max_threads host threads
@@ -269,7 +303,9 @@ struct b200jpg_batch {
     b200jpg_plane *h_planes = nullptr, *d_planes = nullptr;
     cudaEvent_t ev_planes[kPlaneSlots] = {};
     int plane_slot = 0;
-    bool oriented = false;  // some live frame leaves with an Exif orientation other than 1: its group stores through descriptors
+    // some live frame leaves with an Exif orientation other than 1 or with a crop: its group stores through rewritten descriptors
+    bool rewritten = false;
+    std::vector<b200jpg_rect> crop;  // [n_user] b200jpg_batch_create_crop's rectangles, {0, 0, 0, 0}: the whole frame
     int last_launches = 0;
     bool timing = false;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // start, after a0, after a1, after b
@@ -280,6 +316,13 @@ struct b200jpg_batch {
 static int applied_orientation(const b200jpg_batch &b, int i) {
     if (!(b.flags & B200JPG_FLAG_EXIF_ORIENTATION)) return 1;
     return b.frames[b.xt_parent[i] >= 0 ? b.xt_parent[i] : i].orientation;
+}
+
+// the rectangle of the output frame i leaves as (a JPEG XT residual codestream: its frame's), nullptr for the whole frame
+static const b200jpg_rect *crop_of(const b200jpg_batch &b, int i) {
+    const int u = b.xt_parent[i] >= 0 ? b.xt_parent[i] : i;
+    if (b.crop.empty() || u >= b.n_user || rect_empty(b.crop[u])) return nullptr;
+    return &b.crop[u];
 }
 
 extern "C" {
@@ -377,6 +420,17 @@ int b200jpg_exif_orientation(const uint8_t *data, size_t len) {
     ParsedFrame pf;
     const int rc = parse_one(data, len, pf);
     return rc != 0 ? rc : pf.orientation;
+}
+
+int b200jpg_output_size(const uint8_t *data, size_t len, unsigned flags, uint32_t *width, uint32_t *height) {
+    if (!width || !height) return B200JPG_ERR_INVALID_PARAMETER;
+    ParsedFrame pf;
+    const int rc = parse_one(data, len, pf);
+    if (rc != 0) return rc;
+    const Extent e = out_extent(pf.info, 0, flags & ~B200JPG_FLAG_NO_UPSAMPLE, (flags & B200JPG_FLAG_EXIF_ORIENTATION) ? pf.orientation : 1);
+    *width = (uint32_t)e.w;
+    *height = (uint32_t)e.h;
+    return B200JPG_OK;
 }
 
 uint64_t b200jpg_build_tables(const uint8_t *data, size_t len, int scan, uint8_t *dst, uint64_t capacity) {
@@ -662,7 +716,7 @@ static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
                 sample_base[i][c] = sample_cur;
                 sample_cur += path == ReconPath::Scaled ? 64ull * ((fi.blocks_w[c] + k - 1) / k) * ((fi.blocks_h[c] + k - 1) / k) : elems;
             }
-            const Extent e = out_extent(fi, c, b.flags, 1);  // the components one after the other (w * h: any orientation)
+            const Extent e = out_extent(fi, c, b.flags, 1, crop_of(b, i));  // the components one after the other (w * h: any orientation)
             samples += e.w * e.h;
         }
         b.out_off[i] = out_cur;
@@ -883,10 +937,13 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         // oriented frames (B200JPG_FLAG_EXIF_ORIENTATION, 2..8) form groups of their own, one per orientation: their destinations
         // are rewritten descriptors, whose store kind is chosen per group
         const int orientation = applied_orientation(b, i);
-        if (orientation != 1) b.oriented = true;
+        // cropped frames too: their launches are sized by the tiles the rectangles cover, and they always store clipped
+        const b200jpg_rect *crop = crop_of(b, i);
+        if (orientation != 1 || crop) b.rewritten = true;
         ReconGroup *g = nullptr;
         for (auto &gg : b.groups)
-            if (gg.ncomp == fi.ncomp && gg.subx == sx && gg.suby == sy && gg.path == path && gg.orientation == orientation) g = &gg;
+            if (gg.ncomp == fi.ncomp && gg.subx == sx && gg.suby == sy && gg.path == path && gg.orientation == orientation && gg.cropped == (crop != nullptr))
+                g = &gg;
         if (!g) {
             b.groups.emplace_back();
             g = &b.groups.back();
@@ -895,6 +952,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
             g->suby = sy;
             g->path = path;
             g->orientation = orientation;
+            g->cropped = crop != nullptr;
         }
         FrameRecon fr{};
         const uint32_t k = downscale_of(b.flags);
@@ -935,13 +993,35 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         fr.ch = (uint32_t)(sy ? (reduced.h + sy - 1) / sy : reduced.h);
         fr.status_idx = (uint32_t)i;
         fr.precision = fi.precision;
+        if (crop) {
+            // the tiles of the path that cover the clip rectangle, from tile (tx0, ty0) on; the launch grid is sized by the largest
+            // such range of the group and every CTA runs tile (tx0 + bx, ty0 + by) exactly as the uncropped decode does
+            const Clip cl = crop_to_decoded(orientation, *crop, reduced.w, reduced.h);
+            const ReconTile t = recon_tile(path);
+            const uint32_t tw = 8 * t.bw, th = 8 * t.bh;
+            fr.clip_x0 = cl.x0, fr.clip_y0 = cl.y0, fr.clip_x1 = cl.x1, fr.clip_y1 = cl.y1;
+            fr.tx0 = cl.x0 / tw, fr.ty0 = cl.y0 / th;
+            const uint32_t ntx = (cl.x1 - 1) / tw - fr.tx0 + 1, nty = (cl.y1 - 1) / th - fr.ty0 + 1;
+            if (path == ReconPath::Tiled && fi.ncomp > 1) {
+                // b1: the chroma blocks under those tiles, one more on each side (the upsampling window), clipped to the plane
+                const int64_t cbx0 = (int64_t)fr.tx0 * t.bw / sx - 1, cby0 = (int64_t)fr.ty0 * t.bh / sy - 1;
+                const int64_t cbx1 = (int64_t)(fr.tx0 + ntx) * t.bw / sx + 1, cby1 = (int64_t)(fr.ty0 + nty) * t.bh / sy + 1;
+                fr.cb_x0 = (uint32_t)std::max<int64_t>(cbx0, 0), fr.cb_y0 = (uint32_t)std::max<int64_t>(cby0, 0);
+                fr.cb_x1 = (uint32_t)std::min<int64_t>(cbx1, fi.blocks_w[1]), fr.cb_y1 = (uint32_t)std::min<int64_t>(cby1, fi.blocks_h[1]);
+                g->max_bwc = std::max(g->max_bwc, fr.cb_x1 - fr.cb_x0);
+                g->max_bhc = std::max(g->max_bhc, fr.cb_y1 - fr.cb_y0);
+            }
+            g->max_bw0 = std::max(g->max_bw0, ntx * t.bw);
+            g->max_bh0 = std::max(g->max_bh0, nty * t.bh);
+        } else {
+            g->max_bw0 = std::max(g->max_bw0, (uint32_t)(reduced.w + 7) / 8);
+            g->max_bh0 = std::max(g->max_bh0, (uint32_t)(reduced.h + 7) / 8);
+        }
         g->frames.push_back(fr);
-        g->max_bw0 = std::max(g->max_bw0, (uint32_t)(reduced.w + 7) / 8);
-        g->max_bh0 = std::max(g->max_bh0, (uint32_t)(reduced.h + 7) / 8);
         if (generic) {  // the largest block grid of any component: the extent of the generic (or scaled) IDCT launch
             for (int c = 0; c < fi.ncomp; c++)
                 if ((uint64_t)fi.blocks_w[c] * fi.blocks_h[c] > (uint64_t)g->max_bwc * g->max_bhc) g->max_bwc = fi.blocks_w[c], g->max_bhc = fi.blocks_h[c];
-        } else if (fi.ncomp > 1) {
+        } else if (fi.ncomp > 1 && !crop) {  // (a cropped Tiled frame: its chroma block range above)
             g->max_bwc = std::max(g->max_bwc, fi.blocks_w[1]);
             g->max_bhc = std::max(g->max_bhc, fi.blocks_h[1]);
         }
@@ -1044,11 +1124,33 @@ static int stage_and_allocate(b200jpg_batch &b, const Codestreams &cs, const std
     return B200JPG_OK;
 }
 
+// b200jpg_batch_create_crop's rectangles: kept for the live frames (a failed frame's is ignored), each checked against the frame's
+// uncropped output extent; returns 0 or the status the call fails with
+static int admit_crops(b200jpg_batch &b, const b200jpg_rect *rects) {
+    b.crop.assign(rects, rects + b.n_user);
+    for (int i = 0; i < b.n_user; i++) {
+        b200jpg_rect &r = b.crop[i];
+        if (b.parse_status[i] != 0) r = b200jpg_rect{0, 0, 0, 0};
+        if (rect_empty(r)) continue;
+        const Extent e = out_extent(b.frames[i].info, 0, b.flags, applied_orientation(b, i));
+        if (r.width == 0 || r.height == 0 || (uint64_t)r.x + r.width > e.w || (uint64_t)r.y + r.height > e.h)
+            return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": crop rectangle (" + std::to_string(r.x) + ", " +
+                                                                  std::to_string(r.y) + ", " + std::to_string(r.width) + ", " + std::to_string(r.height) +
+                                                                  ") is empty or leaves the " + std::to_string(e.w) + " x " + std::to_string(e.h) + " output");
+    }
+    return B200JPG_OK;
+}
+
 static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
-                             b200jpg_batch **out) {
+                             const b200jpg_rect *rects, b200jpg_batch **out) {
     NvtxRange nvtx("b200jpg batch_create: parse + pack");
     if (!out || !frames || !lens || n <= 0) return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "invalid batch arguments");
     *out = nullptr;
+    bool any_crop = false;
+    for (int i = 0; rects && i < n; i++) any_crop = any_crop || !rect_empty(rects[i]);
+    if (!any_crop) rects = nullptr;  // all {0, 0, 0, 0}: exactly the batch of b200jpg_batch_create_ex
+    if (rects && (flags & B200JPG_FLAG_NO_UPSAMPLE))
+        return ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, "crop rectangles are not supported with B200JPG_FLAG_NO_UPSAMPLE");
     cudaError_t ce = cudaSetDevice(ctx->device);
     if (ce != cudaSuccess) return ctx->fail_cuda(ce, "cudaSetDevice");
 
@@ -1068,6 +1170,8 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
     attach_residuals(b, cs, device_index);
     std::vector<std::vector<TableSet>> frame_tables;
     if (int rc = admit_frames(b, cs, tolerate_bad != 0, frame_tables)) return rc;
+    if (rects)
+        if (int rc = admit_crops(b, rects)) return rc;
     const std::vector<uint64_t> byte_off = lay_out_codestreams(b, cs.len);
     const std::vector<std::array<uint64_t, 4>> sample_base = lay_out_planes(b);
     form_scan_classes(b, frame_tables, byte_off);
@@ -1087,9 +1191,14 @@ int b200jpg_batch_create(b200jpg_ctx *ctx, const uint8_t *const *frames, const s
 
 int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
                             b200jpg_batch **out) {
+    return b200jpg_batch_create_crop(ctx, frames, lens, n, tolerate_bad, flags, nullptr, out);
+}
+
+int b200jpg_batch_create_crop(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
+                              const b200jpg_rect *rects, b200jpg_batch **out) {
     if (!ctx) return B200JPG_ERR_INVALID_PARAMETER;
     try {  // no exception crosses the C ABI
-        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, out);
+        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, rects, out);
     } catch (const std::bad_alloc &) {
         if (out) *out = nullptr;
         return ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "out of host memory while preparing the batch");
@@ -1110,7 +1219,7 @@ int b200jpg_batch_output_extent(const b200jpg_batch *b, int i, int c, uint32_t *
     if (b->parse_status[i] != 0) return b->parse_status[i];
     const b200jpg_frame_info &fi = b->frames[i].info;
     if (c < 0 || c >= fi.ncomp) return B200JPG_ERR_INVALID_PARAMETER;
-    const Extent e = out_extent(fi, c, b->flags, applied_orientation(*b, i));
+    const Extent e = out_extent(fi, c, b->flags, applied_orientation(*b, i), crop_of(*b, i));
     *width = (uint32_t)e.w;
     *height = (uint32_t)e.h;
     return B200JPG_OK;
@@ -1364,26 +1473,30 @@ static int stage_planes(b200jpg_batch *b, void *stream, const std::function<void
     return B200JPG_OK;
 }
 
-// Frame i's destinations rewritten for its Exif orientation (orient_plane), in place; planar[i] cleared unless every component
-// then has bytes_per_pixel == size. Returns false when a pixel stride does not fit (only a caller's descriptor can do that).
-static bool orient_frame(const b200jpg_batch *b, int i, b200jpg_plane *pl, uint64_t size, std::vector<char> &planar) {
+// Frame i's destinations, described in its output coordinates, rewritten into the decoded coordinates the kernels walk, in place:
+// translated by its crop rectangle into the uncropped output (translate_plane), then oriented (orient_plane); planar[i] cleared
+// unless every component then has bytes_per_pixel == size. Returns false when a pixel stride does not fit (only a caller's
+// descriptor can do that).
+static bool rewrite_frame(const b200jpg_batch *b, int i, b200jpg_plane *pl, uint64_t size, std::vector<char> &planar) {
     const b200jpg_frame_info &fi = b->frames[i].info;
     const int o = applied_orientation(*b, i);
+    const b200jpg_rect *crop = crop_of(*b, i);
     for (int c = 0; c < fi.ncomp; c++) {
         const Extent d = out_extent(fi, c, b->flags, 1);
+        if (crop) translate_plane(pl[c], *crop);
         if (!orient_plane(pl[c], o, d.w, d.h)) return false;
         if ((uint64_t)pl[c].bytes_per_pixel != size) planar[(size_t)i] = 0;
     }
     return true;
 }
 
-// b200jpg_batch_decode of a batch with oriented frames: each such frame's packed slot in out_dev, seen as an interleaved bitmap of
-// the oriented extent (B200JPG_FLAG_NO_UPSAMPLE: plane after plane), rewritten for its orientation and staged like the table of
-// b200jpg_batch_decode_into. planar[i] as for that table.
+// b200jpg_batch_decode of a batch with oriented or cropped frames: each such frame's packed slot in out_dev, seen as an interleaved
+// bitmap of the oriented (cropped) extent (B200JPG_FLAG_NO_UPSAMPLE: plane after plane), rewritten for its crop and orientation and
+// staged like the table of b200jpg_batch_decode_into. planar[i] as for that table.
 static int stage_slot_planes(b200jpg_batch *b, uint8_t *out_dev, void *stream, std::vector<char> &planar) {
     return stage_planes(b, stream, [&](b200jpg_plane *table) {
         for (int i = 0; i < b->n_user; i++) {
-            if (b->parse_status[i] != 0 || applied_orientation(*b, i) == 1) continue;
+            if (b->parse_status[i] != 0 || (applied_orientation(*b, i) == 1 && !crop_of(*b, i))) continue;
             const b200jpg_frame_info &fi = b->frames[i].info;
             const int o = applied_orientation(*b, i);
             const int64_t size = fi.precision > 8 ? 2 : 1;
@@ -1391,13 +1504,13 @@ static int stage_slot_planes(b200jpg_batch *b, uint8_t *out_dev, void *stream, s
             uint64_t before = 0;
             b200jpg_plane *pl = table + 4 * (size_t)i;
             for (int c = 0; c < fi.ncomp; c++) {
-                const Extent e = out_extent(fi, c, b->flags, o);
+                const Extent e = out_extent(fi, c, b->flags, o, crop_of(*b, i));
                 pl[c].data = out_dev + b->out_off[i] + (planes ? before : (uint64_t)c) * size;
                 pl[c].bytes_per_pixel = (int32_t)(planes ? size : fi.ncomp * size);
                 pl[c].bytes_per_row = (int64_t)e.w * pl[c].bytes_per_pixel;
                 before += e.w * e.h;
             }
-            orient_frame(b, i, pl, (uint64_t)size, planar);  // a slot's row stride always fits the pixel stride
+            rewrite_frame(b, i, pl, (uint64_t)size, planar);  // a slot's row stride always fits the pixel stride
         }
     });
 }
@@ -1407,10 +1520,10 @@ static int stage_slot_planes(b200jpg_batch *b, uint8_t *out_dev, void *stream, s
 static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b200jpg_plane *planes_dev = nullptr,
                      const std::vector<char> *planar = nullptr, const b200jpg_convert *convert = nullptr) {
     NvtxRange nvtx("b200jpg reconstruction: IDCT + upsampling + colour");
-    // into the packed slots with oriented frames: those frames' slots as rewritten descriptors, built for this call's out_dev
+    // into the packed slots with oriented or cropped frames: those frames' slots as rewritten descriptors, built for this call's out_dev
     std::vector<char> slot_planar;
     const b200jpg_plane *slot_planes = nullptr;
-    if (!planes_dev && b->oriented) {
+    if (!planes_dev && b->rewritten) {
         slot_planar.assign((size_t)b->n, 1);
         if (int rc = stage_slot_planes(b, out_dev, stream, slot_planar)) return rc;
         slot_planes = b->d_planes;
@@ -1441,12 +1554,14 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.planes = planes_dev;
         l.convert = convert;
         const std::vector<char> *group_planar = planar;
-        if (slot_planes && g.orientation != 1) l.planes = slot_planes, group_planar = &slot_planar;
+        if (slot_planes && (g.orientation != 1 || g.cropped)) l.planes = slot_planes, group_planar = &slot_planar;
         l.planar = l.planes != nullptr;
         if (l.planes)
             for (const FrameRecon &fr : g.frames) l.planar = l.planar && (*group_planar)[fr.status_idx];
-        // oriented frames into anything but planar destinations: the staged store kinds, runs of eight samples along x or y
-        l.runs = g.orientation != 1 && l.planes && !l.planar;
+        // oriented frames into anything but planar destinations: the staged store kinds, runs of eight samples along x or y; cropped
+        // frames into any destination: the same kinds with the clip (the generic kernels: the strided kinds with the clip)
+        l.runs = (g.orientation != 1 || g.cropped) && l.planes && (!l.planar || g.cropped);
+        l.clip = g.cropped;
         int launches = 0;
         // grid.y carries the frame index: at most 65535 frames per launch. A generic group that is cut runs the IDCT of ALL its
         // frames first: a JPEG XT frame reads the planes of its residual frame, which may sit in another part
@@ -1521,8 +1636,8 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
                 return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "component " + std::to_string(c) + ": scale and bias must be finite");
     }
     std::vector<char> planar((size_t)b->n, 1);
-    // a batch with oriented frames: the table as staged, those frames' descriptors rewritten once here (orient_plane)
-    std::vector<b200jpg_plane> oriented(b->oriented ? 4 * (size_t)b->n_user : 0);
+    // a batch with oriented or cropped frames: the table as staged, those frames' descriptors rewritten once here (rewrite_frame)
+    std::vector<b200jpg_plane> rewritten(b->rewritten ? 4 * (size_t)b->n_user : 0);
     for (int i = 0; i < b->n_user; i++) {
         if (b->parse_status[i] != 0) continue;
         const b200jpg_frame_info &fi = b->frames[i].info;
@@ -1530,7 +1645,7 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
         const int orientation = applied_orientation(*b, i);
         for (int c = 0; c < fi.ncomp; c++) {
             const b200jpg_plane &p = planes[4 * i + c];
-            const auto [w, h] = out_extent(fi, c, b->flags, orientation);  // the rules hold in output coordinates
+            const auto [w, h] = out_extent(fi, c, b->flags, orientation, crop_of(*b, i));  // the rules hold in (cropped) output coordinates
             const uint64_t bpp = magnitude(p.bytes_per_pixel), bpr = magnitude(p.bytes_per_row);
             const std::string at = "frame " + std::to_string(i) + " component " + std::to_string(c) + ": ";
             if (!p.data) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "no destination");
@@ -1547,18 +1662,18 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
                 return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "not device memory of the batch's device");
             if ((uint64_t)p.bytes_per_pixel != size) planar[(size_t)i] = 0;
         }
-        if (b->oriented) {
-            b200jpg_plane *q = oriented.data() + 4 * (size_t)i;
+        if (b->rewritten) {
+            b200jpg_plane *q = rewritten.data() + 4 * (size_t)i;
             memcpy(q, planes + 4 * (size_t)i, sizeof(b200jpg_plane) * fi.ncomp);
-            if (orientation != 1) {  // the kernels store through the rewritten descriptors: planar is decided on those
+            if (orientation != 1 || crop_of(*b, i)) {  // the kernels store through the rewritten descriptors: planar is decided on those
                 planar[(size_t)i] = 1;
-                if (!orient_frame(b, i, q, size, planar))
+                if (!rewrite_frame(b, i, q, size, planar))
                     return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) +
                                                                            ": |bytes_per_row| does not fit the pixel stride of the transposed frame");
             }
         }
     }
-    const b200jpg_plane *src = b->oriented ? oriented.data() : planes;
+    const b200jpg_plane *src = b->rewritten ? rewritten.data() : planes;
     const int rc = stage_planes(b, stream, [&](b200jpg_plane *table) {
         for (int i = 0; i < b->n_user; i++)
             if (b->parse_status[i] == 0) memcpy(table + 4 * (size_t)i, src + 4 * (size_t)i, sizeof(b200jpg_plane) * b->frames[i].info.ncomp);

@@ -229,6 +229,25 @@ struct FrameRecon {       // per frame, for the reconstruction kernels
     // downscaled frames (ReconPath::Scaled / Scaled420): the coefficient block grid; bw / bh are then the grid of the reduced
     // sample planes, ceil(coef_bw / k) x ceil(coef_bh / k), and width / height the reduced frame
     uint32_t coef_bw[4], coef_bh[4];
+    // cropped frames (groups launched with the clip kinds): the CTA at grid position (bx, by) runs tile (tx0 + bx, ty0 + by) of
+    // the path's tile grid (recon_tile), and a sample (x, y) is stored only inside [clip_x0, clip_x1) x [clip_y0, clip_y1), in the
+    // decoded coordinates of width x height. ReconPath::Tiled: b1 computes only chroma blocks [cb_x0, cb_x1) x [cb_y0, cb_y1)
+    uint32_t tx0, ty0;
+    uint32_t clip_x0, clip_y0, clip_x1, clip_y1;
+    uint32_t cb_x0, cb_y0, cb_x1, cb_y1;
+};
+
+// The tiles of the reconstruction kernels, in luma blocks (8 x 8 samples of the decoded frame): reconstruct_kernel (b2) runs 32 x
+// kThreadsB / 32 blocks per CTA, reconstruct420_kernel and reconstruct420_scaled_kernel 32 x kRows420, generic_reconstruct_kernel
+// kGenericTileBlocks x 1
+constexpr int kThreadsB = 128;
+#ifndef B200JPG_R420_ROWS
+#define B200JPG_R420_ROWS 4
+#endif
+constexpr int kRows420 = B200JPG_R420_ROWS;
+constexpr int kGenericTileBlocks = 64;
+struct ReconTile {
+    uint32_t bw, bh;
 };
 
 // kernel launchers (huffman_sm100.cu, recon_sm100.cu). All asynchronous on `stream`.
@@ -270,6 +289,11 @@ int launch_progressive_dequant(const ProgFrame *frames_dev, uint32_t n_frames, u
 // then the generic kernels on a FrameRecon of the reduced width and height; Scaled420 (downscaled 8-bit 4:2:0 frames with
 // upsampling): reconstruct420_scaled_kernel, no planes
 enum class ReconPath : int { Tiled, Fused420, Generic, Scaled, Scaled420 };
+inline ReconTile recon_tile(ReconPath p) {
+    if (p == ReconPath::Fused420 || p == ReconPath::Scaled420) return {32, (uint32_t)kRows420};
+    if (p == ReconPath::Tiled) return {32, (uint32_t)kThreadsB / 32};
+    return {(uint32_t)kGenericTileBlocks, 1};
+}
 struct ReconLaunch {
     const FrameRecon *frames;  // device
     uint32_t n_frames;
@@ -291,7 +315,8 @@ struct ReconLaunch {
     // null: the packed slots of `out`
     const b200jpg_plane *planes;
     bool planar;                   // every plane of the group's frames has bytes_per_pixel == sample size (element size with `convert`)
-    bool runs;                     // a group of Exif-oriented frames that is not planar: kStoreRuns / kStoreRunsF
+    bool runs;                     // a group of Exif-oriented frames that is not planar, or of cropped frames: kStoreRuns / kStoreRunsF
+    bool clip;                     // a group of cropped frames: the kinds with kStoreClip, grid over the tiles the crops cover
     // b200jpg_batch_decode_into_ex: the samples leave as float32 / float16 / bfloat16 through this map (host memory, passed to
     // the kernels by value); null: as integers
     const b200jpg_convert *convert;
@@ -305,9 +330,15 @@ struct ReconLaunch {
 // kStoreRuns / kStoreRunsF (groups of Exif-oriented frames on the tiled 8-bit paths): the block is staged in the kernel's luma tile
 // and leaves as runs of eight contiguous samples along x (mirrored rows) or along y (transposed), in either direction, a packed
 // interleaved slot as 24-byte runs of pixels; whatever has no contiguous axis, one store per sample.
-enum StoreKind : int { kStoreCanvas = 0, kStorePlanar = 1, kStoreStrided = 2, kStorePlanarF = 3, kStoreStridedF = 4, kStoreRuns = 5, kStoreRunsF = 6 };
+// kStoreClip, or-ed into kStoreRuns / kStoreRunsF / kStoreStrided / kStoreStridedF (groups of cropped frames): the CTAs run the tiles
+// from FrameRecon::tx0 / ty0 on and store only inside the frame's clip rectangle; kBaseKind strips it.
+enum StoreKind : int { kStoreCanvas = 0, kStorePlanar = 1, kStoreStrided = 2, kStorePlanarF = 3, kStoreStridedF = 4, kStoreRuns = 5, kStoreRunsF = 6, kStoreClip = 8 };
 template <int k>
-constexpr bool kFloatKind = k == kStorePlanarF || k == kStoreStridedF || k == kStoreRunsF;
+constexpr int kBaseKind = k & ~kStoreClip;
+template <int k>
+constexpr bool kClipKind = (k & kStoreClip) != 0;
+template <int k>
+constexpr bool kFloatKind = kBaseKind<k> == kStorePlanarF || kBaseKind<k> == kStoreStridedF || kBaseKind<k> == kStoreRunsF;
 
 // the destination argument of the float kinds: the descriptors plus the map, both in the kernel's parameter bank
 struct FloatDst {

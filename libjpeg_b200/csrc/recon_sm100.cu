@@ -38,7 +38,6 @@
 namespace b200jpg {
 namespace {
 
-constexpr int kThreadsB = 128;
 constexpr int kWide = 65535;  // |sample| above this may overflow the 32-bit colour arithmetic -> 64-bit path
 
 #define WMUL(a, k) ((int)((unsigned)(a) * (unsigned)(int)(k)))
@@ -261,6 +260,26 @@ idct_planes_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restr
     }
 }
 
+// idct_planes_kernel for cropped frames: only the chroma blocks [cb_x0, cb_x1) x [cb_y0, cb_y1) that the frame's tiles read;
+// grid (range blocks / 128, frames or kWideSlots, components - 1)
+template <typename T, bool kListed>
+__global__ void __launch_bounds__(kThreadsB)
+idct_planes_crop_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, T *__restrict__ samples, uint32_t *__restrict__ flags,
+                        const uint32_t *__restrict__ list, int first_comp) {
+    const int c = first_comp + blockIdx.z;
+    const uint32_t t = blockIdx.x * kThreadsB + threadIdx.x;
+    auto one = [&](const FrameRecon &f) {
+        const uint32_t rw = f.cb_x1 - f.cb_x0, rh = f.cb_y1 - f.cb_y0;
+        if (c < (int)f.ncomp && t < rw * rh) idct_planes_block<T>(f, c, (f.cb_y0 + t / rw) * f.bw[c] + f.cb_x0 + t % rw, coef, samples, flags);
+    };
+    if (!kListed) {
+        one(frames[blockIdx.y]);
+    } else {
+        const uint32_t n = list[0];
+        for (uint32_t k = blockIdx.y; k < n; k += gridDim.y) one(frames[list[1 + k]]);
+    }
+}
+
 // ---- downscaled decoding (B200JPG_FLAG_DOWNSCALE_k): blocks -> (8/k) x (8/k) int32 samples -------------------------------
 // The k x k box average of the exact 8-point IDCT is, per dimension, the (8/k) x 8 matrix
 //     A_k(m, u) = 1/k sum_{j<k} C(u)/2 cos((2 (k m + j) + 1) u pi / 16),   C(0) = 1/sqrt(2), else 1
@@ -355,11 +374,8 @@ narrow_list_kernel(const FrameRecon *__restrict__ frames, uint32_t n_frames, con
 // b2's CTA). Its chroma window holds, per component, the kRows420 / 2 chroma block rows under the tile plus the line above and
 // the line below (kLines lines) and, per line, the 128 columns under the tile plus the column either side. Line l is chroma
 // line 4 kRows420 blockIdx.y - 1 + l, column i is chroma column 128 blockIdx.x - 4 + i: a lane's own four samples start at
-// i = 4 + 4 lane (an aligned 8- / 16-byte load), its left / right neighbour is i = 3 + 4 lane / 8 + 4 lane.
-#ifndef B200JPG_R420_ROWS
-#define B200JPG_R420_ROWS 4
-#endif
-constexpr int kRows420 = B200JPG_R420_ROWS;
+// i = 4 + 4 lane (an aligned 8- / 16-byte load), its left / right neighbour is i = 3 + 4 lane / 8 + 4 lane. (kRows420: internal.hpp,
+// which the planner shares. A cropped frame's CTA runs tile blockIdx + (tx0, ty0) in place of blockIdx: the same window.)
 constexpr int kThreads420 = 32 * kRows420;
 static_assert(kRows420 % 2 == 0 && kRows420 >= 4 && kRows420 <= 8, "whole chroma block rows, enough warps for phase 1, at most 8 warps");
 
@@ -618,7 +634,7 @@ __device__ __forceinline__ void put_run_f(int type, uint8_t *o, uint32_t w0, uin
 
 template <int K, typename D>
 __device__ __forceinline__ void put_run(const D &out, int c, uint8_t *o, uint32_t w0, uint32_t w1) {
-    if constexpr (K == kStoreRunsF) put_run_f(out.type, o, w0, w1, pick4(out.scale, c), pick4(out.bias, c));
+    if constexpr (kBaseKind<K> == kStoreRunsF) put_run_f(out.type, o, w0, w1, pick4(out.scale, c), pick4(out.bias, c));
     else put_run8(o, w0, w1);
 }
 
@@ -647,23 +663,27 @@ __device__ __forceinline__ void staged_column(const int *st, int c, int x, uint3
     hi = __byte_perm(__byte_perm(w[4], w[5], sel), __byte_perm(w[6], w[7], sel), 0x5410u);
 }
 
-// The store phase of kStoreRuns / kStoreRunsF for the valid lane's block at (X, Y), samples x <= xmax, y <= ymax
+// The store phase of kStoreRuns / kStoreRunsF for the valid lane's block at (X, Y), samples xmin <= x <= xmax, ymin <= y <= ymax
+// (xmin = ymin = 0 unless kClipKind<K>: a block cut by the crop's left or top edge). A run of eight leaves whole or not at all.
 template <int K, int NC, uint32_t NT, typename D>
-__device__ __forceinline__ void store_staged(const D &out, const b200jpg_plane *pl, const int *st, int X, int Y, int xmax, int ymax) {
+__device__ __forceinline__ void store_staged(const D &out, const b200jpg_plane *pl, const int *st, int X, int Y, int xmin, int xmax, int ymin, int ymax) {
+    constexpr int KB = kBaseKind<K>;
+    if constexpr (!kClipKind<K>) xmin = ymin = 0;
     int64_t e = 1;  // element size
-    if constexpr (K == kStoreRunsF) e = out.type == B200JPG_SAMPLE_F32 ? 4 : 2;
-    if constexpr (K == kStoreRuns && NC == 3) {
+    if constexpr (KB == kStoreRunsF) e = out.type == B200JPG_SAMPLE_F32 ? 4 : 2;
+    if constexpr (KB == kStoreRuns && NC == 3) {
         // the packed slot seen as an interleaved bitmap: three components one byte apart with one pair of strides
         const PlaneDesc d0 = desc_of(pl), d1 = desc_of(pl + 1), d2 = desc_of(pl + 2);
         const bool inter = d1.data == d0.data + 1 && d2.data == d0.data + 2 && d1.bpp == d0.bpp && d2.bpp == d0.bpp && d1.bpr == d0.bpr &&
                            d2.bpr == d0.bpr;
-        const bool along_x = inter && (d0.bpp == 3 || d0.bpp == -3) && xmax == 7, along_y = inter && (d0.bpr == 3 || d0.bpr == -3) && ymax == 7;
+        const bool along_x = inter && (d0.bpp == 3 || d0.bpp == -3) && xmin == 0 && xmax == 7,
+                   along_y = inter && (d0.bpr == 3 || d0.bpr == -3) && ymin == 0 && ymax == 7;
         if (along_x || along_y) {
             // run j: line y = j (along x) or column x = j (along y); 24 bytes of eight pixels in memory order from the lowest one
             const int64_t step = along_x ? d0.bpp : d0.bpr;
-            const int jmax = along_x ? ymax : xmax;
+            const int jmin = along_x ? ymin : xmin, jmax = along_x ? ymax : xmax;
 #pragma unroll 1
-            for (int j = 0; j <= jmax; j++) {
+            for (int j = jmin; j <= jmax; j++) {
                 uint32_t cl[3], ch[3];  // component c's eight samples of the run, in run order (k = 0 first)
 #pragma unroll
                 for (int c = 0; c < 3; c++) {
@@ -707,28 +727,28 @@ __device__ __forceinline__ void store_staged(const D &out, const b200jpg_plane *
     for (int c = 0; c < NC; c++) {
         const PlaneDesc d = desc_of(pl + c);
         auto at = [&](int x, int y) { return reinterpret_cast<uint8_t *>(d.data + (uint64_t)((int64_t)(X + x) * d.bpp) + (uint64_t)((int64_t)(Y + y) * d.bpr)); };
-        if ((d.bpp == e || d.bpp == -e) && xmax == 7) {  // rows are runs (mirrored: descending)
+        if ((d.bpp == e || d.bpp == -e) && xmin == 0 && xmax == 7) {  // rows are runs (mirrored: descending)
 #pragma unroll 1
-            for (int y = 0; y <= ymax; y++) {
+            for (int y = ymin; y <= ymax; y++) {
                 const uint32_t w0 = (uint32_t)st[(8 * y + 2 * c) * NT], w1 = (uint32_t)st[(8 * y + 2 * c + 1) * NT];
                 if (d.bpp > 0) put_run<K>(out, c, at(0, y), w0, w1);
                 else put_run<K>(out, c, at(7, y), rev4(w1), rev4(w0));
             }
-        } else if ((d.bpr == e || d.bpr == -e) && ymax == 7) {  // columns are runs (transposed)
+        } else if ((d.bpr == e || d.bpr == -e) && ymin == 0 && ymax == 7) {  // columns are runs (transposed)
 #pragma unroll 1
-            for (int x = 0; x <= xmax; x++) {
+            for (int x = xmin; x <= xmax; x++) {
                 uint32_t lo, hi;
                 staged_column<NT>(st, c, x, lo, hi);
                 if (d.bpr > 0) put_run<K>(out, c, at(x, 0), lo, hi);
                 else put_run<K>(out, c, at(x, 7), rev4(hi), rev4(lo));
             }
-        } else {  // partial blocks at the frame edge, or a layout without a contiguous axis: one store per sample
+        } else {  // partial blocks at the frame (or crop) edge, or a layout without a contiguous axis: one store per sample
 #pragma unroll 1
-            for (int y = 0; y <= ymax; y++)
+            for (int y = ymin; y <= ymax; y++)
 #pragma unroll 1
-                for (int x = 0; x <= xmax; x++) {
+                for (int x = xmin; x <= xmax; x++) {
                     const uint32_t v = byte_of((uint32_t)st[(8 * y + 2 * c + (x >> 2)) * NT], x & 3);
-                    if constexpr (K == kStoreRunsF) store_elem(out.type, at(x, y), convert_bits(0x4B000000u | v, pick4(out.scale, c), pick4(out.bias, c)));
+                    if constexpr (KB == kStoreRunsF) store_elem(out.type, at(x, y), convert_bits(0x4B000000u | v, pick4(out.scale, c), pick4(out.bias, c)));
                     else *at(x, y) = (uint8_t)v;
                 }
         }
@@ -770,12 +790,17 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                                                  uint32_t win, bool chroma_wide, StoreDst<K> __restrict__ out) {
     static_assert(!kWin || (NC == 3 && SX == 2 && SY == 2), "the chroma window is 4:2:0 only");
     constexpr uint32_t NT = kWin ? kThreads420 : kThreadsB;  // threads per CTA: the stride of the tile [coefficient][thread]
+    constexpr int KB = kBaseKind<K>;
+    constexpr bool kClip = kClipKind<K>;  // a cropped frame: tile (tx0, ty0) + blockIdx, stores inside the clip rectangle only
     const uint32_t W = f.width, H = f.height;
-    const uint32_t vbw = (W + 7) >> 3, vbh = (H + 7) >> 3;  // blocks that carry visible pixels
+    // blocks that carry visible pixels (cropped: pixels inside the clip rectangle)
+    const uint32_t vbw = ((kClip ? f.clip_x1 : W) + 7) >> 3, vbh = ((kClip ? f.clip_y1 : H) + 7) >> 3;
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t bx0 = blockIdx.x * 32, bx = bx0 + lane, by = blockIdx.y * (NT / 32) + warp;
+    const uint32_t tile_x = kClip ? f.tx0 + blockIdx.x : blockIdx.x, tile_y = kClip ? f.ty0 + blockIdx.y : blockIdx.y;
+    const uint32_t bx0 = tile_x * 32, bx = bx0 + lane, by = tile_y * (NT / 32) + warp;
     if (by >= vbh) return;  // whole warp
-    const bool valid = bx < vbw;
+    if (kClip && by < (f.clip_y0 >> 3)) return;
+    const bool valid = bx < vbw && (!kClip || bx >= (f.clip_x0 >> 3));
     const int X = 8 * (int)bx, Y = 8 * (int)by;
     int *my = ys + threadIdx.x;
 
@@ -869,29 +894,34 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
         }
     }
 
-    const int xmax = (X + 7 < (int)W) ? 7 : (int)((W - 1) & 7);
-    const int ymax = (Y + 7 < (int)H) ? 7 : (int)((H - 1) & 7);
+    int xmax = (X + 7 < (int)W) ? 7 : (int)((W - 1) & 7);
+    int ymax = (Y + 7 < (int)H) ? 7 : (int)((H - 1) & 7);
+    int xmin = 0, ymin = 0;
+    if constexpr (kClip) {
+        xmin = max((int)f.clip_x0 - X, 0), xmax = min((int)f.clip_x1 - 1 - X, 7);
+        ymin = max((int)f.clip_y0 - Y, 0), ymax = min((int)f.clip_y1 - 1 - Y, 7);
+    }
     const uint32_t opitch = W * NC;
     uint8_t *obase = nullptr;
     const b200jpg_plane *pl = nullptr;  // described kinds: the frame's component descriptors
-    if constexpr (K == kStoreCanvas) obase = out + f.out_base + (uint64_t)Y * opitch + (uint64_t)X * NC;
+    if constexpr (KB == kStoreCanvas) obase = out + f.out_base + (uint64_t)Y * opitch + (uint64_t)X * NC;
     else pl = planes_of(out) + 4u * f.status_idx;
 
     if (NC == 1) {  // identity, COLOR_TO_INT (numerics.hpp:69) + clamp
         if (!valid) return;
 #pragma unroll 1
         for (int r = 0; r <= ymax; r++) {
-            uint8_t *o = (K == kStoreCanvas) ? obase + (uint64_t)r * opitch : ((K == kStoreRuns || K == kStoreRunsF) ? nullptr : plane_at(pl, X, Y + r));
+            uint8_t *o = (KB == kStoreCanvas) ? obase + (uint64_t)r * opitch : ((KB == kStoreRuns || KB == kStoreRunsF) ? nullptr : plane_at(pl, X, Y + r));
             int px[8];
 #pragma unroll
             for (int x = 0; x < 8; x++) px[x] = WADD(my[(8 * r + x) * NT], 8) >> 4;
             const uint32_t w0 = pack_sat4(px[0], px[1], px[2], px[3]), w1 = pack_sat4(px[4], px[5], px[6], px[7]);
-            if constexpr (K == kStoreRuns || K == kStoreRunsF) {  // staged in the line's luma slots, which are consumed
+            if constexpr (KB == kStoreRuns || KB == kStoreRunsF) {  // staged in the line's luma slots, which are consumed
                 my[(8 * r) * NT] = (int)w0;
                 my[(8 * r + 1) * NT] = (int)w1;
                 continue;
             }
-            if (K == kStoreCanvas) {
+            if (KB == kStoreCanvas) {
                 if (xmax == 7 && ((reinterpret_cast<uintptr_t>(o) & 7u) == 0)) {
                     *reinterpret_cast<uint2 *>(o) = make_uint2(w0, w1);
                 } else {
@@ -903,7 +933,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                 store_row<K>(out, 0, pl, o, w0, w1, xmax);
             }
         }
-        if constexpr (K == kStoreRuns || K == kStoreRunsF) store_staged<K, 1, NT>(out, pl, my, X, Y, xmax, ymax);
+        if constexpr (KB == kStoreRuns || KB == kStoreRunsF) store_staged<K, 1, NT>(out, pl, my, X, Y, xmin, xmax, ymin, ymax);
         return;
     }
 
@@ -924,7 +954,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
     const bool fast = (bx0 + 32 <= vbw) && ((int)((bx0 + 32) * OWN) <= cw);
     const int xl = (cx0 > 0) ? cx0 : 0, xr = (cx0 + NW - 1 < cw) ? cx0 + NW - 1 : cw - 1;
     // chroma (line 0, column 0) of the shared-memory window (Window420)
-    const int wy0 = 4 * (int)(NT / 32) * (int)blockIdx.y - 1, wx0 = 128 * (int)blockIdx.x - 4;
+    const int wy0 = 4 * (int)(NT / 32) * (int)tile_y - 1, wx0 = 128 * (int)tile_x - 4;
     auto fetch = [&](int y, int (&d1)[NW], int (&d2)[NW]) {
         if (kWin) {
             using Wn = Window420<T>;
@@ -1021,7 +1051,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                     px[3 * x + 1] = G;
                     px[3 * x + 2] = B;
                 }
-                if (K == kStoreCanvas) {
+                if (KB == kStoreCanvas) {
 #pragma unroll
                     for (int k = 0; k < 6; k++) wd[k] = pack_sat4(px[4 * k], px[4 * k + 1], px[4 * k + 2], px[4 * k + 3]);
                 } else {  // component by component: wd[2 c], wd[2 c + 1] = the eight samples of component c
@@ -1032,12 +1062,12 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                     }
                 }
             }
-            if constexpr (K == kStoreRuns || K == kStoreRunsF) {  // staged in the line's luma slots, which are consumed
+            if constexpr (KB == kStoreRuns || KB == kStoreRunsF) {  // staged in the line's luma slots, which are consumed
                 if (valid) {
 #pragma unroll
                     for (int k = 0; k < 6; k++) my[(8 * r + k) * NT] = (int)wd[k];
                 }
-            } else if (K != kStoreCanvas) {
+            } else if (KB != kStoreCanvas) {
                 if (valid) {
 #pragma unroll
                     for (int c = 0; c < 3; c++) store_row<K>(out, c, pl + c, plane_at(pl + c, X, Y + r), wd[2 * c], wd[2 * c + 1], xmax);
@@ -1090,8 +1120,8 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
     if (!ycbcr) lines(std::integral_constant<int, 2>());
     else if (wide) lines(std::integral_constant<int, 1>());
     else lines(std::integral_constant<int, 0>());
-    if constexpr (K == kStoreRuns || K == kStoreRunsF) {
-        if (valid) store_staged<K, 3, NT>(out, pl, my, X, Y, xmax, ymax);
+    if constexpr (KB == kStoreRuns || KB == kStoreRunsF) {
+        if (valid) store_staged<K, 3, NT>(out, pl, my, X, Y, xmin, xmax, ymin, ymax);
     }
 }
 
@@ -1240,11 +1270,13 @@ __device__ __forceinline__ void reconstruct420_tile(const FrameRecon &f, int *ys
                                                     uint32_t *__restrict__ narrow_flags, StoreDst<K> __restrict__ out) {
     using Wn = Window420<T>;
     constexpr int kHalf = kRows420 / 2;  // chroma block rows under the tile
-    const uint32_t vbw = (f.width + 7) >> 3, vbh = (f.height + 7) >> 3;
-    if (blockIdx.x * 32u >= vbw || blockIdx.y * (uint32_t)kRows420 >= vbh) return;  // whole CTA
+    constexpr bool kClip = kClipKind<K>;  // a cropped frame: tile (tx0, ty0) + blockIdx, past the clip rectangle nothing
+    const uint32_t vbw = ((kClip ? f.clip_x1 : f.width) + 7) >> 3, vbh = ((kClip ? f.clip_y1 : f.height) + 7) >> 3;
+    const uint32_t tile_x = kClip ? f.tx0 + blockIdx.x : blockIdx.x, tile_y = kClip ? f.ty0 + blockIdx.y : blockIdx.y;
+    if (tile_x * 32u >= vbw || tile_y * (uint32_t)kRows420 >= vbh) return;  // whole CTA
     const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int bwc = (int)f.bw[1], bhc = (int)f.bh[1];
-    const int cbx0 = 16 * (int)blockIdx.x, cby0 = kHalf * (int)blockIdx.y;
+    const int cbx0 = 16 * (int)tile_x, cby0 = kHalf * (int)tile_y;
     auto at = [&](uint32_t comp, int line, int col) {
         return win + comp * (uint32_t)Wn::kCompBytes + (uint32_t)line * (uint32_t)Wn::kLineBytes + (uint32_t)col * (uint32_t)sizeof(T);
     };
@@ -1344,10 +1376,12 @@ reconstruct420_scaled_kernel(const FrameRecon *__restrict__ frames, const int16_
     int *ys = reinterpret_cast<int *>(smem420s);
     const uint32_t win = (uint32_t)__cvta_generic_to_shared(smem420s) + (uint32_t)Wn::kYsBytes;
     const FrameRecon &f = frames[blockIdx.z];
-    const uint32_t vbw = (f.width + 7) >> 3, vbh = (f.height + 7) >> 3;
-    if (blockIdx.x * 32u >= vbw || blockIdx.y * (uint32_t)kRows420 >= vbh) return;  // whole CTA
+    constexpr bool kClip = kClipKind<K>;  // a cropped frame: tile (tx0, ty0) + blockIdx, past the clip rectangle nothing
+    const uint32_t vbw = ((kClip ? f.clip_x1 : f.width) + 7) >> 3, vbh = ((kClip ? f.clip_y1 : f.height) + 7) >> 3;
+    const uint32_t tile_x = kClip ? f.tx0 + blockIdx.x : blockIdx.x, tile_y = kClip ? f.ty0 + blockIdx.y : blockIdx.y;
+    if (tile_x * 32u >= vbw || tile_y * (uint32_t)kRows420 >= vbh) return;  // whole CTA
     const int cw = (int)f.cw, ch = (int)f.ch;
-    const int wy0 = 4 * kRows420 * (int)blockIdx.y - 1, wx0 = 128 * (int)blockIdx.x - 4;  // window line 0 / column 0
+    const int wy0 = 4 * kRows420 * (int)tile_y - 1, wx0 = 128 * (int)tile_x - 4;  // window line 0 / column 0
     // the window positions that lie in the plane: lines y0..y1, columns x0..x1 (columns 3..132 of the window)
     const int y0 = max(wy0, 0), y1 = min(wy0 + Wn::kLines - 1, ch - 1), x0 = max(wx0 + 3, 0), x1 = min(wx0 + 132, cw - 1);
     int mn = 0, mx = 0;
@@ -1499,14 +1533,18 @@ __device__ void generic_upsample_block(const int32_t *__restrict__ plane, uint32
 }
 
 // grid (output block columns / 64, output block rows, frames). K: kStoreCanvas, or kStoreStrided / kStoreStridedF for every
-// described destination (this path stores one sample at a time anyway)
+// described destination (this path stores one sample at a time anyway); with kStoreClip (cropped frames) the grid covers the
+// tiles of kGenericTileBlocks x 1 blocks from (tx0, ty0) on, and only samples inside the clip rectangle are stored
 template <int K>
 __global__ void __launch_bounds__(64)
 generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restrict__ samples, StoreDst<K> __restrict__ out) {
+    constexpr int KB = kBaseKind<K>;
+    constexpr bool kClip = kClipKind<K>;
     const FrameRecon &f = frames[blockIdx.z];
     const uint32_t W = f.width, H = f.height, nc = f.ncomp;
-    const uint32_t bx = blockIdx.x * 64 + threadIdx.x, by = blockIdx.y;
+    const uint32_t bx = (kClip ? f.tx0 * kGenericTileBlocks : 0u) + blockIdx.x * 64 + threadIdx.x, by = (kClip ? f.ty0 : 0u) + blockIdx.y;
     if (bx >= (W + 7) / 8 || by >= (H + 7) / 8) return;
+    if (kClip && (bx < f.clip_x0 / 8 || bx >= (f.clip_x1 + 7) / 8 || by < f.clip_y0 / 8 || by >= (f.clip_y1 + 7) / 8)) return;
     const int X = 8 * (int)bx, Y = 8 * (int)by;
     // 64 upsampled samples per subsampled component (local memory: this path is not tuned); a component at full resolution is
     // read where it lies -- inside the image its sample plane IS the upsampled image
@@ -1519,7 +1557,11 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
         else generic_upsample_block(samples + f.sample_base[c], 8u * f.bw[c], w, h, sx, sy, X, Y, buf[c]);
     }
     auto base_at = [&](uint32_t c, int x, int y) -> int { return direct[c] ? direct[c][(uint64_t)y * (8u * f.bw[c]) + (uint32_t)x] : buf[c][8 * y + x]; };
-    const int xmax = (X + 7 < (int)W) ? 7 : (int)((W - 1) & 7), ymax = (Y + 7 < (int)H) ? 7 : (int)((H - 1) & 7);
+    int xmax = (X + 7 < (int)W) ? 7 : (int)((W - 1) & 7), ymax = (Y + 7 < (int)H) ? 7 : (int)((H - 1) & 7), xmin = 0, ymin = 0;
+    if constexpr (kClip) {
+        xmin = max((int)f.clip_x0 - X, 0), xmax = min((int)f.clip_x1 - 1 - X, xmax);
+        ymin = max((int)f.clip_y0 - Y, 0), ymax = min((int)f.clip_y1 - 1 - Y, ymax);
+    }
     if (f.xt & 1u) {
         // ---- JPEG XT (SURVEY 8f3): base image + residual image, YCbCrTrafo<..., Residual | Extended | ClampFlag, ...>::YCbCr2RGB
         // colortrafo/ycbcrtrafo.cpp:747-880 with the tables of the 8-bit integer profile (colortransformerfactory.cpp:300-352,
@@ -1535,10 +1577,10 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
         }
         auto res_at = [&](uint32_t c, int x, int y) -> int { return rdirect[c] ? rdirect[c][(uint64_t)y * (8u * f.res_bw[c]) + (uint32_t)x] : rbuf[c][8 * y + x]; };
         auto clamp_to = [](long long v, long long mx) { return v < 0 ? 0ll : (v > mx ? mx : v); };
-        for (int y = 0; y <= ymax; y++) {
+        for (int y = ymin; y <= ymax; y++) {
             uint8_t *o = nullptr;
-            if constexpr (K == kStoreCanvas) o = out + f.out_base + ((uint64_t)(Y + y) * W + (uint64_t)X) * nc;
-            for (int x = 0; x <= xmax; x++) {
+            if constexpr (KB == kStoreCanvas) o = out + f.out_base + ((uint64_t)(Y + y) * W + (uint64_t)X) * nc;
+            for (int x = xmin; x <= xmax; x++) {
                 const int i = 8 * y + x;
                 long long res[3] = {128, 128, 128}, v[3] = {0, 0, 0};
                 if (nc == 3 && (f.xt & 4u)) {  // the residual: Q table, R transformation (FIX_COLOR_TO_INTCOLOR), R2 table
@@ -1559,8 +1601,8 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
                 }
                 for (uint32_t c = 0; c < nc; c++) {  // merge and clamp (:863-878, :935-947)
                     const uint8_t m = (uint8_t)clamp_to(clamp_to(v[c], 255) + ((clamp_to(res[c], 4095) + 8) >> 4) - 128, 255);
-                    if constexpr (K == kStoreCanvas) o[nc * x + c] = m;
-                    else if constexpr (K == kStoreStridedF)
+                    if constexpr (KB == kStoreCanvas) o[nc * x + c] = m;
+                    else if constexpr (KB == kStoreStridedF)
                         store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, X + x, Y + y), convert_int(m, pick4(out.scale, c), pick4(out.bias, c)));
                     else *plane_at(out + 4u * f.status_idx + c, X + x, Y + y) = m;
                 }
@@ -1572,15 +1614,15 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
     // (what the reference writes into CTYP_UWORD bitmaps)
     const bool deep = f.precision > 8;
     const long long maxval = (1ll << f.precision) - 1, coff = 16ll << (f.precision - 1u);
-    for (int y = 0; y <= ymax; y++) {
+    for (int y = ymin; y <= ymax; y++) {
         const uint64_t at = ((uint64_t)(Y + y) * W + (uint64_t)X) * nc;
         uint8_t *o8 = nullptr;
         uint16_t *o16 = nullptr;
-        if constexpr (K == kStoreCanvas) {
+        if constexpr (KB == kStoreCanvas) {
             o8 = out + f.out_base + at;
             o16 = reinterpret_cast<uint16_t *>(out + f.out_base) + at;
         }
-        for (int x = 0; x <= xmax; x++) {
+        for (int x = xmin; x <= xmax; x++) {
             long long v[4];
             if (nc == 3 && f.ycbcr) {
                 const long long yv = base_at(0, x, y), cb = (long long)base_at(1, x, y) - coff, cr = (long long)base_at(2, x, y) - coff;
@@ -1592,10 +1634,10 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
             }
             for (uint32_t c = 0; c < nc; c++) {
                 const long long w = v[c] < 0 ? 0 : (v[c] > maxval ? maxval : v[c]);
-                if constexpr (K == kStoreCanvas) {
+                if constexpr (KB == kStoreCanvas) {
                     if (deep) o16[nc * x + c] = (uint16_t)w;
                     else o8[nc * x + c] = (uint8_t)w;
-                } else if constexpr (K == kStoreStridedF) {
+                } else if constexpr (KB == kStoreStridedF) {
                     store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, X + x, Y + y), convert_int((int)w, pick4(out.scale, c), pick4(out.bias, c)));
                 } else {
                     uint8_t *o = plane_at(out + 4u * f.status_idx + c, X + x, Y + y);
@@ -1724,11 +1766,14 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
         return (int)cudaGetLastError();
     }
     n++;
-    if (l.planes_out) {
-        const uint32_t gx = std::min<uint32_t>((l.max_bw0 * l.max_bh0 * 64u + 255u) / 256u, 4096u);
-        planes_out_kernel<K><<<dim3(gx, l.n_frames, l.ncomp), 256, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
+    if (l.planes_out) {  // never cropped (b200jpg_batch_create_crop refuses B200JPG_FLAG_NO_UPSAMPLE with a rectangle)
+        if constexpr (!kClipKind<K>) {
+            const uint32_t gx = std::min<uint32_t>((l.max_bw0 * l.max_bh0 * 64u + 255u) / 256u, 4096u);
+            planes_out_kernel<K><<<dim3(gx, l.n_frames, l.ncomp), 256, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
+        }
     } else {
-        generic_reconstruct_kernel<K><<<dim3((l.max_bw0 + 63) / 64, l.max_bh0, l.n_frames), 64, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
+        generic_reconstruct_kernel<K><<<dim3((l.max_bw0 + kGenericTileBlocks - 1) / kGenericTileBlocks, l.max_bh0, l.n_frames), 64, 0, s>>>(l.frames, l.samples32,
+                                                                                                                                     dst_of<K>(l));
     }
     if (launches) *launches = n;
     return (int)cudaGetLastError();
@@ -1736,7 +1781,8 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
 
 template <int K>
 static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches) {
-    if (l.path == ReconPath::Generic || l.path == ReconPath::Scaled) return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : (kFloatKind<K> ? kStoreStridedF : kStoreStrided)>(l, s, launches);
+    if (l.path == ReconPath::Generic || l.path == ReconPath::Scaled)
+        return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : ((kFloatKind<K> ? kStoreStridedF : kStoreStrided) | (K & kStoreClip))>(l, s, launches);
     if (l.path == ReconPath::Fused420) return launch_recon420<K>(l, s, launches);
     if (l.path == ReconPath::Scaled420) return launch_recon420_scaled<K>(l, s, launches);
     int n = 0;  // ReconPath::Tiled
@@ -1754,7 +1800,10 @@ static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches
         ReconLaunch c = l;
         c.frames = l.frames + f0;
         if (l.ncomp > 1) {
-            idct_planes_kernel<int16_t, false><<<dim3(cblocks, nf, l.ncomp - 1), kThreadsB, 0, s>>>(c.frames, l.coef, l.samples16, l.narrow_flags, nullptr, 1);
+            if constexpr (kClipKind<K>)  // cropped frames: the chroma blocks their tiles read (FrameRecon::cb_*)
+                idct_planes_crop_kernel<int16_t, false><<<dim3(cblocks, nf, l.ncomp - 1), kThreadsB, 0, s>>>(c.frames, l.coef, l.samples16, l.narrow_flags, nullptr, 1);
+            else
+                idct_planes_kernel<int16_t, false><<<dim3(cblocks, nf, l.ncomp - 1), kThreadsB, 0, s>>>(c.frames, l.coef, l.samples16, l.narrow_flags, nullptr, 1);
             n++;
         }
         launch_b2<int16_t, false, K>(c, dim3(gx, gy, nf), l.samples16, s);
@@ -1763,7 +1812,10 @@ static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches
     // the exact pass over the frames that were flagged `narrow` (none for real images: three near-empty launches)
     if (l.ncomp > 1) {
         narrow_list_kernel<<<1, 256, 0, s>>>(l.frames, l.n_frames, l.narrow_flags, l.narrow_list);
-        idct_planes_kernel<int32_t, true><<<dim3(cblocks, kWideSlots, l.ncomp - 1), kThreadsB, 0, s>>>(l.frames, l.coef, l.samples32, l.wide_flags, l.narrow_list, 1);
+        if constexpr (kClipKind<K>)  // the exact pass recomputes the same chroma blocks
+            idct_planes_crop_kernel<int32_t, true><<<dim3(cblocks, kWideSlots, l.ncomp - 1), kThreadsB, 0, s>>>(l.frames, l.coef, l.samples32, l.wide_flags, l.narrow_list, 1);
+        else
+            idct_planes_kernel<int32_t, true><<<dim3(cblocks, kWideSlots, l.ncomp - 1), kThreadsB, 0, s>>>(l.frames, l.coef, l.samples32, l.wide_flags, l.narrow_list, 1);
         launch_b2<int32_t, true, K>(l, dim3(gx, gy, kWideSlots), l.samples32, s);
         n += 3;
     }
@@ -1775,6 +1827,7 @@ static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches
 int launch_recon(const ReconLaunch &l, void *stream, int *launches) {
     cudaStream_t s = (cudaStream_t)stream;
     if (!l.planes) return launch_recon_kind<kStoreCanvas>(l, s, launches);
+    if (l.clip) return l.convert ? launch_recon_kind<kStoreRunsF | kStoreClip>(l, s, launches) : launch_recon_kind<kStoreRuns | kStoreClip>(l, s, launches);
     if (l.runs) return l.convert ? launch_recon_kind<kStoreRunsF>(l, s, launches) : launch_recon_kind<kStoreRuns>(l, s, launches);
     if (l.convert) return l.planar ? launch_recon_kind<kStorePlanarF>(l, s, launches) : launch_recon_kind<kStoreStridedF>(l, s, launches);
     if (l.planar) return launch_recon_kind<kStorePlanar>(l, s, launches);

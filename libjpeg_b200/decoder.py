@@ -75,6 +75,41 @@ def exif_orientation(data):
     return rc
 
 
+def output_size(data, downscale=1, exif_orientation=False):
+    """(h, w) of the whole output image of one codestream as BatchDecoder(frames, downscale=..., exif_orientation=...) writes it
+    without a crop: the frame size divided by `downscale` (rounded up), height and width swapped for the Exif orientations 5..8
+    when exif_orientation is set. The coordinates the `crop` rectangles of BatchDecoder are given in; host only, no GPU. Raises
+    NativeError where parse() does."""
+    if isinstance(downscale, bool) or not isinstance(downscale, int) or downscale not in native.DOWNSCALE_FLAGS:
+        raise ValueError("downscale must be 1, 2, 4 or 8, got %r" % (downscale,))
+    flags = native.DOWNSCALE_FLAGS[downscale] | (native.FLAG_EXIF_ORIENTATION if exif_orientation else 0)
+    addr, n, keep = _as_buffer(data)
+    w, h = ctypes.c_uint32(), ctypes.c_uint32()
+    rc = lib.b200jpg_output_size(addr, n, flags, ctypes.byref(w), ctypes.byref(h))
+    del keep
+    native.check(rc)
+    return h.value, w.value
+
+
+def crop_table(crop, n):
+    """The b200jpg_rect table of BatchDecoder(crop=...): n entries, each None (the whole frame) or (x, y, width, height) as
+    non-negative integers. Raises ValueError; the rectangles themselves are checked against the frames by the batch."""
+    import numbers
+    if len(crop) != n:
+        raise ValueError("crop: %d rectangles for %d frames" % (len(crop), n))
+    table = (native.RectStruct * n)()
+    for i, r in enumerate(crop):
+        if r is None:
+            continue
+        vals = tuple(r)
+        if len(vals) != 4 or any(isinstance(v, bool) or not isinstance(v, numbers.Integral) for v in vals):
+            raise ValueError("crop[%d]: expected None or four integers (x, y, width, height), got %r" % (i, r))
+        if any(v < 0 or v > 0xFFFFFFFF for v in vals):
+            raise ValueError("crop[%d]: x, y, width and height must be 0 .. 2**32 - 1, got %r" % (i, vals))
+        table[i].x, table[i].y, table[i].width, table[i].height = (int(v) for v in vals)
+    return table
+
+
 def component_shapes(info, upsample=True):
     """[(h, w)] of every component of a frame as the decoder writes it: the frame size, or without upsampling each
     component's own ceil(H / suby) x ceil(W / subx)."""
@@ -236,7 +271,7 @@ class BatchDecoder:
     """One batch of codestreams: parse + pack on construction, then upload() / decode() on a CUDA stream."""
 
     def __init__(self, frames, device=-1, tolerate_bad=False, ctx=None, color_transform=True, upsample=True, downscale=1,
-                 exif_orientation=False):
+                 exif_orientation=False, crop=None):
         """downscale = 2, 4 or 8 decodes every frame at ceil(W / k) x ceil(H / k) (B200JPG_FLAG_DOWNSCALE_k): each 8x8 block is
         inverse transformed straight to (8/k) x (8/k) samples, the k x k box average of its IDCT, and the rest of the
         reconstruction runs on the smaller frame. geometry(), frame_view() and plane_views() give the reduced sizes. Not to be
@@ -245,9 +280,19 @@ class BatchDecoder:
         exif_orientation=True (B200JPG_FLAG_EXIF_ORIENTATION) writes every frame as its Exif-oriented image, what PIL's
         ImageOps.exif_transpose gives: mirrored and rotated in the reconstruction's store, width and height swapped for the
         orientations 5..8. output_shape(), geometry(), frame_view(), plane_views() and the destinations of decode_into() are
-        then in oriented shapes. orientation(i) gives a frame's Exif value either way."""
+        then in oriented shapes. orientation(i) gives a frame's Exif value either way.
+
+        crop (b200jpg_batch_create_crop) is one entry per frame: None for the whole frame, or (x, y, width, height) -- the order
+        of b200jpg_rect -- a rectangle of the frame's output image after downscaling and Exif orientation (output_size() gives that
+        image's (h, w)). The frame is then written as exactly out[y:y + height, x:x + width] of its uncropped output, bit for bit,
+        and output_shape(), geometry(), frame_view() and the destinations of decode_into() are the rectangle's. Only the tiles
+        under the rectangle are reconstructed; every scan is still decoded, and status(i) is the frame's status without the
+        crop. A rectangle that is empty or leaves the frame raises NativeError (B200JPG_ERR_INVALID_PARAMETER), as does a
+        crop with upsample=False (B200JPG_ERR_NOT_IMPLEMENTED); a wrong length or an entry that is not four non-negative
+        integers raises ValueError."""
         if isinstance(downscale, bool) or not isinstance(downscale, int) or downscale not in native.DOWNSCALE_FLAGS:
             raise ValueError("downscale must be 1, 2, 4 or 8, got %r" % (downscale,))
+        rects = None if crop is None else crop_table(crop, len(frames))
         self.ctx = ctx or Context(device)
         self._keep = []
         n = len(frames)
@@ -268,7 +313,7 @@ class BatchDecoder:
         self.exif_orientation = bool(exif_orientation)
         if exif_orientation:
             flags |= native.FLAG_EXIF_ORIENTATION
-        rc = lib.b200jpg_batch_create_ex(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, ctypes.byref(self.handle))
+        rc = lib.b200jpg_batch_create_crop(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, rects, ctypes.byref(self.handle))
         native.check(rc, self.ctx.handle)
         self._keep = []  # the batch holds its own pinned copy
         self.n = n
@@ -282,7 +327,8 @@ class BatchDecoder:
 
     def output_shape(self, i, c):
         """(h, w) of component c of frame i as decode() / decode_into() write it: the frame size divided by `downscale`
-        (rounded up), or without upsampling the component's own size. Raises NativeError for a frame that failed."""
+        (rounded up), or without upsampling the component's own size; the rectangle's size for a cropped frame. Raises
+        NativeError for a frame that failed."""
         w, h = ctypes.c_uint32(), ctypes.c_uint32()
         native.check(lib.b200jpg_batch_output_extent(self.handle, i, c, ctypes.byref(w), ctypes.byref(h)), self.ctx.handle)
         return h.value, w.value
@@ -426,7 +472,7 @@ class BatchDecoder:
 
     def frame_view(self, out, i):
         """Frame i of a decoded output tensor as [H, W, C] (H x W reduced by `downscale`, swapped by an applied Exif orientation
-        5..8)."""
+        5..8, the rectangle's size for a cropped frame)."""
         fi = self.info(i)
         off = self.out_offset(i)
         h, w = self._shape(i, 0, fi)

@@ -36,6 +36,11 @@ class ConvertStruct(ctypes.Structure):
     _fields_ = [("type", ctypes.c_int32), ("scale", ctypes.c_float * 4), ("bias", ctypes.c_float * 4)]
 
 
+class RectStruct(ctypes.Structure):
+    """b200jpg_rect: a crop rectangle of b200jpg_batch_create_crop, in output coordinates; all zero = the whole frame."""
+    _fields_ = [("x", ctypes.c_uint32), ("y", ctypes.c_uint32), ("width", ctypes.c_uint32), ("height", ctypes.c_uint32)]
+
+
 SAMPLE_F32, SAMPLE_F16, SAMPLE_BF16 = 1, 2, 3
 FLAG_NO_COLOR_TRANSFORM, FLAG_NO_UPSAMPLE = 1, 2
 DOWNSCALE_FLAGS = {1: 0x0, 2: 0x4, 4: 0x8, 8: 0xC}  # B200JPG_FLAG_DOWNSCALE_k
@@ -56,6 +61,7 @@ def _load():
     sig = {
         "b200jpg_parse": (i32, [vp, ctypes.c_size_t, ctypes.POINTER(FrameInfoStruct)]),
         "b200jpg_exif_orientation": (i32, [vp, ctypes.c_size_t]),
+        "b200jpg_output_size": (i32, [vp, ctypes.c_size_t, ctypes.c_uint, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint32)]),
         "b200jpg_build_tables": (u64, [vp, ctypes.c_size_t, i32, vp, u64]),
         "b200jpg_create": (i32, [i32, ctypes.POINTER(vp)]),
         "b200jpg_destroy": (None, [vp]),
@@ -63,6 +69,8 @@ def _load():
         "b200jpg_last_error": (i32, [vp, ctypes.POINTER(ctypes.c_char_p)]),
         "b200jpg_batch_create": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.POINTER(vp)]),
         "b200jpg_batch_create_ex": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.c_uint, ctypes.POINTER(vp)]),
+        "b200jpg_batch_create_crop": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.c_uint,
+                                            ctypes.POINTER(RectStruct), ctypes.POINTER(vp)]),
         "b200jpg_batch_destroy": (None, [vp]),
         "b200jpg_batch_frame_info": (i32, [vp, i32, ctypes.POINTER(FrameInfoStruct)]),
         "b200jpg_batch_output_extent": (i32, [vp, i32, i32, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint32)]),
@@ -116,6 +124,7 @@ ABI_SYMBOLS = [
     "b200jpg_batch_last_launch_count", "b200jpg_batch_enable_timing", "b200jpg_batch_last_timing", "b200jpg_batch_last_unstuff_ms", "b200jpg_decode_to_host", "b200jpg_decode_to_host_ex", "b200jpg_decode_to_device_ex",
     "b200jpg_device_free", "b200jpg_device_copy_rect", "b200jpg_selftest_restartless", "b200jpg_selftest_restartless_items",
     "b200jpg_selftest_table_cache", "b200jpg_microbench_int32", "b200jpg_exif_orientation", "b200jpg_batch_frame_orientation",
+    "b200jpg_batch_create_crop", "b200jpg_output_size",
 ]
 
 
