@@ -621,10 +621,21 @@ static int admit_frames(b200jpg_batch &b, Codestreams &cs, bool tolerate_bad, st
             } else {
                 // A sequential frame codes a component at most once. A component no scan codes (the stream ends early: the
                 // reference just stops at the EOI / the end of the data, Frame::ParseTrailer marker/frame.cpp:1062-1092)
-                // keeps zero coefficients: the coefficient store is cleared for such batches.
+                // keeps zero coefficients: the coefficient store is cleared for such batches. So do the blocks a single-component
+                // scan leaves out: it codes the component's own block grid, ceil(ceil(W * h / hmax) / 8) x ceil(ceil(H * v / vmax)
+                // / 8) (T.81 A.2.2), which can be smaller than the MCU-padded grid the store keeps (Y 3 x 3 next to 1 x 1 chroma,
+                // 517 pixels wide: 65 of 66 block columns).
                 int seen[4] = {0, 0, 0, 0};
-                for (auto &sc : pf.scans)
+                uint32_t hmax = 1, vmax = 1;
+                for (int c = 0; c < fi.ncomp; c++) hmax = std::max<uint32_t>(hmax, fi.hs[c]), vmax = std::max<uint32_t>(vmax, fi.vs[c]);
+                for (auto &sc : pf.scans) {
                     for (int k = 0; k < sc.ns; k++) seen[sc.comp[k]]++;
+                    if (sc.ns == 1) {
+                        const int c = sc.comp[0];
+                        const uint32_t own_w = ((fi.width * fi.hs[c] + hmax - 1) / hmax + 7) / 8, own_h = ((fi.height * fi.vs[c] + vmax - 1) / vmax + 7) / 8;
+                        if (own_w < fi.blocks_w[c] || own_h < fi.blocks_h[c]) b.clear_coef = true;
+                    }
+                }
                 for (int c = 0; c < fi.ncomp; c++) {
                     if (fi.frame_type != 2 && seen[c] > 1) {
                         st = B200JPG_ERR_NOT_IMPLEMENTED;

@@ -171,9 +171,13 @@ __device__ __forceinline__ void idct8t(int &v0, int &v1, int &v2, int &v3, int &
 }
 
 // eight dequantised int16 coefficients -> ints WITHOUT the << 4 preshift of dct/idct.cpp:105. The row pass is linear in front
-// of its rounding shift, so with inputs 16 times smaller ((16 x + 256) >> 9) == ((x + 16) >> 5) for every integer x; the
-// reference's int32 arithmetic cannot wrap in this pass for coefficients that fit int16 (|16 x| <= 16 * 3825 * (32768 + 1024)
-// < 2^31), so nothing is lost by never forming 16 x.
+// of its rounding shift, so with inputs 16 times smaller ((16 x + 256) >> 9) == ((x + 16) >> 5) for every integer x. The
+// reference's int32 arithmetic cannot wrap in this pass: the absolute weights of every output sum to 3825 (the DC's is 512),
+// so for coefficients within +-32767 no sum exceeds 16 (3825 * 32767 + 512 * (dcoffset << 3)) + 256, which is 2,013,729,264
+// for 8 bit (dcoffset << 3 = 1024) and 2,139,558,384 for 12 bit (16384); a row of DC 32767 and ACs of 32767 with the signs of
+// one output's weights reaches it (tests/recon_cases.py, rowmax_8 / rowmax_12). A dequantised -32768 where a weight is
+// negative adds at most 16 * 2434: 2,013,768,208 and 2,139,597,328 (0.4 % below 2^31). So nothing is lost by never forming
+// 16 x.
 __device__ __forceinline__ void unpack_row_raw(const uint4 q, int (&v)[8]) {
     v[0] = (int)(short)(q.x & 0xffffu);
     v[1] = (int)q.x >> 16;

@@ -10,7 +10,7 @@ import pytest
 
 from tests import recon420_cases as rc
 from tests.test_decode_convert_cpu import convert
-from tests.test_decode_into import GOLDEN, SETS, _read, _reference, _set
+from tests.test_decode_into import GOLDEN, SETS, _read, _recon_case_batches, _reference, _set
 
 pytestmark = pytest.mark.gpu
 
@@ -240,6 +240,16 @@ def test_recon420_cases_through_the_float_stores(built, ctx, dt):
     for name in ("nchw", "channels_last", "bottom_up"):
         _roundtrip(dec, refs, launches, LAYOUTS[name], _dtypes()[dt], "recon420/%s/%s" % (dt, name))
     _roundtrip(dec, refs, launches, layout_unaligned, _dtypes()[dt], "recon420/%s/unaligned" % dt)
+
+
+@pytest.mark.parametrize("dt", ["f32", "f16", "bf16"])
+def test_recon_cases_through_the_float_stores(built, ctx, dt):
+    """the Tiled, Generic and wrapping-IDCT cases of tests/recon_cases.py (8- and 12-bit batches) through both float kinds"""
+    for k, frames in enumerate(_recon_case_batches()):
+        dec = _batch(built, ctx, frames)
+        refs, launches = _reference(dec)
+        for name in ("nchw", "channels_last", "bottom_up"):
+            _roundtrip(dec, refs, launches, LAYOUTS[name], _dtypes()[dt], "recon/%d/%s/%s" % (k, dt, name))
 
 
 @pytest.mark.parametrize("dt", ["f32", "f16", "bf16"])

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from tests import recon420_cases as rc
+from tests import recon_cases
 
 pytestmark = pytest.mark.gpu
 
@@ -264,6 +265,23 @@ def test_recon420_cases_through_the_new_stores(built, ctx, layout):
     refs, launches = _reference(dec)
     _roundtrip(dec, refs, layout, "recon420/%s" % layout)
     assert dec.launches == launches
+
+
+def _recon_case_batches():
+    """the cases of tests/recon_cases.py in two batches: 8-bit frames (Tiled, Fused420, Generic) and 12-bit frames"""
+    names = recon_cases.NAMES
+    return [[recon_cases.case(n)[1] for n in names if recon_cases.case(n)[0].precision == p] for p in (8, 12)]
+
+
+@pytest.mark.parametrize("layout", ["nchw", "odd", "bottom_up"])
+def test_recon_cases_through_the_new_stores(built, ctx, layout):
+    """tile seams, the `narrow` exact pass, 64-bit colour, the generic layouts and wrapping IDCTs of tests/recon_cases.py
+    through the planar and the strided kinds"""
+    for k, frames in enumerate(_recon_case_batches()):
+        dec = _batch(built, ctx, frames)
+        refs, launches = _reference(dec)
+        _roundtrip(dec, refs, layout, "recon/%d/%s" % (k, layout))
+        assert dec.launches == launches
 
 
 @pytest.mark.parametrize("kw", [{"upsample": False}, {"color_transform": False}])

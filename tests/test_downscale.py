@@ -8,6 +8,7 @@ import pytest
 
 from tests import downscale_model as dm
 from tests import recon420_cases as rc
+from tests import recon_cases
 from tests import spec_cases as sc
 from tests.test_decode_into import GOLDEN, SETS, _read, _set
 
@@ -19,6 +20,7 @@ DOWN_SETS = {name: fn for name, fn in SETS.items() if name != "xt"}
 DOWN_SETS["noeoi"] = lambda: _set("noeoi")
 DOWN_SETS["reference"] = lambda: [_read(p) for p in sorted(glob.glob(os.path.join(GOLDEN, "reference", "sub_*.jpg")))]
 DOWN_SETS["restartless"] = lambda: [sc.case(n)[1] for n in sc.NAMES]
+DOWN_SETS["recon"] = lambda: [recon_cases.case(n)[1] for n in recon_cases.NAMES]
 
 
 @pytest.fixture(scope="module")

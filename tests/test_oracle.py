@@ -92,6 +92,9 @@ def reference_cases():
     from tests import recon420_cases
     for name in recon420_cases.NAMES:
         yield "recon420[%s]" % name, recon420_cases.case(name)[1]
+    from tests import recon_cases
+    for name in recon_cases.NAMES:
+        yield "recon[%s]" % name, recon_cases.case(name)[1]
 
 
 def check_reference(key, data, rc, px):
@@ -326,6 +329,23 @@ def test_oracle_matches_reference_on_hand_built_reconstruction_frames(oracle, na
     data = recon420_cases.case(name)[1]
     rc, px = oracle.decode(data)
     check_reference("recon420[%s]" % name, data, rc, px)
+
+
+def _recon_case_names():
+    from tests import recon_cases
+    return recon_cases.NAMES
+
+
+@pytest.mark.parametrize("name", _recon_case_names())
+def test_oracle_matches_reference_on_hand_built_tiled_and_generic_frames(oracle, name):
+    """Frames of the test writer aimed at the Tiled and Generic reconstruction and at the IDCT's 32-bit limits
+    (tests/recon_cases.py: tile seams, size sweeps, the int16 edge, 64-bit colour through a neighbour, factors 3 and 4, two and
+    four components, 12 bit, row-pass maxima, wrapping column passes): the reference's samples."""
+    from tests import recon_cases
+    data = recon_cases.case(name)[1]
+    ret, s = oracle.info(data)
+    rc, px = oracle.decode16(data) if s.precision > 8 else oracle.decode(data)
+    check_reference("recon[%s]" % name, data, rc, px)
 
 
 @pytest.mark.parametrize("name", NO_COLOR_TRANSFORM)

@@ -10,6 +10,7 @@ import pytest
 
 from tests import orientation_model as om
 from tests import recon420_cases as rc
+from tests import recon_cases
 from tests import spec_cases as sc
 from tests.test_decode_into import GOLDEN, SETS, _read
 
@@ -20,6 +21,7 @@ ORIENT_SETS = dict(SETS)
 ORIENT_SETS["reference"] = lambda: [_read(p) for p in sorted(glob.glob(os.path.join(GOLDEN, "reference", "sub_*.jpg")))]
 ORIENT_SETS["restartless"] = lambda: [sc.case(n)[1] for n in sc.NAMES]
 ORIENT_SETS["recon420"] = lambda: [rc.case(n)[1] for n in rc.NAMES]
+ORIENT_SETS["recon"] = lambda: [recon_cases.case(n)[1] for n in recon_cases.NAMES]
 
 
 def _synth(w, h, seed, sub=(2, 2), q=80, restart=0):
