@@ -164,6 +164,48 @@ typedef struct b200jpg_rect {
  * frames: one small H2D copy per call (see B200JPG_FLAG_EXIF_ORIENTATION). */
 B200JPG_API int b200jpg_batch_create_crop(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
                                           unsigned flags, const b200jpg_rect *rects, b200jpg_batch **batch);
+/* A target size of b200jpg_batch_create_resize. {0, 0}: the frame is not resized. */
+typedef struct b200jpg_size {
+    uint32_t width, height;
+} b200jpg_size;
+/* The filters of b200jpg_batch_create_resize, with the values of PIL's Image.Resampling (NEAREST, 0, is not one of them). */
+#define B200JPG_RESAMPLE_LANCZOS 1
+#define B200JPG_RESAMPLE_BILINEAR 2
+#define B200JPG_RESAMPLE_BICUBIC 3
+#define B200JPG_RESAMPLE_BOX 4
+#define B200JPG_RESAMPLE_HAMMING 5
+/* b200jpg_batch_create_crop with a target size per frame (no counterpart in the reference). Let C be what the batch writes for the
+ * caller's frame i without a size: O[y : y + height, x : x + width] of b200jpg_batch_create_crop (O itself without a rectangle),
+ * uint8, [h, w, ncomp]. With sizes[i] = {W_t, H_t}, frame i is written as R(C), bit for bit, where R is Pillow's convolution
+ * resampler, Image.resize((W_t, H_t), resample) of a mode L / RGB / CMYK image (box=None, reducing_gap=None), applied to every
+ * channel on its own: horizontal pass over the rows the vertical table touches, then vertical pass, in Pillow's 22-bit fixed
+ * point; an axis whose size does not change is not resampled (DESIGN §13 states R exactly, including the one case where Pillow
+ * runs the passes the other way round). A float destination of b200jpg_batch_decode_into_ex receives R(C) converted by its map:
+ * the resize comes first. The composition is downscale -> orientation -> crop -> resize.
+ * b200jpg_batch_output_extent, out_bytes / out_offset (the slot of a resized frame holds W_t x H_t x ncomp samples) and the
+ * descriptor rules of b200jpg_batch_decode_into(_ex) then describe W_t x H_t, so one [N, C, H_t, W_t] tensor takes frames of any
+ * size. A frame's status is its status without the size. Upscaling is allowed; a size too large to allocate is
+ * B200JPG_ERR_OUT_OF_MEMORY (as is a side above 2^24 or W_t x H_t x ncomp above 2^34 bytes). The reconstruction writes C into a
+ * scratch the batch owns, resized frames in reconstruction groups of their own, and two launches (two per 65535 resized frames)
+ * resample it: a batch whose frames are all resized issues the launches of the same batch of b200jpg_batch_create_crop, with a
+ * rectangle covering the whole output for a frame that has none, plus those two.
+ * sizes == NULL, or every entry {0, 0}: exactly b200jpg_batch_create_crop (resample is then not looked at). Otherwise
+ * B200JPG_ERR_INVALID_PARAMETER for the call, tolerate_bad or not, with the frame named in the message: a size with exactly one
+ * zero field, or an unknown `resample`. A size together with B200JPG_FLAG_NO_UPSAMPLE is B200JPG_ERR_NOT_IMPLEMENTED for the call.
+ * A 12-bit frame with a size has the status B200JPG_ERR_NOT_IMPLEMENTED: it fails the call, or with tolerate_bad it is skipped; it
+ * is never written unresized. The size of a frame that fails to parse is ignored; a JPEG XT frame's residual codestream takes its
+ * frame's size. b200jpg_batch_decode / b200jpg_batch_reconstruct of a batch with resized frames describe their slots like those of
+ * cropped frames: one small H2D copy per call (see B200JPG_FLAG_EXIF_ORIENTATION). */
+B200JPG_API int b200jpg_batch_create_resize(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
+                                            unsigned flags, const b200jpg_rect *rects, const b200jpg_size *sizes, int resample,
+                                            b200jpg_batch **batch);
+/* The fixed-point tables b200jpg_batch_create_resize uses to resample one axis of in_size samples to out_size (tests only, host
+ * only, no device): bounds[2 j] is the first source index and bounds[2 j + 1] the number of taps of output j, coeffs[j * ksize + t]
+ * the int32 coefficient of tap t (zero behind the taps). *ksize receives the row length. The tables are written when bounds and
+ * coeffs are both non-NULL: bounds needs 2 * out_size entries and coeffs `capacity` >= out_size * ksize entries, else the call
+ * returns B200JPG_ERR_INVALID_PARAMETER. Also B200JPG_ERR_INVALID_PARAMETER: a zero size, an unknown filter or a NULL ksize. */
+B200JPG_API int b200jpg_resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, int32_t *bounds, int32_t *coeffs,
+                                              uint64_t capacity, uint32_t *ksize);
 /* The uncropped output size W_o x H_o of one codestream under `flags` (B200JPG_FLAG_DOWNSCALE_k, and width and height swapped for
  * the Exif orientations 5..8 with B200JPG_FLAG_EXIF_ORIENTATION; the frame size, B200JPG_FLAG_NO_UPSAMPLE or not): what the crop
  * rectangles of b200jpg_batch_create_crop are checked against. Returns B200JPG_OK or the error code b200jpg_parse returns for it

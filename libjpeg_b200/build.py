@@ -18,8 +18,11 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hidden",
           "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
-CUDA_SOURCES = ["huffman_sm100.cu", "specsync_sm100.cu", "progressive_sm100.cu", "progfused_sm100.cu", "recon_sm100.cu", "bitmap_sm100.cu", "microbench_sm100.cu"]
+CUDA_SOURCES = ["huffman_sm100.cu", "specsync_sm100.cu", "progressive_sm100.cu", "progfused_sm100.cu", "recon_sm100.cu", "bitmap_sm100.cu",
+                "microbench_sm100.cu", "resample_sm100.cu"]
 HOST_SOURCES = ["abi.cpp", "parse.cpp", "jpeg_shim.cpp"]
+# the resample tables are computed on the host in double precision: no contraction into FMA, so every host computes the same bits
+EXTRA = {"resample_sm100.cu": ["-Xcompiler", "-ffp-contract=off"]}
 
 
 def _nvcc():
@@ -51,7 +54,7 @@ def build(force=False, verbose=False, ptxas_info=False):
     """Compile every translation unit for sm_90a and link the shared objects. Returns the library path."""
     nvcc = _nvcc()
     os.makedirs(OBJ, exist_ok=True)
-    headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".hpp")]
+    headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".hpp", ".cuh"))]
     headers += [os.path.join(ROOT, "include", "b200jpg.h")]
     headers += [os.path.abspath(__file__)]  # the flags (ARCH, COMMON) live here: objects built with other flags are stale
     idir = os.path.join(ROOT, "include", "interface")
@@ -65,7 +68,7 @@ def build(force=False, verbose=False, ptxas_info=False):
         obj = os.path.join(OBJ, src + ".o")
         objs.append(obj)
         if force or _newer(obj, [path] + headers):
-            cmd = [nvcc] + ARCH + COMMON
+            cmd = [nvcc] + ARCH + COMMON + EXTRA.get(src, [])
             if src.endswith(".cu") and ptxas_info:
                 cmd += ["-Xptxas", "-v"]
             cmd += ["-c", path, "-o", obj]

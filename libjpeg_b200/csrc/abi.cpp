@@ -137,6 +137,7 @@ struct ReconGroup {
     ReconPath path = ReconPath::Tiled;
     int orientation = 1;  // B200JPG_FLAG_EXIF_ORIENTATION: the frames' orientation; 2..8 store through rewritten descriptors
     bool cropped = false; // b200jpg_batch_create_crop: the frames' tiles cover their rectangles, clipped stores (FrameRecon::clip_*)
+    bool resized = false; // b200jpg_batch_create_resize: cropped frames stored as uint8 into the scratch, never converted
     std::vector<FrameRecon> frames;
     uint32_t max_bw0 = 0, max_bh0 = 0, max_bwc = 0, max_bhc = 0;
     uint64_t dev_frames = 0;
@@ -164,12 +165,16 @@ struct Extent {
 uint32_t downscale_of(unsigned flags) { return 1u << ((flags & B200JPG_FLAG_DOWNSCALE_MASK) >> 2); }
 
 bool rect_empty(const b200jpg_rect &r) { return r.x == 0 && r.y == 0 && r.width == 0 && r.height == 0; }
+bool size_empty(const b200jpg_size &s) { return s.width == 0 && s.height == 0; }
+bool resample_known(int r) { return r >= B200JPG_RESAMPLE_LANCZOS && r <= B200JPG_RESAMPLE_HAMMING; }  // PIL's values 1 .. 5
 
 // component c as it leaves the decoder: the frame size W' x H' = ceil(W / k) x ceil(H / k), or without upsampling its own
 // ceil(W' / subx) x ceil(H' / suby); width and height swapped for the Exif orientations 5..8 (`orientation`: the one the frame
 // leaves with, 1 for the extent the kernels decode); the rectangle's size for a frame with a crop (`crop`, given in those output
-// coordinates and checked against them; never together with B200JPG_FLAG_NO_UPSAMPLE)
-Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags, int orientation, const b200jpg_rect *crop = nullptr) {
+// coordinates and checked against them; never together with B200JPG_FLAG_NO_UPSAMPLE); the target size of a resized frame (`size`)
+Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags, int orientation, const b200jpg_rect *crop = nullptr,
+                  const b200jpg_size *size = nullptr) {
+    if (size) return {size->width, size->height};
     if (crop) return {crop->width, crop->height};
     const uint64_t k = downscale_of(flags);
     uint64_t w = (fi.width + k - 1) / k, h = (fi.height + k - 1) / k;
@@ -306,6 +311,20 @@ struct b200jpg_batch {
     // some live frame leaves with an Exif orientation other than 1 or with a crop: its group stores through rewritten descriptors
     bool rewritten = false;
     std::vector<b200jpg_rect> crop;  // [n_user] b200jpg_batch_create_crop's rectangles, {0, 0, 0, 0}: the whole frame
+    // b200jpg_batch_create_resize: [n_user] target sizes ({0, 0}: not resized) and the filter; per resized frame its resample
+    // descriptor, its caller frame and its tables (h bounds, h coefficients, v bounds, v coefficients). The descriptor table of
+    // a decode holds 4 * (n + resized frames) entries: the destinations of resized frame r at 4 * (n + r)
+    std::vector<b200jpg_size> size;
+    int resample = 0;
+    std::vector<ResampleFrame> rs_frames;
+    std::vector<int> rs_user, rs_index;  // [resized] caller frame; [n_user] index into rs_frames or -1
+    std::vector<std::array<std::vector<int32_t>, 4>> rs_tables;
+    uint64_t dev_rs_frames = 0;
+    uint32_t rs_max_rows = 0;
+    uint64_t rs_max_pixels = 0;
+    uint8_t *d_scratch = nullptr, *d_inter = nullptr;  // C of every resized frame; the horizontal pass's rows
+    uint64_t scratch_bytes = 0, inter_bytes = 0;
+    size_t n_planes() const { return 4 * ((size_t)n + rs_frames.size()); }
     int last_launches = 0;
     bool timing = false;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // start, after a0, after a1, after b
@@ -323,6 +342,13 @@ static const b200jpg_rect *crop_of(const b200jpg_batch &b, int i) {
     const int u = b.xt_parent[i] >= 0 ? b.xt_parent[i] : i;
     if (b.crop.empty() || u >= b.n_user || rect_empty(b.crop[u])) return nullptr;
     return &b.crop[u];
+}
+
+// the target size of frame i (a JPEG XT residual codestream: its frame's), nullptr for a frame that is not resized
+static const b200jpg_size *size_of(const b200jpg_batch &b, int i) {
+    const int u = b.xt_parent[i] >= 0 ? b.xt_parent[i] : i;
+    if (b.size.empty() || u >= b.n_user || size_empty(b.size[u])) return nullptr;
+    return &b.size[u];
 }
 
 extern "C" {
@@ -433,6 +459,24 @@ int b200jpg_output_size(const uint8_t *data, size_t len, unsigned flags, uint32_
     return B200JPG_OK;
 }
 
+int b200jpg_resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, int32_t *bounds, int32_t *coeffs, uint64_t capacity,
+                                  uint32_t *ksize) {
+    if (!ksize || in_size == 0 || out_size == 0 || !resample_known(resample)) return B200JPG_ERR_INVALID_PARAMETER;
+    std::vector<int32_t> b, k;
+    uint32_t ks = 0;
+    try {
+        if (int rc = resample_coefficients(in_size, out_size, resample, b, k, ks)) return rc;
+    } catch (const std::bad_alloc &) {
+        return B200JPG_ERR_OUT_OF_MEMORY;
+    }
+    *ksize = ks;
+    if (!bounds || !coeffs) return B200JPG_OK;
+    if (capacity < (uint64_t)out_size * ks) return B200JPG_ERR_INVALID_PARAMETER;
+    memcpy(bounds, b.data(), b.size() * sizeof(int32_t));
+    memcpy(coeffs, k.data(), k.size() * sizeof(int32_t));
+    return B200JPG_OK;
+}
+
 uint64_t b200jpg_build_tables(const uint8_t *data, size_t len, int scan, uint8_t *dst, uint64_t capacity) {
     ParsedFrame pf;
     std::string err;
@@ -528,8 +572,10 @@ void b200jpg_batch_destroy(b200jpg_batch *b) {
     if (b->d_spec) b->ctx->put(1, b->d_spec, b->sz_spec);
     if (b->d_dcplane) b->ctx->put(1, b->d_dcplane, b->coef_elems / 64 * sizeof(int16_t));
     b->ctx->put(1, b->d_status, b->sz_status);
-    b->ctx->put(0, b->h_planes, sizeof(b200jpg_plane) * 4 * (size_t)b->n * b200jpg_batch::kPlaneSlots);
-    b->ctx->put(1, b->d_planes, sizeof(b200jpg_plane) * 4 * (size_t)b->n);
+    b->ctx->put(0, b->h_planes, sizeof(b200jpg_plane) * b->n_planes() * b200jpg_batch::kPlaneSlots);
+    b->ctx->put(1, b->d_planes, sizeof(b200jpg_plane) * b->n_planes());
+    if (b->d_scratch) b->ctx->put(1, b->d_scratch, b->scratch_bytes);
+    if (b->d_inter) b->ctx->put(1, b->d_inter, b->inter_bytes);
     for (auto &e : b->ev_planes)
         if (e) cudaEventDestroy(e);
     for (auto &e : b->ev)
@@ -568,6 +614,11 @@ static void attach_residuals(b200jpg_batch &b, Codestreams &cs, bool device_inde
     const int n_user = b.n_user;
     b.xt_child.assign(n_user, -1);
     for (int i = 0; i < n_user; i++) {
+        if (b.parse_status[i] == 0 && !b.size.empty() && !size_empty(b.size[i]) && b.frames[i].info.precision != 8) {
+            b.parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;  // never written unresized
+            cs.err[i] = "only 8-bit frames are resized";
+            continue;
+        }
         if (b.parse_status[i] != 0 || !b.frames[i].xt.present) continue;
         if (b.flags & (B200JPG_FLAG_NO_COLOR_TRANSFORM | B200JPG_FLAG_NO_UPSAMPLE)) {
             b.parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;
@@ -727,7 +778,7 @@ static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
                 sample_base[i][c] = sample_cur;
                 sample_cur += path == ReconPath::Scaled ? 64ull * ((fi.blocks_w[c] + k - 1) / k) * ((fi.blocks_h[c] + k - 1) / k) : elems;
             }
-            const Extent e = out_extent(fi, c, b.flags, 1, crop_of(b, i));  // the components one after the other (w * h: any orientation)
+            const Extent e = out_extent(fi, c, b.flags, 1, crop_of(b, i), size_of(b, i));  // the components one after the other (w * h: any orientation)
             samples += e.w * e.h;
         }
         b.out_off[i] = out_cur;
@@ -951,9 +1002,12 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         // cropped frames too: their launches are sized by the tiles the rectangles cover, and they always store clipped
         const b200jpg_rect *crop = crop_of(b, i);
         if (orientation != 1 || crop) b.rewritten = true;
+        // resized frames too (every one of them is cropped, admit_sizes): they store into the scratch, unconverted
+        const bool resized = size_of(b, i) != nullptr;
         ReconGroup *g = nullptr;
         for (auto &gg : b.groups)
-            if (gg.ncomp == fi.ncomp && gg.subx == sx && gg.suby == sy && gg.path == path && gg.orientation == orientation && gg.cropped == (crop != nullptr))
+            if (gg.ncomp == fi.ncomp && gg.subx == sx && gg.suby == sy && gg.path == path && gg.orientation == orientation && gg.cropped == (crop != nullptr) &&
+                gg.resized == resized)
                 g = &gg;
         if (!g) {
             b.groups.emplace_back();
@@ -964,6 +1018,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
             g->path = path;
             g->orientation = orientation;
             g->cropped = crop != nullptr;
+            g->resized = resized;
         }
         FrameRecon fr{};
         const uint32_t k = downscale_of(b.flags);
@@ -1061,6 +1116,17 @@ static void lay_out_descriptors(b200jpg_batch &b) {
         g.dev_frames = cur;
         cur = align_up(cur + g.frames.size() * sizeof(FrameRecon), 256);
     }
+    b.dev_rs_frames = cur;
+    cur = align_up(cur + b.rs_frames.size() * sizeof(ResampleFrame), 256);
+    for (size_t r = 0; r < b.rs_frames.size(); r++) {  // the tables, 16-byte aligned and padded (resample_h_kernel stages them in uint4)
+        ResampleFrame &f = b.rs_frames[r];
+        uint64_t *at[4] = {&f.h_bounds, &f.h_coef, &f.v_bounds, &f.v_coef};
+        for (int t = 0; t < 4; t++) {
+            *at[t] = cur;
+            cur = align_up(cur + b.rs_tables[r][t].size() * sizeof(int32_t), 16);
+        }
+    }
+    cur = align_up(cur, 256);
     b.dev_prog_frames = cur;
     cur = align_up(cur + b.prog_frames.size() * sizeof(ProgFrame), 256);
     b.dev_index_scans = cur;
@@ -1111,6 +1177,17 @@ static int stage_and_allocate(b200jpg_batch &b, const Codestreams &cs, const std
     for (auto &g : b.groups) memcpy(b.h_input + g.dev_frames, g.frames.data(), g.frames.size() * sizeof(FrameRecon));
     if (!b.index_scans.empty()) memcpy(b.h_input + b.dev_index_scans, b.index_scans.data(), b.index_scans.size() * sizeof(IndexScan));
     if (!b.prog_frames.empty()) memcpy(b.h_input + b.dev_prog_frames, b.prog_frames.data(), b.prog_frames.size() * sizeof(ProgFrame));
+    if (!b.rs_frames.empty()) memcpy(b.h_input + b.dev_rs_frames, b.rs_frames.data(), b.rs_frames.size() * sizeof(ResampleFrame));
+    for (size_t r = 0; r < b.rs_frames.size(); r++) {
+        const ResampleFrame &f = b.rs_frames[r];
+        const uint64_t at[4] = {f.h_bounds, f.h_coef, f.v_bounds, f.v_coef};
+        for (int t = 0; t < 4; t++) {
+            const std::vector<int32_t> &v = b.rs_tables[r][t];
+            const uint64_t bytes = v.size() * sizeof(int32_t);
+            if (bytes) memcpy(b.h_input + at[t], v.data(), bytes);
+            memset(b.h_input + at[t] + bytes, 0, align_up(bytes, 16) - bytes);
+        }
+    }
 
     b.sz_ilen = sizeof(uint32_t) * (size_t)std::max<uint64_t>(b.n_intervals, 1);
     b.sz_status = sizeof(uint32_t) * (5 * (size_t)b.n + 1);  // status words, wide flags, narrow flags, narrow list, index status
@@ -1129,6 +1206,8 @@ static int stage_and_allocate(b200jpg_batch &b, const Codestreams &cs, const std
         b.sz_spec = (size_t)align_up(b.n_spec, 4) * (sizeof(SpecSegment) + 8 + 8 + 4 + 16 + sizeof(SpecLog)) + 256;
         b.d_spec = (uint8_t *)ctx->get(1, b.sz_spec, &ce);
     }
+    if (ce == cudaSuccess && b.scratch_bytes) b.d_scratch = (uint8_t *)ctx->get(1, b.scratch_bytes, &ce);
+    if (ce == cudaSuccess && b.inter_bytes) b.d_inter = (uint8_t *)ctx->get(1, b.inter_bytes, &ce);
     if (ce == cudaSuccess) ce = cudaEventCreateWithFlags(&b.ev_last, cudaEventDisableTiming);
     if (ce != cudaSuccess) return ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, std::string("device allocation failed: ") + cudaGetErrorString(ce));
     b.h_status.assign(b.n, 0);
@@ -1152,16 +1231,95 @@ static int admit_crops(b200jpg_batch &b, const b200jpg_rect *rects) {
     return B200JPG_OK;
 }
 
+// b200jpg_batch_create_resize's sizes: kept for the live frames (a failed frame's is ignored). A resized frame without a rectangle is
+// cropped to its whole output, so that the reconstruction writes C through the cropped path; returns 0 or the status the call fails
+// with (a size whose bitmaps could never be allocated)
+static int admit_sizes(b200jpg_batch &b, const b200jpg_size *sizes) {
+    b.size.assign(sizes, sizes + b.n_user);
+    if (b.crop.empty()) b.crop.assign(b.n_user, b200jpg_rect{0, 0, 0, 0});
+    for (int i = 0; i < b.n_user; i++) {
+        b200jpg_size &s = b.size[i];
+        if (b.parse_status[i] != 0) s = b200jpg_size{0, 0};
+        if (size_empty(s)) continue;
+        const b200jpg_frame_info &fi = b.frames[i].info;
+        if (s.width > (1u << 24) || s.height > (1u << 24) || (uint64_t)s.width * s.height * fi.ncomp > (1ull << 34))
+            return b.ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "frame " + std::to_string(i) + ": target size " + std::to_string(s.width) + " x " +
+                                                              std::to_string(s.height) + " is too large to allocate");
+        if (rect_empty(b.crop[i])) {
+            const Extent e = out_extent(fi, 0, b.flags, applied_orientation(b, i));
+            b.crop[i] = b200jpg_rect{0, 0, (uint32_t)e.w, (uint32_t)e.h};
+        }
+    }
+    return B200JPG_OK;
+}
+
+// The resample descriptors and tables of the resized frames (tables built on host threads, one frame each) and the layout of the
+// scratch (C: h rows of align16(w * ncomp) bytes per frame) and of the intermediate (rows y0 .. y1 - 1 of tw * ncomp bytes, for
+// frames whose width changes)
+static void plan_resample(b200jpg_batch &b) {
+    b.rs_index.assign(b.n_user, -1);
+    for (int i = 0; i < b.n_user; i++)
+        if (b.parse_status[i] == 0 && size_of(b, i)) {
+            b.rs_index[i] = (int)b.rs_user.size();
+            b.rs_user.push_back(i);
+        }
+    const int nr = (int)b.rs_user.size();
+    b.rs_frames.assign(nr, ResampleFrame{});
+    b.rs_tables.assign(nr, {});
+    for_frames(nr, 16, [&](int r) {
+        const int i = b.rs_user[r];
+        const b200jpg_frame_info &fi = b.frames[i].info;
+        const Extent e = out_extent(fi, 0, b.flags, applied_orientation(b, i), crop_of(b, i));  // C
+        const b200jpg_size &s = *size_of(b, i);
+        ResampleFrame &f = b.rs_frames[r];
+        auto &t = b.rs_tables[r];
+        f.w = (uint32_t)e.w, f.h = (uint32_t)e.h, f.tw = s.width, f.th = s.height, f.ncomp = fi.ncomp;
+        f.src_pitch = (uint32_t)align_up((uint64_t)f.w * f.ncomp, 16);
+        f.plane = (uint32_t)(b.n + r);
+        f.y0 = 0, f.y1 = f.h;
+        if (f.th != f.h) {  // (the arguments are valid: the calls cannot fail)
+            resample_coefficients(f.h, f.th, b.resample, t[2], t[3], f.v_ksize);
+            f.y0 = (uint32_t)t[2][0];
+            f.y1 = (uint32_t)(t[2][2 * (size_t)f.th - 2] + t[2][2 * (size_t)f.th - 1]);
+        }
+        if (f.tw != f.w) resample_coefficients(f.w, f.tw, b.resample, t[0], t[1], f.h_ksize);
+        if (f.src_pitch <= kResampleRowSmem) f.stage |= kStageRow;
+        if (f.tw != f.w && align_up(t[1].size() * sizeof(int32_t), 16) <= kResampleCoefSmem) f.stage |= kStageCoef;
+    });
+    for (ResampleFrame &f : b.rs_frames) {
+        f.src = b.scratch_bytes;
+        b.scratch_bytes = align_up(b.scratch_bytes + (uint64_t)f.src_pitch * f.h, 256);
+        if (f.tw != f.w) {
+            f.inter = b.inter_bytes;
+            b.inter_bytes = align_up(b.inter_bytes + (uint64_t)(f.y1 - f.y0) * f.tw * f.ncomp, 256);
+            b.rs_max_rows = std::max(b.rs_max_rows, f.y1 - f.y0);
+        }
+        b.rs_max_pixels = std::max(b.rs_max_pixels, (uint64_t)f.tw * f.th);
+    }
+}
+
 static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
-                             const b200jpg_rect *rects, b200jpg_batch **out) {
+                             const b200jpg_rect *rects, const b200jpg_size *sizes, int resample, b200jpg_batch **out) {
     NvtxRange nvtx("b200jpg batch_create: parse + pack");
     if (!out || !frames || !lens || n <= 0) return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "invalid batch arguments");
     *out = nullptr;
     bool any_crop = false;
     for (int i = 0; rects && i < n; i++) any_crop = any_crop || !rect_empty(rects[i]);
     if (!any_crop) rects = nullptr;  // all {0, 0, 0, 0}: exactly the batch of b200jpg_batch_create_ex
+    bool any_size = false;
+    for (int i = 0; sizes && i < n; i++) {
+        if ((sizes[i].width == 0) != (sizes[i].height == 0))
+            return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": target size " + std::to_string(sizes[i].width) + " x " +
+                                                                std::to_string(sizes[i].height) + " has exactly one zero side");
+        if (!size_empty(sizes[i]) && !resample_known(resample))
+            return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": unknown resample filter " + std::to_string(resample));
+        any_size = any_size || !size_empty(sizes[i]);
+    }
+    if (!any_size) sizes = nullptr;  // all {0, 0}: exactly the batch of b200jpg_batch_create_crop
     if (rects && (flags & B200JPG_FLAG_NO_UPSAMPLE))
         return ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, "crop rectangles are not supported with B200JPG_FLAG_NO_UPSAMPLE");
+    if (sizes && (flags & B200JPG_FLAG_NO_UPSAMPLE))
+        return ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, "target sizes are not supported with B200JPG_FLAG_NO_UPSAMPLE");
     cudaError_t ce = cudaSetDevice(ctx->device);
     if (ce != cudaSuccess) return ctx->fail_cuda(ce, "cudaSetDevice");
 
@@ -1170,6 +1328,7 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
     b.ctx = ctx;
     b.n = b.n_user = n;
     b.flags = flags;
+    if (sizes) b.size.assign(sizes, sizes + n), b.resample = resample;  // (attach_residuals refuses 12-bit frames with a size)
     Codestreams cs;
     cs.data.assign(frames, frames + n);
     cs.len.assign(lens, lens + n);
@@ -1183,12 +1342,15 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
     if (int rc = admit_frames(b, cs, tolerate_bad != 0, frame_tables)) return rc;
     if (rects)
         if (int rc = admit_crops(b, rects)) return rc;
+    if (sizes)
+        if (int rc = admit_sizes(b, sizes)) return rc;
     const std::vector<uint64_t> byte_off = lay_out_codestreams(b, cs.len);
     const std::vector<std::array<uint64_t, 4>> sample_base = lay_out_planes(b);
     form_scan_classes(b, frame_tables, byte_off);
     form_progressive_groups(b);
     lay_out_unstuffed(b);
     form_recon_groups(b, sample_base);
+    plan_resample(b);
     lay_out_descriptors(b);
     if (int rc = stage_and_allocate(b, cs, byte_off)) return rc;
     *out = bp.release();
@@ -1207,9 +1369,14 @@ int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, cons
 
 int b200jpg_batch_create_crop(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
                               const b200jpg_rect *rects, b200jpg_batch **out) {
+    return b200jpg_batch_create_resize(ctx, frames, lens, n, tolerate_bad, flags, rects, nullptr, 0, out);
+}
+
+int b200jpg_batch_create_resize(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
+                                const b200jpg_rect *rects, const b200jpg_size *sizes, int resample, b200jpg_batch **out) {
     if (!ctx) return B200JPG_ERR_INVALID_PARAMETER;
     try {  // no exception crosses the C ABI
-        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, rects, out);
+        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, rects, sizes, resample, out);
     } catch (const std::bad_alloc &) {
         if (out) *out = nullptr;
         return ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "out of host memory while preparing the batch");
@@ -1230,7 +1397,7 @@ int b200jpg_batch_output_extent(const b200jpg_batch *b, int i, int c, uint32_t *
     if (b->parse_status[i] != 0) return b->parse_status[i];
     const b200jpg_frame_info &fi = b->frames[i].info;
     if (c < 0 || c >= fi.ncomp) return B200JPG_ERR_INVALID_PARAMETER;
-    const Extent e = out_extent(fi, c, b->flags, applied_orientation(*b, i), crop_of(*b, i));
+    const Extent e = out_extent(fi, c, b->flags, applied_orientation(*b, i), crop_of(*b, i), size_of(*b, i));
     *width = (uint32_t)e.w;
     *height = (uint32_t)e.h;
     return B200JPG_OK;
@@ -1449,10 +1616,10 @@ static int run_entropy(b200jpg_batch *b, void *stream) {
     return B200JPG_OK;
 }
 
-// The descriptor table [4 * n] that fill(table) writes (on zeros: residual codestreams and failed frames have no destination) to
+// The descriptor table [b->n_planes()] that fill(table) writes (on zeros: residual codestreams and failed frames have no destination) to
 // b->d_planes on `stream`, staged in the next slot of the pinned ring (b200jpg_batch::kPlaneSlots)
 static int stage_planes(b200jpg_batch *b, void *stream, const std::function<void(b200jpg_plane *)> &fill) {
-    const size_t bytes = sizeof(b200jpg_plane) * 4 * (size_t)b->n;
+    const size_t bytes = sizeof(b200jpg_plane) * b->n_planes();
     cudaError_t ce = cudaSuccess;
     constexpr int kSlots = b200jpg_batch::kPlaneSlots;
     if (!b->d_planes) {  // everything is allocated before any of it is kept: a failure leaves the batch as it was
@@ -1474,7 +1641,7 @@ static int stage_planes(b200jpg_batch *b, void *stream, const std::function<void
     const int slot = b->plane_slot;
     ce = cudaEventSynchronize(b->ev_planes[slot]);  // the copy kSlots calls ago has read this slot (at once when never recorded)
     if (ce != cudaSuccess) return b->ctx->fail_cuda(ce, "descriptor table");
-    b200jpg_plane *stage = b->h_planes + 4 * (size_t)b->n * slot;
+    b200jpg_plane *stage = b->h_planes + b->n_planes() * slot;
     memset(stage, 0, bytes);
     fill(stage);
     ce = cudaMemcpyAsync(b->d_planes, stage, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream);
@@ -1501,13 +1668,37 @@ static bool rewrite_frame(const b200jpg_batch *b, int i, b200jpg_plane *pl, uint
     return true;
 }
 
+// The reconstruction's destination of resized frame i: its C in the scratch, an interleaved uint8 bitmap, rewritten like a cropped
+// frame's slot (rewrite_frame)
+static void scratch_planes(const b200jpg_batch *b, int i, b200jpg_plane *pl, std::vector<char> &planar) {
+    const ResampleFrame &f = b->rs_frames[(size_t)b->rs_index[i]];
+    for (uint32_t c = 0; c < f.ncomp; c++) {
+        pl[c].data = b->d_scratch + f.src + c;
+        pl[c].bytes_per_pixel = (int32_t)f.ncomp;
+        pl[c].bytes_per_row = f.src_pitch;
+    }
+    rewrite_frame(b, i, pl, 1, planar);  // a scratch row always fits the pixel stride
+}
+
 // b200jpg_batch_decode of a batch with oriented or cropped frames: each such frame's packed slot in out_dev, seen as an interleaved
 // bitmap of the oriented (cropped) extent (B200JPG_FLAG_NO_UPSAMPLE: plane after plane), rewritten for its crop and orientation and
-// staged like the table of b200jpg_batch_decode_into. planar[i] as for that table.
+// staged like the table of b200jpg_batch_decode_into. A resized frame: its scratch, and its slot as the resample pass's
+// destination at 4 * (n + r), in output coordinates. planar[i] as for that table.
 static int stage_slot_planes(b200jpg_batch *b, uint8_t *out_dev, void *stream, std::vector<char> &planar) {
     return stage_planes(b, stream, [&](b200jpg_plane *table) {
+        for (size_t r = 0; r < b->rs_frames.size(); r++) {
+            const int i = b->rs_user[r];
+            const ResampleFrame &f = b->rs_frames[r];
+            scratch_planes(b, i, table + 4 * (size_t)i, planar);
+            for (uint32_t c = 0; c < f.ncomp; c++) {
+                b200jpg_plane &p = table[4 * (size_t)f.plane + c];
+                p.data = out_dev + b->out_off[i] + c;
+                p.bytes_per_pixel = (int32_t)f.ncomp;
+                p.bytes_per_row = (int64_t)f.tw * f.ncomp;
+            }
+        }
         for (int i = 0; i < b->n_user; i++) {
-            if (b->parse_status[i] != 0 || (applied_orientation(*b, i) == 1 && !crop_of(*b, i))) continue;
+            if (b->parse_status[i] != 0 || (applied_orientation(*b, i) == 1 && !crop_of(*b, i)) || size_of(*b, i)) continue;
             const b200jpg_frame_info &fi = b->frames[i].info;
             const int o = applied_orientation(*b, i);
             const int64_t size = fi.precision > 8 ? 2 : 1;
@@ -1566,6 +1757,7 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.convert = convert;
         const std::vector<char> *group_planar = planar;
         if (slot_planes && (g.orientation != 1 || g.cropped)) l.planes = slot_planes, group_planar = &slot_planar;
+        if (g.resized) l.convert = nullptr;  // C leaves as uint8; the resample pass converts
         l.planar = l.planes != nullptr;
         if (l.planes)
             for (const FrameRecon &fr : g.frames) l.planar = l.planar && (*group_planar)[fr.status_idx];
@@ -1588,6 +1780,24 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
                 b->last_launches += launches;
             }
         }
+    }
+    // resized frames: C in the scratch -> the destinations (grid.y carries the frame: at most 65535 frames per launch)
+    const uint32_t nr = (uint32_t)b->rs_frames.size();
+    for (uint32_t first = 0; first < nr; first += 65535u) {
+        ResampleLaunch rl{};
+        rl.frames = reinterpret_cast<const ResampleFrame *>(b->d_input + b->dev_rs_frames) + first;
+        rl.n_frames = std::min<uint32_t>(65535u, nr - first);
+        rl.max_rows = b->rs_max_rows;
+        rl.max_pixels = b->rs_max_pixels;
+        rl.input = b->d_input;
+        rl.scratch = b->d_scratch;
+        rl.inter = b->d_inter;
+        rl.planes = planes_dev ? planes_dev : slot_planes;
+        rl.convert = convert;
+        int launches = 0;
+        int rc = launch_resample(rl, stream, &launches);
+        if (rc != 0) return b->ctx->fail_cuda((cudaError_t)rc, "resample kernel launch");
+        b->last_launches += launches;
     }
     cudaEventRecord(b->ev_last, (cudaStream_t)stream);
     return B200JPG_OK;
@@ -1656,7 +1866,7 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
         const int orientation = applied_orientation(*b, i);
         for (int c = 0; c < fi.ncomp; c++) {
             const b200jpg_plane &p = planes[4 * i + c];
-            const auto [w, h] = out_extent(fi, c, b->flags, orientation, crop_of(*b, i));  // the rules hold in (cropped) output coordinates
+            const auto [w, h] = out_extent(fi, c, b->flags, orientation, crop_of(*b, i), size_of(*b, i));  // the rules hold in (cropped, resized) output coordinates
             const uint64_t bpp = magnitude(p.bytes_per_pixel), bpr = magnitude(p.bytes_per_row);
             const std::string at = "frame " + std::to_string(i) + " component " + std::to_string(c) + ": ";
             if (!p.data) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "no destination");
@@ -1676,7 +1886,9 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
         if (b->rewritten) {
             b200jpg_plane *q = rewritten.data() + 4 * (size_t)i;
             memcpy(q, planes + 4 * (size_t)i, sizeof(b200jpg_plane) * fi.ncomp);
-            if (orientation != 1 || crop_of(*b, i)) {  // the kernels store through the rewritten descriptors: planar is decided on those
+            if (size_of(*b, i)) {  // the reconstruction stores into the scratch; the caller's descriptors go to the resample pass
+                scratch_planes(b, i, q, planar);
+            } else if (orientation != 1 || crop_of(*b, i)) {  // the kernels store through the rewritten descriptors: planar is decided on those
                 planar[(size_t)i] = 1;
                 if (!rewrite_frame(b, i, q, size, planar))
                     return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) +
@@ -1688,6 +1900,8 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
     const int rc = stage_planes(b, stream, [&](b200jpg_plane *table) {
         for (int i = 0; i < b->n_user; i++)
             if (b->parse_status[i] == 0) memcpy(table + 4 * (size_t)i, src + 4 * (size_t)i, sizeof(b200jpg_plane) * b->frames[i].info.ncomp);
+        for (size_t r = 0; r < b->rs_frames.size(); r++)  // the caller's descriptors of resized frames: the resample pass's, as given
+            memcpy(table + 4 * (size_t)b->rs_frames[r].plane, planes + 4 * (size_t)b->rs_user[r], sizeof(b200jpg_plane) * b->rs_frames[r].ncomp);
     });
     if (rc) return rc;
     return run_decode(b, nullptr, stream, b->d_planes, &planar, convert);

@@ -348,6 +348,39 @@ struct FloatDst {
 };
 int launch_recon(const ReconLaunch &l, void *stream, int *launches);
 
+// ---- resize (b200jpg_batch_create_resize, DESIGN §13), resample_sm100.cu. The reconstruction writes C, the frame's cropped
+// output, as an interleaved uint8 bitmap into the batch's scratch; resample_h_kernel runs the horizontal pass over the rows of C
+// the vertical table touches into the intermediate, resample_v_kernel the vertical pass into the caller's destinations.
+// The fixed-point tables of one axis: bounds [out_size][2] int32 (first source index, taps), coefficients [out_size][ksize] int32
+// (zero behind the taps), PIL's convolution resampler; computed without floating-point contraction (build.py).
+int resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, std::vector<int32_t> &bounds, std::vector<int32_t> &coef,
+                          uint32_t &ksize);
+struct ResampleFrame {
+    uint64_t src;                             // byte offset of C in the scratch: h rows of src_pitch bytes, ncomp bytes per pixel
+    uint64_t inter;                           // byte offset of the horizontal pass's rows y0 .. y1 - 1 in the intermediate (tw * ncomp each)
+    uint64_t h_bounds, h_coef, v_bounds, v_coef;  // byte offsets of the tables in the input buffer (16-byte aligned)
+    uint32_t w, h, tw, th;                    // C's extent and the target size; an axis of equal size is not resampled
+    uint32_t ncomp, src_pitch, h_ksize, v_ksize;
+    uint32_t y0, y1;                          // the rows of C the vertical table touches (0, h when the height does not change)
+    uint32_t plane;                           // destinations: planes[4 * plane + c], in output coordinates
+    uint32_t stage;                           // kStageRow: a row of C fits the shared row buffer; kStageCoef: the horizontal table fits
+};
+constexpr uint32_t kStageRow = 1, kStageCoef = 2;
+constexpr uint32_t kResampleRowSmem = 16 * 1024, kResampleCoefSmem = 32 * 1024;  // the shared buffers of resample_h_kernel
+constexpr uint32_t kResampleRows = 8;                                            // rows of the intermediate per CTA
+struct ResampleLaunch {
+    const ResampleFrame *frames;  // device
+    uint32_t n_frames;
+    uint32_t max_rows;            // largest y1 - y0 of a frame whose width changes
+    uint64_t max_pixels;          // largest tw * th
+    const uint8_t *input;         // the batch's input buffer (tables)
+    const uint8_t *scratch;
+    uint8_t *inter;
+    const b200jpg_plane *planes;  // device
+    const b200jpg_convert *convert;  // host; null: uint8 destinations
+};
+int launch_resample(const ResampleLaunch &l, void *stream, int *launches);
+
 // JPEG::DisplayRectangle into device bitmaps (bitmap_sm100.cu): the rectangle x0..x1, y0..y1 (inclusive, in the coordinates of
 // the decoded samples) of every requested component goes from the decoded frame to the client's bitmap. Sample (x, y) of
 // component k is src[comp[k].src_off + y * src_pitch + x * src_step] (samples of 1 or 2 bytes, `deep`) and lands at

@@ -34,6 +34,7 @@
 #include <type_traits>
 
 #include "internal.hpp"
+#include "store_sm90.cuh"
 
 namespace b200jpg {
 namespace {
@@ -508,21 +509,10 @@ using StoreDst = std::conditional_t<K == kStoreCanvas, uint8_t *, std::condition
 __device__ __forceinline__ const b200jpg_plane *planes_of(const b200jpg_plane *p) { return p; }
 __device__ __forceinline__ const b200jpg_plane *planes_of(const FloatDst &d) { return d.planes; }
 
-// ---- float elements. The samples arrive as clamped integers 0 <= v < 2^23: 0x4B000000 | v is the float 2^23 + v, so one
-// subtraction makes (float)v exactly -- a LOP3 (or the PRMT that takes the byte out of its packed word) and an FADD on the
-// otherwise idle FP32 pipe, where I2F would issue at a fraction of that rate. Then fp32_round(fp32_round(v * s) + b), never
-// fused.
-__device__ __forceinline__ float convert_bits(uint32_t bits, float s, float b) {
-    return __fadd_rn(__fmul_rn(__fsub_rn(__uint_as_float(bits), 8388608.f), s), b);
-}
-__device__ __forceinline__ float convert_int(int v, float s, float b) { return convert_bits(0x4B000000u | (uint32_t)v, s, b); }
+// ---- float elements: convert_bits / convert_int / pick4 / store_elem (store_sm90.cuh)
 // byte k of a packed word of four 8-bit samples as 0x4B0000vv: bytes 4..7 of the permute are those of 0x4B000000
 __device__ __forceinline__ float convert_byte(uint32_t w, int k, float s, float b) {
     return convert_bits(__byte_perm(w, 0x4B000000u, 0x7440u | (uint32_t)k), s, b);
-}
-// scale[c] / bias[c] of a component index known only at run time (a select chain: the parameter bank is not indexed)
-__device__ __forceinline__ float pick4(const float (&a)[B200JPG_MAX_COMPONENTS], uint32_t c) {
-    return c == 0 ? a[0] : (c == 1 ? a[1] : (c == 2 ? a[2] : a[3]));
 }
 __device__ __forceinline__ uint32_t pack2(int type, float lo, float hi) {
     if (type == B200JPG_SAMPLE_F16) {
@@ -531,12 +521,6 @@ __device__ __forceinline__ uint32_t pack2(int type, float lo, float hi) {
     }
     const __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
     return *reinterpret_cast<const uint32_t *>(&h);
-}
-// one element at o, rounded to the destination type
-__device__ __forceinline__ void store_elem(int type, uint8_t *o, float y) {
-    if (type == B200JPG_SAMPLE_F32) *reinterpret_cast<float *>(o) = y;
-    else if (type == B200JPG_SAMPLE_F16) *reinterpret_cast<__half *>(o) = __float2half_rn(y);
-    else *reinterpret_cast<__nv_bfloat16 *>(o) = __float2bfloat16_rn(y);
 }
 // the first xmax + 1 of eight converted samples from o on: a whole 16-byte aligned planar row leaves as one 16-byte store
 // (fp16 / bf16) or two (fp32), else one store per element
@@ -559,17 +543,7 @@ __device__ __forceinline__ void store_row_f(int type, const b200jpg_plane *p, ui
         if (x <= xmax) store_elem(type, o + x * s, y[x]);
 }
 
-// the sample (x, y) of a described component, signed 64-bit addressing (ImageBitMap, interface/imagebitmap.hpp:104-109).
-// The descriptor is read again at every call (L1 hits): held in registers through the line loop of reconstruct_tile, three of
-// them push the 4:2:0 kernel over its 96-register budget.
-__device__ __forceinline__ uint8_t *plane_at(const b200jpg_plane *p, int x, int y) {
-    uint64_t data, bpr;
-    int bpp;
-    asm volatile("ld.global.nc.u64 %0, [%1];" : "=l"(data) : "l"(&p->data));
-    asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(bpp) : "l"(&p->bytes_per_pixel));
-    asm volatile("ld.global.nc.u64 %0, [%1];" : "=l"(bpr) : "l"(&p->bytes_per_row));
-    return reinterpret_cast<uint8_t *>(data + (uint64_t)((int64_t)x * bpp) + (uint64_t)((int64_t)y * (int64_t)bpr));
-}
+// the sample (x, y) of a described component: plane_at (store_sm90.cuh)
 
 // the first xmax + 1 of eight 8-bit samples (w0 | w1, sample 0 in the low byte of w0) from o on: one 8-byte store for a whole
 // aligned planar row, else one store per sample

@@ -1,0 +1,200 @@
+// resample_sm100.cu -- the resize stage of b200jpg_batch_create_resize (DESIGN §13): Pillow's convolution resampler on the
+// reconstruction's uint8 output, every channel on its own, in the int32 fixed point of Pillow's 8-bit path.
+//
+//   resample_h_kernel: grid (row band, frame). A CTA takes kResampleRows rows of the intermediate (rows y0.. of C); each row of C
+//     comes into shared memory with 16-byte loads, and every thread computes output columns x channels from it. The frame's
+//     horizontal table is read from shared memory where it fits, otherwise from global memory through L1. A frame whose width does
+//     not change has no horizontal pass: the vertical pass reads C in the scratch directly.
+//   resample_v_kernel: one thread per output pixel, all channels. The taps go down a column of the intermediate, so a warp's loads
+//     are contiguous along x and the tap's coefficient is one broadcast load; the clamped sample leaves through the caller's
+//     b200jpg_plane descriptor (any signed strides), converted by the float map of b200jpg_batch_decode_into_ex where one is given.
+// The host half: resample_coefficients, the only place the fixed-point tables are built (the batch's planning and the test entry
+// point b200jpg_resample_coefficients both call it). build.py compiles this file with -ffp-contract=off: the double-precision
+// arithmetic is evaluated as written, one rounding per operation, on every host.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cmath>
+#include <cstdint>
+#include <vector>
+
+#include "internal.hpp"
+#include "store_sm90.cuh"
+
+namespace b200jpg {
+
+namespace {
+
+constexpr int kPrecisionBits = 22;  // Pillow's PRECISION_BITS for 8-bit images: 32 - 8 - 2
+
+double box_filter(double x) { return (x > -0.5 && x <= 0.5) ? 1.0 : 0.0; }
+double bilinear_filter(double x) {
+    if (x < 0.0) x = -x;
+    return x < 1.0 ? 1.0 - x : 0.0;
+}
+double hamming_filter(double x) {
+    if (x < 0.0) x = -x;
+    if (x == 0.0) return 1.0;
+    if (x >= 1.0) return 0.0;
+    x = x * M_PI;
+    return sin(x) / x * (0.54 + 0.46 * cos(x));
+}
+double bicubic_filter(double x) {  // Keys, a = -0.5
+    const double a = -0.5;
+    if (x < 0.0) x = -x;
+    if (x < 1.0) return ((a + 2.0) * x - (a + 3.0)) * x * x + 1;
+    if (x < 2.0) return (((x - 5) * x + 8) * x - 4) * a;
+    return 0.0;
+}
+double sinc_filter(double x) {
+    if (x == 0.0) return 1.0;
+    x = x * M_PI;
+    return sin(x) / x;
+}
+double lanczos_filter(double x) { return (-3.0 <= x && x < 3.0) ? sinc_filter(x) * sinc_filter(x / 3) : 0.0; }
+
+__device__ __forceinline__ int clamp8(int acc) {
+    const int v = acc >> kPrecisionBits;
+    return v < 0 ? 0 : (v > 255 ? 255 : v);
+}
+
+__global__ void __launch_bounds__(256) resample_h_kernel(const ResampleFrame *__restrict__ frames, const uint8_t *__restrict__ input,
+                                                         const uint8_t *__restrict__ scratch, uint8_t *__restrict__ inter) {
+    extern __shared__ uint4 smem[];
+    const ResampleFrame &f = frames[blockIdx.y];
+    if (f.tw == f.w) return;
+    const uint32_t rows = f.y1 - f.y0, r0 = blockIdx.x * kResampleRows;
+    if (r0 >= rows) return;
+    const uint32_t r1 = min(rows, r0 + kResampleRows), nc = f.ncomp, outs = f.tw * nc, ksize = f.h_ksize;
+    uint8_t *row_s = reinterpret_cast<uint8_t *>(smem);
+    int32_t *coef_s = reinterpret_cast<int32_t *>(row_s + kResampleRowSmem);
+    const int32_t *bounds = reinterpret_cast<const int32_t *>(input + f.h_bounds);
+    const int32_t *coef = reinterpret_cast<const int32_t *>(input + f.h_coef);
+    const bool row_staged = (f.stage & kStageRow) != 0;
+    if (f.stage & kStageCoef) {  // (the table is padded to 16 bytes in the input buffer)
+        const uint32_t n16 = ((uint32_t)f.tw * ksize + 3) / 4;
+        for (uint32_t k = threadIdx.x; k < n16; k += 256) reinterpret_cast<uint4 *>(coef_s)[k] = __ldg(reinterpret_cast<const uint4 *>(coef) + k);
+        coef = coef_s;
+    }
+    __syncthreads();
+    for (uint32_t r = r0; r < r1; r++) {
+        const uint8_t *src = scratch + f.src + (uint64_t)(f.y0 + r) * f.src_pitch;
+        if (row_staged) {  // a scratch row is 16-byte aligned and padded to 16 bytes
+            for (uint32_t k = threadIdx.x; k < f.src_pitch / 16; k += 256)
+                reinterpret_cast<uint4 *>(row_s)[k] = __ldg(reinterpret_cast<const uint4 *>(src) + k);
+            __syncthreads();
+            src = row_s;
+        }
+        uint8_t *o = inter + f.inter + (uint64_t)r * outs;
+        for (uint32_t k = threadIdx.x; k < outs; k += 256) {
+            const uint32_t x = k / nc, c = k - x * nc;
+            const int xmin = __ldg(bounds + 2 * x), n = __ldg(bounds + 2 * x + 1);
+            const int32_t *kk = coef + (uint64_t)x * ksize;
+            const uint8_t *s = src + (uint32_t)xmin * nc + c;
+            int acc = 1 << (kPrecisionBits - 1);
+            for (int t = 0; t < n; t++) acc += kk[t] * (int)s[(uint32_t)t * nc];
+            o[k] = (uint8_t)clamp8(acc);
+        }
+        if (row_staged) __syncthreads();  // the row buffer is rewritten for the next row
+    }
+}
+
+template <bool kFloat>
+__global__ void __launch_bounds__(256) resample_v_kernel(const ResampleFrame *__restrict__ frames, const uint8_t *__restrict__ input,
+                                                         const uint8_t *__restrict__ scratch, const uint8_t *__restrict__ inter, FloatDst out) {
+    const ResampleFrame &f = frames[blockIdx.y];
+    const uint64_t i = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (i >= (uint64_t)f.tw * f.th) return;
+    const uint32_t y = (uint32_t)(i / f.tw), x = (uint32_t)(i - (uint64_t)y * f.tw), nc = f.ncomp;
+    const bool hpass = f.tw != f.w;
+    const uint8_t *src = hpass ? inter + f.inter : scratch + f.src;  // row 0 of src is row y0 of C
+    const uint64_t pitch = hpass ? (uint64_t)f.tw * nc : f.src_pitch;
+    int acc[B200JPG_MAX_COMPONENTS];
+    if (f.th != f.h) {
+        const int32_t *vb = reinterpret_cast<const int32_t *>(input + f.v_bounds);
+        const int32_t *kk = reinterpret_cast<const int32_t *>(input + f.v_coef) + (uint64_t)y * f.v_ksize;
+        const int n = __ldg(vb + 2 * y + 1);
+        const uint8_t *col = src + (uint64_t)(__ldg(vb + 2 * y) - (int)f.y0) * pitch + (uint64_t)x * nc;
+#pragma unroll
+        for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) acc[c] = 1 << (kPrecisionBits - 1);
+        for (int t = 0; t < n; t++) {
+            const int k = __ldg(kk + t);
+            const uint8_t *p = col + (uint64_t)t * pitch;
+#pragma unroll
+            for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++)
+                if (c < (int)nc) acc[c] += k * (int)__ldg(p + c);
+        }
+#pragma unroll
+        for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) acc[c] = clamp8(acc[c]);
+    } else {
+        const uint8_t *p = src + (uint64_t)y * pitch + (uint64_t)x * nc;
+#pragma unroll
+        for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) acc[c] = c < (int)nc ? (int)__ldg(p + c) : 0;
+    }
+#pragma unroll
+    for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) {
+        if (c >= (int)nc) break;
+        uint8_t *o = plane_at(out.planes + 4u * f.plane + c, (int)x, (int)y);
+        if constexpr (kFloat) store_elem(out.type, o, convert_int(acc[c], pick4(out.scale, c), pick4(out.bias, c)));
+        else *o = (uint8_t)acc[c];
+    }
+}
+
+}  // namespace
+
+int resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, std::vector<int32_t> &bounds, std::vector<int32_t> &coef,
+                          uint32_t &ksize) {
+    double (*filter)(double);
+    double s;
+    switch (resample) {
+    case B200JPG_RESAMPLE_BOX: filter = box_filter, s = 0.5; break;
+    case B200JPG_RESAMPLE_BILINEAR: filter = bilinear_filter, s = 1.0; break;
+    case B200JPG_RESAMPLE_HAMMING: filter = hamming_filter, s = 1.0; break;
+    case B200JPG_RESAMPLE_BICUBIC: filter = bicubic_filter, s = 2.0; break;
+    case B200JPG_RESAMPLE_LANCZOS: filter = lanczos_filter, s = 3.0; break;
+    default: return B200JPG_ERR_INVALID_PARAMETER;
+    }
+    if (in_size == 0 || out_size == 0) return B200JPG_ERR_INVALID_PARAMETER;
+    const double scale = (double)in_size / out_size, fs = std::max(scale, 1.0), support = s * fs;
+    ksize = (uint32_t)ceil(support) * 2 + 1;
+    bounds.assign(2 * (size_t)out_size, 0);
+    coef.assign((size_t)out_size * ksize, 0);
+    std::vector<double> w(ksize);
+    for (uint32_t j = 0; j < out_size; j++) {
+        const double center = (j + 0.5) * scale;
+        const int64_t xmin = std::max<int64_t>((int64_t)(center - support + 0.5), 0);
+        const int64_t n = std::min<int64_t>((int64_t)(center + support + 0.5), in_size) - xmin;
+        double ww = 0.0;
+        for (int64_t t = 0; t < n; t++) {
+            w[t] = filter((t + xmin - center + 0.5) / fs);
+            ww += w[t];
+        }
+        for (int64_t t = 0; t < n; t++) {
+            const double v = ww != 0.0 ? w[t] / ww : w[t];
+            coef[(size_t)j * ksize + t] = (int32_t)(v < 0 ? -0.5 + v * (1 << kPrecisionBits) : 0.5 + v * (1 << kPrecisionBits));
+        }
+        bounds[2 * (size_t)j] = (int32_t)xmin;
+        bounds[2 * (size_t)j + 1] = (int32_t)n;
+    }
+    return B200JPG_OK;
+}
+
+int launch_resample(const ResampleLaunch &l, void *stream, int *launches) {
+    cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t gh = std::max<uint32_t>(1u, (l.max_rows + kResampleRows - 1) / kResampleRows);
+    resample_h_kernel<<<dim3(gh, l.n_frames), 256, kResampleRowSmem + kResampleCoefSmem, s>>>(l.frames, l.input, l.scratch, l.inter);
+    const uint32_t gv = (uint32_t)std::max<uint64_t>(1u, (l.max_pixels + 255) / 256);
+    FloatDst d{};
+    d.planes = l.planes;
+    if (l.convert) {
+        d.type = l.convert->type;
+        for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) d.scale[c] = l.convert->scale[c], d.bias[c] = l.convert->bias[c];
+        resample_v_kernel<true><<<dim3(gv, l.n_frames), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);
+    } else {
+        resample_v_kernel<false><<<dim3(gv, l.n_frames), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);
+    }
+    if (launches) *launches = 2;
+    return (int)cudaGetLastError();
+}
+
+}  // namespace b200jpg

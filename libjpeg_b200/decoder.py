@@ -110,6 +110,41 @@ def crop_table(crop, n):
     return table
 
 
+def resize_table(resize, n):
+    """The b200jpg_size table of BatchDecoder(resize=...): one (h, w) for every frame, or n entries each None or (h, w), as
+    non-negative integers; (0, 0) leaves a frame unresized. Raises ValueError."""
+    import numbers
+
+    def is_int(v):
+        return not isinstance(v, bool) and isinstance(v, numbers.Integral)
+
+    vals = tuple(resize)
+    if len(vals) == 2 and all(is_int(v) for v in vals):
+        vals = (vals,) * n
+    elif len(vals) != n:
+        raise ValueError("resize: %d sizes for %d frames" % (len(vals), n))
+    table = (native.SizeStruct * n)()
+    for i, r in enumerate(vals):
+        if r is None:
+            continue
+        hw = tuple(r) if isinstance(r, (tuple, list)) else None
+        if hw is None or len(hw) != 2 or not all(is_int(v) for v in hw):
+            raise ValueError("resize[%d]: expected None or two integers (h, w), got %r" % (i, r))
+        if any(v < 0 or v > 0xFFFFFFFF for v in hw):
+            raise ValueError("resize[%d]: h and w must be 0 .. 2**32 - 1, got %r" % (i, hw))
+        if (hw[0] == 0) != (hw[1] == 0):
+            raise ValueError("resize[%d]: exactly one of h and w is zero: %r" % (i, hw))
+        table[i].height, table[i].width = int(hw[0]), int(hw[1])
+    return table
+
+
+def resample_filter(name):
+    """B200JPG_RESAMPLE_* of a filter name: "box", "bilinear", "hamming", "bicubic" or "lanczos". Raises ValueError."""
+    if not isinstance(name, str) or name not in native.RESAMPLE:
+        raise ValueError("resample must be one of %s, got %r" % (", ".join(sorted(native.RESAMPLE)), name))
+    return native.RESAMPLE[name]
+
+
 def component_shapes(info, upsample=True):
     """[(h, w)] of every component of a frame as the decoder writes it: the frame size, or without upsampling each
     component's own ceil(H / suby) x ceil(W / subx)."""
@@ -271,7 +306,7 @@ class BatchDecoder:
     """One batch of codestreams: parse + pack on construction, then upload() / decode() on a CUDA stream."""
 
     def __init__(self, frames, device=-1, tolerate_bad=False, ctx=None, color_transform=True, upsample=True, downscale=1,
-                 exif_orientation=False, crop=None):
+                 exif_orientation=False, crop=None, resize=None, resample="bilinear"):
         """downscale = 2, 4 or 8 decodes every frame at ceil(W / k) x ceil(H / k) (B200JPG_FLAG_DOWNSCALE_k): each 8x8 block is
         inverse transformed straight to (8/k) x (8/k) samples, the k x k box average of its IDCT, and the rest of the
         reconstruction runs on the smaller frame. geometry(), frame_view() and plane_views() give the reduced sizes. Not to be
@@ -289,10 +324,21 @@ class BatchDecoder:
         under the rectangle are reconstructed; every scan is still decoded, and status(i) is the frame's status without the
         crop. A rectangle that is empty or leaves the frame raises NativeError (B200JPG_ERR_INVALID_PARAMETER), as does a
         crop with upsample=False (B200JPG_ERR_NOT_IMPLEMENTED); a wrong length or an entry that is not four non-negative
-        integers raises ValueError."""
+        integers raises ValueError.
+
+        resize (b200jpg_batch_create_resize) is one (h, w) for every frame, or one entry per frame: None, or (h, w). The frame's
+        output -- after downscaling, Exif orientation and the crop -- is then resized to h x w with `resample`, one of "box",
+        "bilinear", "hamming", "bicubic" and "lanczos": bit for bit what PIL's Image.resize((w, h), filter) gives for that uint8
+        image (DESIGN §13), and a float destination of decode_into() receives the resized samples through its map.
+        output_shape(), geometry(), frame_view() and the destinations of decode_into() are then h x w, so one [N, C, h, w] tensor
+        takes frames of any size. status(i) is the frame's status without the size; a 12-bit frame with a size is
+        B200JPG_ERR_NOT_IMPLEMENTED, and a size with upsample=False raises NativeError (B200JPG_ERR_NOT_IMPLEMENTED). A wrong length,
+        an entry that is not two non-negative integers, exactly one zero in a size or an unknown filter name raises ValueError."""
         if isinstance(downscale, bool) or not isinstance(downscale, int) or downscale not in native.DOWNSCALE_FLAGS:
             raise ValueError("downscale must be 1, 2, 4 or 8, got %r" % (downscale,))
         rects = None if crop is None else crop_table(crop, len(frames))
+        sizes = None if resize is None else resize_table(resize, len(frames))
+        filt = resample_filter(resample)
         self.ctx = ctx or Context(device)
         self._keep = []
         n = len(frames)
@@ -313,7 +359,7 @@ class BatchDecoder:
         self.exif_orientation = bool(exif_orientation)
         if exif_orientation:
             flags |= native.FLAG_EXIF_ORIENTATION
-        rc = lib.b200jpg_batch_create_crop(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, rects, ctypes.byref(self.handle))
+        rc = lib.b200jpg_batch_create_resize(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, rects, sizes, filt, ctypes.byref(self.handle))
         native.check(rc, self.ctx.handle)
         self._keep = []  # the batch holds its own pinned copy
         self.n = n
@@ -327,8 +373,8 @@ class BatchDecoder:
 
     def output_shape(self, i, c):
         """(h, w) of component c of frame i as decode() / decode_into() write it: the frame size divided by `downscale`
-        (rounded up), or without upsampling the component's own size; the rectangle's size for a cropped frame. Raises
-        NativeError for a frame that failed."""
+        (rounded up), or without upsampling the component's own size; the rectangle's size for a cropped frame, the target size
+        for a resized one. Raises NativeError for a frame that failed."""
         w, h = ctypes.c_uint32(), ctypes.c_uint32()
         native.check(lib.b200jpg_batch_output_extent(self.handle, i, c, ctypes.byref(w), ctypes.byref(h)), self.ctx.handle)
         return h.value, w.value
@@ -472,7 +518,7 @@ class BatchDecoder:
 
     def frame_view(self, out, i):
         """Frame i of a decoded output tensor as [H, W, C] (H x W reduced by `downscale`, swapped by an applied Exif orientation
-        5..8, the rectangle's size for a cropped frame)."""
+        5..8, the rectangle's size for a cropped frame, the target size for a resized one)."""
         fi = self.info(i)
         off = self.out_offset(i)
         h, w = self._shape(i, 0, fi)

@@ -41,10 +41,16 @@ class RectStruct(ctypes.Structure):
     _fields_ = [("x", ctypes.c_uint32), ("y", ctypes.c_uint32), ("width", ctypes.c_uint32), ("height", ctypes.c_uint32)]
 
 
+class SizeStruct(ctypes.Structure):
+    """b200jpg_size: a target size of b200jpg_batch_create_resize; all zero = not resized."""
+    _fields_ = [("width", ctypes.c_uint32), ("height", ctypes.c_uint32)]
+
+
 SAMPLE_F32, SAMPLE_F16, SAMPLE_BF16 = 1, 2, 3
 FLAG_NO_COLOR_TRANSFORM, FLAG_NO_UPSAMPLE = 1, 2
 DOWNSCALE_FLAGS = {1: 0x0, 2: 0x4, 4: 0x8, 8: 0xC}  # B200JPG_FLAG_DOWNSCALE_k
 FLAG_EXIF_ORIENTATION = 0x10
+RESAMPLE = {"lanczos": 1, "bilinear": 2, "bicubic": 3, "box": 4, "hamming": 5}  # B200JPG_RESAMPLE_*, PIL's values
 
 
 def library_path():
@@ -71,6 +77,9 @@ def _load():
         "b200jpg_batch_create_ex": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.c_uint, ctypes.POINTER(vp)]),
         "b200jpg_batch_create_crop": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.c_uint,
                                             ctypes.POINTER(RectStruct), ctypes.POINTER(vp)]),
+        "b200jpg_batch_create_resize": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.c_uint,
+                                              ctypes.POINTER(RectStruct), ctypes.POINTER(SizeStruct), i32, ctypes.POINTER(vp)]),
+        "b200jpg_resample_coefficients": (i32, [ctypes.c_uint32, ctypes.c_uint32, i32, vp, vp, u64, ctypes.POINTER(ctypes.c_uint32)]),
         "b200jpg_batch_destroy": (None, [vp]),
         "b200jpg_batch_frame_info": (i32, [vp, i32, ctypes.POINTER(FrameInfoStruct)]),
         "b200jpg_batch_output_extent": (i32, [vp, i32, i32, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint32)]),
@@ -124,7 +133,7 @@ ABI_SYMBOLS = [
     "b200jpg_batch_last_launch_count", "b200jpg_batch_enable_timing", "b200jpg_batch_last_timing", "b200jpg_batch_last_unstuff_ms", "b200jpg_decode_to_host", "b200jpg_decode_to_host_ex", "b200jpg_decode_to_device_ex",
     "b200jpg_device_free", "b200jpg_device_copy_rect", "b200jpg_selftest_restartless", "b200jpg_selftest_restartless_items",
     "b200jpg_selftest_table_cache", "b200jpg_microbench_int32", "b200jpg_exif_orientation", "b200jpg_batch_frame_orientation",
-    "b200jpg_batch_create_crop", "b200jpg_output_size",
+    "b200jpg_batch_create_crop", "b200jpg_output_size", "b200jpg_batch_create_resize", "b200jpg_resample_coefficients",
 ]
 
 
