@@ -142,6 +142,25 @@ B200JPG_API int b200jpg_batch_create(b200jpg_ctx *ctx, const uint8_t *const *fra
  * before it reuses its pinned staging slot. Without oriented (or cropped, b200jpg_batch_create_crop) frames these calls stay as
  * before: no copy, no host wait. */
 #define B200JPG_FLAG_EXIF_ORIENTATION 0x10u
+/* Output modes (DESIGN §14; no counterpart in the reference): every frame of the batch leaves with the same number of components,
+ * whatever it was coded with. B200JPG_FLAG_OUTPUT_RGB: 3 components. A 3-component frame is written as without the flag; a grey
+ * frame's sample v goes to all three components (PIL's convert("RGB") of an L image), 8- and 12-bit alike.
+ * B200JPG_FLAG_OUTPUT_L: 1 component. A grey frame is written as without the flag; a YCbCr frame (ycbcr == 1) as its component 0
+ * with B200JPG_FLAG_NO_COLOR_TRANSFORM, the luma upsampled to the frame size (libjpeg's JCS_GRAYSCALE output) -- reconstructed
+ * alone, its chroma entropy decoded but never transformed; a 3-component frame without colour transformation (ycbcr == 0) and a JPEG
+ * XT frame after its merge as L = (19595 R + 38470 G + 7471 B + 32768) >> 16 of the clamped samples (PIL's convert("L")).
+ * The mode is a per-pixel map between the colour transformation (and clamp) and the Exif orientation: the composition is
+ * downscale -> mode -> orientation -> crop -> resize -> float map, whose scale[c] / bias[c] are those of the OUTPUT component c.
+ * b200jpg_batch_output_extent (c below the output component count), out_bytes / out_offset (h x w x output components per slot)
+ * and the descriptors of b200jpg_batch_decode_into(_ex) follow the output components (b200jpg_batch_output_components). A frame's
+ * status is its status without the mode; a frame of 2 or 4 components has the status B200JPG_ERR_NOT_IMPLEMENTED (it fails the
+ * call, or with tolerate_bad it is skipped). Both bits, or a mode bit with B200JPG_FLAG_NO_COLOR_TRANSFORM, is
+ * B200JPG_ERR_INVALID_PARAMETER for the call; a mode bit with B200JPG_FLAG_NO_UPSAMPLE is B200JPG_ERR_NOT_IMPLEMENTED. Accepted
+ * wherever request flags are (b200jpg_output_size answers as without them). b200jpg_batch_decode / b200jpg_batch_reconstruct
+ * describe the slots of the frames whose mode changes them like those of oriented frames: one small H2D copy per call. Without
+ * either bit a batch is planned exactly as before. */
+#define B200JPG_FLAG_OUTPUT_RGB 0x20u
+#define B200JPG_FLAG_OUTPUT_L 0x40u
 B200JPG_API int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
                             unsigned flags, b200jpg_batch **batch);
 /* A rectangle of a frame's output: columns x .. x + width - 1, rows y .. y + height - 1. {0, 0, 0, 0} is the whole frame. */
@@ -221,6 +240,9 @@ B200JPG_API int b200jpg_batch_frame_info(const b200jpg_batch *batch, int i, b200
  * status for a frame that failed (nothing written), or B200JPG_ERR_INVALID_PARAMETER. b200jpg_batch_frame_info keeps the
  * codestream's geometry. */
 B200JPG_API int b200jpg_batch_output_extent(const b200jpg_batch *batch, int i, int c, uint32_t *width, uint32_t *height);
+/* The number of components frame i is written with: its own, or 3 / 1 with B200JPG_FLAG_OUTPUT_RGB / B200JPG_FLAG_OUTPUT_L. The
+ * frame's status for a frame that failed, B200JPG_ERR_INVALID_PARAMETER for a bad index. */
+B200JPG_API int b200jpg_batch_output_components(const b200jpg_batch *batch, int i);
 /* Frame i's Exif orientation 1..8, whether or not the batch applies it (B200JPG_FLAG_EXIF_ORIENTATION); the frame's status for a
  * frame that failed, B200JPG_ERR_INVALID_PARAMETER for a bad index. */
 B200JPG_API int b200jpg_batch_frame_orientation(const b200jpg_batch *batch, int i);

@@ -138,6 +138,7 @@ struct ReconGroup {
     int orientation = 1;  // B200JPG_FLAG_EXIF_ORIENTATION: the frames' orientation; 2..8 store through rewritten descriptors
     bool cropped = false; // b200jpg_batch_create_crop: the frames' tiles cover their rectangles, clipped stores (FrameRecon::clip_*)
     bool resized = false; // b200jpg_batch_create_resize: cropped frames stored as uint8 into the scratch, never converted
+    OutMode mode = OutMode::Coded;  // B200JPG_FLAG_OUTPUT_RGB / _L: the frames' slots are described (rewritten descriptors)
     std::vector<FrameRecon> frames;
     uint32_t max_bw0 = 0, max_bh0 = 0, max_bwc = 0, max_bhc = 0;
     uint64_t dev_frames = 0;
@@ -163,6 +164,7 @@ struct Extent {
 };
 // the factor k of B200JPG_FLAG_DOWNSCALE_k: 1, 2, 4 or 8
 uint32_t downscale_of(unsigned flags) { return 1u << ((flags & B200JPG_FLAG_DOWNSCALE_MASK) >> 2); }
+constexpr unsigned kOutputModes = B200JPG_FLAG_OUTPUT_RGB | B200JPG_FLAG_OUTPUT_L;
 
 bool rect_empty(const b200jpg_rect &r) { return r.x == 0 && r.y == 0 && r.width == 0 && r.height == 0; }
 bool size_empty(const b200jpg_size &s) { return s.width == 0 && s.height == 0; }
@@ -318,6 +320,7 @@ struct b200jpg_batch {
     int resample = 0;
     std::vector<ResampleFrame> rs_frames;
     std::vector<int> rs_user, rs_index;  // [resized] caller frame; [n_user] index into rs_frames or -1
+    uint32_t rs_plain = 0;  // resized frames [rs_plain, ..) are grey frames of B200JPG_FLAG_OUTPUT_RGB (ResampleLaunch::n_plain)
     std::vector<std::array<std::vector<int32_t>, 4>> rs_tables;
     uint64_t dev_rs_frames = 0;
     uint32_t rs_max_rows = 0;
@@ -619,6 +622,12 @@ static void attach_residuals(b200jpg_batch &b, Codestreams &cs, bool device_inde
             cs.err[i] = "only 8-bit frames are resized";
             continue;
         }
+        const int ncomp = b.frames[i].info.ncomp;
+        if (b.parse_status[i] == 0 && (b.flags & kOutputModes) && ncomp != 1 && ncomp != 3) {
+            b.parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;  // never written with its own components
+            cs.err[i] = "an output mode takes frames of one or three components";
+            continue;
+        }
         if (b.parse_status[i] != 0 || !b.frames[i].xt.present) continue;
         if (b.flags & (B200JPG_FLAG_NO_COLOR_TRANSFORM | B200JPG_FLAG_NO_UPSAMPLE)) {
             b.parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;
@@ -753,6 +762,43 @@ static ReconPath recon_path(const b200jpg_batch &b, int i) {
     return scaled ? ReconPath::Scaled : ReconPath::Tiled;
 }
 
+// What live frame i reconstructs and what it writes (B200JPG_FLAG_OUTPUT_RGB / _L, DESIGN §14): the path, the components the
+// reconstruction covers and the components the frame leaves with. Without a mode bit: recon_path and the frame's own components.
+struct FramePlan {
+    ReconPath path;
+    uint32_t ncomp;      // components reconstructed, from component 0 on
+    uint32_t out_ncomp;  // components written
+    OutMode mode;
+};
+
+static FramePlan frame_plan(const b200jpg_batch &b, int i) {
+    if (b.xt_parent[i] >= 0) {  // a JPEG XT residual codestream stays in its frame's group: the frame's plan
+        FramePlan p = frame_plan(b, b.xt_parent[i]);
+        p.ncomp = b.frames[i].info.ncomp;  // (the frame's own: parse_residual checks that they agree)
+        return p;
+    }
+    const b200jpg_frame_info &fi = b.frames[i].info;
+    FramePlan p{recon_path(b, i), fi.ncomp, fi.ncomp, OutMode::Coded};
+    const bool xt = i < b.n_user && b.xt_child[i] >= 0;
+    if ((b.flags & B200JPG_FLAG_OUTPUT_L) && fi.ncomp == 3) {
+        p.out_ncomp = 1;
+        if (fi.ycbcr && !xt) {
+            // luma alone: a grey frame over component 0 on the MCU-padded block grid; libjpeg's JCS_GRAYSCALE for YCbCr input
+            p.ncomp = 1;
+            if (downscale_of(b.flags) > 1) p.path = ReconPath::Scaled;
+            else p.path = (fi.precision != 8 || fi.subx[0] != 1 || fi.suby[0] != 1) ? ReconPath::Generic : ReconPath::Tiled;
+        } else {  // RGB-coded and JPEG XT frames: the L formula after the colour transformation (merge) and clamp, in the generic kernels
+            p.mode = OutMode::Luma;
+            p.path = downscale_of(b.flags) > 1 ? ReconPath::Scaled : ReconPath::Generic;
+        }
+    }
+    if ((b.flags & B200JPG_FLAG_OUTPUT_RGB) && fi.ncomp == 1) {
+        p.out_ncomp = 3;
+        p.mode = OutMode::Replicate;
+    }
+    return p;
+}
+
 // Coefficient, sample and output layout of the live frames; returns the sample plane offsets. The sample planes a frame gets
 // follow its reconstruction path: Generic one per component, Tiled one per component from 1 on, Fused420 none (its chroma samples
 // live in shared memory), Scaled one per component of 8 ceil(blocks_w / k) x 8 ceil(blocks_h / k) samples, Scaled420 none.
@@ -766,19 +812,22 @@ static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
     for (int i = 0; i < n; i++) {
         if (b.parse_status[i] != 0) continue;
         const b200jpg_frame_info &fi = b.frames[i].info;
-        const ReconPath path = recon_path(b, i);
+        const FramePlan plan = frame_plan(b, i);
+        const ReconPath path = plan.path;
         const int first_plane = (path == ReconPath::Generic || path == ReconPath::Scaled) ? 0 : (path == ReconPath::Tiled ? 1 : fi.ncomp);
         const uint32_t k = downscale_of(b.flags);
         uint64_t samples = 0;
-        for (int c = 0; c < fi.ncomp; c++) {
+        for (int c = 0; c < fi.ncomp; c++) {  // every component is entropy decoded; only the reconstructed ones get sample planes
             const uint64_t elems = (uint64_t)fi.blocks_w[c] * fi.blocks_h[c] * 64;
             b.coef_base[i][c] = coef_cur;
             coef_cur += elems;
-            if (c >= first_plane) {
+            if (c >= first_plane && c < (int)plan.ncomp) {
                 sample_base[i][c] = sample_cur;
                 sample_cur += path == ReconPath::Scaled ? 64ull * ((fi.blocks_w[c] + k - 1) / k) * ((fi.blocks_h[c] + k - 1) / k) : elems;
             }
-            const Extent e = out_extent(fi, c, b.flags, 1, crop_of(b, i), size_of(b, i));  // the components one after the other (w * h: any orientation)
+        }
+        for (uint32_t c = 0; c < plan.out_ncomp; c++) {
+            const Extent e = out_extent(fi, (int)c, b.flags, 1, crop_of(b, i), size_of(b, i));  // the components one after the other (w * h: any orientation)
             samples += e.w * e.h;
         }
         b.out_off[i] = out_cur;
@@ -992,27 +1041,33 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         if (b.parse_status[i] != 0) continue;
         const b200jpg_frame_info &fi = b.frames[i].info;
         const int xt_res = (i < b.n_user) ? b.xt_child[i] : -1;  // JPEG XT: this frame's residual frame
-        const ReconPath path = recon_path(b, i);
+        const FramePlan plan = frame_plan(b, i);
+        const ReconPath path = plan.path;
+        const uint32_t nc = plan.ncomp;
         const bool generic = path == ReconPath::Generic || path == ReconPath::Scaled;
-        uint32_t sx = fi.ncomp > 1 ? fi.subx[1] : 1, sy = fi.ncomp > 1 ? fi.suby[1] : 1;
+        uint32_t sx = nc > 1 ? fi.subx[1] : 1, sy = nc > 1 ? fi.suby[1] : 1;
         if (generic) sx = sy = 0;  // one group per component count: the generic kernels read the factors per frame
         // oriented frames (B200JPG_FLAG_EXIF_ORIENTATION, 2..8) form groups of their own, one per orientation: their destinations
         // are rewritten descriptors, whose store kind is chosen per group
         const int orientation = applied_orientation(b, i);
         // cropped frames too: their launches are sized by the tiles the rectangles cover, and they always store clipped
         const b200jpg_rect *crop = crop_of(b, i);
-        if (orientation != 1 || crop) b.rewritten = true;
         // resized frames too (every one of them is cropped, admit_sizes): they store into the scratch, unconverted
         const bool resized = size_of(b, i) != nullptr;
+        // and the frames of an output mode, keyed by it, their slots described like those of oriented frames. A resized grey frame
+        // of B200JPG_FLAG_OUTPUT_RGB writes its one channel into the scratch: the resample pass replicates it
+        const OutMode mode = (resized && plan.mode == OutMode::Replicate) ? OutMode::Coded : plan.mode;
+        if (orientation != 1 || crop || plan.mode != OutMode::Coded) b.rewritten = true;
         ReconGroup *g = nullptr;
         for (auto &gg : b.groups)
-            if (gg.ncomp == fi.ncomp && gg.subx == sx && gg.suby == sy && gg.path == path && gg.orientation == orientation && gg.cropped == (crop != nullptr) &&
-                gg.resized == resized)
+            if (gg.ncomp == nc && gg.subx == sx && gg.suby == sy && gg.path == path && gg.orientation == orientation && gg.cropped == (crop != nullptr) &&
+                gg.resized == resized && gg.mode == mode)
                 g = &gg;
         if (!g) {
             b.groups.emplace_back();
             g = &b.groups.back();
-            g->ncomp = fi.ncomp;
+            g->ncomp = nc;
+            g->mode = mode;
             g->subx = sx;
             g->suby = sy;
             g->path = path;
@@ -1022,7 +1077,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         }
         FrameRecon fr{};
         const uint32_t k = downscale_of(b.flags);
-        for (int c = 0; c < fi.ncomp; c++) {
+        for (uint32_t c = 0; c < nc; c++) {
             fr.coef_base[c] = b.coef_base[i][c];
             fr.sample_base[c] = sample_base[i][c];
             fr.bw[c] = fi.blocks_w[c];
@@ -1051,7 +1106,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
                 fr.res_csy[c] = ri.suby[c];
             }
         }
-        fr.ncomp = fi.ncomp;
+        fr.ncomp = nc;
         fr.ycbcr = (b.flags & B200JPG_FLAG_NO_COLOR_TRANSFORM) ? 0 : fi.ycbcr;  // JPGTAG_MATRIX_LTRAFO = ..._NONE (rectanglerequest.cpp:150-152)
         fr.subx = sx;
         fr.suby = sy;
@@ -1068,7 +1123,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
             fr.clip_x0 = cl.x0, fr.clip_y0 = cl.y0, fr.clip_x1 = cl.x1, fr.clip_y1 = cl.y1;
             fr.tx0 = cl.x0 / tw, fr.ty0 = cl.y0 / th;
             const uint32_t ntx = (cl.x1 - 1) / tw - fr.tx0 + 1, nty = (cl.y1 - 1) / th - fr.ty0 + 1;
-            if (path == ReconPath::Tiled && fi.ncomp > 1) {
+            if (path == ReconPath::Tiled && nc > 1) {
                 // b1: the chroma blocks under those tiles, one more on each side (the upsampling window), clipped to the plane
                 const int64_t cbx0 = (int64_t)fr.tx0 * t.bw / sx - 1, cby0 = (int64_t)fr.ty0 * t.bh / sy - 1;
                 const int64_t cbx1 = (int64_t)(fr.tx0 + ntx) * t.bw / sx + 1, cby1 = (int64_t)(fr.ty0 + nty) * t.bh / sy + 1;
@@ -1085,9 +1140,9 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         }
         g->frames.push_back(fr);
         if (generic) {  // the largest block grid of any component: the extent of the generic (or scaled) IDCT launch
-            for (int c = 0; c < fi.ncomp; c++)
+            for (uint32_t c = 0; c < nc; c++)
                 if ((uint64_t)fi.blocks_w[c] * fi.blocks_h[c] > (uint64_t)g->max_bwc * g->max_bhc) g->max_bwc = fi.blocks_w[c], g->max_bhc = fi.blocks_h[c];
-        } else if (fi.ncomp > 1 && !crop) {  // (a cropped Tiled frame: its chroma block range above)
+        } else if (nc > 1 && !crop) {  // (a cropped Tiled frame: its chroma block range above)
             g->max_bwc = std::max(g->max_bwc, fi.blocks_w[1]);
             g->max_bhc = std::max(g->max_bhc, fi.blocks_h[1]);
         }
@@ -1242,7 +1297,7 @@ static int admit_sizes(b200jpg_batch &b, const b200jpg_size *sizes) {
         if (b.parse_status[i] != 0) s = b200jpg_size{0, 0};
         if (size_empty(s)) continue;
         const b200jpg_frame_info &fi = b.frames[i].info;
-        if (s.width > (1u << 24) || s.height > (1u << 24) || (uint64_t)s.width * s.height * fi.ncomp > (1ull << 34))
+        if (s.width > (1u << 24) || s.height > (1u << 24) || (uint64_t)s.width * s.height * frame_plan(b, i).out_ncomp > (1ull << 34))
             return b.ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "frame " + std::to_string(i) + ": target size " + std::to_string(s.width) + " x " +
                                                               std::to_string(s.height) + " is too large to allocate");
         if (rect_empty(b.crop[i])) {
@@ -1255,14 +1310,17 @@ static int admit_sizes(b200jpg_batch &b, const b200jpg_size *sizes) {
 
 // The resample descriptors and tables of the resized frames (tables built on host threads, one frame each) and the layout of the
 // scratch (C: h rows of align16(w * ncomp) bytes per frame) and of the intermediate (rows y0 .. y1 - 1 of tw * ncomp bytes, for
-// frames whose width changes)
+// frames whose width changes). The grey frames of B200JPG_FLAG_OUTPUT_RGB come last, with one channel: the vertical pass replicates it.
 static void plan_resample(b200jpg_batch &b) {
     b.rs_index.assign(b.n_user, -1);
-    for (int i = 0; i < b.n_user; i++)
-        if (b.parse_status[i] == 0 && size_of(b, i)) {
-            b.rs_index[i] = (int)b.rs_user.size();
-            b.rs_user.push_back(i);
-        }
+    for (int rgb = 0; rgb < 2; rgb++) {
+        for (int i = 0; i < b.n_user; i++)
+            if (b.parse_status[i] == 0 && size_of(b, i) && (frame_plan(b, i).mode == OutMode::Replicate) == (rgb == 1)) {
+                b.rs_index[i] = (int)b.rs_user.size();
+                b.rs_user.push_back(i);
+            }
+        if (rgb == 0) b.rs_plain = (uint32_t)b.rs_user.size();
+    }
     const int nr = (int)b.rs_user.size();
     b.rs_frames.assign(nr, ResampleFrame{});
     b.rs_tables.assign(nr, {});
@@ -1273,7 +1331,9 @@ static void plan_resample(b200jpg_batch &b) {
         const b200jpg_size &s = *size_of(b, i);
         ResampleFrame &f = b.rs_frames[r];
         auto &t = b.rs_tables[r];
-        f.w = (uint32_t)e.w, f.h = (uint32_t)e.h, f.tw = s.width, f.th = s.height, f.ncomp = fi.ncomp;
+        const FramePlan plan = frame_plan(b, i);  // C has the components the reconstruction stores
+        f.w = (uint32_t)e.w, f.h = (uint32_t)e.h, f.tw = s.width, f.th = s.height;
+        f.ncomp = plan.mode == OutMode::Replicate ? plan.ncomp : plan.out_ncomp;
         f.src_pitch = (uint32_t)align_up((uint64_t)f.w * f.ncomp, 16);
         f.plane = (uint32_t)(b.n + r);
         f.y0 = 0, f.y1 = f.h;
@@ -1320,6 +1380,12 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
         return ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, "crop rectangles are not supported with B200JPG_FLAG_NO_UPSAMPLE");
     if (sizes && (flags & B200JPG_FLAG_NO_UPSAMPLE))
         return ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, "target sizes are not supported with B200JPG_FLAG_NO_UPSAMPLE");
+    if ((flags & kOutputModes) == kOutputModes)
+        return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "B200JPG_FLAG_OUTPUT_RGB and B200JPG_FLAG_OUTPUT_L exclude each other");
+    if ((flags & kOutputModes) && (flags & B200JPG_FLAG_NO_UPSAMPLE))
+        return ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, "an output mode is not supported with B200JPG_FLAG_NO_UPSAMPLE");
+    if ((flags & kOutputModes) && (flags & B200JPG_FLAG_NO_COLOR_TRANSFORM))
+        return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "an output mode needs the colour transformation (no B200JPG_FLAG_NO_COLOR_TRANSFORM)");
     cudaError_t ce = cudaSetDevice(ctx->device);
     if (ce != cudaSuccess) return ctx->fail_cuda(ce, "cudaSetDevice");
 
@@ -1396,11 +1462,17 @@ int b200jpg_batch_output_extent(const b200jpg_batch *b, int i, int c, uint32_t *
     if (!b || i < 0 || i >= b->n_user || !width || !height) return B200JPG_ERR_INVALID_PARAMETER;
     if (b->parse_status[i] != 0) return b->parse_status[i];
     const b200jpg_frame_info &fi = b->frames[i].info;
-    if (c < 0 || c >= fi.ncomp) return B200JPG_ERR_INVALID_PARAMETER;
+    if (c < 0 || c >= (int)frame_plan(*b, i).out_ncomp) return B200JPG_ERR_INVALID_PARAMETER;
     const Extent e = out_extent(fi, c, b->flags, applied_orientation(*b, i), crop_of(*b, i), size_of(*b, i));
     *width = (uint32_t)e.w;
     *height = (uint32_t)e.h;
     return B200JPG_OK;
+}
+
+int b200jpg_batch_output_components(const b200jpg_batch *b, int i) {
+    if (!b || i < 0 || i >= b->n_user) return B200JPG_ERR_INVALID_PARAMETER;
+    if (b->parse_status[i] != 0) return b->parse_status[i];
+    return (int)frame_plan(*b, i).out_ncomp;
 }
 
 int b200jpg_batch_frame_orientation(const b200jpg_batch *b, int i) {
@@ -1654,12 +1726,13 @@ static int stage_planes(b200jpg_batch *b, void *stream, const std::function<void
 // Frame i's destinations, described in its output coordinates, rewritten into the decoded coordinates the kernels walk, in place:
 // translated by its crop rectangle into the uncropped output (translate_plane), then oriented (orient_plane); planar[i] cleared
 // unless every component then has bytes_per_pixel == size. Returns false when a pixel stride does not fit (only a caller's
-// descriptor can do that).
-static bool rewrite_frame(const b200jpg_batch *b, int i, b200jpg_plane *pl, uint64_t size, std::vector<char> &planar) {
+// descriptor can do that). nc: the descriptors the reconstruction stores through (frame_plan's output components, or C's in the
+// scratch).
+static bool rewrite_frame(const b200jpg_batch *b, int i, b200jpg_plane *pl, uint64_t size, std::vector<char> &planar, uint32_t nc) {
     const b200jpg_frame_info &fi = b->frames[i].info;
     const int o = applied_orientation(*b, i);
     const b200jpg_rect *crop = crop_of(*b, i);
-    for (int c = 0; c < fi.ncomp; c++) {
+    for (uint32_t c = 0; c < nc; c++) {
         const Extent d = out_extent(fi, c, b->flags, 1);
         if (crop) translate_plane(pl[c], *crop);
         if (!orient_plane(pl[c], o, d.w, d.h)) return false;
@@ -1677,7 +1750,7 @@ static void scratch_planes(const b200jpg_batch *b, int i, b200jpg_plane *pl, std
         pl[c].bytes_per_pixel = (int32_t)f.ncomp;
         pl[c].bytes_per_row = f.src_pitch;
     }
-    rewrite_frame(b, i, pl, 1, planar);  // a scratch row always fits the pixel stride
+    rewrite_frame(b, i, pl, 1, planar, f.ncomp);  // a scratch row always fits the pixel stride
 }
 
 // b200jpg_batch_decode of a batch with oriented or cropped frames: each such frame's packed slot in out_dev, seen as an interleaved
@@ -1690,29 +1763,32 @@ static int stage_slot_planes(b200jpg_batch *b, uint8_t *out_dev, void *stream, s
             const int i = b->rs_user[r];
             const ResampleFrame &f = b->rs_frames[r];
             scratch_planes(b, i, table + 4 * (size_t)i, planar);
-            for (uint32_t c = 0; c < f.ncomp; c++) {
+            const uint32_t no = frame_plan(*b, i).out_ncomp;
+            for (uint32_t c = 0; c < no; c++) {
                 b200jpg_plane &p = table[4 * (size_t)f.plane + c];
                 p.data = out_dev + b->out_off[i] + c;
-                p.bytes_per_pixel = (int32_t)f.ncomp;
-                p.bytes_per_row = (int64_t)f.tw * f.ncomp;
+                p.bytes_per_pixel = (int32_t)no;
+                p.bytes_per_row = (int64_t)f.tw * no;
             }
         }
         for (int i = 0; i < b->n_user; i++) {
-            if (b->parse_status[i] != 0 || (applied_orientation(*b, i) == 1 && !crop_of(*b, i)) || size_of(*b, i)) continue;
+            if (b->parse_status[i] != 0 || size_of(*b, i)) continue;
+            const uint32_t no = frame_plan(*b, i).out_ncomp;
             const b200jpg_frame_info &fi = b->frames[i].info;
+            if (applied_orientation(*b, i) == 1 && !crop_of(*b, i) && frame_plan(*b, i).mode == OutMode::Coded) continue;
             const int o = applied_orientation(*b, i);
             const int64_t size = fi.precision > 8 ? 2 : 1;
             const bool planes = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
             uint64_t before = 0;
             b200jpg_plane *pl = table + 4 * (size_t)i;
-            for (int c = 0; c < fi.ncomp; c++) {
-                const Extent e = out_extent(fi, c, b->flags, o, crop_of(*b, i));
+            for (uint32_t c = 0; c < no; c++) {
+                const Extent e = out_extent(fi, (int)c, b->flags, o, crop_of(*b, i));
                 pl[c].data = out_dev + b->out_off[i] + (planes ? before : (uint64_t)c) * size;
-                pl[c].bytes_per_pixel = (int32_t)(planes ? size : fi.ncomp * size);
+                pl[c].bytes_per_pixel = (int32_t)(planes ? size : no * size);
                 pl[c].bytes_per_row = (int64_t)e.w * pl[c].bytes_per_pixel;
                 before += e.w * e.h;
             }
-            rewrite_frame(b, i, pl, (uint64_t)size, planar);  // a slot's row stride always fits the pixel stride
+            rewrite_frame(b, i, pl, (uint64_t)size, planar, no);  // a slot's row stride always fits the pixel stride
         }
     });
 }
@@ -1744,6 +1820,7 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.subx = g.subx;
         l.suby = g.suby;
         l.path = g.path;
+        l.mode = g.mode;
         l.downscale = (int)downscale_of(b->flags);
         l.planes_out = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
         l.coef = b->d_coef;
@@ -1756,14 +1833,15 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.planes = planes_dev;
         l.convert = convert;
         const std::vector<char> *group_planar = planar;
-        if (slot_planes && (g.orientation != 1 || g.cropped)) l.planes = slot_planes, group_planar = &slot_planar;
+        const bool described = g.orientation != 1 || g.cropped || g.mode != OutMode::Coded;  // (by stage_slot_planes)
+        if (slot_planes && described) l.planes = slot_planes, group_planar = &slot_planar;
         if (g.resized) l.convert = nullptr;  // C leaves as uint8; the resample pass converts
         l.planar = l.planes != nullptr;
         if (l.planes)
             for (const FrameRecon &fr : g.frames) l.planar = l.planar && (*group_planar)[fr.status_idx];
         // oriented frames into anything but planar destinations: the staged store kinds, runs of eight samples along x or y; cropped
         // frames into any destination: the same kinds with the clip (the generic kernels: the strided kinds with the clip)
-        l.runs = (g.orientation != 1 || g.cropped) && l.planes && (!l.planar || g.cropped);
+        l.runs = described && l.planes && (!l.planar || g.cropped);
         l.clip = g.cropped;
         int launches = 0;
         // grid.y carries the frame index: at most 65535 frames per launch. A generic group that is cut runs the IDCT of ALL its
@@ -1794,6 +1872,7 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         rl.inter = b->d_inter;
         rl.planes = planes_dev ? planes_dev : slot_planes;
         rl.convert = convert;
+        rl.n_plain = std::min(rl.n_frames, b->rs_plain > first ? b->rs_plain - first : 0u);
         int launches = 0;
         int rc = launch_resample(rl, stream, &launches);
         if (rc != 0) return b->ctx->fail_cuda((cudaError_t)rc, "resample kernel launch");
@@ -1849,9 +1928,9 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
         if (convert->type == B200JPG_SAMPLE_F32) element = 4;
         else if (convert->type == B200JPG_SAMPLE_F16 || convert->type == B200JPG_SAMPLE_BF16) element = 2;
         else return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "unknown sample type " + std::to_string(convert->type));
-        int ncomp = 0;  // the components some live frame has
+        int ncomp = 0;  // the components some live frame is written with
         for (int i = 0; i < b->n_user; i++)
-            if (b->parse_status[i] == 0) ncomp = std::max(ncomp, (int)b->frames[i].info.ncomp);
+            if (b->parse_status[i] == 0) ncomp = std::max(ncomp, (int)frame_plan(*b, i).out_ncomp);
         for (int c = 0; c < ncomp; c++)
             if (!std::isfinite(convert->scale[c]) || !std::isfinite(convert->bias[c]))
                 return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "component " + std::to_string(c) + ": scale and bias must be finite");
@@ -1864,7 +1943,8 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
         const b200jpg_frame_info &fi = b->frames[i].info;
         const uint64_t size = convert ? element : (fi.precision > 8 ? 2 : 1);
         const int orientation = applied_orientation(*b, i);
-        for (int c = 0; c < fi.ncomp; c++) {
+        const FramePlan plan = frame_plan(*b, i);
+        for (int c = 0; c < (int)plan.out_ncomp; c++) {
             const b200jpg_plane &p = planes[4 * i + c];
             const auto [w, h] = out_extent(fi, c, b->flags, orientation, crop_of(*b, i), size_of(*b, i));  // the rules hold in (cropped, resized) output coordinates
             const uint64_t bpp = magnitude(p.bytes_per_pixel), bpr = magnitude(p.bytes_per_row);
@@ -1885,12 +1965,12 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
         }
         if (b->rewritten) {
             b200jpg_plane *q = rewritten.data() + 4 * (size_t)i;
-            memcpy(q, planes + 4 * (size_t)i, sizeof(b200jpg_plane) * fi.ncomp);
+            memcpy(q, planes + 4 * (size_t)i, sizeof(b200jpg_plane) * plan.out_ncomp);
             if (size_of(*b, i)) {  // the reconstruction stores into the scratch; the caller's descriptors go to the resample pass
                 scratch_planes(b, i, q, planar);
             } else if (orientation != 1 || crop_of(*b, i)) {  // the kernels store through the rewritten descriptors: planar is decided on those
                 planar[(size_t)i] = 1;
-                if (!rewrite_frame(b, i, q, size, planar))
+                if (!rewrite_frame(b, i, q, size, planar, plan.out_ncomp))
                     return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) +
                                                                            ": |bytes_per_row| does not fit the pixel stride of the transposed frame");
             }
@@ -1899,9 +1979,9 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
     const b200jpg_plane *src = b->rewritten ? rewritten.data() : planes;
     const int rc = stage_planes(b, stream, [&](b200jpg_plane *table) {
         for (int i = 0; i < b->n_user; i++)
-            if (b->parse_status[i] == 0) memcpy(table + 4 * (size_t)i, src + 4 * (size_t)i, sizeof(b200jpg_plane) * b->frames[i].info.ncomp);
+            if (b->parse_status[i] == 0) memcpy(table + 4 * (size_t)i, src + 4 * (size_t)i, sizeof(b200jpg_plane) * frame_plan(*b, i).out_ncomp);
         for (size_t r = 0; r < b->rs_frames.size(); r++)  // the caller's descriptors of resized frames: the resample pass's, as given
-            memcpy(table + 4 * (size_t)b->rs_frames[r].plane, planes + 4 * (size_t)b->rs_user[r], sizeof(b200jpg_plane) * b->rs_frames[r].ncomp);
+            memcpy(table + 4 * (size_t)b->rs_frames[r].plane, planes + 4 * (size_t)b->rs_user[r], sizeof(b200jpg_plane) * frame_plan(*b, b->rs_user[r]).out_ncomp);
     });
     if (rc) return rc;
     return run_decode(b, nullptr, stream, b->d_planes, &planar, convert);

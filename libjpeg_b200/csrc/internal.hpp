@@ -289,6 +289,10 @@ int launch_progressive_dequant(const ProgFrame *frames_dev, uint32_t n_frames, u
 // then the generic kernels on a FrameRecon of the reduced width and height; Scaled420 (downscaled 8-bit 4:2:0 frames with
 // upsampling): reconstruct420_scaled_kernel, no planes
 enum class ReconPath : int { Tiled, Fused420, Generic, Scaled, Scaled420 };
+// B200JPG_FLAG_OUTPUT_RGB / _L (DESIGN §14): what a reconstruction group writes besides its components as they are. Luma: the generic
+// kernels reduce three clamped components to L = (19595 R + 38470 G + 7471 B + 32768) >> 16 and store one; Replicate: a grey frame's
+// sample is stored to three components. (An L frame of a YCbCr codestream is planned as a grey frame over its component 0: Coded.)
+enum class OutMode : int { Coded, Luma, Replicate };
 inline ReconTile recon_tile(ReconPath p) {
     if (p == ReconPath::Fused420 || p == ReconPath::Scaled420) return {32, (uint32_t)kRows420};
     if (p == ReconPath::Tiled) return {32, (uint32_t)kThreadsB / 32};
@@ -301,6 +305,7 @@ struct ReconLaunch {
     uint32_t max_bwc, max_bhc;     // largest chroma block grid in the group
     uint32_t ncomp, subx, suby;    // uniform over the group
     ReconPath path;                // uniform over the group
+    OutMode mode;                  // uniform over the group; not Coded only with described destinations (never kStoreCanvas)
     bool planes_out;               // B200JPG_FLAG_NO_UPSAMPLE: the components leave as planes at their own resolution
     int generic_phase;             // generic groups: 0 = IDCT then reconstruction, 1 = IDCT only, 2 = reconstruction only
     int downscale;                 // Scaled groups: the factor k (2, 4 or 8) of B200JPG_FLAG_DOWNSCALE_k
@@ -378,6 +383,8 @@ struct ResampleLaunch {
     uint8_t *inter;
     const b200jpg_plane *planes;  // device
     const b200jpg_convert *convert;  // host; null: uint8 destinations
+    uint32_t n_plain;             // frames [n_plain, n_frames) are grey frames of B200JPG_FLAG_OUTPUT_RGB: one channel in the scratch and
+                                  // the intermediate, each resampled value stored to three destinations
 };
 int launch_resample(const ResampleLaunch &l, void *stream, int *launches);
 

@@ -763,13 +763,17 @@ __device__ __forceinline__ void to_rgb(int y, int cbv, int crv, int &r, int &g, 
 // planes. chroma_wide: a chroma sample the tile reads may leave the 32-bit colour range.
 // K: the destination kind (StoreKind). KS > 1: the frame is downscaled by KS (B200JPG_FLAG_DOWNSCALE_k) -- the luma of an output
 // block comes from the KS x KS coefficient blocks under it through scaled_idct_block instead of the 8x8 IDCT of one block.
-template <int NC, int SX, int SY, typename T, bool kWin = false, int K = kStoreCanvas, int KS = 1>
+// NO = 3 with NC = 1 (B200JPG_FLAG_OUTPUT_RGB, described kinds only): the grey row leaves through the descriptors of components 0, 1
+// and 2, each converted with its own component's map.
+template <int NC, int SX, int SY, typename T, bool kWin = false, int K = kStoreCanvas, int KS = 1, int NO = NC>
 __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, const int16_t *__restrict__ coef, const T *__restrict__ samples,
                                                  uint32_t win, bool chroma_wide, StoreDst<K> __restrict__ out) {
     static_assert(!kWin || (NC == 3 && SX == 2 && SY == 2), "the chroma window is 4:2:0 only");
     constexpr uint32_t NT = kWin ? kThreads420 : kThreadsB;  // threads per CTA: the stride of the tile [coefficient][thread]
     constexpr int KB = kBaseKind<K>;
     constexpr bool kClip = kClipKind<K>;  // a cropped frame: tile (tx0, ty0) + blockIdx, stores inside the clip rectangle only
+    constexpr bool kRep = NC == 1 && NO == 3;
+    static_assert(NO == NC || (kRep && KB != kStoreCanvas), "a grey frame leaves as three components through descriptors only");
     const uint32_t W = f.width, H = f.height;
     // blocks that carry visible pixels (cropped: pixels inside the clip rectangle)
     const uint32_t vbw = ((kClip ? f.clip_x1 : W) + 7) >> 3, vbh = ((kClip ? f.clip_y1 : H) + 7) >> 3;
@@ -897,6 +901,10 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
             if constexpr (KB == kStoreRuns || KB == kStoreRunsF) {  // staged in the line's luma slots, which are consumed
                 my[(8 * r) * NT] = (int)w0;
                 my[(8 * r + 1) * NT] = (int)w1;
+                if constexpr (kRep) {  // the same words as components 1 and 2 of the line
+                    my[(8 * r + 2) * NT] = my[(8 * r + 4) * NT] = (int)w0;
+                    my[(8 * r + 3) * NT] = my[(8 * r + 5) * NT] = (int)w1;
+                }
                 continue;
             }
             if (KB == kStoreCanvas) {
@@ -909,9 +917,13 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                 }
             } else {
                 store_row<K>(out, 0, pl, o, w0, w1, xmax);
+                if constexpr (kRep) {
+                    store_row<K>(out, 1, pl + 1, plane_at(pl + 1, X, Y + r), w0, w1, xmax);
+                    store_row<K>(out, 2, pl + 2, plane_at(pl + 2, X, Y + r), w0, w1, xmax);
+                }
             }
         }
-        if constexpr (KB == kStoreRuns || KB == kStoreRunsF) store_staged<K, 1, NT>(out, pl, my, X, Y, xmin, xmax, ymin, ymax);
+        if constexpr (KB == kStoreRuns || KB == kStoreRunsF) store_staged<K, kRep ? 3 : 1, NT>(out, pl, my, X, Y, xmin, xmax, ymin, ymax);
         return;
     }
 
@@ -1125,6 +1137,14 @@ reconstruct_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restr
             __syncwarp();
         }
     }
+}
+
+// B200JPG_FLAG_OUTPUT_RGB: the grey instance of b2 whose rows leave through three descriptors (grey frames have no exact pass)
+template <int K>
+__global__ void __launch_bounds__(kThreadsB, B200JPG_B2_MINCTAS)
+reconstruct_rgb_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, StoreDst<K> __restrict__ out) {
+    __shared__ int ys[64 * kThreadsB];
+    reconstruct_tile<1, 1, 1, int16_t, false, K, 1, 3>(frames[blockIdx.z], ys, coef, nullptr, 0u, false, out);
 }
 
 
@@ -1513,7 +1533,31 @@ __device__ void generic_upsample_block(const int32_t *__restrict__ plane, uint32
 // grid (output block columns / 64, output block rows, frames). K: kStoreCanvas, or kStoreStrided / kStoreStridedF for every
 // described destination (this path stores one sample at a time anyway); with kStoreClip (cropped frames) the grid covers the
 // tiles of kGenericTileBlocks x 1 blocks from (tx0, ty0) on, and only samples inside the clip rectangle are stored
-template <int K>
+
+// B200JPG_FLAG_OUTPUT_* (MODE = OutMode, described kinds only): the clamped samples w[0 .. nc) of pixel (x, y) as the frame's output
+// components. Luma: L = (19595 w0 + 38470 w1 + 7471 w2 + 32768) >> 16 (PIL's convert("L"), libjpeg's rgb_gray_convert; below 2^31 for
+// 12-bit samples too) into component 0; Replicate: w0 into components 0, 1 and 2, each with its own component's map
+template <int K, int MODE>
+__device__ __forceinline__ void store_mode_pixel(StoreDst<K> out, uint32_t status_idx, int x, int y, const int (&w)[4], bool deep) {
+    constexpr int KB = kBaseKind<K>;
+    static_assert(KB == kStoreStrided || KB == kStoreStridedF, "output modes store through descriptors");
+    const int v = MODE == (int)OutMode::Luma ? (19595 * w[0] + 38470 * w[1] + 7471 * w[2] + 32768) >> 16 : w[0];
+    constexpr uint32_t no = MODE == (int)OutMode::Luma ? 1u : 3u;
+#pragma unroll
+    for (uint32_t c = 0; c < no; c++) {
+        if constexpr (KB == kStoreStridedF) {
+            store_elem(out.type, plane_at(out.planes + 4u * status_idx + c, x, y), convert_int(v, pick4(out.scale, c), pick4(out.bias, c)));
+        } else {
+            uint8_t *o = plane_at(out + 4u * status_idx + c, x, y);
+            if (deep) *reinterpret_cast<uint16_t *>(o) = (uint16_t)v;
+            else *o = (uint8_t)v;
+        }
+    }
+}
+
+// MODE (OutMode): Coded, or for the groups of an output mode (B200JPG_FLAG_OUTPUT_RGB / _L) Luma or Replicate, K then kStoreStrided
+// or kStoreStridedF, with or without the clip
+template <int K, int MODE = (int)OutMode::Coded>
 __global__ void __launch_bounds__(64)
 generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restrict__ samples, StoreDst<K> __restrict__ out) {
     constexpr int KB = kBaseKind<K>;
@@ -1577,6 +1621,12 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
                 } else {
                     for (uint32_t c = 0; c < nc; c++) v[c] = ((long long)base_at(c, x, y) + 8) >> 4;
                 }
+                if constexpr (MODE != (int)OutMode::Coded) {
+                    int w[4] = {0, 0, 0, 0};
+                    for (uint32_t c = 0; c < nc; c++) w[c] = (int)clamp_to(clamp_to(v[c], 255) + ((clamp_to(res[c], 4095) + 8) >> 4) - 128, 255);
+                    store_mode_pixel<K, MODE>(out, f.status_idx, X + x, Y + y, w, false);
+                    continue;
+                }
                 for (uint32_t c = 0; c < nc; c++) {  // merge and clamp (:863-878, :935-947)
                     const uint8_t m = (uint8_t)clamp_to(clamp_to(v[c], 255) + ((clamp_to(res[c], 4095) + 8) >> 4) - 128, 255);
                     if constexpr (KB == kStoreCanvas) o[nc * x + c] = m;
@@ -1609,6 +1659,12 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
                 v[2] = (yv * 8192 + cb * 14516 + 65536) >> 17;
             } else {
                 for (uint32_t c = 0; c < nc; c++) v[c] = ((long long)base_at(c, x, y) + 8) >> 4;
+            }
+            if constexpr (MODE != (int)OutMode::Coded) {
+                int w[4] = {0, 0, 0, 0};
+                for (uint32_t c = 0; c < nc; c++) w[c] = (int)(v[c] < 0 ? 0 : (v[c] > maxval ? maxval : v[c]));
+                store_mode_pixel<K, MODE>(out, f.status_idx, X + x, Y + y, w, deep);
+                continue;
             }
             for (uint32_t c = 0; c < nc; c++) {
                 const long long w = v[c] < 0 ? 0 : (v[c] > maxval ? maxval : v[c]);
@@ -1678,6 +1734,12 @@ static StoreDst<K> dst_of(const ReconLaunch &l) {
 template <typename T, bool kListed, int K>
 static void launch_b2(const ReconLaunch &l, dim3 grid, const T *samples, cudaStream_t s) {
     const StoreDst<K> out = dst_of<K>(l);
+    if constexpr (!kListed && K != kStoreCanvas) {
+        if (l.mode == OutMode::Replicate) {
+            reconstruct_rgb_kernel<K><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, out);
+            return;
+        }
+    }
     if (l.ncomp == 1) {
         reconstruct_kernel<1, 1, 1, T, kListed, K><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, samples, l.wide_flags, l.narrow_list, out);
     } else if (l.subx == 2 && l.suby == 1) {
@@ -1750,8 +1812,14 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
             planes_out_kernel<K><<<dim3(gx, l.n_frames, l.ncomp), 256, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
         }
     } else {
-        generic_reconstruct_kernel<K><<<dim3((l.max_bw0 + kGenericTileBlocks - 1) / kGenericTileBlocks, l.max_bh0, l.n_frames), 64, 0, s>>>(l.frames, l.samples32,
-                                                                                                                                     dst_of<K>(l));
+        const dim3 grid((l.max_bw0 + kGenericTileBlocks - 1) / kGenericTileBlocks, l.max_bh0, l.n_frames);
+        bool done = false;  // an output mode's group (never the canvas: its slots are described)
+        if constexpr (K != kStoreCanvas) {
+            if (l.mode == OutMode::Luma) generic_reconstruct_kernel<K, (int)OutMode::Luma><<<grid, 64, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
+            if (l.mode == OutMode::Replicate) generic_reconstruct_kernel<K, (int)OutMode::Replicate><<<grid, 64, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
+            done = l.mode != OutMode::Coded;
+        }
+        if (!done) generic_reconstruct_kernel<K><<<grid, 64, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
     }
     if (launches) *launches = n;
     return (int)cudaGetLastError();

@@ -8,6 +8,8 @@
 //   resample_v_kernel: one thread per output pixel, all channels. The taps go down a column of the intermediate, so a warp's loads
 //     are contiguous along x and the tap's coefficient is one broadcast load; the clamped sample leaves through the caller's
 //     b200jpg_plane descriptor (any signed strides), converted by the float map of b200jpg_batch_decode_into_ex where one is given.
+//   resample_v_rgb_kernel: the same for the grey frames of B200JPG_FLAG_OUTPUT_RGB (DESIGN §14), which come last in the frame list:
+//     one channel, each value stored to three destinations.
 // The host half: resample_coefficients, the only place the fixed-point tables are built (the batch's planning and the test entry
 // point b200jpg_resample_coefficients both call it). build.py compiles this file with -ffp-contract=off: the double-precision
 // arithmetic is evaluated as written, one rounding per operation, on every host.
@@ -140,6 +142,38 @@ __global__ void __launch_bounds__(256) resample_v_kernel(const ResampleFrame *__
     }
 }
 
+// resample_v_kernel for the grey frames of B200JPG_FLAG_OUTPUT_RGB: one channel in the scratch and the intermediate, each resampled
+// value stored through the frame's three destinations, each with its own component's map
+template <bool kFloat>
+__global__ void __launch_bounds__(256) resample_v_rgb_kernel(const ResampleFrame *__restrict__ frames, const uint8_t *__restrict__ input,
+                                                             const uint8_t *__restrict__ scratch, const uint8_t *__restrict__ inter, FloatDst out) {
+    const ResampleFrame &f = frames[blockIdx.y];
+    const uint64_t i = (uint64_t)blockIdx.x * 256 + threadIdx.x;
+    if (i >= (uint64_t)f.tw * f.th) return;
+    const uint32_t y = (uint32_t)(i / f.tw), x = (uint32_t)(i - (uint64_t)y * f.tw);
+    const bool hpass = f.tw != f.w;
+    const uint8_t *src = hpass ? inter + f.inter : scratch + f.src;  // row 0 of src is row y0 of C
+    const uint64_t pitch = hpass ? (uint64_t)f.tw : f.src_pitch;
+    int v;
+    if (f.th != f.h) {
+        const int32_t *vb = reinterpret_cast<const int32_t *>(input + f.v_bounds);
+        const int32_t *kk = reinterpret_cast<const int32_t *>(input + f.v_coef) + (uint64_t)y * f.v_ksize;
+        const int n = __ldg(vb + 2 * y + 1);
+        const uint8_t *col = src + (uint64_t)(__ldg(vb + 2 * y) - (int)f.y0) * pitch + x;
+        int acc = 1 << (kPrecisionBits - 1);
+        for (int t = 0; t < n; t++) acc += __ldg(kk + t) * (int)__ldg(col + (uint64_t)t * pitch);
+        v = clamp8(acc);
+    } else {
+        v = __ldg(src + (uint64_t)y * pitch + x);
+    }
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+        uint8_t *o = plane_at(out.planes + 4u * f.plane + c, (int)x, (int)y);
+        if constexpr (kFloat) store_elem(out.type, o, convert_int(v, out.scale[c], out.bias[c]));
+        else *o = (uint8_t)v;
+    }
+}
+
 }  // namespace
 
 int resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, std::vector<int32_t> &bounds, std::vector<int32_t> &coef,
@@ -189,11 +223,21 @@ int launch_resample(const ResampleLaunch &l, void *stream, int *launches) {
     if (l.convert) {
         d.type = l.convert->type;
         for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) d.scale[c] = l.convert->scale[c], d.bias[c] = l.convert->bias[c];
-        resample_v_kernel<true><<<dim3(gv, l.n_frames), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);
-    } else {
-        resample_v_kernel<false><<<dim3(gv, l.n_frames), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);
     }
-    if (launches) *launches = 2;
+    const uint32_t n_rgb = l.n_frames - l.n_plain;
+    int n = 1;
+    if (l.n_plain) {
+        if (l.convert) resample_v_kernel<true><<<dim3(gv, l.n_plain), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);
+        else resample_v_kernel<false><<<dim3(gv, l.n_plain), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);
+        n++;
+    }
+    if (n_rgb) {
+        const ResampleFrame *rgb = l.frames + l.n_plain;
+        if (l.convert) resample_v_rgb_kernel<true><<<dim3(gv, n_rgb), 256, 0, s>>>(rgb, l.input, l.scratch, l.inter, d);
+        else resample_v_rgb_kernel<false><<<dim3(gv, n_rgb), 256, 0, s>>>(rgb, l.input, l.scratch, l.inter, d);
+        n++;
+    }
+    if (launches) *launches = n;
     return (int)cudaGetLastError();
 }
 

@@ -4,6 +4,7 @@ PyTorch is plumbing here: it owns the output tensor and the CUDA stream; every b
 in the hand-written kernels of libb200jpg.so.
 """
 import ctypes
+import threading
 from dataclasses import dataclass
 
 import numpy as np
@@ -285,6 +286,9 @@ def _batch_tensor_table(geometry, t, device_type):
 class Context:
     def __init__(self, device=-1):
         self.handle = ctypes.c_void_p()
+        self._batches = 0  # live BatchDecoders on this context (batches may be created on several threads: under the lock)
+        self._closing = False
+        self._lock = threading.Lock()
         rc = lib.b200jpg_create(device, ctypes.byref(self.handle))
         native.check(rc)
 
@@ -294,9 +298,30 @@ class Context:
             lib.b200jpg_trim(self.handle)
 
     def close(self):
-        if self.handle:
-            lib.b200jpg_destroy(self.handle)
-            self.handle = ctypes.c_void_p()
+        """Destroys the context; with batches still open, when the last of them closes: a batch returns its buffers to the
+        context's pool. (The garbage collector may finalise a context before the batches of the same reference cycle.)"""
+        lock = getattr(self, "_lock", None)
+        if lock is None:  # b200jpg_create failed
+            return
+        with lock:
+            if self._batches:
+                self._closing = True
+                return
+            if self.handle:
+                lib.b200jpg_destroy(self.handle)
+                self.handle = ctypes.c_void_p()
+
+    def _batch_opened(self):
+        with self._lock:
+            self._batches += 1
+
+    def _batch_closed(self):
+        with self._lock:
+            self._batches -= 1
+            if not (self._closing and self._batches == 0):
+                return
+            self._closing = False
+        self.close()
 
     def __del__(self):
         self.close()
@@ -306,7 +331,7 @@ class BatchDecoder:
     """One batch of codestreams: parse + pack on construction, then upload() / decode() on a CUDA stream."""
 
     def __init__(self, frames, device=-1, tolerate_bad=False, ctx=None, color_transform=True, upsample=True, downscale=1,
-                 exif_orientation=False, crop=None, resize=None, resample="bilinear"):
+                 exif_orientation=False, crop=None, resize=None, resample="bilinear", mode=None):
         """downscale = 2, 4 or 8 decodes every frame at ceil(W / k) x ceil(H / k) (B200JPG_FLAG_DOWNSCALE_k): each 8x8 block is
         inverse transformed straight to (8/k) x (8/k) samples, the k x k box average of its IDCT, and the rest of the
         reconstruction runs on the smaller frame. geometry(), frame_view() and plane_views() give the reduced sizes. Not to be
@@ -333,7 +358,19 @@ class BatchDecoder:
         output_shape(), geometry(), frame_view() and the destinations of decode_into() are then h x w, so one [N, C, h, w] tensor
         takes frames of any size. status(i) is the frame's status without the size; a 12-bit frame with a size is
         B200JPG_ERR_NOT_IMPLEMENTED, and a size with upsample=False raises NativeError (B200JPG_ERR_NOT_IMPLEMENTED). A wrong length,
-        an entry that is not two non-negative integers, exactly one zero in a size or an unknown filter name raises ValueError."""
+        an entry that is not two non-negative integers, exactly one zero in a size or an unknown filter name raises ValueError.
+
+        mode (B200JPG_FLAG_OUTPUT_RGB / _L, DESIGN §14), named after PIL's Image.convert(mode): None writes every frame with its own
+        components; "RGB" writes every frame with three -- a grey frame's sample in all three, as convert("RGB") does -- and "L"
+        with one: a YCbCr frame's luma (the component 0 that color_transform=False gives, reconstructed without its chroma), an
+        RGB-coded or JPEG XT frame's (19595 R + 38470 G + 7471 B + 32768) >> 16, as convert("L") does. The mode comes before the
+        orientation, the crop, the resize and the float map (scale[c] / bias[c] of the output component c), so a batch of grey and
+        colour frames fills one [N, 3, H, W] tensor. output_components(i) gives the count; geometry(), frame_view() and the
+        destinations of decode_into() follow it. A frame of 2 or 4 components is then B200JPG_ERR_NOT_IMPLEMENTED (skipped with
+        tolerate_bad); a mode with color_transform=False raises NativeError (B200JPG_ERR_INVALID_PARAMETER), with upsample=False
+        NativeError (B200JPG_ERR_NOT_IMPLEMENTED); any other value than None, "RGB" and "L" raises ValueError."""
+        if not isinstance(mode, (str, type(None))) or mode not in native.MODE_FLAGS:
+            raise ValueError('mode must be None, "RGB" or "L", got %r' % (mode,))
         if isinstance(downscale, bool) or not isinstance(downscale, int) or downscale not in native.DOWNSCALE_FLAGS:
             raise ValueError("downscale must be 1, 2, 4 or 8, got %r" % (downscale,))
         rects = None if crop is None else crop_table(crop, len(frames))
@@ -359,8 +396,11 @@ class BatchDecoder:
         self.exif_orientation = bool(exif_orientation)
         if exif_orientation:
             flags |= native.FLAG_EXIF_ORIENTATION
+        self.mode = mode
+        flags |= native.MODE_FLAGS[mode]
         rc = lib.b200jpg_batch_create_resize(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, rects, sizes, filt, ctypes.byref(self.handle))
         native.check(rc, self.ctx.handle)
+        self.ctx._batch_opened()
         self._keep = []  # the batch holds its own pinned copy
         self.n = n
         self.out_bytes = lib.b200jpg_batch_out_bytes(self.handle, -1)
@@ -378,6 +418,19 @@ class BatchDecoder:
         w, h = ctypes.c_uint32(), ctypes.c_uint32()
         native.check(lib.b200jpg_batch_output_extent(self.handle, i, c, ctypes.byref(w), ctypes.byref(h)), self.ctx.handle)
         return h.value, w.value
+
+    def output_components(self, i):
+        """The number of components frame i is written with: its own without a mode, 3 with mode="RGB", 1 with mode="L". Raises
+        NativeError for a frame that failed."""
+        rc = lib.b200jpg_batch_output_components(self.handle, i)
+        if rc < 0:
+            native.check(rc, self.ctx.handle)
+        return rc
+
+    def _components(self, i, fi):
+        """output_components, or for a frame that failed the component count of its partial frame info"""
+        rc = lib.b200jpg_batch_output_components(self.handle, i)
+        return rc if rc > 0 else fi.ncomp
 
     def orientation(self, i):
         """Frame i's Exif orientation 1..8, whether or not the batch applies it; the (negative) status of a frame that failed."""
@@ -457,7 +510,7 @@ class BatchDecoder:
                 s = native.FrameInfoStruct()
                 rc = lib.b200jpg_batch_frame_info(self.handle, i, ctypes.byref(s))
                 fi = FrameInfo.from_struct(s)
-                geo.append(None if rc != 0 else ([self.output_shape(i, c) for c in range(fi.ncomp)], fi.precision > 8))
+                geo.append(None if rc != 0 else ([self.output_shape(i, c) for c in range(self._components(i, fi))], fi.precision > 8))
             self._geometry = geo
         return self._geometry
 
@@ -522,11 +575,12 @@ class BatchDecoder:
         fi = self.info(i)
         off = self.out_offset(i)
         h, w = self._shape(i, 0, fi)
-        n = w * h * fi.ncomp
+        nc = self._components(i, fi)
+        n = w * h * nc
         if fi.precision > 8:  # 12-bit frames: native-endian 16-bit samples
             import torch
-            return out[off:off + 2 * n].view(torch.int16).view(h, w, fi.ncomp)
-        return out[off:off + n].view(h, w, fi.ncomp)
+            return out[off:off + 2 * n].view(torch.int16).view(h, w, nc)
+        return out[off:off + n].view(h, w, nc)
 
     def plane_views(self, out, i):
         """upsample=False: the components of frame i as planes [ceil(H/suby), ceil(W/subx)] at their own resolution (H x W
@@ -547,6 +601,7 @@ class BatchDecoder:
         if getattr(self, "handle", None):
             lib.b200jpg_batch_destroy(self.handle)
             self.handle = ctypes.c_void_p()
+            self.ctx._batch_closed()
 
     def __del__(self):
         try:
