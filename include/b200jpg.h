@@ -76,6 +76,20 @@ B200JPG_API int b200jpg_parse(const uint8_t *data, size_t len, b200jpg_frame_inf
 /* The Exif orientation 1..8 that B200JPG_FLAG_EXIF_ORIENTATION applies to this codestream (1 without a valid Exif orientation),
  * or the negative error code b200jpg_parse returns for it. Host only, no device. */
 B200JPG_API int b200jpg_exif_orientation(const uint8_t *data, size_t len);
+/* The colour space the output modes (B200JPG_FLAG_OUTPUT_RGB / _L, DESIGN §14 and §15) read a codestream's samples in. One
+ * component: GREY. Three: YCBCR when b200jpg_frame_info::ycbcr is 1, else RGB. Four, 8-bit, with an APP14 segment in front of the
+ * first scan whose payload has at least 12 bytes and starts with "Adobe" (the last such segment counts, libjpeg's examine_app14):
+ * CMYK when its transform byte (payload[11]) is 0, YCCK for any other value (libjpeg's default_decompress_parms). Anything else --
+ * two components, a four-component frame without such a segment or of 12 bits -- is UNKNOWN: a mode gives such a frame the status
+ * B200JPG_ERR_NOT_IMPLEMENTED. Returns one of B200JPG_COLORSPACE_*, or the negative error code b200jpg_parse returns for it. Host
+ * only, no device. */
+#define B200JPG_COLORSPACE_UNKNOWN 0
+#define B200JPG_COLORSPACE_GREY 1
+#define B200JPG_COLORSPACE_YCBCR 2
+#define B200JPG_COLORSPACE_RGB 3
+#define B200JPG_COLORSPACE_CMYK 4
+#define B200JPG_COLORSPACE_YCCK 5
+B200JPG_API int b200jpg_colorspace(const uint8_t *data, size_t len);
 
 /* Builds the device-independent Huffman / quantisation table blob of scan `scan` of one codestream on the host
  * (replaces HuffmanTemplate::BuildDecoder coding/huffmantemplate.cpp:802-874 and IDCT::DefineQuant dct/idct.cpp:98-108).
@@ -149,13 +163,17 @@ B200JPG_API int b200jpg_batch_create(b200jpg_ctx *ctx, const uint8_t *const *fra
  * with B200JPG_FLAG_NO_COLOR_TRANSFORM, the luma upsampled to the frame size (libjpeg's JCS_GRAYSCALE output) -- reconstructed
  * alone, its chroma entropy decoded but never transformed; a 3-component frame without colour transformation (ycbcr == 0) and a JPEG
  * XT frame after its merge as L = (19595 R + 38470 G + 7471 B + 32768) >> 16 of the clamped samples (PIL's convert("L")).
+ * A CMYK or YCCK frame (b200jpg_colorspace; DESIGN §15) is converted as Pillow converts a four-component JPEG it reads as
+ * Adobe-inverted CMYK: from the clamped samples s0..s3 written without the mode, a_c = 255 - s_c (CMYK), or a = R, G, B of libjpeg's
+ * YCC -> RGB on s0, s1, s2 (YCCK), clamped; then out_c = s3 - MULDIV255(a_c, s3) with MULDIV255(a, b) = ((t >> 8) + t) >> 8,
+ * t = a b + 128 (PIL's convert("RGB")), and under B200JPG_FLAG_OUTPUT_L the L formula of that RGB (PIL's convert("L")).
  * The mode is a per-pixel map between the colour transformation (and clamp) and the Exif orientation: the composition is
  * downscale -> mode -> orientation -> crop -> resize -> float map, whose scale[c] / bias[c] are those of the OUTPUT component c.
  * b200jpg_batch_output_extent (c below the output component count), out_bytes / out_offset (h x w x output components per slot)
  * and the descriptors of b200jpg_batch_decode_into(_ex) follow the output components (b200jpg_batch_output_components). A frame's
- * status is its status without the mode; a frame of 2 or 4 components has the status B200JPG_ERR_NOT_IMPLEMENTED (it fails the
- * call, or with tolerate_bad it is skipped). Both bits, or a mode bit with B200JPG_FLAG_NO_COLOR_TRANSFORM, is
- * B200JPG_ERR_INVALID_PARAMETER for the call; a mode bit with B200JPG_FLAG_NO_UPSAMPLE is B200JPG_ERR_NOT_IMPLEMENTED. Accepted
+ * status is its status without the mode; a frame whose b200jpg_colorspace is B200JPG_COLORSPACE_UNKNOWN (2 components, 4 without
+ * an Adobe segment or of 12 bits) has the status B200JPG_ERR_NOT_IMPLEMENTED (it fails the call, or with tolerate_bad it is
+ * skipped). Both bits, or a mode bit with B200JPG_FLAG_NO_COLOR_TRANSFORM, is B200JPG_ERR_INVALID_PARAMETER for the call; a mode bit with B200JPG_FLAG_NO_UPSAMPLE is B200JPG_ERR_NOT_IMPLEMENTED. Accepted
  * wherever request flags are (b200jpg_output_size answers as without them). b200jpg_batch_decode / b200jpg_batch_reconstruct
  * describe the slots of the frames whose mode changes them like those of oriented frames: one small H2D copy per call. Without
  * either bit a batch is planned exactly as before. */

@@ -451,6 +451,12 @@ int b200jpg_exif_orientation(const uint8_t *data, size_t len) {
     return rc != 0 ? rc : pf.orientation;
 }
 
+int b200jpg_colorspace(const uint8_t *data, size_t len) {
+    ParsedFrame pf;
+    const int rc = parse_one(data, len, pf);
+    return rc != 0 ? rc : frame_colorspace(pf);
+}
+
 int b200jpg_output_size(const uint8_t *data, size_t len, unsigned flags, uint32_t *width, uint32_t *height) {
     if (!width || !height) return B200JPG_ERR_INVALID_PARAMETER;
     ParsedFrame pf;
@@ -622,10 +628,9 @@ static void attach_residuals(b200jpg_batch &b, Codestreams &cs, bool device_inde
             cs.err[i] = "only 8-bit frames are resized";
             continue;
         }
-        const int ncomp = b.frames[i].info.ncomp;
-        if (b.parse_status[i] == 0 && (b.flags & kOutputModes) && ncomp != 1 && ncomp != 3) {
+        if (b.parse_status[i] == 0 && (b.flags & kOutputModes) && frame_colorspace(b.frames[i]) == B200JPG_COLORSPACE_UNKNOWN) {
             b.parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;  // never written with its own components
-            cs.err[i] = "an output mode takes frames of one or three components";
+            cs.err[i] = "an output mode takes grey, YCbCr, RGB, and 8-bit Adobe CMYK or YCCK frames";
             continue;
         }
         if (b.parse_status[i] != 0 || !b.frames[i].xt.present) continue;
@@ -795,6 +800,12 @@ static FramePlan frame_plan(const b200jpg_batch &b, int i) {
     if ((b.flags & B200JPG_FLAG_OUTPUT_RGB) && fi.ncomp == 1) {
         p.out_ncomp = 3;
         p.mode = OutMode::Replicate;
+    }
+    if ((b.flags & kOutputModes) && fi.ncomp == 4) {  // CMYK / YCCK (attach_residuals refused the rest): all four reconstructed,
+        const bool rgb = (b.flags & B200JPG_FLAG_OUTPUT_RGB) != 0;  // Pillow's conversion in the generic kernels (DESIGN §15)
+        p.out_ncomp = rgb ? 3 : 1;
+        p.mode = rgb ? OutMode::CmykRgb : OutMode::CmykLuma;
+        p.path = downscale_of(b.flags) > 1 ? ReconPath::Scaled : ReconPath::Generic;
     }
     return p;
 }
@@ -1108,6 +1119,8 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         }
         fr.ncomp = nc;
         fr.ycbcr = (b.flags & B200JPG_FLAG_NO_COLOR_TRANSFORM) ? 0 : fi.ycbcr;  // JPGTAG_MATRIX_LTRAFO = ..._NONE (rectanglerequest.cpp:150-152)
+        // CMYK and YCCK frames of an output mode share their groups: the YCC -> RGB step is a per-frame switch
+        fr.ycck = (plan.mode == OutMode::CmykRgb || plan.mode == OutMode::CmykLuma) && frame_colorspace(b.frames[i]) == B200JPG_COLORSPACE_YCCK;
         fr.subx = sx;
         fr.suby = sy;
         fr.cw = (uint32_t)(sx ? (reduced.w + sx - 1) / sx : reduced.w);  // (generic groups carry the factors per component: csx / csy)

@@ -80,7 +80,15 @@ struct ParsedFrame {
     // Exif orientation (tag 0x0112 of IFD0 in the first APP1 "Exif\0\0" segment in front of the first scan), 1..8; 1 when there
     // is none or it is malformed. Applied only with B200JPG_FLAG_EXIF_ORIENTATION; never changes the parse status
     int orientation = 1;
+    // the transform byte (payload[11]) of the last APP14 segment in front of the first scan whose payload has at least 12 bytes and
+    // starts with "Adobe" (libjpeg's examine_app14), -1 when there is none. Only the colour space of four-component frames follows
+    // it (frame_colorspace); three-component frames keep the reference's rule (b200jpg_frame_info::ycbcr)
+    int adobe_transform = -1;
 };
+
+// B200JPG_COLORSPACE_* of a parsed frame: grey, YCbCr / RGB by b200jpg_frame_info::ycbcr, CMYK / YCCK for an 8-bit four-component
+// frame with an Adobe segment (transform 0: CMYK, any other value: YCCK, libjpeg's default_decompress_parms), else unknown
+int frame_colorspace(const ParsedFrame &pf);
 
 // The orientation an APP1 payload (the bytes behind the length field) gives: 0 when it is not an Exif segment, else 1..8
 // (1 for anything malformed)
@@ -221,8 +229,9 @@ struct FrameRecon {       // per frame, for the reconstruction kernels
     uint32_t status_idx, precision;     // sample precision of the frame (8, or 12: generic reconstruction, 16-bit samples out)
     uint8_t csx[4], csy[4];             // generic reconstruction: subsampling factors of every component (1..4)
     // JPEG XT (generic reconstruction): bit 0 = merge with the residual image whose int32 sample planes start at
-    // res_sample_base (block grid width res_bw, factors res_csx / res_csy), bit 1 / 2 = YCbCr -> RGB on the base / residual side
-    uint32_t xt, xt_pad;
+    // res_sample_base (block grid width res_bw, factors res_csx / res_csy), bit 1 / 2 = YCbCr -> RGB on the base / residual side.
+    // ycck (groups of OutMode::CmykRgb / CmykLuma): 1 = the frame is YCCK, its first three samples go through YCC -> RGB first
+    uint32_t xt, ycck;
     uint64_t res_sample_base[4];
     uint32_t res_bw[4];
     uint8_t res_csx[4], res_csy[4];
@@ -292,7 +301,9 @@ enum class ReconPath : int { Tiled, Fused420, Generic, Scaled, Scaled420 };
 // B200JPG_FLAG_OUTPUT_RGB / _L (DESIGN §14): what a reconstruction group writes besides its components as they are. Luma: the generic
 // kernels reduce three clamped components to L = (19595 R + 38470 G + 7471 B + 32768) >> 16 and store one; Replicate: a grey frame's
 // sample is stored to three components. (An L frame of a YCbCr codestream is planned as a grey frame over its component 0: Coded.)
-enum class OutMode : int { Coded, Luma, Replicate };
+// CmykRgb / CmykLuma (DESIGN §15): the generic kernels turn four clamped samples of a CMYK or YCCK frame (FrameRecon::ycck) into
+// Pillow's convert("RGB") and store three, or into its convert("L") and store one.
+enum class OutMode : int { Coded, Luma, Replicate, CmykRgb, CmykLuma };
 inline ReconTile recon_tile(ReconPath p) {
     if (p == ReconPath::Fused420 || p == ReconPath::Scaled420) return {32, (uint32_t)kRows420};
     if (p == ReconPath::Tiled) return {32, (uint32_t)kThreadsB / 32};

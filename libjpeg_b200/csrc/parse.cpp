@@ -150,6 +150,7 @@ int parse_codestream(const uint8_t *data, size_t len, ParsedFrame &out, std::str
     memset(&fi, 0, sizeof(fi));
     out.scans.clear();
     out.orientation = 1;
+    out.adobe_transform = -1;
     bool exif_seen = false;  // the first Exif segment decides
     if (!data || len < 4) FAIL(B200JPG_ERR_UNEXPECTED_EOF, "stream is too short to be a JPEG codestream");
     if (c.u16(0) != 0xffd8) FAIL(B200JPG_ERR_MALFORMED_STREAM, "stream does not start with SOI, not a JPEG codestream");
@@ -237,7 +238,10 @@ int parse_codestream(const uint8_t *data, size_t len, ParsedFrame &out, std::str
             dri = (uint32_t)c.u16(pos + 2);
             break;
         case 0xee:  // APP14: Adobe colour information (tables.cpp:2023-2025)
-            if (rem >= 12 && memcmp(s, "Adobe", 5) == 0) adobe_none = (s[11] == 0);
+            if (rem >= 12 && memcmp(s, "Adobe", 5) == 0) {
+                adobe_none = (s[11] == 0);
+                if (out.scans.empty()) out.adobe_transform = s[11];  // libjpeg's examine_app14: the last one in front of the first scan
+            }
             break;
         case 0xe1:  // APP1: Exif orientation, read in front of the first scan only (the reference skips the segment)
             if (out.scans.empty() && !exif_seen) {
@@ -530,6 +534,15 @@ parsed:
         }
     }
     return B200JPG_OK;
+}
+
+int frame_colorspace(const ParsedFrame &pf) {
+    const b200jpg_frame_info &fi = pf.info;
+    if (fi.ncomp == 1) return B200JPG_COLORSPACE_GREY;
+    if (fi.ncomp == 3) return fi.ycbcr ? B200JPG_COLORSPACE_YCBCR : B200JPG_COLORSPACE_RGB;
+    if (fi.ncomp == 4 && fi.precision == 8 && pf.adobe_transform >= 0)
+        return pf.adobe_transform == 0 ? B200JPG_COLORSPACE_CMYK : B200JPG_COLORSPACE_YCCK;
+    return B200JPG_COLORSPACE_UNKNOWN;  // two components, an unmarked or a 12-bit four-component frame
 }
 
 uint32_t TableSet::lut_words() const {

@@ -1536,34 +1536,62 @@ __device__ void generic_upsample_block(const int32_t *__restrict__ plane, uint32
 
 // B200JPG_FLAG_OUTPUT_* (MODE = OutMode, described kinds only): the clamped samples w[0 .. nc) of pixel (x, y) as the frame's output
 // components. Luma: L = (19595 w0 + 38470 w1 + 7471 w2 + 32768) >> 16 (PIL's convert("L"), libjpeg's rgb_gray_convert; below 2^31 for
-// 12-bit samples too) into component 0; Replicate: w0 into components 0, 1 and 2, each with its own component's map
+// 12-bit samples too) into component 0; Replicate: w0 into components 0, 1 and 2, each with its own component's map. CmykRgb /
+// CmykLuma: w[0 .. 3) is the frame's RGB (cmyk_to_rgb), stored as three components / as L like Luma
 template <int K, int MODE>
 __device__ __forceinline__ void store_mode_pixel(StoreDst<K> out, uint32_t status_idx, int x, int y, const int (&w)[4], bool deep) {
     constexpr int KB = kBaseKind<K>;
     static_assert(KB == kStoreStrided || KB == kStoreStridedF, "output modes store through descriptors");
-    const int v = MODE == (int)OutMode::Luma ? (19595 * w[0] + 38470 * w[1] + 7471 * w[2] + 32768) >> 16 : w[0];
-    constexpr uint32_t no = MODE == (int)OutMode::Luma ? 1u : 3u;
+    constexpr bool kL = MODE == (int)OutMode::Luma || MODE == (int)OutMode::CmykLuma;
+    constexpr bool kRgb = MODE == (int)OutMode::CmykRgb;  // w[0 .. 3) is already the RGB of the frame (cmyk_to_rgb)
+    const int v = kL ? (19595 * w[0] + 38470 * w[1] + 7471 * w[2] + 32768) >> 16 : w[0];
+    constexpr uint32_t no = kL ? 1u : 3u;
 #pragma unroll
     for (uint32_t c = 0; c < no; c++) {
+        const int u = kRgb ? w[c] : v;
         if constexpr (KB == kStoreStridedF) {
-            store_elem(out.type, plane_at(out.planes + 4u * status_idx + c, x, y), convert_int(v, pick4(out.scale, c), pick4(out.bias, c)));
+            store_elem(out.type, plane_at(out.planes + 4u * status_idx + c, x, y), convert_int(u, pick4(out.scale, c), pick4(out.bias, c)));
         } else {
             uint8_t *o = plane_at(out + 4u * status_idx + c, x, y);
-            if (deep) *reinterpret_cast<uint16_t *>(o) = (uint16_t)v;
-            else *o = (uint8_t)v;
+            if (deep) *reinterpret_cast<uint16_t *>(o) = (uint16_t)u;
+            else *o = (uint8_t)u;
         }
     }
 }
 
-// MODE (OutMode): Coded, or for the groups of an output mode (B200JPG_FLAG_OUTPUT_RGB / _L) Luma or Replicate, K then kStoreStrided
-// or kStoreStridedF, with or without the clip
+// OutMode::CmykRgb / CmykLuma (DESIGN §15): the clamped 8-bit samples s[0 .. 4) of a CMYK or YCCK frame, in place, as the RGB that
+// Pillow's convert("RGB") gives for the frame it reads as Adobe-inverted CMYK ("CMYK;I"). YCCK: Y = s0, Cb = s1 - 128, Cr = s2 - 128
+// through libjpeg's ycck_cmyk_convert tables (arithmetic shifts), whose C = 255 - clamp(R) Pillow inverts back to a = clamp(R);
+// CMYK: a = 255 - s. Then Pillow's cmyk2rgb with nk = 255 - (255 - s3) = s3: out = s3 - MULDIV255(a, s3)
+__device__ __forceinline__ void cmyk_to_rgb(int (&s)[4], bool ycck) {
+    int a[3];
+    if (ycck) {
+        const int y = s[0], cb = s[1] - 128, cr = s[2] - 128;
+        a[0] = y + ((91881 * cr + 32768) >> 16);
+        a[1] = y + ((-22554 * cb - 46802 * cr + 32768) >> 16);
+        a[2] = y + ((116130 * cb + 32768) >> 16);
+        for (int c = 0; c < 3; c++) a[c] = a[c] < 0 ? 0 : (a[c] > 255 ? 255 : a[c]);
+    } else {
+        for (int c = 0; c < 3; c++) a[c] = 255 - s[c];
+    }
+    const int k = s[3];
+    for (int c = 0; c < 3; c++) {
+        const int t = a[c] * k + 128;  // MULDIV255
+        s[c] = k - (((t >> 8) + t) >> 8);
+    }
+}
+
+// MODE (OutMode): Coded, or for the groups of an output mode (B200JPG_FLAG_OUTPUT_RGB / _L) Luma, Replicate, CmykRgb or CmykLuma,
+// K then kStoreStrided or kStoreStridedF, with or without the clip
 template <int K, int MODE = (int)OutMode::Coded>
 __global__ void __launch_bounds__(64)
 generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restrict__ samples, StoreDst<K> __restrict__ out) {
     constexpr int KB = kBaseKind<K>;
     constexpr bool kClip = kClipKind<K>;
+    constexpr bool kCmyk = MODE == (int)OutMode::CmykRgb || MODE == (int)OutMode::CmykLuma;  // 8-bit four-component frames only
     const FrameRecon &f = frames[blockIdx.z];
-    const uint32_t W = f.width, H = f.height, nc = f.ncomp;
+    // (a CMYK / YCCK group's frames all have four components: a constant count keeps the per-component arrays in registers)
+    const uint32_t W = f.width, H = f.height, nc = kCmyk ? 4u : f.ncomp;
     const uint32_t bx = (kClip ? f.tx0 * kGenericTileBlocks : 0u) + blockIdx.x * 64 + threadIdx.x, by = (kClip ? f.ty0 : 0u) + blockIdx.y;
     if (bx >= (W + 7) / 8 || by >= (H + 7) / 8) return;
     if (kClip && (bx < f.clip_x0 / 8 || bx >= (f.clip_x1 + 7) / 8 || by < f.clip_y0 / 8 || by >= (f.clip_y1 + 7) / 8)) return;
@@ -1584,7 +1612,7 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
         xmin = max((int)f.clip_x0 - X, 0), xmax = min((int)f.clip_x1 - 1 - X, xmax);
         ymin = max((int)f.clip_y0 - Y, 0), ymax = min((int)f.clip_y1 - 1 - Y, ymax);
     }
-    if (f.xt & 1u) {
+    if (!kCmyk && (f.xt & 1u)) {  // (a four-component frame is never a JPEG XT frame: parse_codestream refuses it)
         // ---- JPEG XT (SURVEY 8f3): base image + residual image, YCbCrTrafo<..., Residual | Extended | ClampFlag, ...>::YCbCr2RGB
         // colortrafo/ycbcrtrafo.cpp:747-880 with the tables of the 8-bit integer profile (colortransformerfactory.cpp:300-352,
         // 425-520; ParametricToneMappingBox::ScaledTableOf boxes/parametrictonemappingbox.cpp:387-426): Q = identity over the
@@ -1663,6 +1691,7 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
             if constexpr (MODE != (int)OutMode::Coded) {
                 int w[4] = {0, 0, 0, 0};
                 for (uint32_t c = 0; c < nc; c++) w[c] = (int)(v[c] < 0 ? 0 : (v[c] > maxval ? maxval : v[c]));
+                if constexpr (kCmyk) cmyk_to_rgb(w, f.ycck != 0);
                 store_mode_pixel<K, MODE>(out, f.status_idx, X + x, Y + y, w, deep);
                 continue;
             }
@@ -1817,6 +1846,8 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
         if constexpr (K != kStoreCanvas) {
             if (l.mode == OutMode::Luma) generic_reconstruct_kernel<K, (int)OutMode::Luma><<<grid, 64, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
             if (l.mode == OutMode::Replicate) generic_reconstruct_kernel<K, (int)OutMode::Replicate><<<grid, 64, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
+            if (l.mode == OutMode::CmykRgb) generic_reconstruct_kernel<K, (int)OutMode::CmykRgb><<<grid, 64, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
+            if (l.mode == OutMode::CmykLuma) generic_reconstruct_kernel<K, (int)OutMode::CmykLuma><<<grid, 64, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));
             done = l.mode != OutMode::Coded;
         }
         if (!done) generic_reconstruct_kernel<K><<<grid, 64, 0, s>>>(l.frames, l.samples32, dst_of<K>(l));

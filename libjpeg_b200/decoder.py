@@ -76,6 +76,18 @@ def exif_orientation(data):
     return rc
 
 
+def colorspace(data):
+    """The colour space BatchDecoder(mode=...) reads one codestream's samples in (b200jpg_colorspace, DESIGN §15): "L", "YCbCr",
+    "RGB", "CMYK", "YCCK", or None for a frame a mode refuses (two components, four without an Adobe segment in front of the first
+    scan, or four of 12 bits). Host only, no GPU. Raises NativeError where parse() does."""
+    addr, n, keep = _as_buffer(data)
+    rc = lib.b200jpg_colorspace(addr, n)
+    del keep
+    if rc < 0:
+        native.check(rc)
+    return native.COLORSPACES[rc]
+
+
 def output_size(data, downscale=1, exif_orientation=False):
     """(h, w) of the whole output image of one codestream as BatchDecoder(frames, downscale=..., exif_orientation=...) writes it
     without a crop: the frame size divided by `downscale` (rounded up), height and width swapped for the Exif orientations 5..8
@@ -366,8 +378,10 @@ class BatchDecoder:
         RGB-coded or JPEG XT frame's (19595 R + 38470 G + 7471 B + 32768) >> 16, as convert("L") does. The mode comes before the
         orientation, the crop, the resize and the float map (scale[c] / bias[c] of the output component c), so a batch of grey and
         colour frames fills one [N, 3, H, W] tensor. output_components(i) gives the count; geometry(), frame_view() and the
-        destinations of decode_into() follow it. A frame of 2 or 4 components is then B200JPG_ERR_NOT_IMPLEMENTED (skipped with
-        tolerate_bad); a mode with color_transform=False raises NativeError (B200JPG_ERR_INVALID_PARAMETER), with upsample=False
+        destinations of decode_into() follow it. A CMYK or YCCK frame (an 8-bit four-component frame with an Adobe segment,
+        colorspace(data); DESIGN §15) is written as Pillow's convert("RGB") / convert("L") of the image it reads as Adobe-inverted
+        CMYK. A frame colorspace() gives None for -- two components, four without an Adobe segment or of 12 bits -- is then
+        B200JPG_ERR_NOT_IMPLEMENTED (skipped with tolerate_bad); a mode with color_transform=False raises NativeError (B200JPG_ERR_INVALID_PARAMETER), with upsample=False
         NativeError (B200JPG_ERR_NOT_IMPLEMENTED); any other value than None, "RGB" and "L" raises ValueError."""
         if not isinstance(mode, (str, type(None))) or mode not in native.MODE_FLAGS:
             raise ValueError('mode must be None, "RGB" or "L", got %r' % (mode,))

@@ -51,6 +51,7 @@ FLAG_NO_COLOR_TRANSFORM, FLAG_NO_UPSAMPLE = 1, 2
 DOWNSCALE_FLAGS = {1: 0x0, 2: 0x4, 4: 0x8, 8: 0xC}  # B200JPG_FLAG_DOWNSCALE_k
 FLAG_EXIF_ORIENTATION = 0x10
 MODE_FLAGS = {None: 0x0, "RGB": 0x20, "L": 0x40}  # B200JPG_FLAG_OUTPUT_RGB / _L, named after PIL's Image.convert(mode)
+COLORSPACES = [None, "L", "YCbCr", "RGB", "CMYK", "YCCK"]  # B200JPG_COLORSPACE_UNKNOWN .. _YCCK, named after PIL's modes
 RESAMPLE = {"lanczos": 1, "bilinear": 2, "bicubic": 3, "box": 4, "hamming": 5}  # B200JPG_RESAMPLE_*, PIL's values
 
 
@@ -68,6 +69,7 @@ def _load():
     sig = {
         "b200jpg_parse": (i32, [vp, ctypes.c_size_t, ctypes.POINTER(FrameInfoStruct)]),
         "b200jpg_exif_orientation": (i32, [vp, ctypes.c_size_t]),
+        "b200jpg_colorspace": (i32, [vp, ctypes.c_size_t]),
         "b200jpg_output_size": (i32, [vp, ctypes.c_size_t, ctypes.c_uint, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint32)]),
         "b200jpg_build_tables": (u64, [vp, ctypes.c_size_t, i32, vp, u64]),
         "b200jpg_create": (i32, [i32, ctypes.POINTER(vp)]),
@@ -136,7 +138,7 @@ ABI_SYMBOLS = [
     "b200jpg_device_free", "b200jpg_device_copy_rect", "b200jpg_selftest_restartless", "b200jpg_selftest_restartless_items",
     "b200jpg_selftest_table_cache", "b200jpg_microbench_int32", "b200jpg_exif_orientation", "b200jpg_batch_frame_orientation",
     "b200jpg_batch_create_crop", "b200jpg_output_size", "b200jpg_batch_create_resize", "b200jpg_resample_coefficients",
-    "b200jpg_batch_output_components",
+    "b200jpg_batch_output_components", "b200jpg_colorspace",
 ]
 
 
