@@ -179,6 +179,30 @@ B200JPG_API int b200jpg_batch_create(b200jpg_ctx *ctx, const uint8_t *const *fra
  * either bit a batch is planned exactly as before. */
 #define B200JPG_FLAG_OUTPUT_RGB 0x20u
 #define B200JPG_FLAG_OUTPUT_L 0x40u
+/* B200JPG_FLAG_LIBJPEG_TURBO (DESIGN §16; no counterpart in the reference): every frame is reconstructed as libjpeg-turbo (and so
+ * Pillow) reconstructs it, in place of the reference's numerics, from the same dequantised coefficients:
+ *   1. IDCT: libjpeg-turbo's JDCT_ISLOW in its C form with 64-bit intermediates. Constants (13 bits) 2446, 3196, 4433, 6270, 7373,
+ *      9633, 12299, 15137, 16069, 16819, 20995, 25172; pass 1 down the columns descales by 11, (x + 2^10) >> 11, pass 2 along the
+ *      rows by 18; the result v goes through the post-IDCT range-limit table at v & 1023 (0..127 -> v + 128, 128..511 -> 255,
+ *      512..895 -> 0, 896..1023 -> v - 896): one uint8 plane per component.
+ *   2. Upsampling of component c by fx = hmax / h_c, fy = vmax / v_c from its real size w x h = ceil(W h_c / hmax) x
+ *      ceil(H v_c / vmax): 2x1 with w > 2: out[2j] = (3 a[j] + a[j-1] + 1) >> 2, out[2j+1] = (3 a[j] + a[j+1] + 2) >> 2,
+ *      out[0] = a[0], out[2w-1] = a[w-1]; 1x2: upper (3 near + above + 1) >> 2, lower (3 near + below + 2) >> 2; 2x2 with w > 2:
+ *      cs = 3 near + far (far: the row above for the upper output row, below for the lower), out[2j] = (3 cs[j] + cs[j-1] + 8) >> 4,
+ *      out[2j+1] = (3 cs[j] + cs[j+1] + 7) >> 4, ends (4 cs[0] + 8) >> 4 and (4 cs[w-1] + 7) >> 4; any other integer ratio, and
+ *      2x1 / 2x2 with w <= 2, replicates. The row above the first row and below row h - 1 is that row itself.
+ *   3. Colour (b200jpg_colorspace YCbCr), b = Cb - 128, r = Cr - 128: R = Y + ((91881 r + 32768) >> 16), G = Y + ((-22554 b -
+ *      46802 r + 32768) >> 16), B = Y + ((116130 b + 32768) >> 16), clamped to 0..255. RGB-coded frames: the identity; grey frames:
+ *      the plane; B200JPG_FLAG_NO_COLOR_TRANSFORM: the upsampled components as they are.
+ *   4. The output modes keep their meaning on these samples: B200JPG_FLAG_OUTPUT_L of a YCbCr frame is component 0 upsampled by
+ *      rule 2 (Pillow's draft("L")), of an RGB-coded frame the L formula.
+ *   5. A JPEG XT frame is its base codestream alone, as libjpeg-turbo decodes it. A JPEG XT frame whose profile the parser refuses
+ *      (b200jpg_parse: B200JPG_ERR_NOT_IMPLEMENTED) keeps that status under the flag too: its base codestream is not decoded.
+ * Everything after the reconstruction is unchanged (orientation, crop, resize, float map), as are extents, out_bytes and statuses.
+ * The flag together with B200JPG_FLAG_DOWNSCALE_k or B200JPG_FLAG_NO_UPSAMPLE is B200JPG_ERR_NOT_IMPLEMENTED for the call; a 12-bit
+ * frame, a two- or a four-component frame has the status B200JPG_ERR_NOT_IMPLEMENTED (it fails the call, or with tolerate_bad it
+ * is skipped). Accepted wherever request flags are. Without the flag a batch is planned exactly as before. */
+#define B200JPG_FLAG_LIBJPEG_TURBO 0x80u
 B200JPG_API int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
                             unsigned flags, b200jpg_batch **batch);
 /* A rectangle of a frame's output: columns x .. x + width - 1, rows y .. y + height - 1. {0, 0, 0, 0} is the whole frame. */

@@ -19,7 +19,7 @@ COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-fvisibility=hi
           "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
 CUDA_SOURCES = ["huffman_sm100.cu", "specsync_sm100.cu", "progressive_sm100.cu", "progfused_sm100.cu", "recon_sm100.cu", "bitmap_sm100.cu",
-                "microbench_sm100.cu", "resample_sm100.cu"]
+                "microbench_sm100.cu", "resample_sm100.cu", "turbo_sm90.cu"]
 HOST_SOURCES = ["abi.cpp", "parse.cpp", "jpeg_shim.cpp"]
 # the resample tables are computed on the host in double precision: no contraction into FMA, so every host computes the same bits
 EXTRA = {"resample_sm100.cu": ["-Xcompiler", "-ffp-contract=off"]}

@@ -287,6 +287,8 @@ struct b200jpg_batch {
     int32_t *d_samples = nullptr;     // int32 planes: exact pass of frames flagged `narrow`
     int16_t *d_samples16 = nullptr;   // int16 planes: every frame
     uint64_t sample_elems = 0;
+    uint8_t *d_planes8 = nullptr;     // B200JPG_FLAG_LIBJPEG_TURBO: the uint8 planes of turbo_idct_kernel
+    uint64_t plane8_bytes = 0;
     uint8_t *d_clean = nullptr;
     uint64_t clean_bytes = 0;
     uint32_t *d_interval_len = nullptr;
@@ -575,6 +577,7 @@ void b200jpg_batch_destroy(b200jpg_batch *b) {
     b->ctx->put(1, b->d_coef, b->coef_elems * sizeof(int16_t));
     b->ctx->put(1, b->d_samples, b->sample_elems * sizeof(int32_t));
     b->ctx->put(1, b->d_samples16, b->sample_elems * sizeof(int16_t));
+    if (b->d_planes8) b->ctx->put(1, b->d_planes8, b->plane8_bytes);
     b->ctx->put(1, b->d_clean, b->clean_bytes);
     b->ctx->put(1, b->d_interval_len, b->sz_ilen);
     b->ctx->put(1, b->d_overrun, b->sz_overrun);
@@ -633,7 +636,14 @@ static void attach_residuals(b200jpg_batch &b, Codestreams &cs, bool device_inde
             cs.err[i] = "an output mode takes grey, YCbCr, RGB, and 8-bit Adobe CMYK or YCCK frames";
             continue;
         }
-        if (b.parse_status[i] != 0 || !b.frames[i].xt.present) continue;
+        if (b.parse_status[i] == 0 && (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) &&
+            (b.frames[i].info.precision != 8 || (b.frames[i].info.ncomp != 1 && b.frames[i].info.ncomp != 3))) {
+            b.parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;
+            cs.err[i] = "B200JPG_FLAG_LIBJPEG_TURBO takes 8-bit frames of one or three components";
+            continue;
+        }
+        // libjpeg-turbo decodes the base codestream of a JPEG XT frame alone: no residual frame
+        if (b.parse_status[i] != 0 || !b.frames[i].xt.present || (b.flags & B200JPG_FLAG_LIBJPEG_TURBO)) continue;
         if (b.flags & (B200JPG_FLAG_NO_COLOR_TRANSFORM | B200JPG_FLAG_NO_UPSAMPLE)) {
             b.parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;
             cs.err[i] = "JPEG XT frames are only reconstructed with upsampling and colour transformation";
@@ -754,9 +764,22 @@ static std::vector<uint64_t> lay_out_codestreams(b200jpg_batch &b, const std::ve
 // upsampling and both codestreams of a JPEG XT frame go through the generic kernels. Downscaled frames: 8-bit 4:2:0 frames with
 // upsampling take reconstruct420_scaled_kernel, every other one the scaled IDCT into int32 planes and then the generic kernels (a
 // JPEG XT frame never gets here downscaled: attach_residuals refuses it).
+// B200JPG_FLAG_LIBJPEG_TURBO (8-bit grey and three-component frames: attach_residuals): the tiled turbo_reconstruct_kernel covers
+// component 0 at full resolution, alone or with two chroma components of equal factors 1 or 2 whose fancy upsampling has both
+// neighbours (more than 2 chroma samples per row when halved horizontally); everything else the generic turbo kernel. ncomp: the
+// components reconstructed (1 for mode "L" of a YCbCr frame)
+static ReconPath turbo_path(const b200jpg_frame_info &fi, int ncomp) {
+    if (fi.subx[0] != 1 || fi.suby[0] != 1) return ReconPath::TurboGeneric;
+    if (ncomp == 1) return ReconPath::Turbo;
+    const uint32_t sx = fi.subx[1], sy = fi.suby[1];
+    if (sx != fi.subx[2] || sy != fi.suby[2] || sx > 2 || sy > 2) return ReconPath::TurboGeneric;
+    return (sx == 2 && (fi.width + 1) / 2 <= 2) ? ReconPath::TurboGeneric : ReconPath::Turbo;
+}
+
 static ReconPath recon_path(const b200jpg_batch &b, int i) {
     const b200jpg_frame_info &fi = b.frames[i].info;
     const bool scaled = downscale_of(b.flags) > 1;
+    if (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) return turbo_path(fi, fi.ncomp);
     if (b.xt_parent[i] >= 0 || (i < b.n_user && b.xt_child[i] >= 0)) return ReconPath::Generic;
     if (b.flags & B200JPG_FLAG_NO_UPSAMPLE) return scaled ? ReconPath::Scaled : ReconPath::Generic;  // planes of every component, then one sample -> one output value
     if (fi.precision != 8) return scaled ? ReconPath::Scaled : ReconPath::Generic;  // 12-bit frames: int32 planes, 16-bit samples out
@@ -790,11 +813,15 @@ static FramePlan frame_plan(const b200jpg_batch &b, int i) {
         if (fi.ycbcr && !xt) {
             // luma alone: a grey frame over component 0 on the MCU-padded block grid; libjpeg's JCS_GRAYSCALE for YCbCr input
             p.ncomp = 1;
+            if (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) {  // the turbo kernels over component 0
+                p.path = turbo_path(fi, 1);
+                return p;
+            }
             if (downscale_of(b.flags) > 1) p.path = ReconPath::Scaled;
             else p.path = (fi.precision != 8 || fi.subx[0] != 1 || fi.suby[0] != 1) ? ReconPath::Generic : ReconPath::Tiled;
         } else {  // RGB-coded and JPEG XT frames: the L formula after the colour transformation (merge) and clamp, in the generic kernels
             p.mode = OutMode::Luma;
-            p.path = downscale_of(b.flags) > 1 ? ReconPath::Scaled : ReconPath::Generic;
+            if (!(b.flags & B200JPG_FLAG_LIBJPEG_TURBO)) p.path = downscale_of(b.flags) > 1 ? ReconPath::Scaled : ReconPath::Generic;
         }
     }
     if ((b.flags & B200JPG_FLAG_OUTPUT_RGB) && fi.ncomp == 1) {
@@ -812,27 +839,32 @@ static FramePlan frame_plan(const b200jpg_batch &b, int i) {
 
 // Coefficient, sample and output layout of the live frames; returns the sample plane offsets. The sample planes a frame gets
 // follow its reconstruction path: Generic one per component, Tiled one per component from 1 on, Fused420 none (its chroma samples
-// live in shared memory), Scaled one per component of 8 ceil(blocks_w / k) x 8 ceil(blocks_h / k) samples, Scaled420 none.
+// live in shared memory), Scaled one per component of 8 ceil(blocks_w / k) x 8 ceil(blocks_h / k) samples, Scaled420 none,
+// TurboGeneric one uint8 plane per reconstructed component and Turbo one per component from 1 on, byte offsets into the batch's
+// uint8 plane buffer.
 static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
     const int n = b.n;
     b.coef_base.assign(n, {});
     b.out_off.assign(n, 0);
     b.out_bytes.assign(n, 0);
     std::vector<std::array<uint64_t, 4>> sample_base(n);
-    uint64_t coef_cur = 0, sample_cur = 0, out_cur = 0;
+    uint64_t coef_cur = 0, sample_cur = 0, out_cur = 0, plane8_cur = 0;
     for (int i = 0; i < n; i++) {
         if (b.parse_status[i] != 0) continue;
         const b200jpg_frame_info &fi = b.frames[i].info;
         const FramePlan plan = frame_plan(b, i);
         const ReconPath path = plan.path;
-        const int first_plane = (path == ReconPath::Generic || path == ReconPath::Scaled) ? 0 : (path == ReconPath::Tiled ? 1 : fi.ncomp);
+        const int first_plane = (path == ReconPath::Generic || path == ReconPath::Scaled || path == ReconPath::TurboGeneric) ? 0 : (path == ReconPath::Tiled ? 1 : fi.ncomp);
         const uint32_t k = downscale_of(b.flags);
         uint64_t samples = 0;
         for (int c = 0; c < fi.ncomp; c++) {  // every component is entropy decoded; only the reconstructed ones get sample planes
             const uint64_t elems = (uint64_t)fi.blocks_w[c] * fi.blocks_h[c] * 64;
             b.coef_base[i][c] = coef_cur;
             coef_cur += elems;
-            if (c >= first_plane && c < (int)plan.ncomp) {
+            if ((path == ReconPath::TurboGeneric || (path == ReconPath::Turbo && c >= 1)) && c < (int)plan.ncomp) {
+                sample_base[i][c] = plane8_cur;
+                plane8_cur = align_up(plane8_cur + elems, 256);
+            } else if (c >= first_plane && c < (int)plan.ncomp) {
                 sample_base[i][c] = sample_cur;
                 sample_cur += path == ReconPath::Scaled ? 64ull * ((fi.blocks_w[c] + k - 1) / k) * ((fi.blocks_h[c] + k - 1) / k) : elems;
             }
@@ -850,6 +882,7 @@ static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
     b.out_total = out_cur;
     b.coef_elems = coef_cur;
     b.sample_elems = sample_cur;
+    b.plane8_bytes = plane8_cur;
     return sample_base;
 }
 
@@ -1055,7 +1088,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         const FramePlan plan = frame_plan(b, i);
         const ReconPath path = plan.path;
         const uint32_t nc = plan.ncomp;
-        const bool generic = path == ReconPath::Generic || path == ReconPath::Scaled;
+        const bool generic = path == ReconPath::Generic || path == ReconPath::Scaled || path == ReconPath::TurboGeneric;
         uint32_t sx = nc > 1 ? fi.subx[1] : 1, sy = nc > 1 ? fi.suby[1] : 1;
         if (generic) sx = sy = 0;  // one group per component count: the generic kernels read the factors per frame
         // oriented frames (B200JPG_FLAG_EXIF_ORIENTATION, 2..8) form groups of their own, one per orientation: their destinations
@@ -1136,7 +1169,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
             fr.clip_x0 = cl.x0, fr.clip_y0 = cl.y0, fr.clip_x1 = cl.x1, fr.clip_y1 = cl.y1;
             fr.tx0 = cl.x0 / tw, fr.ty0 = cl.y0 / th;
             const uint32_t ntx = (cl.x1 - 1) / tw - fr.tx0 + 1, nty = (cl.y1 - 1) / th - fr.ty0 + 1;
-            if (path == ReconPath::Tiled && nc > 1) {
+            if ((path == ReconPath::Tiled || path == ReconPath::Turbo) && nc > 1) {
                 // b1: the chroma blocks under those tiles, one more on each side (the upsampling window), clipped to the plane
                 const int64_t cbx0 = (int64_t)fr.tx0 * t.bw / sx - 1, cby0 = (int64_t)fr.ty0 * t.bh / sy - 1;
                 const int64_t cbx1 = (int64_t)(fr.tx0 + ntx) * t.bw / sx + 1, cby1 = (int64_t)(fr.ty0 + nty) * t.bh / sy + 1;
@@ -1264,6 +1297,7 @@ static int stage_and_allocate(b200jpg_batch &b, const Codestreams &cs, const std
     if (ce == cudaSuccess && b.sample_elems) b.d_samples = (int32_t *)ctx->get(1, b.sample_elems * sizeof(int32_t), &ce);
     // the int16 planes serve the Tiled path only, which downscaled batches never take
     if (ce == cudaSuccess && b.sample_elems && downscale_of(b.flags) == 1) b.d_samples16 = (int16_t *)ctx->get(1, b.sample_elems * sizeof(int16_t), &ce);
+    if (ce == cudaSuccess && b.plane8_bytes) b.d_planes8 = (uint8_t *)ctx->get(1, b.plane8_bytes, &ce);
     if (ce == cudaSuccess) b.d_clean = (uint8_t *)ctx->get(1, b.clean_bytes, &ce);
     if (ce == cudaSuccess) b.d_interval_len = (uint32_t *)ctx->get(1, b.sz_ilen, &ce);
     b.sz_overrun = sizeof(uint32_t) * (size_t)(b.n_intervals + b.classes.size() + 1);
@@ -1319,6 +1353,18 @@ static int admit_sizes(b200jpg_batch &b, const b200jpg_size *sizes) {
         }
     }
     return B200JPG_OK;
+}
+
+// B200JPG_FLAG_LIBJPEG_TURBO: every live frame without a rectangle is cropped to its whole output, as admit_sizes does for
+// resized frames. Its slot is then described (rewritten descriptors), and turbo_generic_kernel needs only the clipped strided
+// store kinds, whatever the destination.
+static void crop_whole_frames(b200jpg_batch &b) {
+    if (b.crop.empty()) b.crop.assign(b.n_user, b200jpg_rect{0, 0, 0, 0});
+    for (int i = 0; i < b.n_user; i++) {
+        if (b.parse_status[i] != 0 || !rect_empty(b.crop[i])) continue;
+        const Extent e = out_extent(b.frames[i].info, 0, b.flags, applied_orientation(b, i));
+        b.crop[i] = b200jpg_rect{0, 0, (uint32_t)e.w, (uint32_t)e.h};
+    }
 }
 
 // The resample descriptors and tables of the resized frames (tables built on host threads, one frame each) and the layout of the
@@ -1399,6 +1445,8 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
         return ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, "an output mode is not supported with B200JPG_FLAG_NO_UPSAMPLE");
     if ((flags & kOutputModes) && (flags & B200JPG_FLAG_NO_COLOR_TRANSFORM))
         return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "an output mode needs the colour transformation (no B200JPG_FLAG_NO_COLOR_TRANSFORM)");
+    if ((flags & B200JPG_FLAG_LIBJPEG_TURBO) && (flags & (B200JPG_FLAG_DOWNSCALE_MASK | B200JPG_FLAG_NO_UPSAMPLE)))
+        return ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, "B200JPG_FLAG_LIBJPEG_TURBO is not supported with B200JPG_FLAG_DOWNSCALE_k or B200JPG_FLAG_NO_UPSAMPLE");
     cudaError_t ce = cudaSetDevice(ctx->device);
     if (ce != cudaSuccess) return ctx->fail_cuda(ce, "cudaSetDevice");
 
@@ -1423,6 +1471,7 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
         if (int rc = admit_crops(b, rects)) return rc;
     if (sizes)
         if (int rc = admit_sizes(b, sizes)) return rc;
+    if (flags & B200JPG_FLAG_LIBJPEG_TURBO) crop_whole_frames(b);
     const std::vector<uint64_t> byte_off = lay_out_codestreams(b, cs.len);
     const std::vector<std::array<uint64_t, 4>> sample_base = lay_out_planes(b);
     form_scan_classes(b, frame_tables, byte_off);
@@ -1839,6 +1888,7 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.coef = b->d_coef;
         l.samples16 = b->d_samples16;
         l.samples32 = b->d_samples;
+        l.planes8 = b->d_planes8;
         l.wide_flags = b->d_status + b->n;
         l.narrow_flags = b->d_status + 2 * (size_t)b->n;
         l.narrow_list = b->d_status + 3 * (size_t)b->n;

@@ -296,8 +296,11 @@ int launch_progressive_dequant(const ProgFrame *frames_dev, uint32_t n_frames, u
 // 4:2:2, 4:4:0); Fused420: reconstruct420_kernel, no planes; Generic: int32 planes of every component + the generic kernels
 // Scaled (B200JPG_FLAG_DOWNSCALE_*): idct_scaled_planes_kernel into int32 planes laid out as the IDCT output of the reduced frame,
 // then the generic kernels on a FrameRecon of the reduced width and height; Scaled420 (downscaled 8-bit 4:2:0 frames with
-// upsampling): reconstruct420_scaled_kernel, no planes
-enum class ReconPath : int { Tiled, Fused420, Generic, Scaled, Scaled420 };
+// upsampling): reconstruct420_scaled_kernel, no planes. B200JPG_FLAG_LIBJPEG_TURBO (DESIGN §16, turbo_sm90.cu): Turbo (grey, and
+// three components with full-resolution component 0 and chroma factors 1 or 2, wider than 2 chroma samples when halved
+// horizontally): turbo_idct_kernel into uint8 planes of components 1.., then turbo_reconstruct_kernel; TurboGeneric (every other
+// such frame): uint8 planes of every reconstructed component, then turbo_generic_kernel
+enum class ReconPath : int { Tiled, Fused420, Generic, Scaled, Scaled420, TurboGeneric, Turbo };
 // B200JPG_FLAG_OUTPUT_RGB / _L (DESIGN §14): what a reconstruction group writes besides its components as they are. Luma: the generic
 // kernels reduce three clamped components to L = (19595 R + 38470 G + 7471 B + 32768) >> 16 and store one; Replicate: a grey frame's
 // sample is stored to three components. (An L frame of a YCbCr codestream is planned as a grey frame over its component 0: Coded.)
@@ -306,7 +309,7 @@ enum class ReconPath : int { Tiled, Fused420, Generic, Scaled, Scaled420 };
 enum class OutMode : int { Coded, Luma, Replicate, CmykRgb, CmykLuma };
 inline ReconTile recon_tile(ReconPath p) {
     if (p == ReconPath::Fused420 || p == ReconPath::Scaled420) return {32, (uint32_t)kRows420};
-    if (p == ReconPath::Tiled) return {32, (uint32_t)kThreadsB / 32};
+    if (p == ReconPath::Tiled || p == ReconPath::Turbo) return {32, (uint32_t)kThreadsB / 32};
     return {(uint32_t)kGenericTileBlocks, 1};
 }
 struct ReconLaunch {
@@ -323,6 +326,7 @@ struct ReconLaunch {
     const int16_t *coef;
     int16_t *samples16;            // chroma sample planes every frame goes through
     int32_t *samples32;            // the same planes for the exact pass over frames flagged `narrow`
+    uint8_t *planes8;              // TurboGeneric groups: the uint8 planes (FrameRecon::sample_base are byte offsets into them)
     uint32_t *narrow_flags;        // [frames in batch], zeroed per decode: a chroma sample does not fit int16
     uint32_t *wide_flags;          // [frames in batch], zeroed per decode: a chroma sample leaves the 32-bit colour range
     uint32_t *narrow_list;         // [1 + frames in group] scratch: {count, group-local indices of the flagged frames}
@@ -363,6 +367,10 @@ struct FloatDst {
     float scale[B200JPG_MAX_COMPONENTS], bias[B200JPG_MAX_COMPONENTS];
 };
 int launch_recon(const ReconLaunch &l, void *stream, int *launches);
+// turbo_sm90.cu: a Turbo or TurboGeneric group, every frame cropped (ReconLaunch::clip), K = kStoreStrided or kStoreStridedF with
+// kStoreClip
+template <int K>
+int launch_turbo(const ReconLaunch &l, void *stream, int *launches);
 
 // ---- resize (b200jpg_batch_create_resize, DESIGN §13), resample_sm100.cu. The reconstruction writes C, the frame's cropped
 // output, as an interleaved uint8 bitmap into the batch's scratch; resample_h_kernel runs the horizontal pass over the rows of C

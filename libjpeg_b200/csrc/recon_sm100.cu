@@ -1858,6 +1858,10 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
 
 template <int K>
 static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches) {
+    if (l.path == ReconPath::Turbo || l.path == ReconPath::TurboGeneric) {  // (every frame of such a group is cropped: crop_whole_frames)
+        if constexpr (kClipKind<K>) return launch_turbo<(kFloatKind<K> ? kStoreStridedF : kStoreStrided) | kStoreClip>(l, s, launches);
+        return (int)cudaErrorInvalidValue;
+    }
     if (l.path == ReconPath::Generic || l.path == ReconPath::Scaled)
         return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : ((kFloatKind<K> ? kStoreStridedF : kStoreStrided) | (K & kStoreClip))>(l, s, launches);
     if (l.path == ReconPath::Fused420) return launch_recon420<K>(l, s, launches);

@@ -343,7 +343,7 @@ class BatchDecoder:
     """One batch of codestreams: parse + pack on construction, then upload() / decode() on a CUDA stream."""
 
     def __init__(self, frames, device=-1, tolerate_bad=False, ctx=None, color_transform=True, upsample=True, downscale=1,
-                 exif_orientation=False, crop=None, resize=None, resample="bilinear", mode=None):
+                 exif_orientation=False, crop=None, resize=None, resample="bilinear", mode=None, reconstruction="reference"):
         """downscale = 2, 4 or 8 decodes every frame at ceil(W / k) x ceil(H / k) (B200JPG_FLAG_DOWNSCALE_k): each 8x8 block is
         inverse transformed straight to (8/k) x (8/k) samples, the k x k box average of its IDCT, and the rest of the
         reconstruction runs on the smaller frame. geometry(), frame_view() and plane_views() give the reduced sizes. Not to be
@@ -382,9 +382,19 @@ class BatchDecoder:
         colorspace(data); DESIGN §15) is written as Pillow's convert("RGB") / convert("L") of the image it reads as Adobe-inverted
         CMYK. A frame colorspace() gives None for -- two components, four without an Adobe segment or of 12 bits -- is then
         B200JPG_ERR_NOT_IMPLEMENTED (skipped with tolerate_bad); a mode with color_transform=False raises NativeError (B200JPG_ERR_INVALID_PARAMETER), with upsample=False
-        NativeError (B200JPG_ERR_NOT_IMPLEMENTED); any other value than None, "RGB" and "L" raises ValueError."""
+        NativeError (B200JPG_ERR_NOT_IMPLEMENTED); any other value than None, "RGB" and "L" raises ValueError.
+
+        reconstruction (B200JPG_FLAG_LIBJPEG_TURBO, DESIGN §16): "reference" (the default) reconstructs as the reference decoder
+        does; "libjpeg-turbo" as libjpeg-turbo does, so as Pillow's Image.open(f) -- its islow IDCT, fancy upsampling and YCbCr ->
+        RGB conversion -- with "L" of a YCbCr frame as Pillow's draft("L") and a JPEG XT frame as its base codestream alone.
+        Orientation, crop, resize and the float map follow unchanged, so Image.open(f).convert("RGB").crop(box).resize(size)
+        is what the GPU writes, byte for byte, for intact codestreams. A 12-bit, two- or four-component frame is then
+        B200JPG_ERR_NOT_IMPLEMENTED (skipped with tolerate_bad); "libjpeg-turbo" with downscale > 1 or upsample=False raises
+        NativeError (B200JPG_ERR_NOT_IMPLEMENTED); any other value raises ValueError before a device is touched."""
         if not isinstance(mode, (str, type(None))) or mode not in native.MODE_FLAGS:
             raise ValueError('mode must be None, "RGB" or "L", got %r' % (mode,))
+        if not isinstance(reconstruction, str) or reconstruction not in native.RECONSTRUCTION_FLAGS:
+            raise ValueError('reconstruction must be "reference" or "libjpeg-turbo", got %r' % (reconstruction,))
         if isinstance(downscale, bool) or not isinstance(downscale, int) or downscale not in native.DOWNSCALE_FLAGS:
             raise ValueError("downscale must be 1, 2, 4 or 8, got %r" % (downscale,))
         rects = None if crop is None else crop_table(crop, len(frames))
@@ -412,6 +422,8 @@ class BatchDecoder:
             flags |= native.FLAG_EXIF_ORIENTATION
         self.mode = mode
         flags |= native.MODE_FLAGS[mode]
+        self.reconstruction = reconstruction
+        flags |= native.RECONSTRUCTION_FLAGS[reconstruction]
         rc = lib.b200jpg_batch_create_resize(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, rects, sizes, filt, ctypes.byref(self.handle))
         native.check(rc, self.ctx.handle)
         self.ctx._batch_opened()

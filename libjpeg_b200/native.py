@@ -51,6 +51,7 @@ FLAG_NO_COLOR_TRANSFORM, FLAG_NO_UPSAMPLE = 1, 2
 DOWNSCALE_FLAGS = {1: 0x0, 2: 0x4, 4: 0x8, 8: 0xC}  # B200JPG_FLAG_DOWNSCALE_k
 FLAG_EXIF_ORIENTATION = 0x10
 MODE_FLAGS = {None: 0x0, "RGB": 0x20, "L": 0x40}  # B200JPG_FLAG_OUTPUT_RGB / _L, named after PIL's Image.convert(mode)
+RECONSTRUCTION_FLAGS = {"reference": 0x0, "libjpeg-turbo": 0x80}  # B200JPG_FLAG_LIBJPEG_TURBO
 COLORSPACES = [None, "L", "YCbCr", "RGB", "CMYK", "YCCK"]  # B200JPG_COLORSPACE_UNKNOWN .. _YCCK, named after PIL's modes
 RESAMPLE = {"lanczos": 1, "bilinear": 2, "bicubic": 3, "box": 4, "hamming": 5}  # B200JPG_RESAMPLE_*, PIL's values
 
