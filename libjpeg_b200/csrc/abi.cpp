@@ -989,7 +989,11 @@ static void form_progressive_groups(b200jpg_batch &b) {
             bool ok = !ids.empty();
             for (uint32_t id : ids) ok = ok && b.frames[id].scans.size() == cls.size();
             PfGroupHost grp;
-            const b200jpg_frame_info &fi0 = b.frames[ids[0]].info;
+            const ParsedFrame &pf0 = b.frames[ids[0]];
+            const b200jpg_frame_info &fi0 = pf0.info;
+            // one DC quantiser per component serves the whole group
+            for (uint32_t id : ids)
+                for (int c = 0; c < fi0.ncomp; c++) ok = ok && b.frames[id].comp_quant[c][0] == pf0.comp_quant[c][0];
             for (int ci : cls) {
                 const ScanClassParams &p = b.classes[(size_t)ci].p;
                 if (!ok) break;
@@ -1015,9 +1019,7 @@ static void form_progressive_groups(b200jpg_batch &b) {
             if (!ok) continue;
             for (int ci : cls) b.classes[(size_t)ci].fused = true;
             for (uint32_t id : ids) frame_fused[id] = 1;
-            const ParsedFrame &pf0 = b.frames[ids[0]];
-            for (int c = 0; c < 4; c++)
-                b.pf_dc_quant.push_back(c < fi0.ncomp && pf0.scans[0].quant_defined[fi0.tq[c]] ? pf0.scans[0].quant[fi0.tq[c]][0] : 0);
+            for (int c = 0; c < 4; c++) b.pf_dc_quant.push_back(c < fi0.ncomp ? pf0.comp_quant[c][0] : 0);
             b.pf_groups.push_back(std::move(grp));
         }
     }
@@ -1030,8 +1032,7 @@ static void form_progressive_groups(b200jpg_batch &b) {
             f.coef_base[c] = b.coef_base[i][c];
             f.n_blocks[c] = pf.info.blocks_w[c] * pf.info.blocks_h[c];
             b.prog_max_blocks = std::max(b.prog_max_blocks, f.n_blocks[c]);
-            const ScanInfo &last = pf.scans.back();  // quantisers in effect at the end of the frame
-            for (int k = 0; k < 64; k++) f.q_raster[c][kZigZagToRaster[k]] = last.quant_defined[pf.info.tq[c]] ? last.quant[pf.info.tq[c]][k] : 0;
+            for (int k = 0; k < 64; k++) f.q_raster[c][kZigZagToRaster[k]] = pf.comp_quant[c][k];
         }
         b.prog_frames.push_back(f);
     }

@@ -57,7 +57,7 @@ struct ScanInfo {  // one SOS + its entropy coded segment
     // points (specsync.hpp) instead of by a single lane
     bool spec = false;
     HuffSpec dc[4], ac[4];       // tables in effect at this SOS
-    uint16_t quant[4][64];       // zig-zag order as transmitted, in effect at this SOS
+    uint16_t quant[4][64];       // zig-zag order; slot tq of a scan component holds that component's ParsedFrame::comp_quant
     bool quant_defined[4] = {false, false, false, false};
 };
 
@@ -84,6 +84,12 @@ struct ParsedFrame {
     // starts with "Adobe" (libjpeg's examine_app14), -1 when there is none. Only the colour space of four-component frames follows
     // it (frame_colorspace); three-component frames keep the reference's rule (b200jpg_frame_info::ycbcr)
     int adobe_transform = -1;
+    // the quantiser of each frame component (zig-zag order), latched at the first scan that contains the component: the
+    // reference builds a component's inverse DCT once, at that scan (BlockBuffer::ResetToStartOfScan control/blockbuffer.cpp:
+    // 185-197, IDCT::DefineQuant dct/idct.cpp:98-108), so a DQT that redefines the slot later does not reach it. Every
+    // consumer reads this: the scans' table sets (ScanInfo::quant of the scan's components), the fused DC kernel and the
+    // scan-by-scan dequantisation
+    uint16_t comp_quant[4][64];
 };
 
 // B200JPG_COLORSPACE_* of a parsed frame: grey, YCbCr / RGB by b200jpg_frame_info::ycbcr, CMYK / YCCK for an 8-bit four-component

@@ -158,6 +158,8 @@ int parse_codestream(const uint8_t *data, size_t len, ParsedFrame &out, std::str
     HuffSpec dc[4], ac[4];
     uint16_t quant[4][64];
     bool quant_defined[4] = {false, false, false, false};
+    bool quant_latched[4] = {false, false, false, false};  // per frame component: ParsedFrame::comp_quant is set
+    memset(out.comp_quant, 0, sizeof(out.comp_quant));
     uint32_t dri = 0;
     bool have_sof = false, adobe_none = false;
     int hmax = 0, vmax = 0;
@@ -413,7 +415,15 @@ int parse_codestream(const uint8_t *data, size_t len, ParsedFrame &out, std::str
                     FAIL(B200JPG_ERR_MALFORMED_STREAM, "Huffman decoder not specified for all components included in scan");  // sequentialscan.cpp:117-129
                 if (!quant_defined[fi.tq[sc.comp[i]]])
                     FAIL(B200JPG_ERR_MALFORMED_STREAM, "quantization table for a component of the scan is not defined");
+                if (!quant_latched[sc.comp[i]]) {
+                    memcpy(out.comp_quant[sc.comp[i]], quant[fi.tq[sc.comp[i]]], sizeof(quant[0]));
+                    quant_latched[sc.comp[i]] = true;
+                }
             }
+            // the table set of the scan dequantises with the components' latched quantisers (the sequential and the fused AC
+            // kernels read it). Two components of one slot latch different tables only when they first appear in different
+            // scans; in an interleaved progressive DC scan that is harmless, the DC kernels take comp_quant itself
+            for (int i = 0; i < sc.ns; i++) memcpy(sc.quant[fi.tq[sc.comp[i]]], out.comp_quant[sc.comp[i]], sizeof(quant[0]));
             uint64_t total = (uint64_t)sc.mcu_cols * sc.mcu_rows;
             uint64_t per = sc.dri ? sc.dri : total;
             uint64_t nint = (total + per - 1) / per;
@@ -637,7 +647,10 @@ int build_table_set(const ScanInfo &scan, TableSet &out, std::string &err) {
                 uint32_t delta = scan.quant_defined[t] ? scan.quant[t][k] : 0;
                 if (((uint64_t)delta << scan.lowbit) >= (1u << 24))
                     FAIL(B200JPG_ERR_NOT_IMPLEMENTED, "quantisation step times point transform too large for the GPU path");
+                // a step beyond 32768 turns every non-zero level into a coefficient beyond int16: 32769 stands for all of
+                // them, so that |level| x q (|level| < 2^15) stays within int32 in the kernels
                 q = delta << scan.lowbit;
+                if (q > 32769u) q = 32769u;
                 off = 2u * kZigZagToRaster[k];
             } else {
                 // 64..95: a coefficient whose run left the block (sequentialscan.cpp:764-766). The multiplier 2^16 turns any

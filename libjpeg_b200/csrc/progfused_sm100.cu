@@ -136,11 +136,14 @@ pf_dc_kernel(PfLaunch L) {
                             const uint32_t sz = e & 31u;
                             if (sz) pred[c] += extend(b[0].get(sz), sz);
                         }
-                        level = (int)((uint32_t)pred[c] << first.al);
+                        const long long lv = (long long)pred[c] * (1ll << first.al);
+                        if (lv < -32768 || lv > 32767) bad = true;  // beyond the int16 side plane (DESIGN.md section 7)
+                        level = (int)lv;
                     }
 #pragma unroll
                     for (int s = 1; s < kPfMaxScans; s++)  // refinements: one raw bit per block, refinementscan.cpp:588-592
                         if (s < L.n_scans && present[s]) level |= (int)(b[s].get(1) << L.scan[s].al);
+                    if (level < -32768 || level > 32767) bad = true;
                     const uint32_t bx = mx * L.mw[c] + x, by = my * L.mh[c] + y;
                     const uint64_t blk = cs.coef_base[c] / 64u + (uint64_t)by * L.bw[c] + bx;
                     L.dcplane[blk] = (int16_t)level;
@@ -285,6 +288,7 @@ pf_ac_kernel(PfLaunch L) {
                             if (sz != 0) {
                                 uint2 pq;
                                 asm("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(pq.x), "=r"(pq.y) : "r"(qz + 8u * (uint32_t)kk));
+                                // |level| < 2^15 and the table caps q << Al at 32769 (build_table_set): no int32 wrap
                                 const int d = extend(bits, sz) * (int)pq.x;
                                 ovf |= (uint32_t)(d + 32768);
                                 sts_h(s_stage + pq.y, d);
@@ -344,7 +348,9 @@ pf_ac_kernel(PfLaunch L) {
                             if (target <= se && sign) {  // (its position is behind every position that still owes a bit)
                                 uint2 pq;
                                 asm("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(pq.x), "=r"(pq.y) : "r"(qz + 8u * (uint32_t)target));
-                                sts_h(s_stage + pq.y, sign * (int)pq.x);
+                                const int d = sign * (int)pq.x;
+                                ovf |= (uint32_t)(d + 32768);
+                                sts_h(s_stage + pq.y, d);
                                 H |= 1ull << target;
                             }
                             if (eob) {  // the rest of this block (and of the next skip-1 blocks) only takes correction bits

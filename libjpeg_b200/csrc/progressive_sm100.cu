@@ -72,6 +72,17 @@ __device__ __forceinline__ int extend(uint32_t v, uint32_t s) {  // sequentialsc
     return (v < (1u << (s - 1))) ? (int)v + (int)((~0u) << s) + 1 : (int)v;
 }
 
+__device__ __forceinline__ bool fits_int16(long long v) { return v >= -32768 && v <= 32767; }
+
+// a correction bit of AC refinement: the level moves away from zero by 1 << Al; false (and the level unchanged) when that
+// leaves the int16 store
+__device__ __forceinline__ bool refine(int16_t *q, int cur, int al) {
+    const int level = cur + (cur > 0 ? (1 << al) : -(1 << al));
+    if (!fits_int16(level)) return false;
+    *q = (int16_t)level;
+    return true;
+}
+
 __global__ void __launch_bounds__(kThreadsP)
 progressive_scan_kernel(ScanClassParams p, const uint8_t *__restrict__ clean, const uint64_t *__restrict__ clean_off,
                         const uint32_t *__restrict__ interval_len, const ClassScan *__restrict__ scans, const uint8_t *__restrict__ tables,
@@ -119,9 +130,19 @@ progressive_scan_kernel(ScanClassParams p, const uint8_t *__restrict__ clean, co
                             }
                             const uint32_t s = e & 31u;
                             if (s) pred[c] += extend(b.get(s), s);
-                            blk[0] = (int16_t)((uint32_t)pred[c] << al);
+                            const long long level = (long long)pred[c] * (1ll << al);
+                            if (!fits_int16(level)) {  // a level beyond the store is a coefficient beyond it (DESIGN.md section 7)
+                                bad = true;
+                                break;
+                            }
+                            blk[0] = (int16_t)level;
                         } else {      // DC refinement: one raw bit, refinementscan.cpp:588-592
-                            blk[0] = (int16_t)(blk[0] | (int)(b.get(1) << al));
+                            const int level = blk[0] | (int)(b.get(1) << al);
+                            if (!fits_int16(level)) {
+                                bad = true;
+                                break;
+                            }
+                            blk[0] = (int16_t)level;
                         }
                         continue;
                     }
@@ -149,11 +170,11 @@ progressive_scan_kernel(ScanClassParams p, const uint8_t *__restrict__ clean, co
                             }
                             k += (int)r;
                             const int v = extend(b.get(s), s);
-                            if (k >= 64) {  // the reference tests against 64, not against Se
+                            if (k >= 64 || !fits_int16((long long)v * (1ll << al))) {  // the reference tests against 64, not against Se
                                 bad = true;
                                 break;
                             }
-                            blk[c_zigzag[k]] = (int16_t)((uint32_t)v << al);
+                            blk[c_zigzag[k]] = (int16_t)(v * (1 << al));
                             k++;
                         } while (k <= p.se);
                     } else {          // AC refinement: refinementscan.cpp:594-690
@@ -182,7 +203,7 @@ progressive_scan_kernel(ScanClassParams p, const uint8_t *__restrict__ clean, co
                                     int16_t *q = blk + c_zigzag[k];
                                     const int cur = *q;
                                     if (cur) {
-                                        if (b.get(1)) *q = (int16_t)(cur + (cur > 0 ? (1 << al) : -(1 << al)));
+                                        if (b.get(1)) bad |= !refine(q, cur, al);
                                     } else {
                                         if (r == 0) break;
                                         r--;
@@ -197,7 +218,7 @@ progressive_scan_kernel(ScanClassParams p, const uint8_t *__restrict__ clean, co
                             for (; k <= p.se; k++) {
                                 int16_t *q = blk + c_zigzag[k];
                                 const int cur = *q;
-                                if (cur && b.get(1)) *q = (int16_t)(cur + (cur > 0 ? (1 << al) : -(1 << al)));
+                                if (cur && b.get(1)) bad |= !refine(q, cur, al);
                             }
                             skip--;
                         }

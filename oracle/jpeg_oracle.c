@@ -371,10 +371,14 @@ typedef void (*dht_cb)(void *user, int slot_is_ac, int th, const uint8_t *bits, 
 
 /* Walks the marker segments.  Follows codestream/decoder.cpp:77, codestream/tables.cpp:1003-1420
  * (DQT/DHT/DRI/APPn/COM), marker/frame.cpp:111-214 (SOF), marker/scan.cpp:163-315 (SOS).
- * When `tabs` is non-NULL the Huffman tables in effect at scan `want_scan` are captured.              */
-static int walk(const uint8_t *d, size_t n, jpgo_info *info, decoder_tables *tabs, int want_scan) {
+ * When `tabs` is non-NULL the Huffman tables in effect at scan `want_scan` are captured.
+ * When `latched` is non-NULL it receives the quantiser of every component (raster order): its slot's table as it stood at
+ * the first scan that holds the component -- the reference builds the component's IDCT there (BlockBuffer::
+ * ResetToStartOfScan control/blockbuffer.cpp:185-197) and a later DQT does not reach it; a component no scan holds takes
+ * the slot's last definition.                                                                          */
+static int walk(const uint8_t *d, size_t n, jpgo_info *info, decoder_tables *tabs, int want_scan, uint16_t (*latched)[64]) {
     size_t pos = 2;
-    int have_sof = 0, dri = 0, adobe_none = 0, i;
+    int have_sof = 0, dri = 0, adobe_none = 0, seen = 0, i;
     if (n < 4 || d[0] != 0xff || d[1] != 0xd8) return JPGO_ERR_MALFORMED_STREAM; /* no SOI */
     memset(info, 0, sizeof(*info));
     for (;;) {
@@ -534,6 +538,10 @@ static int walk(const uint8_t *d, size_t n, jpgo_info *info, decoder_tables *tab
                 for (j = 0; j < i; j++)
                     if (sc->comp[j] == found) return JPGO_ERR_MALFORMED_STREAM;
                 sc->comp[i] = found;
+                if (!(seen & (1 << found)) && info->quant_defined[info->tq[found]]) {
+                    if (latched) memcpy(latched[found], info->quant[info->tq[found]], sizeof(latched[found]));
+                    seen |= 1 << found;
+                }
                 sc->td[i] = sel >> 4;
                 sc->ta[i] = sel & 15;
                 if (sc->td[i] > 3 || sc->ta[i] > 3) return JPGO_ERR_MALFORMED_STREAM;
@@ -578,11 +586,30 @@ static int walk(const uint8_t *d, size_t n, jpgo_info *info, decoder_tables *tab
         pos += (size_t)len;
     }
     if (!have_sof || info->nscans == 0) return JPGO_ERR_MALFORMED_STREAM;
+    for (i = 0; latched && i < info->ncomp; i++)
+        if (!(seen & (1 << i))) memcpy(latched[i], info->quant[info->tq[i]], sizeof(latched[i]));
     info->ycbcr = (info->ncomp == 3 && !adobe_none); /* tables.cpp:2023-2030 */
     return JPGO_OK;
 }
 
-int jpgo_read_info(const uint8_t *data, size_t len, jpgo_info *info) { return walk(data, len, info, NULL, -1); }
+int jpgo_read_info(const uint8_t *data, size_t len, jpgo_info *info) { return walk(data, len, info, NULL, -1, NULL); }
+
+/* `info` of the stream rewritten for reconstruction: component c dequantises through slot c, which holds the quantiser it
+ * latched (walk) */
+static int latched_quantisers(const uint8_t *data, size_t len, jpgo_info *info) {
+    uint16_t q[JPGO_MAX_COMP][64];
+    int defined[JPGO_MAX_COMP], c, rc;
+    jpgo_info tmp;
+    rc = walk(data, len, &tmp, NULL, -1, q);
+    if (rc) return rc;
+    for (c = 0; c < info->ncomp; c++) defined[c] = info->quant_defined[info->tq[c]];
+    for (c = 0; c < info->ncomp; c++) {
+        memcpy(info->quant[c], q[c], sizeof(q[c]));
+        info->quant_defined[c] = defined[c];
+        info->tq[c] = c;
+    }
+    return JPGO_OK;
+}
 
 /* ------------------------------------------------------------------------------------------------ */
 /* Entropy decode of one scan.  MCU order follows codestream/sequentialscan.cpp:381-428; restart
@@ -703,7 +730,7 @@ int jpgo_decode_coefficients(const uint8_t *data, size_t len, const jpgo_info *i
         /* tables may be redefined between scans: re-walk up to scan s and take what is in effect there */
         free_tables(tabs);
         memset(tabs, 0, sizeof(*tabs));
-        rc = walk(data, len, &tmp, tabs, s);
+        rc = walk(data, len, &tmp, tabs, s, NULL);
         if (rc) break;
         rc = build_tables(tabs);
         if (rc) break;
@@ -1053,6 +1080,7 @@ int jpgo_decode_planes16(const uint8_t *data, size_t len, uint16_t *out, size_t 
         if (!planes[c]) rc = JPGO_ERR_OUT_OF_MEMORY;
     }
     if (!rc) rc = jpgo_decode_coefficients(data, len, &info, planes);
+    if (!rc) rc = latched_quantisers(data, len, &info);
     if (!rc) rc = jpgo_reconstruct_planes16(&info, planes, out);
     for (c = 0; c < info.ncomp; c++) free(planes[c]);
     return rc;
@@ -1316,6 +1344,7 @@ static int decode_any(const uint8_t *data, size_t len, uint8_t *out8, uint16_t *
         if (!planes[c]) rc = JPGO_ERR_OUT_OF_MEMORY;
     }
     if (!rc) rc = jpgo_decode_coefficients(data, len, &info, planes);
+    if (!rc) rc = latched_quantisers(data, len, &info);
     if (!rc) rc = out16 ? jpgo_reconstruct16(&info, planes, out16) : jpgo_reconstruct(&info, planes, out8);
     for (c = 0; c < info.ncomp; c++) free(planes[c]);
     return rc;

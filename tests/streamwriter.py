@@ -170,6 +170,12 @@ class Scan:
     ah: int = 0
     al: int = 0
     tables: dict = field(default_factory=dict)  # {("dc" | "ac", slot): HuffTable} defined right in front of this scan
+    quant: dict = field(default_factory=dict)   # {slot: 64 quantiser values in RASTER order} defined (DQT) in front of this scan
+    restart_interval: int = None                # a DRI in front of this scan (in effect from here on); None: no DRI
+    # AC refinement only: {block ordinal in the scan's coding order: size 2..15}. The block carries one symbol of run 0 and that
+    # size, without value bits, at the first position of its band that stays zero and ends no run (G.1.2.3 allows only size 1
+    # there; T.81 decoders that go on treat it as "nothing placed, one zero position passed")
+    odd_sizes: dict = field(default_factory=dict)
 
 
 @dataclass
@@ -197,6 +203,16 @@ def _dht(tables):
     for (kind, slot), t in sorted(tables.items()):
         payload += t.dht_payload(0 if kind == "dc" else 1, slot)
     return _segment(0xC4, payload) if payload else b""
+
+
+def _dqt(quant, dqt16):
+    payload = b""
+    for slot, q in sorted(quant.items()):
+        q = np.asarray(q).reshape(64)[ZIGZAG]
+        if q.min() < 1 or q.max() > (65535 if dqt16 else 255):
+            raise ValueError("quantiser out of range")
+        payload += bytes([(0x10 if dqt16 else 0) | slot]) + (b"".join(int(v).to_bytes(2, "big") for v in q) if dqt16 else bytes(int(v) for v in q))
+    return _segment(0xDB, payload) if payload else b""
 
 
 def _cdiv(a, b):
@@ -243,6 +259,7 @@ class _ScanCoder:
         self.pred = [0] * 4
         self.eobrun = 0
         self.be = []  # correction bits that follow the pending EOB run
+        self.n_blocks = 0
 
     def restart(self):
         self.flush_eobrun()
@@ -318,7 +335,7 @@ class _ScanCoder:
 
     def ac_refine(self, blk):
         zz, al = _zz(blk), self.s.al
-        if not np.any(np.abs(zz[self.s.ss:self.s.se + 1]) >> al):
+        if not np.any(np.abs(zz[self.s.ss:self.s.se + 1]) >> al) and self.n_blocks - 1 not in self.s.odd_sizes:
             self.eobrun += 1
             if self.eobrun == 0x7FFF:
                 self.flush_eobrun()
@@ -326,8 +343,16 @@ class _ScanCoder:
         absv = [abs(int(zz[i])) >> al for i in range(64)]
         eob = max([i for i in range(self.s.ss, self.s.se + 1) if absv[i] == 1], default=-1)
         r, br = 0, []
+        odd = self.s.odd_sizes.get(self.n_blocks - 1)
         for i in range(self.s.ss, self.s.se + 1):
             t = absv[i]
+            if t == 0 and r == 0 and odd is not None:  # the odd symbol passes this zero position
+                self.flush_eobrun()
+                self.w.symbol(self.ac[0], odd)
+                for b in br:
+                    self.w.put(b, 1)
+                br, odd = [], None
+                continue
             if t == 0:
                 r += 1
                 continue
@@ -347,6 +372,8 @@ class _ScanCoder:
             for b in br:
                 self.w.put(b, 1)
             br, r = [], 0
+        if odd is not None:
+            raise ValueError("block %d of the scan has no zero position for a symbol of size %d" % (self.n_blocks - 1, odd))
         if r > 0 or br:
             self.eobrun += 1
             self.be += br
@@ -355,6 +382,7 @@ class _ScanCoder:
 
     def block(self, k, blk):
         s = self.s
+        self.n_blocks += 1
         if not self.f.progressive:
             self.w.blocks.append(self.w.bit)
             self.sequential(k, blk)
@@ -378,6 +406,8 @@ def _check_scan(frame, scan):
             raise ValueError("progressive AC scans hold one component")
         if scan.ah and scan.al != scan.ah - 1:
             raise ValueError("successive approximation refines one bit at a time")
+        if scan.odd_sizes and (scan.ss == 0 or scan.ah == 0 or not all(2 <= n <= 15 for n in scan.odd_sizes.values())):
+            raise ValueError("symbols of size 2..15 go into AC refinement scans")
     elif (scan.ss, scan.se, scan.ah, scan.al) != (0, 63, 0, 0):
         raise ValueError("sequential scans code the whole block")
 
@@ -392,13 +422,7 @@ def encode(frame):
         if c.coef.shape != (mcy * c.v, mcx * c.h, 8, 8):
             raise ValueError("component %d: coefficients must cover the MCU-padded grid %r" % (ci, (mcy * c.v, mcx * c.h)))
     out = bytearray(b"\xff\xd8")
-    dqt = b""
-    for slot, q in sorted(frame.quant.items()):
-        q = np.asarray(q).reshape(64)[ZIGZAG]
-        if q.min() < 1 or q.max() > (65535 if frame.dqt16 else 255):
-            raise ValueError("quantiser out of range")
-        dqt += bytes([(0x10 if frame.dqt16 else 0) | slot]) + (b"".join(int(v).to_bytes(2, "big") for v in q) if frame.dqt16 else bytes(int(v) for v in q))
-    out += _segment(0xDB, dqt)
+    out += _dqt(frame.quant, frame.dqt16)
     baseline = (frame.precision == 8 and not frame.dqt16 and not frame.progressive and
                 all(slot < 2 for scan in frame.scans for slot in (scan.td or [0]) + (scan.ta or [0])) and
                 all(slot < 2 for (_, slot) in frame.tables))
@@ -411,9 +435,14 @@ def encode(frame):
     if frame.restart_interval:
         out += _segment(0xDD, list(frame.restart_interval.to_bytes(2, "big")))
     current = dict(frame.tables)
+    ri = frame.restart_interval
     frame.stats = {"symbols": [], "intervals": [], "blocks": []}
     for scan in frame.scans:
         _check_scan(frame, scan)
+        out += _dqt(scan.quant, frame.dqt16)
+        if scan.restart_interval is not None:
+            ri = scan.restart_interval
+            out += _segment(0xDD, list(ri.to_bytes(2, "big")))
         out += _dht(scan.tables)
         current.update(scan.tables)
         ns = len(scan.comps)
@@ -433,7 +462,7 @@ def encode(frame):
             bw, bh = own[scan.comps[0]]
             if np.any(c.coef[bh:]) or np.any(c.coef[:, bw:]):
                 raise ValueError("component %d has coefficients outside the grid a single-component scan codes" % scan.comps[0])
-        ri, rst = frame.restart_interval, 0
+        rst = 0
         for m, unit in enumerate(units):
             if ri and m and m % ri == 0:
                 coder.restart()

@@ -5,6 +5,9 @@ import numpy as np
 import pytest
 
 from tests import entropy_cases as ec
+from tests import oracle_binding
+from tests import progressive_cases as pc
+from tests import progressive_model as pm
 from tests import streamwriter as sw
 
 TABLE_HEADER_BYTES = 16 + 16 + 4 * 160 * 2 * 4  # magic..flags, lut_off[8], qz[4][160][2] (internal.hpp)
@@ -174,3 +177,32 @@ def test_decoder_tables_follow_canonical_codes(built, name):
                 assert (lut[base + (1 << L1) + 32 * sub + np.array(rest, dtype=np.int64)] == UNUSED).all() if rest else True
             expect_words += (1 << L1) + 32 * len(subs)
         assert words == expect_words, (si, words, expect_words)
+
+
+@pytest.mark.parametrize("name", pc.NAMES)
+def test_oracle_reads_back_the_progressive_levels(oracle, name):
+    """every progressive case, the per-scan DQT / DRI and the refinement symbols of sizes 2..15 included, decodes in the oracle to
+    the levels the model says its script codes"""
+    frame, data = pc.case(name)
+    rc, s, planes = oracle.coefficients(data)
+    assert rc == 0
+    for c, want in enumerate(pm.levels(frame)):
+        assert np.array_equal(planes[c], want), "component %d" % c
+
+
+def test_writer_places_per_scan_markers_and_odd_sizes():
+    frame, data = pc.case("dri_changed_between_scans")
+    _, s = oracle_binding.load().info(data)
+    assert [s.scan[i].restart_interval for i in range(s.nscans)] == [2, 3, 0]
+    frame, data = pc.case("dqt_redefined_scan")
+    sos = [i for i in range(len(data) - 1) if data[i:i + 2] == b"\xff\xda"]
+    dqt = [i for i in range(len(data) - 1) if data[i:i + 2] == b"\xff\xdb"]
+    assert len(dqt) == 3 and sos[1] < dqt[1] < sos[2] < dqt[2] < sos[3]  # in front of the third and the fourth scan
+    frame, _ = pc.case("refine_odd_sizes")
+    table = frame.scans[2].tables[("ac", 0)]
+    lengths = {table.codes[n][1] for n in range(2, 16)}
+    assert {n for _, n in frame.stats["symbols"][2]} >= lengths  # the odd symbols carry no value bits
+    with pytest.raises(ValueError, match="no zero position"):
+        bad = pc.refine_odd_sizes(1)
+        bad.components[0].coef[0, 0].reshape(64)[sw.ZIGZAG[1:]] = 2
+        sw.encode(bad)
