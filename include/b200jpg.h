@@ -201,7 +201,8 @@ B200JPG_API int b200jpg_batch_create(b200jpg_ctx *ctx, const uint8_t *const *fra
  * Everything after the reconstruction is unchanged (orientation, crop, resize, float map), as are extents, out_bytes and statuses.
  * The flag together with B200JPG_FLAG_DOWNSCALE_k or B200JPG_FLAG_NO_UPSAMPLE is B200JPG_ERR_NOT_IMPLEMENTED for the call; a 12-bit
  * frame, a two- or a four-component frame has the status B200JPG_ERR_NOT_IMPLEMENTED (it fails the call, or with tolerate_bad it
- * is skipped). Accepted wherever request flags are. Without the flag a batch is planned exactly as before. */
+ * is skipped). Accepted wherever request flags are. Without the flag a batch is planned exactly as before. libjpeg-turbo's reduced
+ * decode at 1/2, 1/4 and 1/8 (Pillow's draft) is a per-frame request of b200jpg_batch_create_draft. */
 #define B200JPG_FLAG_LIBJPEG_TURBO 0x80u
 B200JPG_API int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
                             unsigned flags, b200jpg_batch **batch);
@@ -260,6 +261,31 @@ typedef struct b200jpg_size {
 B200JPG_API int b200jpg_batch_create_resize(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
                                             unsigned flags, const b200jpg_rect *rects, const b200jpg_size *sizes, int resample,
                                             b200jpg_batch **batch);
+/* b200jpg_batch_create_resize with a requested size per frame for libjpeg-turbo's reduced decode, as Pillow's
+ * JpegImageFile.draft(mode, (width, height)) asks for it (DESIGN §17; no counterpart in the reference). With drafts[i] = {w, h},
+ * frame i of codestream size W x H is decoded at scale 1/k, k = b200jpg_draft_scale(frame, w, h), as ceil(W / k) x ceil(H / k), and
+ * everything else follows on that image: the composition is draft -> mode -> orientation -> crop -> resize -> float map, rectangles
+ * are given in the drafted, oriented image (b200jpg_output_size with B200JPG_FLAG_DOWNSCALE_k gives it) and a frame's status is its
+ * status without the draft. At 1/k libjpeg-turbo's reconstruction (B200JPG_FLAG_LIBJPEG_TURBO rules 1-5) changes as follows, with
+ * m = 8 / k and hmax, vmax the largest sampling factors:
+ *   1. Component c is inverse transformed to s_c x s_c samples per block: s_c = m, doubled while s_c < 8, (hmax m) % (2 h_c s_c) == 0
+ *      and (vmax m) % (2 v_c s_c) == 0 (jdmaster.c). s = 8: rule 1; 4: jpeg_idct_4x4; 2: jpeg_idct_2x2; 1: range_limit((F0 + 4) >>
+ *      3) (jidctred.c, C form, 64-bit intermediates, then the range-limit table).
+ *   2. Component c is upsampled by fx = hmax m / (h_c s_c), fy = vmax m / (v_c s_c) from its real size ceil(W' / fx) x ceil(H' / fy)
+ *      of the reduced frame W' x H': by rule 2 for k = 2 and 4, replicated for k = 8 (libjpeg-turbo turns fancy upsampling off at
+ *      1/8).
+ * A frame whose k is 1 is decoded, planned and written exactly as without a draft. drafts == NULL, or every entry {0, 0}: exactly
+ * b200jpg_batch_create_resize. Otherwise, for the call, tolerate_bad or not: an entry with exactly one zero field is
+ * B200JPG_ERR_INVALID_PARAMETER (the message names the frame); a draft without B200JPG_FLAG_LIBJPEG_TURBO is
+ * B200JPG_ERR_NOT_IMPLEMENTED, as B200JPG_FLAG_LIBJPEG_TURBO with B200JPG_FLAG_DOWNSCALE_k or B200JPG_FLAG_NO_UPSAMPLE stays. The
+ * draft of a frame that fails to parse is ignored. */
+B200JPG_API int b200jpg_batch_create_draft(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
+                                           unsigned flags, const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes,
+                                           int resample, b200jpg_batch **batch);
+/* Pillow's draft scale of one codestream for a requested width x height (host only): s = min(W / width, H / height) in integer
+ * division over the codestream's own W x H (before any Exif orientation), and the largest k of 8, 4, 2, 1 with k <= s, or 1 when
+ * none fits. Returns k, or the negative parse error of the codestream; a zero width or height is B200JPG_ERR_INVALID_PARAMETER. */
+B200JPG_API int b200jpg_draft_scale(const uint8_t *data, size_t len, uint32_t width, uint32_t height);
 /* The fixed-point tables b200jpg_batch_create_resize uses to resample one axis of in_size samples to out_size (tests only, host
  * only, no device): bounds[2 j] is the first source index and bounds[2 j + 1] the number of taps of output j, coeffs[j * ksize + t]
  * the int32 coefficient of tap t (zero behind the taps). *ksize receives the row length. The tables are written when bounds and

@@ -141,6 +141,7 @@ struct ReconGroup {
     OutMode mode = OutMode::Coded;  // B200JPG_FLAG_OUTPUT_RGB / _L: the frames' slots are described (rewritten descriptors)
     std::vector<FrameRecon> frames;
     uint32_t max_bw0 = 0, max_bh0 = 0, max_bwc = 0, max_bhc = 0;
+    uint32_t scale = 1;   // the frames' factor k (b200jpg_batch::scale)
     uint64_t dev_frames = 0;
 };
 
@@ -170,15 +171,47 @@ bool rect_empty(const b200jpg_rect &r) { return r.x == 0 && r.y == 0 && r.width 
 bool size_empty(const b200jpg_size &s) { return s.width == 0 && s.height == 0; }
 bool resample_known(int r) { return r >= B200JPG_RESAMPLE_LANCZOS && r <= B200JPG_RESAMPLE_HAMMING; }  // PIL's values 1 .. 5
 
-// component c as it leaves the decoder: the frame size W' x H' = ceil(W / k) x ceil(H / k), or without upsampling its own
-// ceil(W' / subx) x ceil(H' / suby); width and height swapped for the Exif orientations 5..8 (`orientation`: the one the frame
-// leaves with, 1 for the extent the kernels decode); the rectangle's size for a frame with a crop (`crop`, given in those output
-// coordinates and checked against them; never together with B200JPG_FLAG_NO_UPSAMPLE); the target size of a resized frame (`size`)
-Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags, int orientation, const b200jpg_rect *crop = nullptr,
+// Pillow's draft scale (JpegImageFile.draft) of a frame of codestream size W x H for a request of width x height (both >= 1): the
+// largest k of 8, 4, 2, 1 with k <= min(W / width, H / height), 1 when none fits
+uint32_t draft_scale_of(const b200jpg_frame_info &fi, uint32_t width, uint32_t height) {
+    const uint32_t s = std::min(fi.width / width, fi.height / height);
+    for (uint32_t k : {8u, 4u, 2u})
+        if (k <= s) return k;
+    return 1;
+}
+
+// libjpeg-turbo's IDCT output size of component c at scale 1/k (jdmaster.c, DESIGN §17): m = 8 / k, doubled while below 8 and the
+// component's ratios to the largest factors stay even multiples
+uint32_t draft_idct_size(const b200jpg_frame_info &fi, int c, uint32_t k) {
+    uint32_t hmax = 1, vmax = 1;
+    for (int j = 0; j < fi.ncomp; j++) hmax = std::max<uint32_t>(hmax, fi.hs[j]), vmax = std::max<uint32_t>(vmax, fi.vs[j]);
+    const uint32_t m = 8 / k;
+    uint32_t s = m;
+    while (s < 8 && (hmax * m) % (fi.hs[c] * s * 2) == 0 && (vmax * m) % (fi.vs[c] * s * 2) == 0) s *= 2;
+    return s;
+}
+
+// the integer factors component c of a frame decoded at scale 1/k is upsampled by after its IDCT: hmax (8 / k) / (h_c s_c) x
+// vmax (8 / k) / (v_c s_c), s_c = draft_idct_size (DESIGN §17); subx x suby at k = 1
+struct Ratio {
+    uint32_t x, y;
+};
+Ratio draft_ratio(const b200jpg_frame_info &fi, int c, uint32_t k) {
+    uint32_t hmax = 1, vmax = 1;
+    for (int j = 0; j < fi.ncomp; j++) hmax = std::max<uint32_t>(hmax, fi.hs[j]), vmax = std::max<uint32_t>(vmax, fi.vs[j]);
+    const uint32_t s = draft_idct_size(fi, c, k);
+    return {hmax * (8 / k) / (fi.hs[c] * s), vmax * (8 / k) / (fi.vs[c] * s)};
+}
+
+// component c as it leaves the decoder, decoded at scale 1/k (B200JPG_FLAG_DOWNSCALE_k or the frame's draft: b200jpg_batch::scale):
+// the frame size W' x H' = ceil(W / k) x ceil(H / k), or without upsampling its own ceil(W' / subx) x ceil(H' / suby); width and
+// height swapped for the Exif orientations 5..8 (`orientation`: the one the frame leaves with, 1 for the extent the kernels decode);
+// the rectangle's size for a frame with a crop (`crop`, given in those output coordinates and checked against them; never together
+// with B200JPG_FLAG_NO_UPSAMPLE); the target size of a resized frame (`size`)
+Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags, uint64_t k, int orientation, const b200jpg_rect *crop = nullptr,
                   const b200jpg_size *size = nullptr) {
     if (size) return {size->width, size->height};
     if (crop) return {crop->width, crop->height};
-    const uint64_t k = downscale_of(flags);
     uint64_t w = (fi.width + k - 1) / k, h = (fi.height + k - 1) / k;
     if (flags & B200JPG_FLAG_NO_UPSAMPLE) w = (w + fi.subx[c] - 1) / fi.subx[c], h = (h + fi.suby[c] - 1) / fi.suby[c];
     if (orientation >= 5) return {h, w};
@@ -257,6 +290,9 @@ struct b200jpg_batch {
     unsigned flags = 0;  // B200JPG_FLAG_*
     std::vector<ParsedFrame> frames;
     std::vector<int> parse_status;
+    // [n] the factor k every frame is decoded at, 1/k: B200JPG_FLAG_DOWNSCALE_k, or a live frame's draft (admit_drafts). Every
+    // extent, plane layout and path decision of a frame reads it here
+    std::vector<uint32_t> scale;
     int n_user = 0;                       // frames of the caller; [n_user, n) are residual codestreams of JPEG XT frames
     std::vector<int> xt_child, xt_parent;  // [n_user] index of a frame's residual frame or -1; [n] the reverse
     std::vector<uint64_t> out_off, out_bytes;
@@ -464,10 +500,18 @@ int b200jpg_output_size(const uint8_t *data, size_t len, unsigned flags, uint32_
     ParsedFrame pf;
     const int rc = parse_one(data, len, pf);
     if (rc != 0) return rc;
-    const Extent e = out_extent(pf.info, 0, flags & ~B200JPG_FLAG_NO_UPSAMPLE, (flags & B200JPG_FLAG_EXIF_ORIENTATION) ? pf.orientation : 1);
+    const Extent e = out_extent(pf.info, 0, flags & ~B200JPG_FLAG_NO_UPSAMPLE, downscale_of(flags),
+                                (flags & B200JPG_FLAG_EXIF_ORIENTATION) ? pf.orientation : 1);
     *width = (uint32_t)e.w;
     *height = (uint32_t)e.h;
     return B200JPG_OK;
+}
+
+int b200jpg_draft_scale(const uint8_t *data, size_t len, uint32_t width, uint32_t height) {
+    if (width == 0 || height == 0) return B200JPG_ERR_INVALID_PARAMETER;
+    ParsedFrame pf;
+    const int rc = parse_one(data, len, pf);
+    return rc != 0 ? rc : (int)draft_scale_of(pf.info, width, height);
 }
 
 int b200jpg_resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, int32_t *bounds, int32_t *coeffs, uint64_t capacity,
@@ -767,19 +811,23 @@ static std::vector<uint64_t> lay_out_codestreams(b200jpg_batch &b, const std::ve
 // B200JPG_FLAG_LIBJPEG_TURBO (8-bit grey and three-component frames: attach_residuals): the tiled turbo_reconstruct_kernel covers
 // component 0 at full resolution, alone or with two chroma components of equal factors 1 or 2 whose fancy upsampling has both
 // neighbours (more than 2 chroma samples per row when halved horizontally); everything else the generic turbo kernel. ncomp: the
-// components reconstructed (1 for mode "L" of a YCbCr frame)
-static ReconPath turbo_path(const b200jpg_frame_info &fi, int ncomp) {
+// components reconstructed (1 for mode "L" of a YCbCr frame). A frame drafted to 1/k (k > 1, DESIGN §17) is judged on the ratios
+// after its IDCTs (draft_ratio) and its reduced width: its luma block is then 8 / k wide, and its chroma ratios 1 x 1 (4:4:4,
+// 4:2:0), 2 x 1 (4:2:2) or 1 x 2 (4:4:0); 2 x 2 never occurs at k > 1 and is left to the generic kernel
+static ReconPath turbo_path(const b200jpg_frame_info &fi, int ncomp, uint32_t k) {
     if (fi.subx[0] != 1 || fi.suby[0] != 1) return ReconPath::TurboGeneric;
     if (ncomp == 1) return ReconPath::Turbo;
-    const uint32_t sx = fi.subx[1], sy = fi.suby[1];
-    if (sx != fi.subx[2] || sy != fi.suby[2] || sx > 2 || sy > 2) return ReconPath::TurboGeneric;
-    return (sx == 2 && (fi.width + 1) / 2 <= 2) ? ReconPath::TurboGeneric : ReconPath::Turbo;
+    const Ratio r = draft_ratio(fi, 1, k), r2 = draft_ratio(fi, 2, k);
+    if (r.x != r2.x || r.y != r2.y || r.x > 2 || r.y > 2) return ReconPath::TurboGeneric;
+    if (k > 1 && (fi.hs[1] != fi.hs[2] || fi.vs[1] != fi.vs[2] || (r.x == 2 && r.y == 2))) return ReconPath::TurboGeneric;
+    const uint32_t w = (fi.width + k - 1) / k;
+    return (r.x == 2 && (w + 1) / 2 <= 2) ? ReconPath::TurboGeneric : ReconPath::Turbo;
 }
 
 static ReconPath recon_path(const b200jpg_batch &b, int i) {
     const b200jpg_frame_info &fi = b.frames[i].info;
-    const bool scaled = downscale_of(b.flags) > 1;
-    if (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) return turbo_path(fi, fi.ncomp);
+    const bool scaled = b.scale[i] > 1;
+    if (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) return turbo_path(fi, fi.ncomp, b.scale[i]);
     if (b.xt_parent[i] >= 0 || (i < b.n_user && b.xt_child[i] >= 0)) return ReconPath::Generic;
     if (b.flags & B200JPG_FLAG_NO_UPSAMPLE) return scaled ? ReconPath::Scaled : ReconPath::Generic;  // planes of every component, then one sample -> one output value
     if (fi.precision != 8) return scaled ? ReconPath::Scaled : ReconPath::Generic;  // 12-bit frames: int32 planes, 16-bit samples out
@@ -814,14 +862,14 @@ static FramePlan frame_plan(const b200jpg_batch &b, int i) {
             // luma alone: a grey frame over component 0 on the MCU-padded block grid; libjpeg's JCS_GRAYSCALE for YCbCr input
             p.ncomp = 1;
             if (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) {  // the turbo kernels over component 0
-                p.path = turbo_path(fi, 1);
+                p.path = turbo_path(fi, 1, b.scale[i]);
                 return p;
             }
-            if (downscale_of(b.flags) > 1) p.path = ReconPath::Scaled;
+            if (b.scale[i] > 1) p.path = ReconPath::Scaled;
             else p.path = (fi.precision != 8 || fi.subx[0] != 1 || fi.suby[0] != 1) ? ReconPath::Generic : ReconPath::Tiled;
         } else {  // RGB-coded and JPEG XT frames: the L formula after the colour transformation (merge) and clamp, in the generic kernels
             p.mode = OutMode::Luma;
-            if (!(b.flags & B200JPG_FLAG_LIBJPEG_TURBO)) p.path = downscale_of(b.flags) > 1 ? ReconPath::Scaled : ReconPath::Generic;
+            if (!(b.flags & B200JPG_FLAG_LIBJPEG_TURBO)) p.path = b.scale[i] > 1 ? ReconPath::Scaled : ReconPath::Generic;
         }
     }
     if ((b.flags & B200JPG_FLAG_OUTPUT_RGB) && fi.ncomp == 1) {
@@ -832,7 +880,7 @@ static FramePlan frame_plan(const b200jpg_batch &b, int i) {
         const bool rgb = (b.flags & B200JPG_FLAG_OUTPUT_RGB) != 0;  // Pillow's conversion in the generic kernels (DESIGN §15)
         p.out_ncomp = rgb ? 3 : 1;
         p.mode = rgb ? OutMode::CmykRgb : OutMode::CmykLuma;
-        p.path = downscale_of(b.flags) > 1 ? ReconPath::Scaled : ReconPath::Generic;
+        p.path = b.scale[i] > 1 ? ReconPath::Scaled : ReconPath::Generic;
     }
     return p;
 }
@@ -840,8 +888,8 @@ static FramePlan frame_plan(const b200jpg_batch &b, int i) {
 // Coefficient, sample and output layout of the live frames; returns the sample plane offsets. The sample planes a frame gets
 // follow its reconstruction path: Generic one per component, Tiled one per component from 1 on, Fused420 none (its chroma samples
 // live in shared memory), Scaled one per component of 8 ceil(blocks_w / k) x 8 ceil(blocks_h / k) samples, Scaled420 none,
-// TurboGeneric one uint8 plane per reconstructed component and Turbo one per component from 1 on, byte offsets into the batch's
-// uint8 plane buffer.
+// TurboGeneric one uint8 plane per reconstructed component (s_c x s_c bytes per block of a drafted frame, draft_idct_size) and Turbo
+// one per component from 1 on, byte offsets into the batch's uint8 plane buffer.
 static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
     const int n = b.n;
     b.coef_base.assign(n, {});
@@ -855,22 +903,23 @@ static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
         const FramePlan plan = frame_plan(b, i);
         const ReconPath path = plan.path;
         const int first_plane = (path == ReconPath::Generic || path == ReconPath::Scaled || path == ReconPath::TurboGeneric) ? 0 : (path == ReconPath::Tiled ? 1 : fi.ncomp);
-        const uint32_t k = downscale_of(b.flags);
+        const uint32_t k = b.scale[i];
         uint64_t samples = 0;
         for (int c = 0; c < fi.ncomp; c++) {  // every component is entropy decoded; only the reconstructed ones get sample planes
             const uint64_t elems = (uint64_t)fi.blocks_w[c] * fi.blocks_h[c] * 64;
             b.coef_base[i][c] = coef_cur;
             coef_cur += elems;
             if ((path == ReconPath::TurboGeneric || (path == ReconPath::Turbo && c >= 1)) && c < (int)plan.ncomp) {
+                const uint64_t s = draft_idct_size(fi, c, k);  // s x s bytes per block (8 x 8 undrafted)
                 sample_base[i][c] = plane8_cur;
-                plane8_cur = align_up(plane8_cur + elems, 256);
+                plane8_cur = align_up(plane8_cur + elems / 64 * s * s, 256);
             } else if (c >= first_plane && c < (int)plan.ncomp) {
                 sample_base[i][c] = sample_cur;
                 sample_cur += path == ReconPath::Scaled ? 64ull * ((fi.blocks_w[c] + k - 1) / k) * ((fi.blocks_h[c] + k - 1) / k) : elems;
             }
         }
         for (uint32_t c = 0; c < plan.out_ncomp; c++) {
-            const Extent e = out_extent(fi, (int)c, b.flags, 1, crop_of(b, i), size_of(b, i));  // the components one after the other (w * h: any orientation)
+            const Extent e = out_extent(fi, (int)c, b.flags, k, 1, crop_of(b, i), size_of(b, i));  // the components one after the other (w * h: any orientation)
             samples += e.w * e.h;
         }
         b.out_off[i] = out_cur;
@@ -1091,6 +1140,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         const uint32_t nc = plan.ncomp;
         const bool generic = path == ReconPath::Generic || path == ReconPath::Scaled || path == ReconPath::TurboGeneric;
         uint32_t sx = nc > 1 ? fi.subx[1] : 1, sy = nc > 1 ? fi.suby[1] : 1;
+        if (nc > 1 && path == ReconPath::Turbo) sx = draft_ratio(fi, 1, b.scale[i]).x, sy = draft_ratio(fi, 1, b.scale[i]).y;
         if (generic) sx = sy = 0;  // one group per component count: the generic kernels read the factors per frame
         // oriented frames (B200JPG_FLAG_EXIF_ORIENTATION, 2..8) form groups of their own, one per orientation: their destinations
         // are rewritten descriptors, whose store kind is chosen per group
@@ -1103,10 +1153,12 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         // of B200JPG_FLAG_OUTPUT_RGB writes its one channel into the scratch: the resample pass replicates it
         const OutMode mode = (resized && plan.mode == OutMode::Replicate) ? OutMode::Coded : plan.mode;
         if (orientation != 1 || crop || plan.mode != OutMode::Coded) b.rewritten = true;
+        // and the frames of one scale: a group's launches take its factor k (ReconLaunch::downscale)
+        const uint32_t k = b.scale[i];
         ReconGroup *g = nullptr;
         for (auto &gg : b.groups)
             if (gg.ncomp == nc && gg.subx == sx && gg.suby == sy && gg.path == path && gg.orientation == orientation && gg.cropped == (crop != nullptr) &&
-                gg.resized == resized && gg.mode == mode)
+                gg.resized == resized && gg.mode == mode && gg.scale == k)
                 g = &gg;
         if (!g) {
             b.groups.emplace_back();
@@ -1119,25 +1171,36 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
             g->orientation = orientation;
             g->cropped = crop != nullptr;
             g->resized = resized;
+            g->scale = k;
         }
         FrameRecon fr{};
-        const uint32_t k = downscale_of(b.flags);
+        const bool drafted = k > 1 && (path == ReconPath::TurboGeneric || path == ReconPath::Turbo);
+        uint32_t hmax = 1, vmax = 1;
+        for (int c = 0; c < fi.ncomp; c++) hmax = std::max<uint32_t>(hmax, fi.hs[c]), vmax = std::max<uint32_t>(vmax, fi.vs[c]);
         for (uint32_t c = 0; c < nc; c++) {
             fr.coef_base[c] = b.coef_base[i][c];
             fr.sample_base[c] = sample_base[i][c];
             fr.bw[c] = fi.blocks_w[c];
             fr.bh[c] = fi.blocks_h[c];
-            if (k > 1) {  // the grid of the reduced planes; the coefficient grid moves to coef_bw / coef_bh
+            fr.csx[c] = fi.subx[c];
+            fr.csy[c] = fi.suby[c];
+            if (drafted) {  // the coefficient grid on both sides, s x s samples per block, the ratios after the reduced IDCT
+                const uint32_t s = draft_idct_size(fi, (int)c, k);
+                fr.coef_bw[c] = fi.blocks_w[c];
+                fr.coef_bh[c] = fi.blocks_h[c];
+                fr.idct[c] = (uint8_t)s;
+                fr.csx[c] = (uint8_t)(hmax * (8 / k) / (fi.hs[c] * s));
+                fr.csy[c] = (uint8_t)(vmax * (8 / k) / (fi.vs[c] * s));
+            } else if (k > 1) {  // the grid of the reduced planes; the coefficient grid moves to coef_bw / coef_bh
                 fr.coef_bw[c] = fi.blocks_w[c];
                 fr.coef_bh[c] = fi.blocks_h[c];
                 fr.bw[c] = (fi.blocks_w[c] + k - 1) / k;
                 fr.bh[c] = (fi.blocks_h[c] + k - 1) / k;
             }
-            fr.csx[c] = fi.subx[c];
-            fr.csy[c] = fi.suby[c];
         }
+        fr.fancy = k < 8;  // libjpeg-turbo upsamples by replication at 1/8 (min_DCT_scaled_size == 1)
         fr.out_base = b.out_off[i];
-        const Extent reduced = out_extent(fi, 0, b.flags & ~B200JPG_FLAG_NO_UPSAMPLE, 1);  // W' x H' (the full size without downscaling)
+        const Extent reduced = out_extent(fi, 0, b.flags & ~B200JPG_FLAG_NO_UPSAMPLE, k, 1);  // W' x H' (the full size at k = 1)
         fr.width = (uint32_t)reduced.w;
         fr.height = (uint32_t)reduced.h;
         if (b.xt_parent[i] >= 0) fr.width = fr.height = 0;  // a residual codestream: planes only, its frame's reconstruction reads them
@@ -1166,11 +1229,21 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
             // such range of the group and every CTA runs tile (tx0 + bx, ty0 + by) exactly as the uncropped decode does
             const Clip cl = crop_to_decoded(orientation, *crop, reduced.w, reduced.h);
             const ReconTile t = recon_tile(path);
-            const uint32_t tw = 8 * t.bw, th = 8 * t.bh;
+            const uint32_t bpx = (drafted && path == ReconPath::Turbo) ? 8 / k : 8;  // output pixels per tile block: a drafted luma block's
+            const uint32_t tw = bpx * t.bw, th = bpx * t.bh;
             fr.clip_x0 = cl.x0, fr.clip_y0 = cl.y0, fr.clip_x1 = cl.x1, fr.clip_y1 = cl.y1;
             fr.tx0 = cl.x0 / tw, fr.ty0 = cl.y0 / th;
             const uint32_t ntx = (cl.x1 - 1) / tw - fr.tx0 + 1, nty = (cl.y1 - 1) / th - fr.ty0 + 1;
-            if ((path == ReconPath::Tiled || path == ReconPath::Turbo) && nc > 1) {
+            if (drafted && path == ReconPath::Turbo && nc > 1) {
+                // the chroma samples under those tiles, one more on each side (the upsampling window), as blocks of idct[1] samples
+                const int64_t s = fr.idct[1];
+                const int64_t jx0 = (int64_t)fr.tx0 * tw / sx - 1, jy0 = (int64_t)fr.ty0 * th / sy - 1;
+                const int64_t jx1 = ((int64_t)(fr.tx0 + ntx) * tw - 1) / sx + 1, jy1 = ((int64_t)(fr.ty0 + nty) * th - 1) / sy + 1;
+                fr.cb_x0 = (uint32_t)(std::max<int64_t>(jx0, 0) / s), fr.cb_y0 = (uint32_t)(std::max<int64_t>(jy0, 0) / s);
+                fr.cb_x1 = (uint32_t)std::min<int64_t>(jx1 / s + 1, fi.blocks_w[1]), fr.cb_y1 = (uint32_t)std::min<int64_t>(jy1 / s + 1, fi.blocks_h[1]);
+                g->max_bwc = std::max(g->max_bwc, fr.cb_x1 - fr.cb_x0);
+                g->max_bhc = std::max(g->max_bhc, fr.cb_y1 - fr.cb_y0);
+            } else if ((path == ReconPath::Tiled || path == ReconPath::Turbo) && nc > 1) {
                 // b1: the chroma blocks under those tiles, one more on each side (the upsampling window), clipped to the plane
                 const int64_t cbx0 = (int64_t)fr.tx0 * t.bw / sx - 1, cby0 = (int64_t)fr.ty0 * t.bh / sy - 1;
                 const int64_t cbx1 = (int64_t)(fr.tx0 + ntx) * t.bw / sx + 1, cby1 = (int64_t)(fr.ty0 + nty) * t.bh / sy + 1;
@@ -1325,7 +1398,7 @@ static int admit_crops(b200jpg_batch &b, const b200jpg_rect *rects) {
         b200jpg_rect &r = b.crop[i];
         if (b.parse_status[i] != 0) r = b200jpg_rect{0, 0, 0, 0};
         if (rect_empty(r)) continue;
-        const Extent e = out_extent(b.frames[i].info, 0, b.flags, applied_orientation(b, i));
+        const Extent e = out_extent(b.frames[i].info, 0, b.flags, b.scale[i], applied_orientation(b, i));
         if (r.width == 0 || r.height == 0 || (uint64_t)r.x + r.width > e.w || (uint64_t)r.y + r.height > e.h)
             return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": crop rectangle (" + std::to_string(r.x) + ", " +
                                                                   std::to_string(r.y) + ", " + std::to_string(r.width) + ", " + std::to_string(r.height) +
@@ -1349,11 +1422,19 @@ static int admit_sizes(b200jpg_batch &b, const b200jpg_size *sizes) {
             return b.ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "frame " + std::to_string(i) + ": target size " + std::to_string(s.width) + " x " +
                                                               std::to_string(s.height) + " is too large to allocate");
         if (rect_empty(b.crop[i])) {
-            const Extent e = out_extent(fi, 0, b.flags, applied_orientation(b, i));
+            const Extent e = out_extent(fi, 0, b.flags, b.scale[i], applied_orientation(b, i));
             b.crop[i] = b200jpg_rect{0, 0, (uint32_t)e.w, (uint32_t)e.h};
         }
     }
     return B200JPG_OK;
+}
+
+// b200jpg_batch_create_draft's requests (nullptr: none): every frame's factor k, B200JPG_FLAG_DOWNSCALE_k or, for a live caller's
+// frame with a request, Pillow's draft scale (a failed frame's request is ignored)
+static void admit_drafts(b200jpg_batch &b, const b200jpg_size *drafts) {
+    b.scale.assign(b.n, downscale_of(b.flags));
+    for (int i = 0; drafts && i < b.n_user; i++)
+        if (b.parse_status[i] == 0 && !size_empty(drafts[i])) b.scale[i] = draft_scale_of(b.frames[i].info, drafts[i].width, drafts[i].height);
 }
 
 // B200JPG_FLAG_LIBJPEG_TURBO: every live frame without a rectangle is cropped to its whole output, as admit_sizes does for
@@ -1363,7 +1444,7 @@ static void crop_whole_frames(b200jpg_batch &b) {
     if (b.crop.empty()) b.crop.assign(b.n_user, b200jpg_rect{0, 0, 0, 0});
     for (int i = 0; i < b.n_user; i++) {
         if (b.parse_status[i] != 0 || !rect_empty(b.crop[i])) continue;
-        const Extent e = out_extent(b.frames[i].info, 0, b.flags, applied_orientation(b, i));
+        const Extent e = out_extent(b.frames[i].info, 0, b.flags, b.scale[i], applied_orientation(b, i));
         b.crop[i] = b200jpg_rect{0, 0, (uint32_t)e.w, (uint32_t)e.h};
     }
 }
@@ -1387,7 +1468,7 @@ static void plan_resample(b200jpg_batch &b) {
     for_frames(nr, 16, [&](int r) {
         const int i = b.rs_user[r];
         const b200jpg_frame_info &fi = b.frames[i].info;
-        const Extent e = out_extent(fi, 0, b.flags, applied_orientation(b, i), crop_of(b, i));  // C
+        const Extent e = out_extent(fi, 0, b.flags, b.scale[i], applied_orientation(b, i), crop_of(b, i));  // C
         const b200jpg_size &s = *size_of(b, i);
         ResampleFrame &f = b.rs_frames[r];
         auto &t = b.rs_tables[r];
@@ -1419,10 +1500,20 @@ static void plan_resample(b200jpg_batch &b) {
 }
 
 static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
-                             const b200jpg_rect *rects, const b200jpg_size *sizes, int resample, b200jpg_batch **out) {
+                             const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes, int resample, b200jpg_batch **out) {
     NvtxRange nvtx("b200jpg batch_create: parse + pack");
     if (!out || !frames || !lens || n <= 0) return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "invalid batch arguments");
     *out = nullptr;
+    bool any_draft = false;
+    for (int i = 0; drafts && i < n; i++) {
+        if ((drafts[i].width == 0) != (drafts[i].height == 0))
+            return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": draft size " + std::to_string(drafts[i].width) + " x " +
+                                                                std::to_string(drafts[i].height) + " has exactly one zero side");
+        any_draft = any_draft || !size_empty(drafts[i]);
+    }
+    if (!any_draft) drafts = nullptr;  // all {0, 0}: exactly the batch of b200jpg_batch_create_resize
+    if (drafts && !(flags & B200JPG_FLAG_LIBJPEG_TURBO))
+        return ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, "a draft size needs B200JPG_FLAG_LIBJPEG_TURBO (libjpeg-turbo's reduced decode)");
     bool any_crop = false;
     for (int i = 0; rects && i < n; i++) any_crop = any_crop || !rect_empty(rects[i]);
     if (!any_crop) rects = nullptr;  // all {0, 0, 0, 0}: exactly the batch of b200jpg_batch_create_ex
@@ -1468,6 +1559,7 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
     attach_residuals(b, cs, device_index);
     std::vector<std::vector<TableSet>> frame_tables;
     if (int rc = admit_frames(b, cs, tolerate_bad != 0, frame_tables)) return rc;
+    admit_drafts(b, drafts);
     if (rects)
         if (int rc = admit_crops(b, rects)) return rc;
     if (sizes)
@@ -1503,9 +1595,14 @@ int b200jpg_batch_create_crop(b200jpg_ctx *ctx, const uint8_t *const *frames, co
 
 int b200jpg_batch_create_resize(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
                                 const b200jpg_rect *rects, const b200jpg_size *sizes, int resample, b200jpg_batch **out) {
+    return b200jpg_batch_create_draft(ctx, frames, lens, n, tolerate_bad, flags, nullptr, rects, sizes, resample, out);
+}
+
+int b200jpg_batch_create_draft(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
+                               const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes, int resample, b200jpg_batch **out) {
     if (!ctx) return B200JPG_ERR_INVALID_PARAMETER;
     try {  // no exception crosses the C ABI
-        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, rects, sizes, resample, out);
+        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, drafts, rects, sizes, resample, out);
     } catch (const std::bad_alloc &) {
         if (out) *out = nullptr;
         return ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "out of host memory while preparing the batch");
@@ -1526,7 +1623,7 @@ int b200jpg_batch_output_extent(const b200jpg_batch *b, int i, int c, uint32_t *
     if (b->parse_status[i] != 0) return b->parse_status[i];
     const b200jpg_frame_info &fi = b->frames[i].info;
     if (c < 0 || c >= (int)frame_plan(*b, i).out_ncomp) return B200JPG_ERR_INVALID_PARAMETER;
-    const Extent e = out_extent(fi, c, b->flags, applied_orientation(*b, i), crop_of(*b, i), size_of(*b, i));
+    const Extent e = out_extent(fi, c, b->flags, b->scale[i], applied_orientation(*b, i), crop_of(*b, i), size_of(*b, i));
     *width = (uint32_t)e.w;
     *height = (uint32_t)e.h;
     return B200JPG_OK;
@@ -1796,7 +1893,7 @@ static bool rewrite_frame(const b200jpg_batch *b, int i, b200jpg_plane *pl, uint
     const int o = applied_orientation(*b, i);
     const b200jpg_rect *crop = crop_of(*b, i);
     for (uint32_t c = 0; c < nc; c++) {
-        const Extent d = out_extent(fi, c, b->flags, 1);
+        const Extent d = out_extent(fi, c, b->flags, b->scale[i], 1);
         if (crop) translate_plane(pl[c], *crop);
         if (!orient_plane(pl[c], o, d.w, d.h)) return false;
         if ((uint64_t)pl[c].bytes_per_pixel != size) planar[(size_t)i] = 0;
@@ -1845,7 +1942,7 @@ static int stage_slot_planes(b200jpg_batch *b, uint8_t *out_dev, void *stream, s
             uint64_t before = 0;
             b200jpg_plane *pl = table + 4 * (size_t)i;
             for (uint32_t c = 0; c < no; c++) {
-                const Extent e = out_extent(fi, (int)c, b->flags, o, crop_of(*b, i));
+                const Extent e = out_extent(fi, (int)c, b->flags, b->scale[i], o, crop_of(*b, i));
                 pl[c].data = out_dev + b->out_off[i] + (planes ? before : (uint64_t)c) * size;
                 pl[c].bytes_per_pixel = (int32_t)(planes ? size : no * size);
                 pl[c].bytes_per_row = (int64_t)e.w * pl[c].bytes_per_pixel;
@@ -1884,7 +1981,7 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.suby = g.suby;
         l.path = g.path;
         l.mode = g.mode;
-        l.downscale = (int)downscale_of(b->flags);
+        l.downscale = (int)g.scale;
         l.planes_out = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
         l.coef = b->d_coef;
         l.samples16 = b->d_samples16;
@@ -2010,7 +2107,7 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
         const FramePlan plan = frame_plan(*b, i);
         for (int c = 0; c < (int)plan.out_ncomp; c++) {
             const b200jpg_plane &p = planes[4 * i + c];
-            const auto [w, h] = out_extent(fi, c, b->flags, orientation, crop_of(*b, i), size_of(*b, i));  // the rules hold in (cropped, resized) output coordinates
+            const auto [w, h] = out_extent(fi, c, b->flags, b->scale[i], orientation, crop_of(*b, i), size_of(*b, i));  // the rules hold in (cropped, resized) output coordinates
             const uint64_t bpp = magnitude(p.bytes_per_pixel), bpr = magnitude(p.bytes_per_row);
             const std::string at = "frame " + std::to_string(i) + " component " + std::to_string(c) + ": ";
             if (!p.data) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "no destination");

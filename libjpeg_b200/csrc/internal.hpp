@@ -250,6 +250,12 @@ struct FrameRecon {       // per frame, for the reconstruction kernels
     uint32_t tx0, ty0;
     uint32_t clip_x0, clip_y0, clip_x1, clip_y1;
     uint32_t cb_x0, cb_y0, cb_x1, cb_y1;
+    // drafted frames (Turbo / TurboGeneric groups of ReconLaunch::downscale > 1, DESIGN §17): width / height are the reduced frame, bw / bh =
+    // coef_bw / coef_bh the coefficient grid, and block (bx, by) of component c leaves the IDCT as idct[c] x idct[c] samples (8, 4,
+    // 2 or 1) of a plane with row pitch idct[c] bw[c]; csx / csy are then the upsampling ratios after that IDCT, and fancy = 0 (1/8)
+    // replicates every ratio
+    uint8_t idct[4];
+    uint32_t fancy;
 };
 
 // The tiles of the reconstruction kernels, in luma blocks (8 x 8 samples of the decoded frame): reconstruct_kernel (b2) runs 32 x
@@ -305,7 +311,8 @@ int launch_progressive_dequant(const ProgFrame *frames_dev, uint32_t n_frames, u
 // upsampling): reconstruct420_scaled_kernel, no planes. B200JPG_FLAG_LIBJPEG_TURBO (DESIGN §16, turbo_sm90.cu): Turbo (grey, and
 // three components with full-resolution component 0 and chroma factors 1 or 2, wider than 2 chroma samples when halved
 // horizontally): turbo_idct_kernel into uint8 planes of components 1.., then turbo_reconstruct_kernel; TurboGeneric (every other
-// such frame): uint8 planes of every reconstructed component, then turbo_generic_kernel
+// such frame): uint8 planes of every reconstructed component, then turbo_generic_kernel. Frames drafted to 1/2, 1/4 or 1/8 (DESIGN
+// §17) take the same two paths, decided on the ratios after their reduced IDCTs, through the _draft_ kernels
 enum class ReconPath : int { Tiled, Fused420, Generic, Scaled, Scaled420, TurboGeneric, Turbo };
 // B200JPG_FLAG_OUTPUT_RGB / _L (DESIGN §14): what a reconstruction group writes besides its components as they are. Luma: the generic
 // kernels reduce three clamped components to L = (19595 R + 38470 G + 7471 B + 32768) >> 16 and store one; Replicate: a grey frame's
@@ -328,7 +335,7 @@ struct ReconLaunch {
     OutMode mode;                  // uniform over the group; not Coded only with described destinations (never kStoreCanvas)
     bool planes_out;               // B200JPG_FLAG_NO_UPSAMPLE: the components leave as planes at their own resolution
     int generic_phase;             // generic groups: 0 = IDCT then reconstruction, 1 = IDCT only, 2 = reconstruction only
-    int downscale;                 // Scaled groups: the factor k (2, 4 or 8) of B200JPG_FLAG_DOWNSCALE_k
+    int downscale;                 // the group's factor k: B200JPG_FLAG_DOWNSCALE_k of Scaled groups, the draft of TurboGeneric groups
     const int16_t *coef;
     int16_t *samples16;            // chroma sample planes every frame goes through
     int32_t *samples32;            // the same planes for the exact pass over frames flagged `narrow`

@@ -8,6 +8,10 @@
 //                              luma blocks, luma IDCT'd into shared memory, chroma read from the planes, upsampled, converted and
 //                              stored pixel by pixel along x
 //   turbo_generic_kernel       ReconPath::TurboGeneric: one thread per output pixel from the planes of every component
+//   turbo_*_draft_kernel       the same three for drafted frames (DESIGN §17, groups of ReconLaunch::downscale > 1): each block
+//                              leaves the IDCT as FrameRecon::idct[c]^2 samples (islow, jpeg_idct_4x4, jpeg_idct_2x2 or
+//                              jpeg_idct_1x1), the Turbo tile holds luma blocks of S = 8 / k, and the planes are upsampled by the
+//                              ratios after the IDCT
 // Every frame of a flagged batch is cropped (abi.cpp: crop_whole_frames), so both kinds store through described destinations with
 // the clip.
 #include <cuda_runtime.h>
@@ -102,11 +106,111 @@ __device__ __forceinline__ void turbo_idct_block(const int16_t *__restrict__ coe
     }
 }
 
+// jpeg_idct_4x4 / jpeg_idct_2x2 (jidctred.c). As for islow, int32 is exact for a pass while every sum stays inside int32: as a
+// linear form of the pass's inputs no sum has an L1 norm above 77910 (4x4) or 85759 (2x2) (tests/test_draft_cpu.py finds both by
+// brute force), so pass 1 (rounding 2^11 / 2^12) is exact for |F| <= 27563 / 25040 and pass 2 (2^18 / 2^19) for pass-1 results
+// |v| <= 27560 / 25034. int16 coefficients exceed the pass-1 bounds: a block runs each pass in 64 bits when its inputs do
+constexpr int kRed4Pass1Exact = 27563, kRed4Pass2Exact = 27560, kRed2Pass1Exact = 25040, kRed2Pass2Exact = 25034;
+
+// one line of jpeg_idct_4x4 over d[0 .. 8) (d[4] unused) -> 4 outputs (x + 2^(kShift - 1)) >> kShift
+template <typename T, int kShift>
+__device__ __forceinline__ void red4(const T (&d)[8], T (&o)[4]) {
+    const T t0 = d[0] * (T)16384, t2 = d[2] * (T)15137 + d[6] * (T)-6270;
+    const T t10 = t0 + t2, t12 = t0 - t2;
+    const T o0 = d[7] * (T)-1730 + d[5] * (T)11893 + d[3] * (T)-17799 + d[1] * (T)8697;
+    const T o2 = d[7] * (T)-4176 + d[5] * (T)-4926 + d[3] * (T)7373 + d[1] * (T)20995;
+    constexpr T r = (T)1 << (kShift - 1);
+    o[0] = (t10 + o2 + r) >> kShift, o[3] = (t10 - o2 + r) >> kShift;
+    o[1] = (t12 + o0 + r) >> kShift, o[2] = (t12 - o0 + r) >> kShift;
+}
+
+// one line of jpeg_idct_2x2 over d[0 .. 8) (d[2], d[4], d[6] unused) -> 2 outputs
+template <typename T, int kShift>
+__device__ __forceinline__ void red2(const T (&d)[8], T (&o)[2]) {
+    const T t10 = d[0] * (T)32768;
+    const T t0 = d[7] * (T)-5906 + d[5] * (T)6967 + d[3] * (T)-10426 + d[1] * (T)29692;
+    constexpr T r = (T)1 << (kShift - 1);
+    o[0] = (t10 + t0 + r) >> kShift, o[1] = (t10 - t0 + r) >> kShift;
+}
+
+// the inputs an S-point reduced line reads: 4 x 4 skips index 4, 2 x 2 every even index but 0
+template <int S>
+__device__ __forceinline__ constexpr bool red_input(int k) {
+    return k != 4 && !(S == 2 && (k == 2 || k == 6));
+}
+
+// pass 1 of the S-point reduced IDCT (S = 4, 2): the columns of s the second pass reads -> the S rows of ws
+template <int S, typename T>
+__device__ __forceinline__ void red_pass1(const int (&s)[8][8], int (&ws)[S][8]) {
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        if (!red_input<S>(k)) continue;
+        T d[8], o[S];
+#pragma unroll
+        for (int j = 0; j < 8; j++) d[j] = (T)s[j][k];
+        if constexpr (S == 4) red4<T, 12>(d, o);
+        else red2<T, 13>(d, o);
+#pragma unroll
+        for (int j = 0; j < S; j++) ws[j][k] = (int)o[j];
+    }
+}
+
+// pass 2 along the S rows of ws -> S x S samples at dst (row pitch `pitch`)
+template <int S, typename T>
+__device__ __forceinline__ void red_pass2(const int (&ws)[S][8], uint8_t *dst, uint32_t pitch) {
+#pragma unroll
+    for (int r = 0; r < S; r++) {
+        T d[8], o[S];
+#pragma unroll
+        for (int j = 0; j < 8; j++) d[j] = red_input<S>(j) ? (T)ws[r][j] : (T)0;
+        if constexpr (S == 4) {
+            red4<T, 19>(d, o);
+            *reinterpret_cast<uint32_t *>(dst + (uint64_t)r * pitch) =
+                range_limit((int)o[0]) | range_limit((int)o[1]) << 8 | range_limit((int)o[2]) << 16 | range_limit((int)o[3]) << 24;
+        } else {
+            red2<T, 20>(d, o);
+            *reinterpret_cast<uint16_t *>(dst + (uint64_t)r * pitch) = (uint16_t)(range_limit((int)o[0]) | range_limit((int)o[1]) << 8);
+        }
+    }
+}
+
+// one block at the reduced size S (4 or 2): its 64 dequantised coefficients -> S rows of S samples at dst (S-byte aligned); each pass
+// in int32 when the block's inputs to it are inside that pass's bound, else in 64 bits
+template <int S>
+__device__ __forceinline__ void turbo_idct_block_reduced(const int16_t *__restrict__ coef, uint8_t *dst, uint32_t pitch) {
+    constexpr int kB1 = S == 4 ? kRed4Pass1Exact : kRed2Pass1Exact, kB2 = S == 4 ? kRed4Pass2Exact : kRed2Pass2Exact;
+    int s[8][8];
+    const uint4 *src = reinterpret_cast<const uint4 *>(coef);
+    int mx = 0;
+#pragma unroll
+    for (int r = 0; r < 8; r++) {
+        const uint4 q = __ldg(src + r);
+        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            s[r][2 * k] = (int)(int16_t)(w[k] & 0xffffu);
+            s[r][2 * k + 1] = (int)w[k] >> 16;
+            mx = max(mx, max(abs(s[r][2 * k]), abs(s[r][2 * k + 1])));
+        }
+    }
+    int ws[S][8];
+    if (mx <= kB1) red_pass1<S, int>(s, ws);
+    else red_pass1<S, long long>(s, ws);
+    mx = 0;
+#pragma unroll
+    for (int r = 0; r < S; r++)
+#pragma unroll
+        for (int k = 0; k < 8; k++)
+            if (red_input<S>(k)) mx = max(mx, abs(ws[r][k]));
+    if (mx <= kB2) red_pass2<S, int>(ws, dst, pitch);
+    else red_pass2<S, long long>(ws, dst, pitch);
+}
+
 // grid (blocks / 128, frames, components - first): block t of component first + blockIdx.z of frame blockIdx.y -> 8 x 8 bytes of its
-// plane. kRange (ReconPath::Turbo, first = 1): t runs over the chroma blocks [cb_x0, cb_x1) x [cb_y0, cb_y1) only
-template <bool kRange>
-__global__ void __launch_bounds__(kThreadsB)
-turbo_idct_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, uint8_t *__restrict__ planes) {
+// plane. kRange (ReconPath::Turbo, first = 1): t runs over the chroma blocks [cb_x0, cb_x1) x [cb_y0, cb_y1) only. kDraft (drafted
+// groups, turbo_idct_draft_kernel): S x S bytes, S = FrameRecon::idct[c], into a plane of pitch S bw
+template <bool kRange, bool kDraft>
+__device__ __forceinline__ void turbo_idct(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, uint8_t *__restrict__ planes) {
     const FrameRecon &f = frames[blockIdx.y];
     const uint32_t c = (kRange ? 1u : 0u) + blockIdx.z;
     uint32_t t = blockIdx.x * kThreadsB + threadIdx.x;
@@ -118,16 +222,41 @@ turbo_idct_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restri
         t = (f.cb_y0 + t / rw) * bw + f.cb_x0 + t % rw;
     }
     if (t >= bw * bh) return;
-    const uint32_t bx = t % bw, by = t / bw, pitch = 8u * bw;
-    turbo_idct_block(coef + f.coef_base[c] + (uint64_t)t * 64u, planes + f.sample_base[c] + (uint64_t)(8u * by) * pitch + 8u * bx, pitch);
+    const uint32_t bx = t % bw, by = t / bw;
+    const int16_t *src = coef + f.coef_base[c] + (uint64_t)t * 64u;
+    if constexpr (kDraft) {
+        const uint32_t S = f.idct[c], pitch = S * bw;
+        uint8_t *dst = planes + f.sample_base[c] + (uint64_t)(S * by) * pitch + S * bx;
+        if (S == 8) turbo_idct_block(src, dst, pitch);
+        else if (S == 4) turbo_idct_block_reduced<4>(src, dst, pitch);
+        else if (S == 2) turbo_idct_block_reduced<2>(src, dst, pitch);
+        else *dst = (uint8_t)range_limit((src[0] + 4) >> 3);  // jpeg_idct_1x1
+    } else {
+        const uint32_t pitch = 8u * bw;
+        turbo_idct_block(src, planes + f.sample_base[c] + (uint64_t)(8u * by) * pitch + 8u * bx, pitch);
+    }
+}
+
+template <bool kRange>
+__global__ void __launch_bounds__(kThreadsB)
+turbo_idct_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, uint8_t *__restrict__ planes) {
+    turbo_idct<kRange, false>(frames, coef, planes);
+}
+
+template <bool kRange>
+__global__ void __launch_bounds__(kThreadsB)
+turbo_idct_draft_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, uint8_t *__restrict__ planes) {
+    turbo_idct<kRange, true>(frames, coef, planes);
 }
 
 // sample (x, y) of the frame-size image of a component whose plane p (row pitch `pitch`, real size w x h) is upsampled by the
 // integer factors fx x fy: h2v1 / h2v2 fancy for w > 2, h1v2 fancy, every other ratio replicated; the row above the first and
-// below row h - 1 is that row itself
-__device__ __forceinline__ int turbo_upsampled(const uint8_t *__restrict__ p, uint32_t pitch, int fx, int fy, int w, int h, int x, int y) {
+// below row h - 1 is that row itself. fancy = false (a frame drafted at 1/8) replicates every ratio
+__device__ __forceinline__ int turbo_upsampled(const uint8_t *__restrict__ p, uint32_t pitch, int fx, int fy, int w, int h, int x, int y,
+                                               bool fancy = true) {
     auto at = [&](int r, int col) -> int { return __ldg(p + (uint64_t)r * pitch + (uint32_t)col); };
     if (fx == 1 && fy == 1) return at(y, x);
+    if (!fancy) return at(y / fy, x / fx);
     const bool odd_y = (y & 1) != 0, odd_x = (x & 1) != 0;
     if (fx == 1 && fy == 2) {  // h1v2
         const int i = y >> 1;
@@ -163,13 +292,15 @@ constexpr int kTurboTileW = 32, kTurboTileH = kThreadsB / 32;  // luma blocks pe
 // grid (tile columns, tile rows, frames) over the tiles from (tx0, ty0) on, kThreadsB threads. Phase 1: thread (lane, warp) IDCTs
 // luma block (32 tx + lane, 4 ty + warp) into the shared tile when it meets the clip rectangle. Phase 2: the tile's pixels, 128
 // consecutive x per step: luma from the tile, chroma (NC == 3) upsampled by SX x SY from the planes, rule 3, the mode (a
-// launch-uniform OutMode, as for turbo_generic_kernel), the store through the frame's descriptors, read once per thread
-template <int NC, int SX, int SY, int K>
-__global__ void __launch_bounds__(kThreadsB)
-turbo_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, const uint8_t *__restrict__ planes,
-                         int mode, TurboDst<K> out) {
+// launch-uniform OutMode, as for turbo_generic_kernel), the store through the frame's descriptors, read once per thread.
+// S: the luma block's IDCT size, 8 (turbo_reconstruct_kernel) or that of a drafted frame, 4, 2, 1 (turbo_reconstruct_draft_kernel,
+// DESIGN §17): a tile is then 32 S x 4 S output pixels, the chroma planes have pitch FrameRecon::idct[c] bw[c], SX x SY are the
+// ratios after the chroma IDCT, and S == 1 (1/8) replicates
+template <int NC, int S, int SX, int SY, int K>
+__device__ __forceinline__ void turbo_reconstruct(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef,
+                                                  const uint8_t *__restrict__ planes, int mode, TurboDst<K> out) {
     static_assert(kClipKind<K> && (kBaseKind<K> == kStoreStrided || kBaseKind<K> == kStoreStridedF), "described, cropped destinations");
-    constexpr int TW = 8 * kTurboTileW, TH = 8 * kTurboTileH;
+    constexpr int TW = S * kTurboTileW, TH = S * kTurboTileH;
     __shared__ __align__(16) uint8_t tile[TH * TW];
     const FrameRecon &f = frames[blockIdx.z];
     const int X0 = (int)((f.tx0 + blockIdx.x) * TW), Y0 = (int)((f.ty0 + blockIdx.y) * TH);
@@ -177,9 +308,13 @@ turbo_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int16_t *_
     if (X0 >= cx1 || Y0 >= cy1) return;  // (uniform over the CTA) a tile beyond this frame's clip range
     {
         const int lane = (int)threadIdx.x & 31, row = (int)threadIdx.x >> 5;
-        const int bx = X0 / 8 + lane, by = Y0 / 8 + row;
-        if (8 * bx < cx1 && 8 * bx + 8 > cx0 && 8 * by < cy1 && 8 * by + 8 > cy0)
-            turbo_idct_block(coef + f.coef_base[0] + ((uint64_t)by * f.bw[0] + (uint32_t)bx) * 64u, tile + 8 * row * TW + 8 * lane, TW);
+        const int bx = X0 / S + lane, by = Y0 / S + row;
+        if (S * bx < cx1 && S * bx + S > cx0 && S * by < cy1 && S * by + S > cy0) {
+            const int16_t *src = coef + f.coef_base[0] + ((uint64_t)by * f.bw[0] + (uint32_t)bx) * 64u;
+            if constexpr (S == 8) turbo_idct_block(src, tile + 8 * row * TW + 8 * lane, TW);
+            else if constexpr (S == 1) tile[row * TW + lane] = (uint8_t)range_limit((__ldg(src) + 4) >> 3);  // jpeg_idct_1x1
+            else turbo_idct_block_reduced<S>(src, tile + S * row * TW + S * lane, TW);
+        }
     }
     __syncthreads();
     constexpr int kMaxOut = 3;
@@ -206,9 +341,14 @@ turbo_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int16_t *_
         int v[3];
         v[0] = tile[ly * TW + lx];
         v[1] = v[2] = v[0];
-        if constexpr (NC == 3) {
+        if constexpr (NC == 3 && S == 8) {
             v[1] = turbo_upsampled(planes + f.sample_base[1], 8u * f.bw[1], SX, SY, (int)f.cw, (int)f.ch, x, y);
             v[2] = turbo_upsampled(planes + f.sample_base[2], 8u * f.bw[2], SX, SY, (int)f.cw, (int)f.ch, x, y);
+        } else if constexpr (NC == 3) {
+            v[1] = turbo_upsampled(planes + f.sample_base[1], f.idct[1] * f.bw[1], SX, SY, (int)f.cw, (int)f.ch, x, y, S != 1);
+            v[2] = turbo_upsampled(planes + f.sample_base[2], f.idct[2] * f.bw[2], SX, SY, (int)f.cw, (int)f.ch, x, y, S != 1);
+        }
+        if constexpr (NC == 3) {
             if (f.ycbcr) turbo_ycc_rgb(v);
             if (mode == (int)OutMode::Luma) v[0] = (19595 * v[0] + 38470 * v[1] + 7471 * v[2] + 32768) >> 16;
         }
@@ -222,12 +362,27 @@ turbo_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int16_t *_
     }
 }
 
+template <int NC, int SX, int SY, int K>
+__global__ void __launch_bounds__(kThreadsB)
+turbo_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, const uint8_t *__restrict__ planes,
+                         int mode, TurboDst<K> out) {
+    turbo_reconstruct<NC, 8, SX, SY, K>(frames, coef, planes, mode, out);
+}
+
+template <int NC, int S, int SX, int SY, int K>
+__global__ void __launch_bounds__(kThreadsB)
+turbo_reconstruct_draft_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, const uint8_t *__restrict__ planes,
+                               int mode, TurboDst<K> out) {
+    turbo_reconstruct<NC, S, SX, SY, K>(frames, coef, planes, mode, out);
+}
+
 // grid (output columns / 64, tile rows, frames), block 64 x 8: pixel (x, y) of the frame's clip rectangle, x from the frame's first
 // tile column tx0 (tiles of kGenericTileBlocks blocks), y from its first block row ty0. mode (OutMode, uniform over the launch):
-// Coded stores the frame's components, Luma the L formula of three, Replicate one sample to three components
-template <int K>
-__global__ void __launch_bounds__(512)
-turbo_generic_kernel(const FrameRecon *__restrict__ frames, const uint8_t *__restrict__ planes, int mode, TurboDst<K> out) {
+// Coded stores the frame's components, Luma the L formula of three, Replicate one sample to three components. kDraft (drafted
+// frames, turbo_generic_draft_kernel): plane pitch FrameRecon::idct[c] bw[c], csx / csy the ratios after the reduced IDCT,
+// FrameRecon::fancy
+template <int K, bool kDraft>
+__device__ __forceinline__ void turbo_generic(const FrameRecon *__restrict__ frames, const uint8_t *__restrict__ planes, int mode, TurboDst<K> out) {
     static_assert(kClipKind<K> && (kBaseKind<K> == kStoreStrided || kBaseKind<K> == kStoreStridedF), "described, cropped destinations");
     const FrameRecon &f = frames[blockIdx.z];
     const int x = (int)(f.tx0 * (8u * kGenericTileBlocks) + blockIdx.x * 64u + threadIdx.x), y = (int)(8u * (f.ty0 + blockIdx.y) + threadIdx.y);
@@ -239,7 +394,8 @@ turbo_generic_kernel(const FrameRecon *__restrict__ frames, const uint8_t *__res
         if (c >= nc) break;
         const int fx = f.csx[c], fy = f.csy[c];
         const int w = (int)((f.width + fx - 1) / fx), h = (int)((f.height + fy - 1) / fy);
-        v[c] = turbo_upsampled(planes + f.sample_base[c], 8u * f.bw[c], fx, fy, w, h, x, y);
+        if constexpr (kDraft) v[c] = turbo_upsampled(planes + f.sample_base[c], f.idct[c] * f.bw[c], fx, fy, w, h, x, y, f.fancy != 0);
+        else v[c] = turbo_upsampled(planes + f.sample_base[c], 8u * f.bw[c], fx, fy, w, h, x, y);
     }
     if (nc == 3 && f.ycbcr) turbo_ycc_rgb(v);
     uint32_t no = nc;
@@ -255,9 +411,31 @@ turbo_generic_kernel(const FrameRecon *__restrict__ frames, const uint8_t *__res
     }
 }
 
+template <int K>
+__global__ void __launch_bounds__(512)
+turbo_generic_kernel(const FrameRecon *__restrict__ frames, const uint8_t *__restrict__ planes, int mode, TurboDst<K> out) {
+    turbo_generic<K, false>(frames, planes, mode, out);
+}
+
+template <int K>
+__global__ void __launch_bounds__(512)
+turbo_generic_draft_kernel(const FrameRecon *__restrict__ frames, const uint8_t *__restrict__ planes, int mode, TurboDst<K> out) {
+    turbo_generic<K, true>(frames, planes, mode, out);
+}
+
 template <int NC, int SX, int SY, int K>
 static void launch_b(const ReconLaunch &l, dim3 grid, TurboDst<K> out, cudaStream_t s) {
     turbo_reconstruct_kernel<NC, SX, SY, K><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8, (int)l.mode, out);
+}
+
+// a drafted Turbo group: grey, or three components whose chroma ratios after the IDCT are 1 x 1 (4:4:4, 4:2:0), 2 x 1 (4:2:2) or
+// 1 x 2 (4:4:0) (turbo_path)
+template <int S, int K>
+static void launch_b_draft(const ReconLaunch &l, dim3 grid, TurboDst<K> out, cudaStream_t s) {
+    if (l.ncomp == 1) turbo_reconstruct_draft_kernel<1, S, 1, 1, K><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8, (int)l.mode, out);
+    else if (l.subx == 2) turbo_reconstruct_draft_kernel<3, S, 2, 1, K><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8, (int)l.mode, out);
+    else if (l.suby == 2) turbo_reconstruct_draft_kernel<3, S, 1, 2, K><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8, (int)l.mode, out);
+    else turbo_reconstruct_draft_kernel<3, S, 1, 1, K><<<grid, kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8, (int)l.mode, out);
 }
 
 }  // namespace
@@ -275,7 +453,13 @@ int launch_turbo(const ReconLaunch &l, void *stream, int *launches) {
         out = l.planes;
     }
     int n = 0;
-    if (l.path == ReconPath::Turbo) {  // the chroma blocks under the clip tiles (FrameRecon::cb_*), then the tiles
+    if (l.path == ReconPath::Turbo && l.downscale > 1) {  // drafted (DESIGN §17): the luma block is S = 8 / k samples wide
+        if (l.ncomp > 1) turbo_idct_draft_kernel<true><<<dim3(cblocks, l.n_frames, l.ncomp - 1), kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8), n++;
+        const dim3 grid((l.max_bw0 + kTurboTileW - 1) / kTurboTileW, (l.max_bh0 + kTurboTileH - 1) / kTurboTileH, l.n_frames);
+        if (l.downscale == 2) launch_b_draft<4, K>(l, grid, out, s);
+        else if (l.downscale == 4) launch_b_draft<2, K>(l, grid, out, s);
+        else launch_b_draft<1, K>(l, grid, out, s);
+    } else if (l.path == ReconPath::Turbo) {  // the chroma blocks under the clip tiles (FrameRecon::cb_*), then the tiles
         if (l.ncomp > 1) turbo_idct_kernel<true><<<dim3(cblocks, l.n_frames, l.ncomp - 1), kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8), n++;
         const dim3 grid((l.max_bw0 + kTurboTileW - 1) / kTurboTileW, (l.max_bh0 + kTurboTileH - 1) / kTurboTileH, l.n_frames);
         if (l.ncomp == 1) launch_b<1, 1, 1, K>(l, grid, out, s);
@@ -284,9 +468,14 @@ int launch_turbo(const ReconLaunch &l, void *stream, int *launches) {
         else if (l.suby == 2) launch_b<3, 1, 2, K>(l, grid, out, s);
         else launch_b<3, 1, 1, K>(l, grid, out, s);
     } else {
-        turbo_idct_kernel<false><<<dim3(cblocks, l.n_frames, l.ncomp), kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8), n++;
         const dim3 grid((8u * l.max_bw0 + 63u) / 64u, l.max_bh0, l.n_frames);
-        turbo_generic_kernel<K><<<grid, dim3(64, 8), 0, s>>>(l.frames, l.planes8, (int)l.mode, out);
+        if (l.downscale > 1) {  // drafted frames (DESIGN §17)
+            turbo_idct_draft_kernel<false><<<dim3(cblocks, l.n_frames, l.ncomp), kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8), n++;
+            turbo_generic_draft_kernel<K><<<grid, dim3(64, 8), 0, s>>>(l.frames, l.planes8, (int)l.mode, out);
+        } else {
+            turbo_idct_kernel<false><<<dim3(cblocks, l.n_frames, l.ncomp), kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8), n++;
+            turbo_generic_kernel<K><<<grid, dim3(64, 8), 0, s>>>(l.frames, l.planes8, (int)l.mode, out);
+        }
     }
     if (launches) *launches = n + 1;
     return (int)cudaGetLastError();

@@ -104,6 +104,25 @@ def output_size(data, downscale=1, exif_orientation=False):
     return h.value, w.value
 
 
+def draft_scale(data, size):
+    """Pillow's draft scale k (8, 4, 2 or 1) of one codestream for the requested size = (h, w) -- Image.draft(mode, (w, h)) takes
+    (w, h) --, from the codestream's own size before any Exif orientation: the largest k <= min(W // w, H // h), 1 when none fits.
+    BatchDecoder(frames, draft=size) decodes the frame at ceil(W / k) x ceil(H / k); output_size(data, downscale=k,
+    exif_orientation=...) is then the image crop rectangles are given in. Host only, no GPU. Raises ValueError for a size that is
+    not two positive integers, NativeError where parse() does."""
+    import numbers
+    hw = tuple(size) if isinstance(size, (tuple, list)) else None
+    if hw is None or len(hw) != 2 or any(isinstance(v, bool) or not isinstance(v, numbers.Integral) for v in hw) or \
+            any(v < 1 or v > 0xFFFFFFFF for v in hw):
+        raise ValueError("draft size must be two integers (h, w) of 1 .. 2**32 - 1, got %r" % (size,))
+    addr, n, keep = _as_buffer(data)
+    rc = lib.b200jpg_draft_scale(addr, n, int(hw[1]), int(hw[0]))
+    del keep
+    if rc < 0:
+        native.check(rc)
+    return rc
+
+
 def crop_table(crop, n):
     """The b200jpg_rect table of BatchDecoder(crop=...): n entries, each None (the whole frame) or (x, y, width, height) as
     non-negative integers. Raises ValueError; the rectangles themselves are checked against the frames by the batch."""
@@ -123,9 +142,9 @@ def crop_table(crop, n):
     return table
 
 
-def resize_table(resize, n):
-    """The b200jpg_size table of BatchDecoder(resize=...): one (h, w) for every frame, or n entries each None or (h, w), as
-    non-negative integers; (0, 0) leaves a frame unresized. Raises ValueError."""
+def resize_table(resize, n, name="resize"):
+    """The b200jpg_size table of BatchDecoder(resize=...) (or of `name`=..., draft): one (h, w) for every frame, or n entries each
+    None or (h, w), as non-negative integers; (0, 0) leaves a frame unresized (undrafted). Raises ValueError."""
     import numbers
 
     def is_int(v):
@@ -135,18 +154,18 @@ def resize_table(resize, n):
     if len(vals) == 2 and all(is_int(v) for v in vals):
         vals = (vals,) * n
     elif len(vals) != n:
-        raise ValueError("resize: %d sizes for %d frames" % (len(vals), n))
+        raise ValueError("%s: %d sizes for %d frames" % (name, len(vals), n))
     table = (native.SizeStruct * n)()
     for i, r in enumerate(vals):
         if r is None:
             continue
         hw = tuple(r) if isinstance(r, (tuple, list)) else None
         if hw is None or len(hw) != 2 or not all(is_int(v) for v in hw):
-            raise ValueError("resize[%d]: expected None or two integers (h, w), got %r" % (i, r))
+            raise ValueError("%s[%d]: expected None or two integers (h, w), got %r" % (name, i, r))
         if any(v < 0 or v > 0xFFFFFFFF for v in hw):
-            raise ValueError("resize[%d]: h and w must be 0 .. 2**32 - 1, got %r" % (i, hw))
+            raise ValueError("%s[%d]: h and w must be 0 .. 2**32 - 1, got %r" % (name, i, hw))
         if (hw[0] == 0) != (hw[1] == 0):
-            raise ValueError("resize[%d]: exactly one of h and w is zero: %r" % (i, hw))
+            raise ValueError("%s[%d]: exactly one of h and w is zero: %r" % (name, i, hw))
         table[i].height, table[i].width = int(hw[0]), int(hw[1])
     return table
 
@@ -343,7 +362,7 @@ class BatchDecoder:
     """One batch of codestreams: parse + pack on construction, then upload() / decode() on a CUDA stream."""
 
     def __init__(self, frames, device=-1, tolerate_bad=False, ctx=None, color_transform=True, upsample=True, downscale=1,
-                 exif_orientation=False, crop=None, resize=None, resample="bilinear", mode=None, reconstruction="reference"):
+                 exif_orientation=False, crop=None, resize=None, resample="bilinear", mode=None, reconstruction="reference", draft=None):
         """downscale = 2, 4 or 8 decodes every frame at ceil(W / k) x ceil(H / k) (B200JPG_FLAG_DOWNSCALE_k): each 8x8 block is
         inverse transformed straight to (8/k) x (8/k) samples, the k x k box average of its IDCT, and the rest of the
         reconstruction runs on the smaller frame. geometry(), frame_view() and plane_views() give the reduced sizes. Not to be
@@ -390,7 +409,19 @@ class BatchDecoder:
         Orientation, crop, resize and the float map follow unchanged, so Image.open(f).convert("RGB").crop(box).resize(size)
         is what the GPU writes, byte for byte, for intact codestreams. A 12-bit, two- or four-component frame is then
         B200JPG_ERR_NOT_IMPLEMENTED (skipped with tolerate_bad); "libjpeg-turbo" with downscale > 1 or upsample=False raises
-        NativeError (B200JPG_ERR_NOT_IMPLEMENTED); any other value raises ValueError before a device is touched."""
+        NativeError (B200JPG_ERR_NOT_IMPLEMENTED); any other value raises ValueError before a device is touched.
+
+        draft (b200jpg_batch_create_draft, DESIGN §17) is one (h, w) for every frame, or one entry per frame: None, or (h, w) -- the
+        order of `resize`; Pillow's Image.draft(mode, (w, h)) takes (w, h). A frame with a request is decoded as Pillow's draft gives
+        it: at scale 1/k, k = draft_scale(data, (h, w)) of 8, 4, 2 and 1 from the codestream's own size, ceil(W / k) x ceil(H / k),
+        with libjpeg-turbo's reduced IDCTs and its upsampling at that scale. Everything else follows on that image, so for intact
+        codestreams the batch writes, byte for byte, what
+            im = Image.open(f); im.draft(mode, (w, h))
+            ImageOps.exif_transpose(im).convert(mode).crop(box).resize(size, filter)
+        gives; crop rectangles are given in output_size(data, downscale=k, exif_orientation=...). A frame whose k is 1 is decoded
+        exactly as without a draft; status(i) is unchanged. A draft needs reconstruction="libjpeg-turbo" (else NativeError,
+        B200JPG_ERR_NOT_IMPLEMENTED); a wrong length, an entry that is not two non-negative integers or exactly one zero in an
+        entry raises ValueError."""
         if not isinstance(mode, (str, type(None))) or mode not in native.MODE_FLAGS:
             raise ValueError('mode must be None, "RGB" or "L", got %r' % (mode,))
         if not isinstance(reconstruction, str) or reconstruction not in native.RECONSTRUCTION_FLAGS:
@@ -399,6 +430,7 @@ class BatchDecoder:
             raise ValueError("downscale must be 1, 2, 4 or 8, got %r" % (downscale,))
         rects = None if crop is None else crop_table(crop, len(frames))
         sizes = None if resize is None else resize_table(resize, len(frames))
+        drafts = None if draft is None else resize_table(draft, len(frames), "draft")
         filt = resample_filter(resample)
         self.ctx = ctx or Context(device)
         self._keep = []
@@ -424,7 +456,11 @@ class BatchDecoder:
         flags |= native.MODE_FLAGS[mode]
         self.reconstruction = reconstruction
         flags |= native.RECONSTRUCTION_FLAGS[reconstruction]
-        rc = lib.b200jpg_batch_create_resize(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, rects, sizes, filt, ctypes.byref(self.handle))
+        if drafts is None:
+            rc = lib.b200jpg_batch_create_resize(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, rects, sizes, filt, ctypes.byref(self.handle))
+        else:
+            rc = lib.b200jpg_batch_create_draft(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, drafts, rects, sizes, filt,
+                                                ctypes.byref(self.handle))
         native.check(rc, self.ctx.handle)
         self.ctx._batch_opened()
         self._keep = []  # the batch holds its own pinned copy

@@ -83,6 +83,10 @@ def _load():
                                             ctypes.POINTER(RectStruct), ctypes.POINTER(vp)]),
         "b200jpg_batch_create_resize": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.c_uint,
                                               ctypes.POINTER(RectStruct), ctypes.POINTER(SizeStruct), i32, ctypes.POINTER(vp)]),
+        "b200jpg_batch_create_draft": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.c_uint,
+                                             ctypes.POINTER(SizeStruct), ctypes.POINTER(RectStruct), ctypes.POINTER(SizeStruct), i32,
+                                             ctypes.POINTER(vp)]),
+        "b200jpg_draft_scale": (i32, [vp, ctypes.c_size_t, ctypes.c_uint32, ctypes.c_uint32]),
         "b200jpg_resample_coefficients": (i32, [ctypes.c_uint32, ctypes.c_uint32, i32, vp, vp, u64, ctypes.POINTER(ctypes.c_uint32)]),
         "b200jpg_batch_destroy": (None, [vp]),
         "b200jpg_batch_frame_info": (i32, [vp, i32, ctypes.POINTER(FrameInfoStruct)]),
@@ -139,7 +143,7 @@ ABI_SYMBOLS = [
     "b200jpg_device_free", "b200jpg_device_copy_rect", "b200jpg_selftest_restartless", "b200jpg_selftest_restartless_items",
     "b200jpg_selftest_table_cache", "b200jpg_microbench_int32", "b200jpg_exif_orientation", "b200jpg_batch_frame_orientation",
     "b200jpg_batch_create_crop", "b200jpg_output_size", "b200jpg_batch_create_resize", "b200jpg_resample_coefficients",
-    "b200jpg_batch_output_components", "b200jpg_colorspace",
+    "b200jpg_batch_output_components", "b200jpg_colorspace", "b200jpg_batch_create_draft", "b200jpg_draft_scale",
 ]
 
 
