@@ -384,15 +384,20 @@ narrow_list_kernel(const FrameRecon *__restrict__ frames, uint32_t n_frames, con
 constexpr int kThreads420 = 32 * kRows420;
 static_assert(kRows420 % 2 == 0 && kRows420 >= 4 && kRows420 <= 8, "whole chroma block rows, enough warps for phase 1, at most 8 warps");
 
-template <typename T>
+// The luma tile `ys` in front of the window holds a sample per (coefficient, thread): int16 in the int16 instance for the packed
+// and the planar 8-bit stores (Tile420), which then run six CTAs per SM (kWarps420); int32 in the int32 instance (the exact
+// path) and for the other kinds, which stay at five.
+template <typename T, typename Y = int>
 struct Window420 {
     static constexpr int kLines = 4 * kRows420 + 2;
     static constexpr int kLineBytes = 136 * (int)sizeof(T);  // [3 unused][left][128][right][3 unused]
     // + 4 samples: Cr lies two banks off Cb for the int16 stores of phase 1, and 16-byte aligned for the int32 loads
     static constexpr int kCompBytes = kLines * kLineBytes + 4 * (int)sizeof(T);
-    static constexpr int kYsBytes = 64 * kThreads420 * 4;  // the luma tile `ys` in front of the window
+    static constexpr int kYsBytes = 64 * kThreads420 * (int)sizeof(Y);  // the luma tile `ys` in front of the window
     static constexpr int kSmemBytes = kYsBytes + 2 * kCompBytes;
 };
+template <typename T, int K>
+using Tile420 = std::conditional_t<sizeof(T) == 2 && (K == kStoreCanvas || K == kStorePlanar), int16_t, int>;
 
 __device__ __forceinline__ uint32_t lds32(uint32_t a) {
     uint32_t v;
@@ -416,6 +421,12 @@ __device__ __forceinline__ int lds_s16(uint32_t a) {
 }
 __device__ __forceinline__ void sts16(uint32_t a, int v) { asm volatile("st.shared.u16 [%0], %1;" ::"r"(a), "h"((short)v) : "memory"); }
 __device__ __forceinline__ void sts32(uint32_t a, int v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+
+// x, which the compiler cannot see through: what is derived from it is computed where it is used
+__device__ __forceinline__ int opaque(int x) {
+    asm volatile("mov.b32 %0, %0;" : "+r"(x));
+    return x;
+}
 
 // one window sample (T = short / int) at a shared-space byte address
 template <typename T>
@@ -759,17 +770,84 @@ __device__ __forceinline__ void to_rgb(int y, int cbv, int crv, int &r, int &g, 
     }
 }
 
+// ---- the 16-bit tile of reconstruct420_kernel<int16_t> (Tile420) ----------------------------------------------------------
+// Warp w owns the 4 KB from byte 4096 w on, laid out [coefficient][lane]: sample (c, lane) at 2 (32 c + lane). Its 32 blocks of
+// coefficients are exactly those 4 KB, so each block row is reconstructed in place: coefficient row r of the 32 blocks (16-byte
+// piece (block b, row r) at 512 r + 16 (b ^ r)) and, once read, the eight row-pass outputs of every lane (at 512 r + 64 k +
+// 2 lane) take the same 512 bytes. Banks: 512 r is a multiple of 128, so a piece lands in 16-byte bank group (b ^ r) & 7. A
+// 16-byte access is served a quarter warp (eight lanes) at a time: the stores of tile_fetch's piece i * 32 + lane have b = 4 i +
+// lane / 8 fixed and r = lane & 7, the per-lane reads b = lane and r fixed, so the eight lanes hit eight different groups
+// either way; the int16 samples of a warp are 64 contiguous bytes. All conflict-free. (The int32 tile keeps the pieces in its
+// upper half, at the same offsets + 4096: kStash.)
+//
+// Range. The row pass idct8t<16, 5> of int16 coefficients is out_n = (sum_k W[n][k] v_k + 16) >> 5 with sum_k |W[n][k]| = 3825
+// for every n; the negative weights of an output sum to at most 2434 in magnitude (n = 1), the positive ones to 3825 (n = 0). So
+// over v in [-32768, 32767]^8 the outputs lie in [(-(32767 * 3825 + 3825) + 16) >> 5, (32767 * 3825 + 2434 + 16) >> 5] =
+// [-3,916,800, 3,916,757], 120 times the int16 range (tests/test_recon420_tile16_cpu.py): a stored output can wrap. Every
+// output goes through the min / max of its lane before it is stored, and a warp with one outside int16 flags the frame `narrow`
+// (the int32 instance redoes it) -- the min / max the column pass kept for the 32-bit colour range moves here: with the row
+// outputs inside int16 the column pass gives |out| <= (3825 * 32768 + 2048) >> 12 = 30,600, nothing is `wide`.
+// The level shift is left out of the row pass: dcoffset << 3 = 1024 on the DC adds exactly 512 * 1024 = 16384 << 5 to every
+// output of coefficient row 0, and that row's outputs add exactly 512 * 16384 = 2048 << 12 to every column-pass output. So the
+// row pass runs without it and the column pass rounds with 2048 + (2048 << 12) (kRound16): the same sums, bit for bit, with
+// the tile centred on zero -- row 0 of a flat block of 255 is 16256 instead of 32640, and real images stay far inside int16.
+constexpr int kRound16 = 2048 + (2048 << 12);
+
+// the 16-byte pieces of a warp's 32 blocks, eight per lane (piece i * 32 + lane: block 4 i + lane / 8, row lane & 7), into the
+// warp's tile at byte offset kStash (0 for the int16 tile, 4096 for the upper half of the int32 one)
+template <uint32_t kStash>
+__device__ __forceinline__ void tile_stash_at(uint32_t wseg, const uint4 (&pc)[8]) {
+    const uint32_t lane = threadIdx.x & 31, prow = lane & 7u, sub = lane >> 3;
+#pragma unroll
+    for (uint32_t i = 0; i < 8; i++) {
+        const uint32_t blk = 4u * i + sub;
+        const uint32_t dst = wseg + kStash + 512u * prow + 128u * (blk >> 3) + 16u * ((blk & 7u) ^ prow);
+        asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(dst), "r"(pc[i].x), "r"(pc[i].y), "r"(pc[i].z), "r"(pc[i].w) : "memory");
+    }
+    __syncwarp();
+}
+
+// The row pass of the int16 tile yw (the warp's 4 KB) in place, coefficient rows 0 .. kRows - 1, without the level shift
+// (kRound16); mn / mx: the min / max of the outputs (both start at 0)
+template <int kRows>
+__device__ __forceinline__ void tile_rows16(int16_t *yw, int &mn, int &mx) {
+    const uint32_t lane = threadIdx.x & 31;
+    int16_t *my = yw + lane;
+    const uint32_t wseg = (uint32_t)__cvta_generic_to_shared(yw);
+    auto piece = [&](int r) { return lds128(wseg + 512u * (uint32_t)r + 16u * (lane ^ (uint32_t)r)); };
+    mn = 0, mx = 0;
+    uint4 q = piece(0);
+#pragma unroll 1
+    for (int r = 0; r < kRows; r++) {
+        const uint4 qn = piece((r < kRows - 1) ? r + 1 : r);
+        int v[8];
+        unpack_row_raw(q, v);
+        idct8t<16, 5>(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+        mx = __vimax3_s32(__vimax3_s32(mx, v[0], v[1]), __vimax3_s32(v[2], v[3], v[4]), __vimax3_s32(v[5], v[6], v[7]));
+        mn = __vimin3_s32(__vimin3_s32(mn, v[0], v[1]), __vimin3_s32(v[2], v[3], v[4]), __vimin3_s32(v[5], v[6], v[7]));
+        __syncwarp();  // every lane has read piece r before it is overwritten
+#pragma unroll
+        for (int k = 0; k < 8; k++) my[(8 * r + k) * 32] = (int16_t)v[k];
+        q = qn;
+    }
+}
+
 // kWin: the chroma samples come from the window of reconstruct420_kernel at shared-space address `win` instead of the sample
 // planes. chroma_wide: a chroma sample the tile reads may leave the 32-bit colour range.
 // K: the destination kind (StoreKind). KS > 1: the frame is downscaled by KS (B200JPG_FLAG_DOWNSCALE_k) -- the luma of an output
 // block comes from the KS x KS coefficient blocks under it through scaled_idct_block instead of the 8x8 IDCT of one block.
 // NO = 3 with NC = 1 (B200JPG_FLAG_OUTPUT_RGB, described kinds only): the grey row leaves through the descriptors of components 0, 1
 // and 2, each converted with its own component's map.
-template <int NC, int SX, int SY, typename T, bool kWin = false, int K = kStoreCanvas, int KS = 1, int NO = NC>
-__device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, const int16_t *__restrict__ coef, const T *__restrict__ samples,
-                                                 uint32_t win, bool chroma_wide, StoreDst<K> __restrict__ out) {
+// YT = int16_t (reconstruct420_kernel<int16_t>, Canvas and Planar): the luma tile is the warp's 4 KB of the 16-bit tile
+// (tile_rows16), and a row-pass output outside int16 flags the frame in `narrow`.
+template <int NC, int SX, int SY, typename T, bool kWin = false, int K = kStoreCanvas, int KS = 1, int NO = NC, typename YT = int>
+__device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, YT *ys, const int16_t *__restrict__ coef, const T *__restrict__ samples,
+                                                 uint32_t win, bool chroma_wide, StoreDst<K> __restrict__ out, uint32_t *__restrict__ narrow = nullptr) {
     static_assert(!kWin || (NC == 3 && SX == 2 && SY == 2), "the chroma window is 4:2:0 only");
+    constexpr bool k16 = sizeof(YT) == 2;
+    static_assert(!k16 || (kWin && KS == 1 && sizeof(T) == 2 && std::is_same<YT, Tile420<T, K>>::value), "the 16-bit tile is reconstruct420_kernel<int16_t>'s");
     constexpr uint32_t NT = kWin ? kThreads420 : kThreadsB;  // threads per CTA: the stride of the tile [coefficient][thread]
+    constexpr uint32_t TS = k16 ? 32u : NT;                  // the stride of a lane's samples in its tile
     constexpr int KB = kBaseKind<K>;
     constexpr bool kClip = kClipKind<K>;  // a cropped frame: tile (tx0, ty0) + blockIdx, stores inside the clip rectangle only
     constexpr bool kRep = NC == 1 && NO == 3;
@@ -784,10 +862,33 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
     if (kClip && by < (f.clip_y0 >> 3)) return;
     const bool valid = bx < vbw && (!kClip || bx >= (f.clip_x0 >> 3));
     const int X = 8 * (int)bx, Y = 8 * (int)by;
-    int *my = ys + threadIdx.x;
+    YT *my = k16 ? ys + 2048u * warp + lane : ys + threadIdx.x;
 
     int mx = 0, mn = 0;
-    if constexpr (KS > 1) {
+    if constexpr (k16) {
+        // ---- luma coefficients: 4 KB of contiguous HBM for the warp's 32 blocks, eight coalesced 16-byte loads per lane, then
+        // the row pass in place (tile_rows16) and its range check
+        const uint4 *src = reinterpret_cast<const uint4 *>(coef + f.coef_base[0] + ((uint64_t)by * f.bw[0] + bx0) * 64u);
+        const uint32_t sub = lane >> 3;
+        uint4 pc[8];
+#pragma unroll
+        for (uint32_t i = 0; i < 8; i++) pc[i] = (bx0 + 4u * i + sub < f.bw[0]) ? __ldg(src + i * 32u + lane) : make_uint4(0u, 0u, 0u, 0u);
+        YT *yw = ys + 2048u * warp;
+        tile_stash_at<0>((uint32_t)__cvta_generic_to_shared(yw), pc);
+        tile_rows16<8>(yw, mn, mx);
+        if (mx > 32767 || mn < -32768) atomicOr(narrow + f.status_idx, 1u);  // `narrow`: the int32 instance redoes the frame
+        // ---- column pass (:291-334), the level shift in the rounding (kRound16)
+#pragma unroll 1
+        for (int k = 0; k < 8; k++) {
+            int v[8];
+#pragma unroll
+            for (int r = 0; r < 8; r++) v[r] = my[(8 * r + k) * 32];
+            idct8t<kRound16, 12>(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+#pragma unroll
+            for (int r = 0; r < 8; r++) my[(8 * r + k) * 32] = (int16_t)v[r];
+        }
+        mx = mn = 0;  // |luma| <= 30,600 + 2048: never `wide`
+    } else if constexpr (KS > 1) {
         // ---- downscaled: output block (bx, by) holds the (8/KS) x (8/KS) samples of coefficient blocks (KS bx + i, KS by + j)
         constexpr int N = 8 / KS;
 #pragma unroll 1
@@ -896,7 +997,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
             uint8_t *o = (KB == kStoreCanvas) ? obase + (uint64_t)r * opitch : ((KB == kStoreRuns || KB == kStoreRunsF) ? nullptr : plane_at(pl, X, Y + r));
             int px[8];
 #pragma unroll
-            for (int x = 0; x < 8; x++) px[x] = WADD(my[(8 * r + x) * NT], 8) >> 4;
+            for (int x = 0; x < 8; x++) px[x] = WADD(my[(8 * r + x) * TS], 8) >> 4;
             const uint32_t w0 = pack_sat4(px[0], px[1], px[2], px[3]), w1 = pack_sat4(px[4], px[5], px[6], px[7]);
             if constexpr (KB == kStoreRuns || KB == kStoreRunsF) {  // staged in the line's luma slots, which are consumed
                 my[(8 * r) * NT] = (int)w0;
@@ -943,6 +1044,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
     constexpr int OWN = 8 / SX;
     const bool fast = (bx0 + 32 <= vbw) && ((int)((bx0 + 32) * OWN) <= cw);
     const int xl = (cx0 > 0) ? cx0 : 0, xr = (cx0 + NW - 1 < cw) ? cx0 + NW - 1 : cw - 1;
+    const bool lin = cx0 >= 0, rin = cx0 + NW - 1 < cw;  // the window's left / right neighbour columns are not clamped
     // chroma (line 0, column 0) of the shared-memory window (Window420)
     const int wy0 = 4 * (int)(NT / 32) * (int)tile_y - 1, wx0 = 128 * (int)tile_x - 4;
     auto fetch = [&](int y, int (&d1)[NW], int (&d2)[NW]) {
@@ -955,21 +1057,31 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                 for (int c = 0; c < 2; c++) {
                     int (&d)[NW] = c ? d2 : d1;
                     const uint32_t a = line + (uint32_t)c * (uint32_t)Wn::kCompBytes;
+                    const uint32_t own = a + (4u + 4u * lane) * S;  // the lane's own four samples
                     if (S == 2) {
-                        const uint2 o = lds64(a + (4u + 4u * lane) * S);
+                        const uint2 o = lds64(own);
                         d[1] = (int)(short)(o.x & 0xffffu), d[2] = (int)o.x >> 16, d[3] = (int)(short)(o.y & 0xffffu), d[4] = (int)o.y >> 16;
                     } else {
-                        const uint4 o = lds128(a + (4u + 4u * lane) * S);
+                        const uint4 o = lds128(own);
                         d[1] = (int)o.x, d[2] = (int)o.y, d[3] = (int)o.z, d[4] = (int)o.w;
                     }
-                    d[0] = win_load<T>(a + (uint32_t)(xl - wx0) * S);
-                    d[NW - 1] = win_load<T>(a + (uint32_t)(xr - wx0) * S);
+                    if constexpr (k16) {
+                        // the neighbours are the samples either side of the own four (the halo columns for lanes 0 / 31), unless
+                        // the frame edge clamps them onto d[1] / d[4]: immediate offsets, no per-lane columns held in registers
+                        d[0] = lin ? win_load<T>(own - S) : d[1];
+                        d[NW - 1] = rin ? win_load<T>(own + 4u * S) : d[4];
+                    } else {
+                        d[0] = win_load<T>(a + (uint32_t)(xl - wx0) * S);
+                        d[NW - 1] = win_load<T>(a + (uint32_t)(xr - wx0) * S);
+                    }
                 }
             } else if (valid) {
-                // at the frame edge: the clamped addressing below, always inside the window
+                // at the frame edge: the clamped addressing below, always inside the window. 16-bit tile: `opaque` keeps the
+                // compiler from hoisting the six columns out of the line loop, where they held registers (and spilled at 80)
+                const int c0 = k16 ? opaque(cx0) : cx0;
 #pragma unroll
                 for (int j = 0; j < NW; j++) {
-                    const uint32_t a = line + (uint32_t)(clampi(cx0 + j, 0, cw - 1) - wx0) * S;
+                    const uint32_t a = line + (uint32_t)(clampi(c0 + j, 0, cw - 1) - wx0) * S;
                     d1[j] = win_load<T>(a);
                     d2[j] = win_load<T>(a + (uint32_t)Wn::kCompBytes);
                 }
@@ -1034,7 +1146,7 @@ __device__ __forceinline__ void reconstruct_tile(const FrameRecon &f, int *ys, c
                 }
 #pragma unroll
                 for (int x = 0; x < 8; x++) {
-                    const int yv = my[(8 * r + x) * NT];
+                    const int yv = my[(8 * r + x) * TS];
                     int R, G, B;
                     to_rgb<MODE>(yv, c1[x], c2[x], R, G, B);
                     px[3 * x] = R;
@@ -1166,10 +1278,10 @@ reconstruct_rgb_kernel(const FrameRecon *__restrict__ frames, const int16_t *__r
 // redoes it; there a window sample beyond +-kWide selects the 64-bit colour mode for the CTA.
 
 // The warp's 32 blocks of coefficients come in as 4 KB of 16-byte pieces, eight per lane (piece i * 32 + lane): a chroma row is
-// two runs of 2 KB (Cb blocks 0..15, Cr blocks 16..31). tile_stash parks the pieces in the upper half of the warp's tile (piece
-// (block, row) at row segment 32 + 4 row + block / 8, slot (block % 8) ^ row: conflict-free both ways), tile_idct hands every
-// lane its own block and runs the row pass and the column pass (dct/idct.cpp:237-334) as two compact loops over the tile
-// [sample][lane].
+// two runs of 2 KB (Cb blocks 0..15, Cr blocks 16..31). tile_stash parks the pieces in the warp's tile -- the upper half of an
+// int32 tile (piece (block, row) at row segment 32 + 4 row + block / 8, slot (block % 8) ^ row: conflict-free both ways), all of
+// an int16 one (tile_stash_at) --, tile_idct hands every lane its own block and runs the row pass and the column pass
+// (dct/idct.cpp:237-334) as two compact loops over the tile [sample][lane].
 template <typename Have>
 __device__ __forceinline__ void tile_fetch(uint4 (&pc)[8], const uint4 *__restrict__ src_a, const uint4 *__restrict__ src_b, Have have) {
     const uint32_t lane = threadIdx.x & 31, sub = lane >> 3;
@@ -1180,60 +1292,66 @@ __device__ __forceinline__ void tile_fetch(uint4 (&pc)[8], const uint4 *__restri
     }
 }
 
-__device__ __forceinline__ void tile_stash(int *ys, const uint4 (&pc)[8]) {
-    const uint32_t lane = threadIdx.x & 31, prow = lane & 7u, sub = lane >> 3;
-    const uint32_t wseg = (uint32_t)__cvta_generic_to_shared(ys);
-#pragma unroll
-    for (uint32_t i = 0; i < 8; i++) {
-        const uint32_t blk = 4u * i + sub;
-        const uint32_t dst = wseg + 128u * (32u + 4u * prow + (blk >> 3)) + 16u * ((blk & 7u) ^ prow);
-        asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(dst), "r"(pc[i].x), "r"(pc[i].y), "r"(pc[i].z), "r"(pc[i].w) : "memory");
-    }
-    __syncwarp();
+// the byte offset of the pieces in a warp's tile of Y
+template <typename Y>
+constexpr uint32_t kStash = sizeof(Y) == 2 ? 0u : 4096u;
+
+template <typename Y>
+__device__ __forceinline__ void tile_stash(Y *ys, const uint4 (&pc)[8]) {
+    tile_stash_at<kStash<Y>>((uint32_t)__cvta_generic_to_shared(ys), pc);
 }
 
 // `sink(k, r, a, b)` receives the samples (row r, columns k and k + 1) of this lane's block, k even; only = -1: all 64 samples,
 // only = 0 / 7: row 0 / 7 alone. kRows: coefficient rows 0 .. kRows - 1 may be non-zero, the others are zero in every block of
 // the warp: their row pass would only yield zeros, so it is skipped and the column pass sees literal zeros (the same integer
-// arithmetic, folded by the compiler). Returns the min / max of what was sunk in mn / mx (both start at 0).
-template <int kRows, typename Sink>
-__device__ __forceinline__ void tile_idct_rows(int *ys, int only, int &mn, int &mx, Sink sink) {
+// arithmetic, folded by the compiler). Returns in mn / mx (both start at 0) the min / max of what was sunk (int32 tile) or of
+// the row-pass outputs (int16 tile: outside int16 they have wrapped; inside, the samples fit int16, see tile_rows16).
+template <int kRows, typename Y, typename Sink>
+__device__ __forceinline__ void tile_idct_rows(Y *ys, int only, int &mn, int &mx, Sink sink) {
+    constexpr bool k16 = sizeof(Y) == 2;
+    constexpr int kRound = k16 ? kRound16 : 2048;  // the int16 tile's row pass leaves the level shift to the column pass
     const uint32_t lane = threadIdx.x & 31;
-    int *my = ys + lane;
-    const uint32_t wseg = (uint32_t)__cvta_generic_to_shared(ys);
-    const uint32_t mine = wseg + 128u * (32u + (lane >> 3));
-    auto piece = [&](int r) { return lds128(mine + 512u * (uint32_t)r + 16u * ((lane & 7u) ^ (uint32_t)r)); };
-    uint4 q = piece(0);
+    Y *my = ys + lane;
+    if constexpr (k16) {
+        tile_rows16<kRows>(ys, mn, mx);
+    } else {
+        const uint32_t wseg = (uint32_t)__cvta_generic_to_shared(ys);
+        const uint32_t mine = wseg + 128u * (32u + (lane >> 3));
+        auto piece = [&](int r) { return lds128(mine + 512u * (uint32_t)r + 16u * ((lane & 7u) ^ (uint32_t)r)); };
+        uint4 q = piece(0);
 #pragma unroll 1
-    for (int r = 0; r < kRows; r++) {
-        const uint4 qn = piece((r < kRows - 1) ? r + 1 : r);
-        int v[8];
-        unpack_row_raw(q, v);
-        if (r == 0) v[0] = WADD(v[0], 128 << 3);  // dcoffset << 3 (idct.cpp:233,244), the << 4 preshift left out like in the inputs
-        idct8t<16, 5>(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
-        __syncwarp();
+        for (int r = 0; r < kRows; r++) {
+            const uint4 qn = piece((r < kRows - 1) ? r + 1 : r);
+            int v[8];
+            unpack_row_raw(q, v);
+            if (r == 0) v[0] = WADD(v[0], 128 << 3);  // dcoffset << 3 (idct.cpp:233,244), the << 4 preshift left out like in the inputs
+            idct8t<16, 5>(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+            __syncwarp();
 #pragma unroll
-        for (int k = 0; k < 8; k++) my[(8 * r + k) * 32] = v[k];
-        q = qn;
+            for (int k = 0; k < 8; k++) my[(8 * r + k) * 32] = v[k];
+            q = qn;
+        }
+        mx = 0, mn = 0;
     }
-    mx = 0, mn = 0;
 #pragma unroll 1
     for (int k = 0; k < 8; k += 2) {
         int a[8], b[8];
 #pragma unroll
         for (int r = 0; r < 8; r++) {
-            a[r] = (r < kRows) ? my[(8 * r + k) * 32] : 0;
-            b[r] = (r < kRows) ? my[(8 * r + k + 1) * 32] : 0;
+            a[r] = (r < kRows) ? (int)my[(8 * r + k) * 32] : 0;
+            b[r] = (r < kRows) ? (int)my[(8 * r + k + 1) * 32] : 0;
         }
         if (only < 0) {
-            idct8t<2048, 12>(a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7]);
-            idct8t<2048, 12>(b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7]);
+            idct8t<kRound, 12>(a[0], a[1], a[2], a[3], a[4], a[5], a[6], a[7]);
+            idct8t<kRound, 12>(b[0], b[1], b[2], b[3], b[4], b[5], b[6], b[7]);
 #pragma unroll
             for (int r = 0; r < 8; r++) sink(k, r, a[r], b[r]);
+            if constexpr (!k16) {
 #pragma unroll
-            for (int r = 0; r < 8; r += 2) {
-                mx = __vimax3_s32(__vimax3_s32(mx, a[r], a[r + 1]), b[r], b[r + 1]);
-                mn = __vimin3_s32(__vimin3_s32(mn, a[r], a[r + 1]), b[r], b[r + 1]);
+                for (int r = 0; r < 8; r += 2) {
+                    mx = __vimax3_s32(__vimax3_s32(mx, a[r], a[r + 1]), b[r], b[r + 1]);
+                    mn = __vimin3_s32(__vimin3_s32(mn, a[r], a[r + 1]), b[r], b[r + 1]);
+                }
             }
         } else {
             // output 0 / 7 of the column pass is one dot product: the butterfly of idct8t is linear in front of its rounding shift
@@ -1241,22 +1359,24 @@ __device__ __forceinline__ void tile_idct_rows(int *ys, int only, int &mn, int &
             auto one = [&](const int (&v)[8]) {
                 const int even = WADD(WADD(WMUL(v[0], 512), WMUL(v[2], 669)), WADD(WMUL(v[4], 512), WMUL(v[6], 277)));
                 const int odd = WADD(WADD(WMUL(v[1], 710), WMUL(v[3], 602)), WADD(WMUL(v[5], 402), WMUL(v[7], 141)));
-                return WADD(only == 0 ? WADD(even, odd) : WSUB(even, odd), 2048) >> 12;
+                return WADD(only == 0 ? WADD(even, odd) : WSUB(even, odd), kRound) >> 12;
             };
             const int sa = one(a), sb = one(b);
             sink(k, only, sa, sb);
-            mx = __vimax3_s32(mx, sa, sb);
-            mn = __vimin3_s32(mn, sa, sb);
+            if constexpr (!k16) {
+                mx = __vimax3_s32(mx, sa, sb);
+                mn = __vimin3_s32(mn, sa, sb);
+            }
         }
     }
 }
 
 // Chroma blocks of ordinary images rarely carry anything in coefficient rows 6 and 7 (4:2:0 q75 frames of the benchmark: in
 // about 98 % of the warps none of the 32 blocks does), so the warp checks once and takes the shorter instance when it can.
-template <typename Sink>
-__device__ __forceinline__ void tile_idct(int *ys, int only, int &mn, int &mx, Sink sink) {
+template <typename Y, typename Sink>
+__device__ __forceinline__ void tile_idct(Y *ys, int only, int &mn, int &mx, Sink sink) {
     const uint32_t lane = threadIdx.x & 31;
-    const uint32_t mine = (uint32_t)__cvta_generic_to_shared(ys) + 128u * (32u + (lane >> 3));
+    const uint32_t mine = (uint32_t)__cvta_generic_to_shared(ys) + kStash<Y> + 128u * (lane >> 3);
     const uint4 p6 = lds128(mine + 512u * 6u + 16u * ((lane & 7u) ^ 6u)), p7 = lds128(mine + 512u * 7u + 16u * ((lane & 7u) ^ 7u));
     const bool high = ((p6.x | p6.y | p6.z | p6.w) | (p7.x | p7.y | p7.z | p7.w)) != 0u;
     if (__any_sync(0xffffffffu, high)) tile_idct_rows<8>(ys, only, mn, mx, sink);
@@ -1264,9 +1384,10 @@ __device__ __forceinline__ void tile_idct(int *ys, int only, int &mn, int &mx, S
 }
 
 template <typename T, int K>
-__device__ __forceinline__ void reconstruct420_tile(const FrameRecon &f, int *ys, uint32_t win, const int16_t *__restrict__ coef,
+__device__ __forceinline__ void reconstruct420_tile(const FrameRecon &f, Tile420<T, K> *ys, uint32_t win, const int16_t *__restrict__ coef,
                                                     uint32_t *__restrict__ narrow_flags, StoreDst<K> __restrict__ out) {
     using Wn = Window420<T>;
+    using Y = Tile420<T, K>;
     constexpr int kHalf = kRows420 / 2;  // chroma block rows under the tile
     constexpr bool kClip = kClipKind<K>;  // a cropped frame: tile (tx0, ty0) + blockIdx, past the clip rectangle nothing
     const uint32_t vbw = ((kClip ? f.clip_x1 : f.width) + 7) >> 3, vbh = ((kClip ? f.clip_y1 : f.height) + 7) >> 3;
@@ -1285,7 +1406,7 @@ __device__ __forceinline__ void reconstruct420_tile(const FrameRecon &f, int *ys
         const int q = (warp < (uint32_t)kHalf) ? (int)warp : (warp == (uint32_t)kHalf ? -1 : kHalf);
         const int cby = cby0 + q;
         if (cby >= 0 && cby < bhc) {
-            int *yw = ys + warp * 2048u;  // this warp's 8 KB of the luma tile, free until phase 2
+            Y *yw = ys + warp * 2048u;  // this warp's 8 KB (int16 tile: 4 KB) of the luma tile, free until phase 2
             uint4 pc[8];
             const uint4 *src_a = reinterpret_cast<const uint4 *>(coef + f.coef_base[1] + ((uint64_t)cby * (uint32_t)bwc + (uint32_t)cbx0) * 64u);
             const uint4 *src_b = reinterpret_cast<const uint4 *>(coef + f.coef_base[2] + ((uint64_t)cby * (uint32_t)bwc + (uint32_t)cbx0) * 64u);
@@ -1328,23 +1449,36 @@ __device__ __forceinline__ void reconstruct420_tile(const FrameRecon &f, int *ys
             }
         }
     }
+    // int16: a window sample (int32 tile) or a row-pass output of phase 1a (int16 tile) or a sample of phase 1b outside int16
     const bool out_of_range = (sizeof(T) == 2) ? (mx > 32767 || mn < -32768) : (mx > kWide || mn < -kWide);
     const bool flagged = __syncthreads_or(out_of_range) != 0;
     if (sizeof(T) == 2 && flagged && threadIdx.x == 0) atomicOr(narrow_flags + f.status_idx, 1u);  // `narrow`: the int32 instance redoes the frame
 
     // ---- phase 2: the luma rows
-    reconstruct_tile<3, 2, 2, T, true, K>(f, ys, coef, nullptr, win, sizeof(T) == 4 && flagged, out);
+    reconstruct_tile<3, 2, 2, T, true, K, 1, 3, Y>(f, ys, coef, nullptr, win, sizeof(T) == 4 && flagged, out, narrow_flags);
 }
 
-// grid (luma block columns / 32, luma block rows / kRows420, frames or kWideSlots); dynamic shared memory Window420<T>::kSmemBytes.
-// At kRows420 = 4 five CTAs (20 warps) per SM, like b2; the int32 instance (rare frames) three, which keeps it free of spills.
+// Resident warps per SM that reconstruct420_kernel<T, ..., K> is compiled for (__launch_bounds__). The CTA is latency-bound:
+// 16 warps instead of 20 made it 21 % slower (DESIGN §4). With the 16-bit tile (Canvas, Planar) six CTAs = 24 warps fit, at 80
+// registers without spills; the other int16 kinds stay at five (20 warps, 96 registers): the float kinds spill at 80, and the
+// strided store, one byte per instruction, was 16 % slower at six CTAs (DESIGN §9). The int32 instance (rare frames) keeps 12,
+// which keeps it free of spills. (-DB200JPG_R420_WARPS16=20: the 16-bit tile at five CTAs, for comparisons.)
+#ifndef B200JPG_R420_WARPS16
+#define B200JPG_R420_WARPS16 24
+#endif
+template <typename T, int K>
+constexpr int kWarps420 = sizeof(T) == 4 ? 12 : (sizeof(Tile420<T, K>) == 2 ? B200JPG_R420_WARPS16 : 20);
+
+// grid (luma block columns / 32, luma block rows / kRows420, frames or kWideSlots); dynamic shared memory
+// Window420<T, Tile420<T, K>>::kSmemBytes
 template <typename T, bool kListed, int K>
-__global__ void __launch_bounds__(kThreads420, ((sizeof(T) == 2) ? 20 : 12) / kRows420)
+__global__ void __launch_bounds__(kThreads420, kWarps420<T, K> / kRows420)
 reconstruct420_kernel(const FrameRecon *__restrict__ frames, const int16_t *__restrict__ coef, uint32_t *__restrict__ narrow_flags,
                       const uint32_t *__restrict__ list, StoreDst<K> __restrict__ out) {
+    using Y = Tile420<T, K>;
     extern __shared__ __align__(16) uint8_t smem420[];
-    int *ys = reinterpret_cast<int *>(smem420);  // phase 2: [coefficient][thread]; phase 1: 8 KB per warp
-    const uint32_t win = (uint32_t)__cvta_generic_to_shared(smem420) + (uint32_t)Window420<T>::kYsBytes;
+    Y *ys = reinterpret_cast<Y *>(smem420);  // phase 2: the luma tile; phase 1: 8 KB (int16 tile: 4 KB) per warp
+    const uint32_t win = (uint32_t)__cvta_generic_to_shared(smem420) + (uint32_t)Window420<T, Y>::kYsBytes;
     if (!kListed) {
         reconstruct420_tile<T, K>(frames[blockIdx.z], ys, win, coef, narrow_flags, out);
     } else {
@@ -1783,7 +1917,7 @@ static void launch_b2(const ReconLaunch &l, dim3 grid, const T *samples, cudaStr
 template <int K>
 static int launch_recon420(const ReconLaunch &l, cudaStream_t s, int *launches) {
     const uint32_t gx = (l.max_bw0 + 31) / 32, gy = (l.max_bh0 + kRows420 - 1) / kRows420;
-    constexpr int smem16 = Window420<int16_t>::kSmemBytes, smem32 = Window420<int32_t>::kSmemBytes;
+    constexpr int smem16 = Window420<int16_t, Tile420<int16_t, K>>::kSmemBytes, smem32 = Window420<int32_t>::kSmemBytes;
     cudaError_t e = cudaFuncSetAttribute(reconstruct420_kernel<int16_t, false, K>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     if (e == cudaSuccess && smem16 > 48 * 1024) e = cudaFuncSetAttribute(reconstruct420_kernel<int16_t, false, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem16);
     if (e == cudaSuccess && smem32 > 48 * 1024) e = cudaFuncSetAttribute(reconstruct420_kernel<int32_t, true, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem32);
