@@ -198,10 +198,14 @@ B200JPG_API int b200jpg_batch_create(b200jpg_ctx *ctx, const uint8_t *const *fra
  *      rule 2 (Pillow's draft("L")), of an RGB-coded frame the L formula.
  *   5. A JPEG XT frame is its base codestream alone, as libjpeg-turbo decodes it. A JPEG XT frame whose profile the parser refuses
  *      (b200jpg_parse: B200JPG_ERR_NOT_IMPLEMENTED) keeps that status under the flag too: its base codestream is not decoded.
+ *   6. With B200JPG_FLAG_OUTPUT_RGB or _L, a CMYK or YCCK frame (b200jpg_colorspace; DESIGN §18): its four components by rules 1
+ *      and 2, then the conversion of B200JPG_FLAG_OUTPUT_RGB / _L for such frames (Pillow's convert("RGB") / convert("L") of the
+ *      "CMYK" image it opens).
  * Everything after the reconstruction is unchanged (orientation, crop, resize, float map), as are extents, out_bytes and statuses.
  * The flag together with B200JPG_FLAG_DOWNSCALE_k or B200JPG_FLAG_NO_UPSAMPLE is B200JPG_ERR_NOT_IMPLEMENTED for the call; a 12-bit
- * frame, a two- or a four-component frame has the status B200JPG_ERR_NOT_IMPLEMENTED (it fails the call, or with tolerate_bad it
- * is skipped). Accepted wherever request flags are. Without the flag a batch is planned exactly as before. libjpeg-turbo's reduced
+ * frame, a two-component frame and a four-component frame without an output mode have the status B200JPG_ERR_NOT_IMPLEMENTED (it
+ * fails the call, or with tolerate_bad it is skipped), as under a mode does a frame whose colorspace is
+ * B200JPG_COLORSPACE_UNKNOWN. Accepted wherever request flags are. Without the flag a batch is planned exactly as before. libjpeg-turbo's reduced
  * decode at 1/2, 1/4 and 1/8 (Pillow's draft) is a per-frame request of b200jpg_batch_create_draft. */
 #define B200JPG_FLAG_LIBJPEG_TURBO 0x80u
 B200JPG_API int b200jpg_batch_create_ex(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
@@ -274,6 +278,7 @@ B200JPG_API int b200jpg_batch_create_resize(b200jpg_ctx *ctx, const uint8_t *con
  *   2. Component c is upsampled by fx = hmax m / (h_c s_c), fy = vmax m / (v_c s_c) from its real size ceil(W' / fx) x ceil(H' / fy)
  *      of the reduced frame W' x H': by rule 2 for k = 2 and 4, replicated for k = 8 (libjpeg-turbo turns fancy upsampling off at
  *      1/8).
+ * Both apply to all four components of a CMYK or YCCK frame under an output mode (rule 6), hmax and vmax over all four.
  * A frame whose k is 1 is decoded, planned and written exactly as without a draft. drafts == NULL, or every entry {0, 0}: exactly
  * b200jpg_batch_create_resize. Otherwise, for the call, tolerate_bad or not: an entry with exactly one zero field is
  * B200JPG_ERR_INVALID_PARAMETER (the message names the frame); a draft without B200JPG_FLAG_LIBJPEG_TURBO is

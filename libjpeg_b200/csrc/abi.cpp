@@ -680,10 +680,12 @@ static void attach_residuals(b200jpg_batch &b, Codestreams &cs, bool device_inde
             cs.err[i] = "an output mode takes grey, YCbCr, RGB, and 8-bit Adobe CMYK or YCCK frames";
             continue;
         }
+        // (a four-component frame that reaches this under a mode is 8-bit Adobe CMYK or YCCK: the check above refused the rest)
+        const int nc = b.frames[i].info.ncomp;
         if (b.parse_status[i] == 0 && (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) &&
-            (b.frames[i].info.precision != 8 || (b.frames[i].info.ncomp != 1 && b.frames[i].info.ncomp != 3))) {
+            (b.frames[i].info.precision != 8 || (nc != 1 && nc != 3 && !(nc == 4 && (b.flags & kOutputModes))))) {
             b.parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;
-            cs.err[i] = "B200JPG_FLAG_LIBJPEG_TURBO takes 8-bit frames of one or three components";
+            cs.err[i] = "B200JPG_FLAG_LIBJPEG_TURBO takes 8-bit frames of one or three components, and Adobe CMYK or YCCK frames under an output mode";
             continue;
         }
         // libjpeg-turbo decodes the base codestream of a JPEG XT frame alone: no residual frame
@@ -808,14 +810,15 @@ static std::vector<uint64_t> lay_out_codestreams(b200jpg_batch &b, const std::ve
 // upsampling and both codestreams of a JPEG XT frame go through the generic kernels. Downscaled frames: 8-bit 4:2:0 frames with
 // upsampling take reconstruct420_scaled_kernel, every other one the scaled IDCT into int32 planes and then the generic kernels (a
 // JPEG XT frame never gets here downscaled: attach_residuals refuses it).
-// B200JPG_FLAG_LIBJPEG_TURBO (8-bit grey and three-component frames: attach_residuals): the tiled turbo_reconstruct_kernel covers
-// component 0 at full resolution, alone or with two chroma components of equal factors 1 or 2 whose fancy upsampling has both
-// neighbours (more than 2 chroma samples per row when halved horizontally); everything else the generic turbo kernel. ncomp: the
+// B200JPG_FLAG_LIBJPEG_TURBO (8-bit grey and three-component frames, and CMYK / YCCK frames under a mode: attach_residuals): the
+// tiled turbo_reconstruct_kernel covers component 0 at full resolution, alone or with two chroma components of equal factors 1 or
+// 2 whose fancy upsampling has both neighbours (more than 2 chroma samples per row when halved horizontally); everything else,
+// four-component frames always (DESIGN §18), the generic turbo kernel. ncomp: the
 // components reconstructed (1 for mode "L" of a YCbCr frame). A frame drafted to 1/k (k > 1, DESIGN §17) is judged on the ratios
 // after its IDCTs (draft_ratio) and its reduced width: its luma block is then 8 / k wide, and its chroma ratios 1 x 1 (4:4:4,
 // 4:2:0), 2 x 1 (4:2:2) or 1 x 2 (4:4:0); 2 x 2 never occurs at k > 1 and is left to the generic kernel
 static ReconPath turbo_path(const b200jpg_frame_info &fi, int ncomp, uint32_t k) {
-    if (fi.subx[0] != 1 || fi.suby[0] != 1) return ReconPath::TurboGeneric;
+    if (ncomp == 4 || fi.subx[0] != 1 || fi.suby[0] != 1) return ReconPath::TurboGeneric;  // (the tiled kernel has no fourth component)
     if (ncomp == 1) return ReconPath::Turbo;
     const Ratio r = draft_ratio(fi, 1, k), r2 = draft_ratio(fi, 2, k);
     if (r.x != r2.x || r.y != r2.y || r.x > 2 || r.y > 2) return ReconPath::TurboGeneric;
@@ -877,10 +880,11 @@ static FramePlan frame_plan(const b200jpg_batch &b, int i) {
         p.mode = OutMode::Replicate;
     }
     if ((b.flags & kOutputModes) && fi.ncomp == 4) {  // CMYK / YCCK (attach_residuals refused the rest): all four reconstructed,
-        const bool rgb = (b.flags & B200JPG_FLAG_OUTPUT_RGB) != 0;  // Pillow's conversion in the generic kernels (DESIGN §15)
+        const bool rgb = (b.flags & B200JPG_FLAG_OUTPUT_RGB) != 0;  // Pillow's conversion in the generic kernels (DESIGN §15, §18)
         p.out_ncomp = rgb ? 3 : 1;
         p.mode = rgb ? OutMode::CmykRgb : OutMode::CmykLuma;
-        p.path = b.scale[i] > 1 ? ReconPath::Scaled : ReconPath::Generic;
+        if (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) p.path = ReconPath::TurboGeneric;
+        else p.path = b.scale[i] > 1 ? ReconPath::Scaled : ReconPath::Generic;
     }
     return p;
 }

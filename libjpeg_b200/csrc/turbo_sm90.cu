@@ -12,12 +12,15 @@
 //                              leaves the IDCT as FrameRecon::idct[c]^2 samples (islow, jpeg_idct_4x4, jpeg_idct_2x2 or
 //                              jpeg_idct_1x1), the Turbo tile holds luma blocks of S = 8 / k, and the planes are upsampled by the
 //                              ratios after the IDCT
+//   turbo_cmyk_*kernel         turbo_generic_kernel and its draft form for the 8-bit Adobe CMYK / YCCK frames of an output mode
+//                              (DESIGN §18): four components read, Pillow's conversion (cmyk_sm90.cuh), three or one stored
 // Every frame of a flagged batch is cropped (abi.cpp: crop_whole_frames), so both kinds store through described destinations with
 // the clip.
 #include <cuda_runtime.h>
 
 #include <type_traits>
 
+#include "cmyk_sm90.cuh"
 #include "internal.hpp"
 #include "store_sm90.cuh"
 
@@ -380,27 +383,37 @@ turbo_reconstruct_draft_kernel(const FrameRecon *__restrict__ frames, const int1
 // tile column tx0 (tiles of kGenericTileBlocks blocks), y from its first block row ty0. mode (OutMode, uniform over the launch):
 // Coded stores the frame's components, Luma the L formula of three, Replicate one sample to three components. kDraft (drafted
 // frames, turbo_generic_draft_kernel): plane pitch FrameRecon::idct[c] bw[c], csx / csy the ratios after the reduced IDCT,
-// FrameRecon::fancy
-template <int K, bool kDraft>
+// FrameRecon::fancy. CMYK (turbo_cmyk_kernel, turbo_cmyk_draft_kernel: an 8-bit Adobe CMYK or YCCK frame, DESIGN §18): MODE is
+// OutMode::CmykRgb or CmykLuma, fixed at compile time like the component count 4 (a run-time count puts v in local memory); the
+// four samples go through cmyk_to_rgb (FrameRecon::ycck), and three components or L leave
+template <int K, bool kDraft, int MODE = (int)OutMode::Coded>
 __device__ __forceinline__ void turbo_generic(const FrameRecon *__restrict__ frames, const uint8_t *__restrict__ planes, int mode, TurboDst<K> out) {
     static_assert(kClipKind<K> && (kBaseKind<K> == kStoreStrided || kBaseKind<K> == kStoreStridedF), "described, cropped destinations");
+    constexpr bool kCmyk = MODE == (int)OutMode::CmykRgb || MODE == (int)OutMode::CmykLuma;
+    constexpr uint32_t kIn = kCmyk ? 4u : 3u;
     const FrameRecon &f = frames[blockIdx.z];
     const int x = (int)(f.tx0 * (8u * kGenericTileBlocks) + blockIdx.x * 64u + threadIdx.x), y = (int)(8u * (f.ty0 + blockIdx.y) + threadIdx.y);
     if (x < (int)f.clip_x0 || x >= (int)f.clip_x1 || y < (int)f.clip_y0 || y >= (int)f.clip_y1) return;
-    const uint32_t nc = f.ncomp;
-    int v[3] = {0, 0, 0};
+    const uint32_t nc = kCmyk ? 4u : f.ncomp;
+    int v[kIn] = {};
 #pragma unroll
-    for (uint32_t c = 0; c < 3; c++) {
+    for (uint32_t c = 0; c < kIn; c++) {
         if (c >= nc) break;
         const int fx = f.csx[c], fy = f.csy[c];
         const int w = (int)((f.width + fx - 1) / fx), h = (int)((f.height + fy - 1) / fy);
         if constexpr (kDraft) v[c] = turbo_upsampled(planes + f.sample_base[c], f.idct[c] * f.bw[c], fx, fy, w, h, x, y, f.fancy != 0);
         else v[c] = turbo_upsampled(planes + f.sample_base[c], 8u * f.bw[c], fx, fy, w, h, x, y);
     }
-    if (nc == 3 && f.ycbcr) turbo_ycc_rgb(v);
     uint32_t no = nc;
-    if (mode == (int)OutMode::Luma) v[0] = (19595 * v[0] + 38470 * v[1] + 7471 * v[2] + 32768) >> 16, no = 1;
-    if (mode == (int)OutMode::Replicate) v[1] = v[2] = v[0], no = 3;
+    if constexpr (kCmyk) {
+        cmyk_to_rgb(v, f.ycck != 0);
+        no = 3;
+        if (MODE == (int)OutMode::CmykLuma) v[0] = (19595 * v[0] + 38470 * v[1] + 7471 * v[2] + 32768) >> 16, no = 1;
+    } else {
+        if (nc == 3 && f.ycbcr) turbo_ycc_rgb(v);
+        if (mode == (int)OutMode::Luma) v[0] = (19595 * v[0] + 38470 * v[1] + 7471 * v[2] + 32768) >> 16, no = 1;
+        if (mode == (int)OutMode::Replicate) v[1] = v[2] = v[0], no = 3;
+    }
 #pragma unroll
     for (uint32_t c = 0; c < 3; c++) {
         if (c >= no) break;
@@ -421,6 +434,35 @@ template <int K>
 __global__ void __launch_bounds__(512)
 turbo_generic_draft_kernel(const FrameRecon *__restrict__ frames, const uint8_t *__restrict__ planes, int mode, TurboDst<K> out) {
     turbo_generic<K, true>(frames, planes, mode, out);
+}
+
+// the generic kernels of a CMYK / YCCK group (DESIGN §18), MODE = OutMode::CmykRgb or CmykLuma
+template <int K, int MODE>
+__global__ void __launch_bounds__(512)
+turbo_cmyk_kernel(const FrameRecon *__restrict__ frames, const uint8_t *__restrict__ planes, TurboDst<K> out) {
+    turbo_generic<K, false, MODE>(frames, planes, MODE, out);
+}
+
+template <int K, int MODE>
+__global__ void __launch_bounds__(512)
+turbo_cmyk_draft_kernel(const FrameRecon *__restrict__ frames, const uint8_t *__restrict__ planes, TurboDst<K> out) {
+    turbo_generic<K, true, MODE>(frames, planes, MODE, out);
+}
+
+template <int K, bool kDraft, int MODE>
+static void launch_cmyk(const ReconLaunch &l, dim3 grid, TurboDst<K> out, cudaStream_t s) {
+    if constexpr (kDraft) turbo_cmyk_draft_kernel<K, MODE><<<grid, dim3(64, 8), 0, s>>>(l.frames, l.planes8, out);
+    else turbo_cmyk_kernel<K, MODE><<<grid, dim3(64, 8), 0, s>>>(l.frames, l.planes8, out);
+}
+
+// a TurboGeneric group's reconstruction, after its IDCT: the CMYK instances for the modes of four-component frames (DESIGN §18),
+// turbo_generic_kernel / turbo_generic_draft_kernel for every other group
+template <int K, bool kDraft>
+static void launch_c(const ReconLaunch &l, dim3 grid, TurboDst<K> out, cudaStream_t s) {
+    if (l.mode == OutMode::CmykRgb) launch_cmyk<K, kDraft, (int)OutMode::CmykRgb>(l, grid, out, s);
+    else if (l.mode == OutMode::CmykLuma) launch_cmyk<K, kDraft, (int)OutMode::CmykLuma>(l, grid, out, s);
+    else if constexpr (kDraft) turbo_generic_draft_kernel<K><<<grid, dim3(64, 8), 0, s>>>(l.frames, l.planes8, (int)l.mode, out);
+    else turbo_generic_kernel<K><<<grid, dim3(64, 8), 0, s>>>(l.frames, l.planes8, (int)l.mode, out);
 }
 
 template <int NC, int SX, int SY, int K>
@@ -471,10 +513,10 @@ int launch_turbo(const ReconLaunch &l, void *stream, int *launches) {
         const dim3 grid((8u * l.max_bw0 + 63u) / 64u, l.max_bh0, l.n_frames);
         if (l.downscale > 1) {  // drafted frames (DESIGN §17)
             turbo_idct_draft_kernel<false><<<dim3(cblocks, l.n_frames, l.ncomp), kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8), n++;
-            turbo_generic_draft_kernel<K><<<grid, dim3(64, 8), 0, s>>>(l.frames, l.planes8, (int)l.mode, out);
+            launch_c<K, true>(l, grid, out, s);
         } else {
             turbo_idct_kernel<false><<<dim3(cblocks, l.n_frames, l.ncomp), kThreadsB, 0, s>>>(l.frames, l.coef, l.planes8), n++;
-            turbo_generic_kernel<K><<<grid, dim3(64, 8), 0, s>>>(l.frames, l.planes8, (int)l.mode, out);
+            launch_c<K, false>(l, grid, out, s);
         }
     }
     if (launches) *launches = n + 1;

@@ -407,8 +407,11 @@ class BatchDecoder:
         does; "libjpeg-turbo" as libjpeg-turbo does, so as Pillow's Image.open(f) -- its islow IDCT, fancy upsampling and YCbCr ->
         RGB conversion -- with "L" of a YCbCr frame as Pillow's draft("L") and a JPEG XT frame as its base codestream alone.
         Orientation, crop, resize and the float map follow unchanged, so Image.open(f).convert("RGB").crop(box).resize(size)
-        is what the GPU writes, byte for byte, for intact codestreams. A 12-bit, two- or four-component frame is then
-        B200JPG_ERR_NOT_IMPLEMENTED (skipped with tolerate_bad); "libjpeg-turbo" with downscale > 1 or upsample=False raises
+        is what the GPU writes, byte for byte, for intact codestreams. Under mode "RGB" or "L" that holds for CMYK and YCCK frames
+        too (DESIGN §18): libjpeg-turbo's IDCT and upsampling of all four components, then §15's conversion, as Pillow's
+        convert(mode) of the "CMYK" image it opens. A 12-bit or two-component frame, a four-component frame without a mode and
+        one colorspace() gives None for are then B200JPG_ERR_NOT_IMPLEMENTED (skipped with tolerate_bad); "libjpeg-turbo" with
+        downscale > 1 or upsample=False raises
         NativeError (B200JPG_ERR_NOT_IMPLEMENTED); any other value raises ValueError before a device is touched.
 
         draft (b200jpg_batch_create_draft, DESIGN §17) is one (h, w) for every frame, or one entry per frame: None, or (h, w) -- the
@@ -418,7 +421,8 @@ class BatchDecoder:
         codestreams the batch writes, byte for byte, what
             im = Image.open(f); im.draft(mode, (w, h))
             ImageOps.exif_transpose(im).convert(mode).crop(box).resize(size, filter)
-        gives; crop rectangles are given in output_size(data, downscale=k, exif_orientation=...). A frame whose k is 1 is decoded
+        gives, CMYK and YCCK frames under a mode included (their four components at their reduced IDCT sizes, DESIGN §18); crop
+        rectangles are given in output_size(data, downscale=k, exif_orientation=...). A frame whose k is 1 is decoded
         exactly as without a draft; status(i) is unchanged. A draft needs reconstruction="libjpeg-turbo" (else NativeError,
         B200JPG_ERR_NOT_IMPLEMENTED); a wrong length, an entry that is not two non-negative integers or exactly one zero in an
         entry raises ValueError."""
