@@ -287,6 +287,39 @@ B200JPG_API int b200jpg_batch_create_resize(b200jpg_ctx *ctx, const uint8_t *con
 B200JPG_API int b200jpg_batch_create_draft(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
                                            unsigned flags, const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes,
                                            int resample, b200jpg_batch **batch);
+/* A source box of b200jpg_batch_create_resample, Pillow's Image.resize(box=(x0, y0, x1, y1)) in the coordinates of C (below).
+ * {0, 0, 0, 0}: the default box (0, 0, w, h). */
+typedef struct b200jpg_box {
+    double x0, y0, x1, y1;
+} b200jpg_box;
+/* b200jpg_batch_create_draft with a source box and an output window per frame and one reducing_gap for the batch, the rest of
+ * Pillow's Image.resize (DESIGN §19; no counterpart in the reference). Let C be what the batch writes for frame i without a size
+ * (after draft, mode, orientation and crop, uint8, w x h). With sizes[i] = {W_t, H_t}, frame i is written, byte for byte, as
+ *     Image.fromarray(C).resize((W_t, H_t), resample, box=box, reducing_gap=gap).crop((wx, wy, wx + ww, wy + wh))
+ * of Pillow 12.2, where box = boxes[i] (the default box for {0, 0, 0, 0} or boxes == NULL), gap = reducing_gap (None when
+ * reducing_gap <= 0) and (wx, wy, ww, wh) = windows[i] ({0, 0, 0, 0} or windows == NULL: the whole W_t x H_t image). That is:
+ *   1. With a gap, fx = int((x1 - x0) / W_t / gap) or 1 and fy likewise, in double. If either is above 1, C is reduced over
+ *      Pillow's _get_safe_box (the filter's support - 0.5 times the scale around the box, int() low, ceil() high, clamped to C) by
+ *      Image.reduce: each fx x fy block (fewer pixels at the box's right and bottom edges) is ((s + n / 2) floor(2^24 / n)) >> 24
+ *      for the sum s of its n pixels; the box becomes ((x0 - rx0) / fx, (y0 - ry0) / fy, (x1 - rx0) / fx, (y1 - ry0) / fy).
+ *   2. Pillow's convolution resampler runs on the reduced image (or C) with the box as C floats: scale = (double)(x1 - x0) / W_t,
+ *      centre = x0 + (j + 0.5) scale. An axis is resampled when its size changes or its box is not (0, size): Pillow's
+ *      need_horizontal / need_vertical. The tall-image deviation of DESIGN §13 stays.
+ *   3. The window selects output columns and rows of the two tables: every output pixel depends only on its own table row, so the
+ *      cropped resize is exact.
+ * b200jpg_batch_output_extent, out_bytes / out_offset and the descriptor rules of b200jpg_batch_decode_into(_ex) describe ww x wh.
+ * The reconstruction covers only the part of C the tables (or the reduce box) read; the frame's status is its status without
+ * the size. A batch in which some frame reduces issues one launch more than without the reduce.
+ * boxes and windows NULL or all zero, and reducing_gap <= 0: exactly b200jpg_batch_create_draft. Otherwise, for the call,
+ * tolerate_bad or not, B200JPG_ERR_INVALID_PARAMETER with the frame named in the message: a box or window on a frame without a
+ * size; a box that is not finite, has a negative offset, leaves C or has x1 < x0 or y1 < y0; a window outside W_t x H_t or with
+ * a zero side; a reduce box that is empty (Pillow raises there too); a reducing_gap that is NaN or in (0, 1). A frame whose
+ * fx * fy reaches 2^24 is B200JPG_ERR_NOT_IMPLEMENTED for the call. The box and window of a frame that fails to parse are
+ * ignored. */
+B200JPG_API int b200jpg_batch_create_resample(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
+                                              unsigned flags, const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes,
+                                              const b200jpg_box *boxes, const b200jpg_rect *windows, int resample, double reducing_gap,
+                                              b200jpg_batch **batch);
 /* Pillow's draft scale of one codestream for a requested width x height (host only): s = min(W / width, H / height) in integer
  * division over the codestream's own W x H (before any Exif orientation), and the largest k of 8, 4, 2, 1 with k <= s, or 1 when
  * none fits. Returns k, or the negative parse error of the codestream; a zero width or height is B200JPG_ERR_INVALID_PARAMETER. */
@@ -298,6 +331,10 @@ B200JPG_API int b200jpg_draft_scale(const uint8_t *data, size_t len, uint32_t wi
  * returns B200JPG_ERR_INVALID_PARAMETER. Also B200JPG_ERR_INVALID_PARAMETER: a zero size, an unknown filter or a NULL ksize. */
 B200JPG_API int b200jpg_resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, int32_t *bounds, int32_t *coeffs,
                                               uint64_t capacity, uint32_t *ksize);
+/* b200jpg_resample_coefficients for the source box [in0, in1) of b200jpg_batch_create_resample, as Pillow's C resampler takes it in
+ * floats (tests only, host only). Also B200JPG_ERR_INVALID_PARAMETER: a box that is not 0 <= in0 <= in1 <= in_size. */
+B200JPG_API int b200jpg_resample_coefficients_box(uint32_t in_size, float in0, float in1, uint32_t out_size, int resample, int32_t *bounds,
+                                                  int32_t *coeffs, uint64_t capacity, uint32_t *ksize);
 /* The uncropped output size W_o x H_o of one codestream under `flags` (B200JPG_FLAG_DOWNSCALE_k, and width and height swapped for
  * the Exif orientations 5..8 with B200JPG_FLAG_EXIF_ORIENTATION; the frame size, B200JPG_FLAG_NO_UPSAMPLE or not): what the crop
  * rectangles of b200jpg_batch_create_crop are checked against. Returns B200JPG_OK or the error code b200jpg_parse returns for it

@@ -169,6 +169,7 @@ constexpr unsigned kOutputModes = B200JPG_FLAG_OUTPUT_RGB | B200JPG_FLAG_OUTPUT_
 
 bool rect_empty(const b200jpg_rect &r) { return r.x == 0 && r.y == 0 && r.width == 0 && r.height == 0; }
 bool size_empty(const b200jpg_size &s) { return s.width == 0 && s.height == 0; }
+bool box_empty(const b200jpg_box &b) { return b.x0 == 0.0 && b.y0 == 0.0 && b.x1 == 0.0 && b.y1 == 0.0; }
 bool resample_known(int r) { return r >= B200JPG_RESAMPLE_LANCZOS && r <= B200JPG_RESAMPLE_HAMMING; }  // PIL's values 1 .. 5
 
 // Pillow's draft scale (JpegImageFile.draft) of a frame of codestream size W x H for a request of width x height (both >= 1): the
@@ -356,12 +357,18 @@ struct b200jpg_batch {
     // a decode holds 4 * (n + resized frames) entries: the destinations of resized frame r at 4 * (n + r)
     std::vector<b200jpg_size> size;
     int resample = 0;
+    // b200jpg_batch_create_resample (DESIGN §19): [n_user] the target sizes W_t x H_t (`size` holds the window's extent then), the
+    // source boxes and the windows ({0, ..}: the defaults), and the reducing_gap (<= 0: None)
+    std::vector<b200jpg_size> target;
+    std::vector<b200jpg_box> box;
+    std::vector<b200jpg_rect> window;
+    double gap = 0.0;
     std::vector<ResampleFrame> rs_frames;
     std::vector<int> rs_user, rs_index;  // [resized] caller frame; [n_user] index into rs_frames or -1
     uint32_t rs_plain = 0;  // resized frames [rs_plain, ..) are grey frames of B200JPG_FLAG_OUTPUT_RGB (ResampleLaunch::n_plain)
     std::vector<std::array<std::vector<int32_t>, 4>> rs_tables;
     uint64_t dev_rs_frames = 0;
-    uint32_t rs_max_rows = 0;
+    uint32_t rs_max_rows = 0, rs_max_reduce_rows = 0;
     uint64_t rs_max_pixels = 0;
     uint8_t *d_scratch = nullptr, *d_inter = nullptr;  // C of every resized frame; the horizontal pass's rows
     uint64_t scratch_bytes = 0, inter_bytes = 0;
@@ -514,13 +521,14 @@ int b200jpg_draft_scale(const uint8_t *data, size_t len, uint32_t width, uint32_
     return rc != 0 ? rc : (int)draft_scale_of(pf.info, width, height);
 }
 
-int b200jpg_resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, int32_t *bounds, int32_t *coeffs, uint64_t capacity,
-                                  uint32_t *ksize) {
+// the tables of resample_coefficients copied out (b200jpg_resample_coefficients / _box)
+static int coefficients_out(uint32_t in_size, const float *box, uint32_t out_size, int resample, int32_t *bounds, int32_t *coeffs,
+                            uint64_t capacity, uint32_t *ksize) {
     if (!ksize || in_size == 0 || out_size == 0 || !resample_known(resample)) return B200JPG_ERR_INVALID_PARAMETER;
     std::vector<int32_t> b, k;
     uint32_t ks = 0;
     try {
-        if (int rc = resample_coefficients(in_size, out_size, resample, b, k, ks)) return rc;
+        if (int rc = resample_coefficients(in_size, box, out_size, resample, b, k, ks)) return rc;
     } catch (const std::bad_alloc &) {
         return B200JPG_ERR_OUT_OF_MEMORY;
     }
@@ -530,6 +538,18 @@ int b200jpg_resample_coefficients(uint32_t in_size, uint32_t out_size, int resam
     memcpy(bounds, b.data(), b.size() * sizeof(int32_t));
     memcpy(coeffs, k.data(), k.size() * sizeof(int32_t));
     return B200JPG_OK;
+}
+
+int b200jpg_resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, int32_t *bounds, int32_t *coeffs, uint64_t capacity,
+                                  uint32_t *ksize) {
+    return coefficients_out(in_size, nullptr, out_size, resample, bounds, coeffs, capacity, ksize);
+}
+
+int b200jpg_resample_coefficients_box(uint32_t in_size, float in0, float in1, uint32_t out_size, int resample, int32_t *bounds,
+                                      int32_t *coeffs, uint64_t capacity, uint32_t *ksize) {
+    if (!(in0 >= 0.0f && in0 <= in1 && in1 <= (float)in_size)) return B200JPG_ERR_INVALID_PARAMETER;  // (NaN fails too)
+    const float box[2] = {in0, in1};
+    return coefficients_out(in_size, box, out_size, resample, bounds, coeffs, capacity, ksize);
 }
 
 uint64_t b200jpg_build_tables(const uint8_t *data, size_t len, int scan, uint8_t *dst, uint64_t capacity) {
@@ -1430,6 +1450,9 @@ static int admit_sizes(b200jpg_batch &b, const b200jpg_size *sizes) {
             b.crop[i] = b200jpg_rect{0, 0, (uint32_t)e.w, (uint32_t)e.h};
         }
     }
+    b.target = b.size;
+    b.box.assign(b.n_user, b200jpg_box{0, 0, 0, 0});
+    b.window.assign(b.n_user, b200jpg_rect{0, 0, 0, 0});
     return B200JPG_OK;
 }
 
@@ -1453,9 +1476,118 @@ static void crop_whole_frames(b200jpg_batch &b) {
     }
 }
 
+// Pillow's _filters_support
+static double filter_support(int resample) {
+    switch (resample) {
+    case B200JPG_RESAMPLE_BOX: return 0.5;
+    case B200JPG_RESAMPLE_BICUBIC: return 2.0;
+    case B200JPG_RESAMPLE_LANCZOS: return 3.0;
+    default: return 1.0;  // bilinear, hamming
+    }
+}
+
+// Image.resize's reduce step for resized frame i (DESIGN §19), in double as Pillow's Python computes it: the factors, the reduce
+// box rb in C (x0, y0, x1, y1; Image._get_safe_box) and the box the resampler then takes, in the reduced image's coordinates (C's
+// when the frame does not reduce). C is the frame's rectangle b.crop[i], untrimmed.
+struct ReducePlan {
+    uint64_t fx = 1, fy = 1;
+    int64_t rb[4] = {0, 0, 0, 0};
+    double box[4];
+};
+static ReducePlan reduce_plan(const b200jpg_batch &b, int i) {
+    const b200jpg_rect &c = b.crop[i];
+    const b200jpg_size &t = b.target[i];
+    ReducePlan p;
+    const b200jpg_box &bx = b.box[i];
+    const double box[4] = {bx.x0, bx.y0, bx.x1, bx.y1}, whole[4] = {0.0, 0.0, (double)c.width, (double)c.height};
+    memcpy(p.box, box_empty(bx) ? whole : box, sizeof(p.box));
+    if (b.gap <= 0.0) return p;
+    p.fx = std::max<uint64_t>(1, (uint64_t)((p.box[2] - p.box[0]) / t.width / b.gap));  // int(...) or 1
+    p.fy = std::max<uint64_t>(1, (uint64_t)((p.box[3] - p.box[1]) / t.height / b.gap));
+    if (p.fx == 1 && p.fy == 1) return p;
+    const double support = filter_support(b.resample) - 0.5;
+    const double sx = support * ((p.box[2] - p.box[0]) / t.width), sy = support * ((p.box[3] - p.box[1]) / t.height);
+    p.rb[0] = std::max<int64_t>(0, (int64_t)(p.box[0] - sx));
+    p.rb[1] = std::max<int64_t>(0, (int64_t)(p.box[1] - sy));
+    p.rb[2] = std::min<int64_t>(c.width, (int64_t)std::ceil(p.box[2] + sx));
+    p.rb[3] = std::min<int64_t>(c.height, (int64_t)std::ceil(p.box[3] + sy));
+    const double nb[4] = {(p.box[0] - p.rb[0]) / p.fx, (p.box[1] - p.rb[1]) / p.fy, (p.box[2] - p.rb[0]) / p.fx, (p.box[3] - p.rb[1]) / p.fy};
+    memcpy(p.box, nb, sizeof(p.box));
+    return p;
+}
+
+// b200jpg_batch_create_resample's boxes and windows (nullptr: none), checked for the live frames (a failed frame's are ignored)
+// against C (the frame's rectangle, set by admit_sizes) and the target size; a window replaces the frame's output extent
+// (`size`), the target staying in `target` (admit_sizes sets `target`, `box` and `window`; without sizes they stay empty and any
+// box or window is refused). Returns 0 or the status the call fails with.
+static int admit_boxes(b200jpg_batch &b, const b200jpg_box *boxes, const b200jpg_rect *windows) {
+    for (int i = 0; i < b.n_user; i++) {
+        if (b.parse_status[i] != 0) continue;
+        const b200jpg_box bx = boxes ? boxes[i] : b200jpg_box{0, 0, 0, 0};
+        const b200jpg_rect wn = windows ? windows[i] : b200jpg_rect{0, 0, 0, 0};
+        const std::string at = "frame " + std::to_string(i) + ": ";
+        if (!box_empty(bx) || !rect_empty(wn)) {
+            if (b.target.empty() || size_empty(b.target[i])) return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "a box or window needs a target size");
+            const b200jpg_rect &c = b.crop[i];
+            const b200jpg_size &t = b.target[i];
+            if (!box_empty(bx)) {
+                const std::string desc = "box (" + std::to_string(bx.x0) + ", " + std::to_string(bx.y0) + ", " + std::to_string(bx.x1) + ", " +
+                                         std::to_string(bx.y1) + ")";
+                if (!std::isfinite(bx.x0) || !std::isfinite(bx.y0) || !std::isfinite(bx.x1) || !std::isfinite(bx.y1))
+                    return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + desc + " is not finite");
+                if (bx.x0 < 0.0 || bx.y0 < 0.0) return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + desc + " has a negative offset");
+                if (bx.x1 > c.width || bx.y1 > c.height)
+                    return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER,
+                                       at + desc + " leaves the " + std::to_string(c.width) + " x " + std::to_string(c.height) + " image");
+                if (bx.x1 < bx.x0 || bx.y1 < bx.y0) return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + desc + " has a negative extent");
+            }
+            if (!rect_empty(wn) && (wn.width == 0 || wn.height == 0 || (uint64_t)wn.x + wn.width > t.width || (uint64_t)wn.y + wn.height > t.height))
+                return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "window (" + std::to_string(wn.x) + ", " + std::to_string(wn.y) + ", " +
+                                                                      std::to_string(wn.width) + ", " + std::to_string(wn.height) +
+                                                                      ") is empty or leaves the " + std::to_string(t.width) + " x " +
+                                                                      std::to_string(t.height) + " image");
+            b.box[i] = bx;
+            if (!rect_empty(wn)) b.window[i] = wn, b.size[i] = b200jpg_size{wn.width, wn.height};
+        }
+        if (b.target.empty() || size_empty(b.target[i]) || b.gap <= 0.0) continue;
+        const ReducePlan rp = reduce_plan(b, i);
+        if (rp.fx * rp.fy >= (1ull << 24))
+            return b.ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, at + "reduce factors " + std::to_string(rp.fx) + " x " + std::to_string(rp.fy) +
+                                                                " reach 2^24 pixels per block");
+        if ((rp.fx > 1 || rp.fy > 1) && (rp.rb[2] <= rp.rb[0] || rp.rb[3] <= rp.rb[1]))
+            return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "the reduce box of the source box is empty");
+    }
+    return B200JPG_OK;
+}
+
+// One axis of resized frame i: the table of the source's `in` samples for `out` outputs (box: Pillow's floats, nullptr for the
+// default box), restricted to the window's outputs [w0, w0 + wn), or none when Pillow does not resample the axis. Returns the
+// source range [lo, hi) the window reads, the tables rebased to lo.
+static void plan_axis(uint32_t in, const float *box, uint32_t out, uint32_t w0, uint32_t wn, int resample, bool pass,
+                      std::vector<int32_t> &bounds, std::vector<int32_t> &coef, uint32_t &ksize, uint32_t &lo, uint32_t &hi) {
+    if (!pass) {  // the window's own samples (out == in)
+        lo = w0, hi = w0 + wn;
+        return;
+    }
+    resample_coefficients(in, box, out, resample, bounds, coef, ksize);  // (the arguments are valid: the call cannot fail)
+    if (w0 != 0 || wn != out) {
+        bounds.erase(bounds.begin() + 2 * ((size_t)w0 + wn), bounds.end());
+        bounds.erase(bounds.begin(), bounds.begin() + 2 * (size_t)w0);
+        coef.erase(coef.begin() + ((size_t)w0 + wn) * ksize, coef.end());
+        coef.erase(coef.begin(), coef.begin() + (size_t)w0 * ksize);
+    }
+    lo = in, hi = 0;
+    for (uint32_t j = 0; j < wn; j++)
+        if (bounds[2 * j + 1] > 0) lo = std::min<uint32_t>(lo, bounds[2 * j]), hi = std::max<uint32_t>(hi, bounds[2 * j] + bounds[2 * j + 1]);
+    if (lo >= hi) lo = 0, hi = 1;  // no output reads a sample (a zero-width box at the edge): one sample stays
+    for (uint32_t j = 0; j < wn; j++) bounds[2 * j] = bounds[2 * j + 1] > 0 ? bounds[2 * j] - (int32_t)lo : 0;
+}
+
 // The resample descriptors and tables of the resized frames (tables built on host threads, one frame each) and the layout of the
-// scratch (C: h rows of align16(w * ncomp) bytes per frame) and of the intermediate (rows y0 .. y1 - 1 of tw * ncomp bytes, for
-// frames whose width changes). The grey frames of B200JPG_FLAG_OUTPUT_RGB come last, with one channel: the vertical pass replicates it.
+// scratch (C: c_h rows of align16(c_w * ncomp) bytes per frame, then R where the frame reduces) and of the intermediate (rows y0 ..
+// y1 - 1 of tw * ncomp bytes, for frames with a horizontal pass). The grey frames of B200JPG_FLAG_OUTPUT_RGB come last, with one
+// channel: the vertical pass replicates it. Each frame's rectangle shrinks to the part of C its tables (or its reduce box) read,
+// which is all of C without a box, a window and a reduce (DESIGN §19): the reconstruction covers no more.
 static void plan_resample(b200jpg_batch &b) {
     b.rs_index.assign(b.n_user, -1);
     for (int rgb = 0; rgb < 2; rgb++) {
@@ -1471,30 +1603,54 @@ static void plan_resample(b200jpg_batch &b) {
     b.rs_tables.assign(nr, {});
     for_frames(nr, 16, [&](int r) {
         const int i = b.rs_user[r];
-        const b200jpg_frame_info &fi = b.frames[i].info;
-        const Extent e = out_extent(fi, 0, b.flags, b.scale[i], applied_orientation(b, i), crop_of(b, i));  // C
-        const b200jpg_size &s = *size_of(b, i);
+        b200jpg_rect &c = b.crop[i];  // C, trimmed below to what the resize reads
+        const b200jpg_size &s = b.target[i];
+        const b200jpg_rect &wn = b.window[i];
         ResampleFrame &f = b.rs_frames[r];
         auto &t = b.rs_tables[r];
         const FramePlan plan = frame_plan(b, i);  // C has the components the reconstruction stores
-        f.w = (uint32_t)e.w, f.h = (uint32_t)e.h, f.tw = s.width, f.th = s.height;
+        const ReducePlan rp = reduce_plan(b, i);
+        const bool reduces = rp.fx > 1 || rp.fy > 1;
+        f.fx = (uint32_t)rp.fx, f.fy = (uint32_t)rp.fy;
+        // the source S: R, (rb.x1 - rb.x0) / fx x (rb.y1 - rb.y0) / fy rounded up, or C
+        const uint32_t sw = reduces ? (uint32_t)((rp.rb[2] - rp.rb[0] + rp.fx - 1) / rp.fx) : c.width;
+        const uint32_t sh = reduces ? (uint32_t)((rp.rb[3] - rp.rb[1] + rp.fy - 1) / rp.fy) : c.height;
+        const float fb[4] = {(float)rp.box[0], (float)rp.box[1], (float)rp.box[2], (float)rp.box[3]};  // Pillow's "(ffff)"
+        const bool plain = !reduces && box_empty(b.box[i]);  // DESIGN §13's tables, computed as they always were
+        f.pass = (s.width != sw || fb[0] != 0.0f || fb[2] != (float)s.width ? kPassH : 0u) |
+                 (s.height != sh || fb[1] != 0.0f || fb[3] != (float)s.height ? kPassV : 0u);
+        f.tw = rect_empty(wn) ? s.width : wn.width, f.th = rect_empty(wn) ? s.height : wn.height;
+        const float fbh[2] = {fb[0], fb[2]}, fbv[2] = {fb[1], fb[3]};
+        uint32_t x0, x1, y0, y1;  // the part of S the window reads
+        plan_axis(sw, plain ? nullptr : fbh, s.width, wn.x, f.tw, b.resample, f.pass & kPassH, t[0], t[1], f.h_ksize, x0, x1);
+        plan_axis(sh, plain ? nullptr : fbv, s.height, wn.y, f.th, b.resample, f.pass & kPassV, t[2], t[3], f.v_ksize, y0, y1);
+        f.w = x1 - x0, f.h = y1 - y0;
         f.ncomp = plan.mode == OutMode::Replicate ? plan.ncomp : plan.out_ncomp;
         f.src_pitch = (uint32_t)align_up((uint64_t)f.w * f.ncomp, 16);
+        if (reduces) {  // R's blocks x0 .. x1 - 1, y0 .. y1 - 1: the pixels of C they cover (the last ones partial only at rb's edges)
+            const uint64_t cx = rp.rb[0] + (uint64_t)x0 * rp.fx, cy = rp.rb[1] + (uint64_t)y0 * rp.fy;
+            c.x += (uint32_t)cx, c.y += (uint32_t)cy;
+            c.width = (uint32_t)(std::min<uint64_t>(rp.rb[2], rp.rb[0] + (uint64_t)x1 * rp.fx) - cx);
+            c.height = (uint32_t)(std::min<uint64_t>(rp.rb[3], rp.rb[1] + (uint64_t)y1 * rp.fy) - cy);
+        } else {
+            c.x += x0, c.y += y0, c.width = f.w, c.height = f.h;
+        }
+        f.c_w = c.width, f.c_h = c.height;
+        f.c_pitch = (uint32_t)align_up((uint64_t)f.c_w * f.ncomp, 16);
         f.plane = (uint32_t)(b.n + r);
         f.y0 = 0, f.y1 = f.h;
-        if (f.th != f.h) {  // (the arguments are valid: the calls cannot fail)
-            resample_coefficients(f.h, f.th, b.resample, t[2], t[3], f.v_ksize);
-            f.y0 = (uint32_t)t[2][0];
-            f.y1 = (uint32_t)(t[2][2 * (size_t)f.th - 2] + t[2][2 * (size_t)f.th - 1]);
-        }
-        if (f.tw != f.w) resample_coefficients(f.w, f.tw, b.resample, t[0], t[1], f.h_ksize);
         if (f.src_pitch <= kResampleRowSmem) f.stage |= kStageRow;
-        if (f.tw != f.w && align_up(t[1].size() * sizeof(int32_t), 16) <= kResampleCoefSmem) f.stage |= kStageCoef;
+        if ((f.pass & kPassH) && align_up(t[1].size() * sizeof(int32_t), 16) <= kResampleCoefSmem) f.stage |= kStageCoef;
     });
     for (ResampleFrame &f : b.rs_frames) {
-        f.src = b.scratch_bytes;
-        b.scratch_bytes = align_up(b.scratch_bytes + (uint64_t)f.src_pitch * f.h, 256);
-        if (f.tw != f.w) {
+        f.c_src = f.src = b.scratch_bytes;
+        b.scratch_bytes = align_up(b.scratch_bytes + (uint64_t)f.c_pitch * f.c_h, 256);
+        if (f.fx > 1 || f.fy > 1) {  // R behind C
+            f.src = b.scratch_bytes;
+            b.scratch_bytes = align_up(b.scratch_bytes + (uint64_t)f.src_pitch * f.h, 256);
+            b.rs_max_reduce_rows = std::max(b.rs_max_reduce_rows, f.h);
+        }
+        if (f.pass & kPassH) {
             f.inter = b.inter_bytes;
             b.inter_bytes = align_up(b.inter_bytes + (uint64_t)(f.y1 - f.y0) * f.tw * f.ncomp, 256);
             b.rs_max_rows = std::max(b.rs_max_rows, f.y1 - f.y0);
@@ -1504,10 +1660,16 @@ static void plan_resample(b200jpg_batch &b) {
 }
 
 static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
-                             const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes, int resample, b200jpg_batch **out) {
+                             const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes, const b200jpg_box *boxes,
+                             const b200jpg_rect *windows, int resample, double reducing_gap, b200jpg_batch **out) {
     NvtxRange nvtx("b200jpg batch_create: parse + pack");
     if (!out || !frames || !lens || n <= 0) return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "invalid batch arguments");
     *out = nullptr;
+    if (std::isnan(reducing_gap) || (reducing_gap > 0.0 && reducing_gap < 1.0))
+        return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "reducing_gap " + std::to_string(reducing_gap) + " is NaN or below 1.0");
+    bool any_box = false;
+    for (int i = 0; i < n; i++) any_box = any_box || (boxes && !box_empty(boxes[i])) || (windows && !rect_empty(windows[i]));
+    if (!any_box) boxes = nullptr, windows = nullptr;  // all zero: exactly the batch of b200jpg_batch_create_draft
     bool any_draft = false;
     for (int i = 0; drafts && i < n; i++) {
         if ((drafts[i].width == 0) != (drafts[i].height == 0))
@@ -1568,14 +1730,17 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
         if (int rc = admit_crops(b, rects)) return rc;
     if (sizes)
         if (int rc = admit_sizes(b, sizes)) return rc;
+    if (sizes) b.gap = reducing_gap;  // (<= 0: None)
+    if (boxes || windows || b.gap > 0.0)
+        if (int rc = admit_boxes(b, boxes, windows)) return rc;
     if (flags & B200JPG_FLAG_LIBJPEG_TURBO) crop_whole_frames(b);
+    plan_resample(b);  // (before the reconstruction groups: it trims the rectangles of resized frames)
     const std::vector<uint64_t> byte_off = lay_out_codestreams(b, cs.len);
     const std::vector<std::array<uint64_t, 4>> sample_base = lay_out_planes(b);
     form_scan_classes(b, frame_tables, byte_off);
     form_progressive_groups(b);
     lay_out_unstuffed(b);
     form_recon_groups(b, sample_base);
-    plan_resample(b);
     lay_out_descriptors(b);
     if (int rc = stage_and_allocate(b, cs, byte_off)) return rc;
     *out = bp.release();
@@ -1604,9 +1769,15 @@ int b200jpg_batch_create_resize(b200jpg_ctx *ctx, const uint8_t *const *frames, 
 
 int b200jpg_batch_create_draft(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
                                const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes, int resample, b200jpg_batch **out) {
+    return b200jpg_batch_create_resample(ctx, frames, lens, n, tolerate_bad, flags, drafts, rects, sizes, nullptr, nullptr, resample, 0.0, out);
+}
+
+int b200jpg_batch_create_resample(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
+                                  const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes, const b200jpg_box *boxes,
+                                  const b200jpg_rect *windows, int resample, double reducing_gap, b200jpg_batch **out) {
     if (!ctx) return B200JPG_ERR_INVALID_PARAMETER;
     try {  // no exception crosses the C ABI
-        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, drafts, rects, sizes, resample, out);
+        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, drafts, rects, sizes, boxes, windows, resample, reducing_gap, out);
     } catch (const std::bad_alloc &) {
         if (out) *out = nullptr;
         return ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "out of host memory while preparing the batch");
@@ -1910,9 +2081,9 @@ static bool rewrite_frame(const b200jpg_batch *b, int i, b200jpg_plane *pl, uint
 static void scratch_planes(const b200jpg_batch *b, int i, b200jpg_plane *pl, std::vector<char> &planar) {
     const ResampleFrame &f = b->rs_frames[(size_t)b->rs_index[i]];
     for (uint32_t c = 0; c < f.ncomp; c++) {
-        pl[c].data = b->d_scratch + f.src + c;
+        pl[c].data = b->d_scratch + f.c_src + c;
         pl[c].bytes_per_pixel = (int32_t)f.ncomp;
-        pl[c].bytes_per_row = f.src_pitch;
+        pl[c].bytes_per_row = f.c_pitch;
     }
     rewrite_frame(b, i, pl, 1, planar, f.ncomp);  // a scratch row always fits the pixel stride
 }
@@ -2031,6 +2202,7 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         rl.frames = reinterpret_cast<const ResampleFrame *>(b->d_input + b->dev_rs_frames) + first;
         rl.n_frames = std::min<uint32_t>(65535u, nr - first);
         rl.max_rows = b->rs_max_rows;
+        rl.max_reduce_rows = b->rs_max_reduce_rows;
         rl.max_pixels = b->rs_max_pixels;
         rl.input = b->d_input;
         rl.scratch = b->d_scratch;

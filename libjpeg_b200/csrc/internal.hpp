@@ -385,33 +385,42 @@ int launch_recon(const ReconLaunch &l, void *stream, int *launches);
 template <int K>
 int launch_turbo(const ReconLaunch &l, void *stream, int *launches);
 
-// ---- resize (b200jpg_batch_create_resize, DESIGN §13), resample_sm100.cu. The reconstruction writes C, the frame's cropped
-// output, as an interleaved uint8 bitmap into the batch's scratch; resample_h_kernel runs the horizontal pass over the rows of C
-// the vertical table touches into the intermediate, resample_v_kernel the vertical pass into the caller's destinations.
-// The fixed-point tables of one axis: bounds [out_size][2] int32 (first source index, taps), coefficients [out_size][ksize] int32
-// (zero behind the taps), PIL's convolution resampler; computed without floating-point contraction (build.py).
-int resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, std::vector<int32_t> &bounds, std::vector<int32_t> &coef,
-                          uint32_t &ksize);
+// ---- resize (b200jpg_batch_create_resize, DESIGN §13; boxes, reduce and windows of b200jpg_batch_create_resample, DESIGN §19),
+// resample_sm100.cu. The reconstruction writes C, the frame's cropped output (the part of it the resize reads), as an interleaved
+// uint8 bitmap into the batch's scratch; reduce_kernel reduces it to R behind it in the scratch where the frame reduces;
+// resample_h_kernel runs the horizontal pass over the rows of the source (C or R) the vertical table touches into the
+// intermediate, resample_v_kernel the vertical pass into the caller's destinations.
+// The fixed-point tables of one axis of in_size samples for out_size outputs: bounds [out_size][2] int32 (first source index, taps),
+// coefficients [out_size][ksize] int32 (zero behind the taps), PIL's convolution resampler; computed without floating-point
+// contraction (build.py). box = {in0, in1}, Pillow's C floats, or nullptr for the default box (0, in_size) of DESIGN §13.
+int resample_coefficients(uint32_t in_size, const float *box, uint32_t out_size, int resample, std::vector<int32_t> &bounds,
+                          std::vector<int32_t> &coef, uint32_t &ksize);
 struct ResampleFrame {
-    uint64_t src;                             // byte offset of C in the scratch: h rows of src_pitch bytes, ncomp bytes per pixel
+    uint64_t src;                             // byte offset of the source in the scratch: h rows of src_pitch bytes, ncomp bytes per pixel
     uint64_t inter;                           // byte offset of the horizontal pass's rows y0 .. y1 - 1 in the intermediate (tw * ncomp each)
     uint64_t h_bounds, h_coef, v_bounds, v_coef;  // byte offsets of the tables in the input buffer (16-byte aligned)
-    uint32_t w, h, tw, th;                    // C's extent and the target size; an axis of equal size is not resampled
-    uint32_t ncomp, src_pitch, h_ksize, v_ksize;
-    uint32_t y0, y1;                          // the rows of C the vertical table touches (0, h when the height does not change)
-    uint32_t plane;                           // destinations: planes[4 * plane + c], in output coordinates
-    uint32_t stage;                           // kStageRow: a row of C fits the shared row buffer; kStageCoef: the horizontal table fits
+    uint64_t c_src;                           // byte offset of C in the scratch (src unless the frame reduces): c_h rows of c_pitch bytes
+    // (grouped by 16 bytes so that the vertical pass reads its fields in two loads)
+    uint32_t tw, th, ncomp, pass;             // the output's extent (the window's); kPassH / kPassV: the axes Pillow resamples
+    uint32_t src_pitch, v_ksize, y0, plane;   // y0, y1: the rows of the source the vertical table touches (0, h: the source is trimmed
+    uint32_t w, h, h_ksize, y1;               // to them); destinations: planes[4 * plane + c], in output coordinates; w x h: the source
+    uint32_t stage;                           // kStageRow: a row of the source fits the shared row buffer; kStageCoef: the horizontal table fits
+    uint32_t fx, fy;                          // Image.reduce's factors (1, 1: the source is C)
+    uint32_t c_w, c_h, c_pitch;               // C's extent and row pitch; blocks of fx x fy pixels of C from its origin make R
 };
 constexpr uint32_t kStageRow = 1, kStageCoef = 2;
+constexpr uint32_t kPassH = 1, kPassV = 2;
 constexpr uint32_t kResampleRowSmem = 16 * 1024, kResampleCoefSmem = 32 * 1024;  // the shared buffers of resample_h_kernel
 constexpr uint32_t kResampleRows = 8;                                            // rows of the intermediate per CTA
+constexpr uint32_t kReduceRows = 4;                                              // rows of R per reduce_kernel CTA
 struct ResampleLaunch {
     const ResampleFrame *frames;  // device
     uint32_t n_frames;
-    uint32_t max_rows;            // largest y1 - y0 of a frame whose width changes
+    uint32_t max_rows;            // largest y1 - y0 of a frame with a horizontal pass
+    uint32_t max_reduce_rows;     // largest height of R of a frame that reduces (0: no reduce_kernel launch)
     uint64_t max_pixels;          // largest tw * th
     const uint8_t *input;         // the batch's input buffer (tables)
-    const uint8_t *scratch;
+    uint8_t *scratch;
     uint8_t *inter;
     const b200jpg_plane *planes;  // device
     const b200jpg_convert *convert;  // host; null: uint8 destinations

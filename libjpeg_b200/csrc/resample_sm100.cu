@@ -1,17 +1,22 @@
-// resample_sm100.cu -- the resize stage of b200jpg_batch_create_resize (DESIGN §13): Pillow's convolution resampler on the
-// reconstruction's uint8 output, every channel on its own, in the int32 fixed point of Pillow's 8-bit path.
+// resample_sm100.cu -- the resize stage of b200jpg_batch_create_resize (DESIGN §13) and b200jpg_batch_create_resample (DESIGN
+// §19): Pillow's Image.reduce and convolution resampler on the reconstruction's uint8 output, every channel on its own, in the
+// integer arithmetic of Pillow's 8-bit paths.
 //
+//   reduce_kernel: grid (row band, frame). Each thread takes output pixels x channels of R along x and sums its fx x fy block of C
+//     (fewer pixels in the partial blocks at C's right and bottom edges), so a warp reads each of the fy source rows contiguously.
+//     Frames that do not reduce return at once; the kernel is launched only when some frame of the batch reduces.
 //   resample_h_kernel: grid (row band, frame). A CTA takes kResampleRows rows of the intermediate (rows y0.. of C); each row of C
 //     comes into shared memory with 16-byte loads, and every thread computes output columns x channels from it. The frame's
 //     horizontal table is read from shared memory where it fits, otherwise from global memory through L1. A frame whose width does
-//     not change has no horizontal pass: the vertical pass reads C in the scratch directly.
+//     Pillow does not resample horizontally has no horizontal pass: the vertical pass reads the source in the scratch directly.
 //   resample_v_kernel: one thread per output pixel, all channels. The taps go down a column of the intermediate, so a warp's loads
 //     are contiguous along x and the tap's coefficient is one broadcast load; the clamped sample leaves through the caller's
 //     b200jpg_plane descriptor (any signed strides), converted by the float map of b200jpg_batch_decode_into_ex where one is given.
 //   resample_v_rgb_kernel: the same for the grey frames of B200JPG_FLAG_OUTPUT_RGB (DESIGN §14), which come last in the frame list:
 //     one channel, each value stored to three destinations.
+// Which passes run is the descriptor's `pass` (Pillow's need_horizontal / need_vertical); a window only selects the tables' rows.
 // The host half: resample_coefficients, the only place the fixed-point tables are built (the batch's planning and the test entry
-// point b200jpg_resample_coefficients both call it). build.py compiles this file with -ffp-contract=off: the double-precision
+// points b200jpg_resample_coefficients / _box call it). build.py compiles this file with -ffp-contract=off: the double-precision
 // arithmetic is evaluated as written, one rounding per operation, on every host.
 #include <cuda_runtime.h>
 
@@ -60,11 +65,36 @@ __device__ __forceinline__ int clamp8(int acc) {
     return v < 0 ? 0 : (v > 255 ? 255 : v);
 }
 
+// Image.reduce's rounding (Pillow's Reduce.c): ((sum + n / 2) * floor(2^24 / n)) >> 24 for a block of n pixels, in uint32 -- the
+// product is at most (255 n + n / 2) floor(2^24 / n) <= 255.5 * 2^24 < 2^32. The planning keeps n below 2^24 (fx * fy < 2^24).
+__global__ void __launch_bounds__(256) reduce_kernel(const ResampleFrame *__restrict__ frames, uint8_t *__restrict__ scratch) {
+    const ResampleFrame &f = frames[blockIdx.y];
+    const uint32_t fx = f.fx, fy = f.fy;
+    if (fx == 1 && fy == 1) return;
+    const uint32_t r0 = blockIdx.x * kReduceRows;
+    if (r0 >= f.h) return;
+    const uint32_t r1 = min(f.h, r0 + kReduceRows), nc = f.ncomp, outs = f.w * nc;
+    for (uint32_t r = r0; r < r1; r++) {
+        const uint32_t cy = r * fy, ny = min(fy, f.c_h - cy);
+        const uint8_t *rows = scratch + f.c_src + (uint64_t)cy * f.c_pitch;
+        uint8_t *o = scratch + f.src + (uint64_t)r * f.src_pitch;
+        for (uint32_t k = threadIdx.x; k < outs; k += 256) {
+            const uint32_t x = k / nc, c = k - x * nc, cx = x * fx, nx = min(fx, f.c_w - cx);
+            const uint8_t *p = rows + (uint64_t)cx * nc + c;
+            uint32_t sum = 0;
+            for (uint32_t yy = 0; yy < ny; yy++, p += f.c_pitch)
+                for (uint32_t xx = 0; xx < nx; xx++) sum += p[xx * nc];
+            const uint32_t n = nx * ny;
+            o[k] = (uint8_t)(((sum + n / 2) * ((1u << 24) / n)) >> 24);
+        }
+    }
+}
+
 __global__ void __launch_bounds__(256) resample_h_kernel(const ResampleFrame *__restrict__ frames, const uint8_t *__restrict__ input,
                                                          const uint8_t *__restrict__ scratch, uint8_t *__restrict__ inter) {
     extern __shared__ uint4 smem[];
     const ResampleFrame &f = frames[blockIdx.y];
-    if (f.tw == f.w) return;
+    if (!(f.pass & kPassH)) return;
     const uint32_t rows = f.y1 - f.y0, r0 = blockIdx.x * kResampleRows;
     if (r0 >= rows) return;
     const uint32_t r1 = min(rows, r0 + kResampleRows), nc = f.ncomp, outs = f.tw * nc, ksize = f.h_ksize;
@@ -108,11 +138,11 @@ __global__ void __launch_bounds__(256) resample_v_kernel(const ResampleFrame *__
     const uint64_t i = (uint64_t)blockIdx.x * 256 + threadIdx.x;
     if (i >= (uint64_t)f.tw * f.th) return;
     const uint32_t y = (uint32_t)(i / f.tw), x = (uint32_t)(i - (uint64_t)y * f.tw), nc = f.ncomp;
-    const bool hpass = f.tw != f.w;
-    const uint8_t *src = hpass ? inter + f.inter : scratch + f.src;  // row 0 of src is row y0 of C
+    const bool hpass = (f.pass & kPassH) != 0;
+    const uint8_t *src = hpass ? inter + f.inter : scratch + f.src;  // row 0 of src is row y0 of the source
     const uint64_t pitch = hpass ? (uint64_t)f.tw * nc : f.src_pitch;
     int acc[B200JPG_MAX_COMPONENTS];
-    if (f.th != f.h) {
+    if (f.pass & kPassV) {
         const int32_t *vb = reinterpret_cast<const int32_t *>(input + f.v_bounds);
         const int32_t *kk = reinterpret_cast<const int32_t *>(input + f.v_coef) + (uint64_t)y * f.v_ksize;
         const int n = __ldg(vb + 2 * y + 1);
@@ -151,11 +181,11 @@ __global__ void __launch_bounds__(256) resample_v_rgb_kernel(const ResampleFrame
     const uint64_t i = (uint64_t)blockIdx.x * 256 + threadIdx.x;
     if (i >= (uint64_t)f.tw * f.th) return;
     const uint32_t y = (uint32_t)(i / f.tw), x = (uint32_t)(i - (uint64_t)y * f.tw);
-    const bool hpass = f.tw != f.w;
-    const uint8_t *src = hpass ? inter + f.inter : scratch + f.src;  // row 0 of src is row y0 of C
+    const bool hpass = (f.pass & kPassH) != 0;
+    const uint8_t *src = hpass ? inter + f.inter : scratch + f.src;  // row 0 of src is row y0 of the source
     const uint64_t pitch = hpass ? (uint64_t)f.tw : f.src_pitch;
     int v;
-    if (f.th != f.h) {
+    if (f.pass & kPassV) {
         const int32_t *vb = reinterpret_cast<const int32_t *>(input + f.v_bounds);
         const int32_t *kk = reinterpret_cast<const int32_t *>(input + f.v_coef) + (uint64_t)y * f.v_ksize;
         const int n = __ldg(vb + 2 * y + 1);
@@ -176,8 +206,10 @@ __global__ void __launch_bounds__(256) resample_v_rgb_kernel(const ResampleFrame
 
 }  // namespace
 
-int resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, std::vector<int32_t> &bounds, std::vector<int32_t> &coef,
-                          uint32_t &ksize) {
+// Pillow's precompute_coeffs: scale = (double)(in1 - in0) / out_size with the difference taken in float, center = in0 + (j + 0.5)
+// scale in double; without a box, scale = in_size / out_size and center = (j + 0.5) scale (DESIGN §13, for any in_size).
+int resample_coefficients(uint32_t in_size, const float *box, uint32_t out_size, int resample, std::vector<int32_t> &bounds,
+                          std::vector<int32_t> &coef, uint32_t &ksize) {
     double (*filter)(double);
     double s;
     switch (resample) {
@@ -189,13 +221,14 @@ int resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, std
     default: return B200JPG_ERR_INVALID_PARAMETER;
     }
     if (in_size == 0 || out_size == 0) return B200JPG_ERR_INVALID_PARAMETER;
-    const double scale = (double)in_size / out_size, fs = std::max(scale, 1.0), support = s * fs;
+    const double extent = box ? (double)(box[1] - box[0]) : (double)in_size, in0 = box ? (double)box[0] : 0.0;
+    const double scale = extent / out_size, fs = std::max(scale, 1.0), support = s * fs;
     ksize = (uint32_t)ceil(support) * 2 + 1;
     bounds.assign(2 * (size_t)out_size, 0);
     coef.assign((size_t)out_size * ksize, 0);
     std::vector<double> w(ksize);
     for (uint32_t j = 0; j < out_size; j++) {
-        const double center = (j + 0.5) * scale;
+        const double center = box ? in0 + (j + 0.5) * scale : (j + 0.5) * scale;
         const int64_t xmin = std::max<int64_t>((int64_t)(center - support + 0.5), 0);
         const int64_t n = std::min<int64_t>((int64_t)(center + support + 0.5), in_size) - xmin;
         double ww = 0.0;
@@ -215,6 +248,11 @@ int resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, std
 
 int launch_resample(const ResampleLaunch &l, void *stream, int *launches) {
     cudaStream_t s = (cudaStream_t)stream;
+    int n = 1;
+    if (l.max_reduce_rows) {
+        reduce_kernel<<<dim3((l.max_reduce_rows + kReduceRows - 1) / kReduceRows, l.n_frames), 256, 0, s>>>(l.frames, l.scratch);
+        n++;
+    }
     const uint32_t gh = std::max<uint32_t>(1u, (l.max_rows + kResampleRows - 1) / kResampleRows);
     resample_h_kernel<<<dim3(gh, l.n_frames), 256, kResampleRowSmem + kResampleCoefSmem, s>>>(l.frames, l.input, l.scratch, l.inter);
     const uint32_t gv = (uint32_t)std::max<uint64_t>(1u, (l.max_pixels + 255) / 256);
@@ -225,7 +263,6 @@ int launch_resample(const ResampleLaunch &l, void *stream, int *launches) {
         for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) d.scale[c] = l.convert->scale[c], d.bias[c] = l.convert->bias[c];
     }
     const uint32_t n_rgb = l.n_frames - l.n_plain;
-    int n = 1;
     if (l.n_plain) {
         if (l.convert) resample_v_kernel<true><<<dim3(gv, l.n_plain), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);
         else resample_v_kernel<false><<<dim3(gv, l.n_plain), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);

@@ -4,6 +4,7 @@ PyTorch is plumbing here: it owns the output tensor and the CUDA stream; every b
 in the hand-written kernels of libb200jpg.so.
 """
 import ctypes
+import math
 import threading
 from dataclasses import dataclass
 
@@ -123,21 +124,125 @@ def draft_scale(data, size):
     return rc
 
 
-def crop_table(crop, n):
-    """The b200jpg_rect table of BatchDecoder(crop=...): n entries, each None (the whole frame) or (x, y, width, height) as
-    non-negative integers. Raises ValueError; the rectangles themselves are checked against the frames by the batch."""
+def _hw(size, what):
+    """(h, w) of two positive integers; raises ValueError"""
+    import numbers
+    hw = tuple(size) if isinstance(size, (tuple, list)) else None
+    if hw is None or len(hw) != 2 or any(isinstance(v, bool) or not isinstance(v, numbers.Integral) or v < 1 for v in hw):
+        raise ValueError("%s must be two positive integers (h, w), got %r" % (what, size))
+    return int(hw[0]), int(hw[1])
+
+
+def thumbnail_args(data, size, reducing_gap=2.0, exif_orientation=False):
+    """The BatchDecoder entries of one codestream for Pillow's thumbnail, as a dict of "draft", "resize" and "box" (each None or
+    the entry) -- host only, no GPU. size = (h, w); Image.thumbnail takes (w, h). With exif_orientation=False the chain is
+        im = Image.open(f); im.thumbnail((w, h), reducing_gap=reducing_gap)
+    and with exif_orientation=True (the batch's flag too) ImageOps.exif_transpose(Image.open(f)).thumbnail((w, h), ...), which
+    draws no draft: exif_transpose has loaded the image. The batch takes resample="bicubic" and the same reducing_gap (None for
+    None). An image already within the size is left untouched (every entry None), and a frame whose draft already has the
+    thumbnail's size is drafted but not resized. The image the batch resizes is the frame's own, so this holds for grey and
+    YCbCr frames under mode None or "RGB" (DESIGN §19). Raises ValueError, NativeError where parse() does."""
+    h, w = _hw(size, "size")
+    if reducing_gap is not None:
+        reducing_gap_value(reducing_gap)
+    H, W = output_size(data, exif_orientation=exif_orientation)
+    out = {"draft": None, "resize": None, "box": None}
+    if w >= W and h >= H:  # preserve_aspect_ratio: None
+        return out
+    aspect = W / H
+
+    def round_aspect(number, key):
+        return max(min(math.floor(number), math.ceil(number), key=key), 1)
+
+    x, y = w, h
+    if x / y >= aspect:
+        x = round_aspect(y * aspect, key=lambda n: abs(aspect - n / y))
+    else:
+        y = round_aspect(x / aspect, key=lambda n: 0 if n == 0 else abs(aspect - x / n))
+    cur_h, cur_w = H, W
+    if reducing_gap is not None and not exif_orientation:
+        dh, dw = int(h * reducing_gap), int(w * reducing_gap)
+        k = draft_scale(data, (dh, dw))
+        out["draft"] = (dh, dw)
+        cur_h, cur_w = (H + k - 1) // k, (W + k - 1) // k
+        out["box"] = (0.0, 0.0, W / k, H / k)
+    if (cur_w, cur_h) != (x, y):
+        out["resize"] = (y, x)
+    else:
+        out["box"] = None
+    return out
+
+
+def fit_args(data, size, bleed=0.0, centering=(0.5, 0.5), exif_orientation=False):
+    """The BatchDecoder entries of one codestream for ImageOps.fit(im, (w, h), bleed=bleed, centering=centering) of the image the
+    batch writes without a size (Image.open(f), or its exif_transpose with exif_orientation=True), as a dict of "resize" and "box":
+    Pillow's own box arithmetic, including its fallbacks (a centering outside [0, 1] is 0.5, a bleed outside [0, 0.5) is 0). The
+    batch takes resample="bicubic" (fit's default method) and no reducing_gap. size = (h, w). Host only; raises ValueError,
+    NativeError where parse() does."""
+    h, w = _hw(size, "size")
+    H, W = output_size(data, exif_orientation=exif_orientation)
+    cx, cy = centering
+    if not 0.0 <= cx <= 1.0:
+        cx = 0.5
+    if not 0.0 <= cy <= 1.0:
+        cy = 0.5
+    if not 0.0 <= bleed < 0.5:
+        bleed = 0.0
+    bx, by = bleed * W, bleed * H
+    lw, lh = W - bx * 2, H - by * 2
+    live_ratio, out_ratio = lw / lh, w / h
+    if live_ratio == out_ratio:
+        cw, ch = lw, lh
+    elif live_ratio >= out_ratio:
+        cw, ch = out_ratio * lh, lh
+    else:
+        cw, ch = lw, lw / out_ratio
+    left, top = bx + (lw - cw) * cx, by + (lh - ch) * cy
+    return {"resize": (h, w), "box": (left, top, left + cw, top + ch)}
+
+
+def resize_center_crop_args(data, resize, crop, exif_orientation=False):
+    """The BatchDecoder entries of one codestream for torchvision's Resize(resize) then CenterCrop(crop) on the PIL image the batch
+    writes without a size, as a dict of "resize" and "window". resize is an int (the shorter side: the longer becomes
+    int(resize * long / short)) or (h, w); crop an int or (h, w). The window is at (int(round((W_r - w) / 2)), int(round((H_r - h)
+    / 2))) of the resized W_r x H_r image, Python's round. The batch takes resample="bilinear" (Resize's default) and no
+    reducing_gap. A crop larger than the resized image raises ValueError: torchvision pads there. Host only; NativeError where
+    parse() does."""
+    import numbers
+    H, W = output_size(data, exif_orientation=exif_orientation)
+    if isinstance(resize, numbers.Integral) and not isinstance(resize, bool):
+        if resize < 1:
+            raise ValueError("resize must be positive, got %r" % (resize,))
+        short, long = (W, H) if W <= H else (H, W)
+        new_short, new_long = int(resize), int(resize * long / short)
+        rw, rh = (new_short, new_long) if W <= H else (new_long, new_short)
+    else:
+        rh, rw = _hw(resize, "resize")
+    if isinstance(crop, numbers.Integral) and not isinstance(crop, bool):
+        crop = (crop, crop)
+    ch, cw = _hw(crop, "crop")
+    if ch > rh or cw > rw:
+        raise ValueError("crop %d x %d is larger than the resized %d x %d image (torchvision pads there)" % (ch, cw, rh, rw))
+    top, left = int(round((rh - ch) / 2.0)), int(round((rw - cw) / 2.0))
+    return {"resize": (rh, rw), "window": (left, top, cw, ch)}
+
+
+def crop_table(crop, n, name="crop"):
+    """The b200jpg_rect table of BatchDecoder(crop=...) (or of `name`=..., window): n entries, each None (the whole frame) or (x, y,
+    width, height) as non-negative integers. Raises ValueError; the rectangles themselves are checked against the frames by the
+    batch."""
     import numbers
     if len(crop) != n:
-        raise ValueError("crop: %d rectangles for %d frames" % (len(crop), n))
+        raise ValueError("%s: %d rectangles for %d frames" % (name, len(crop), n))
     table = (native.RectStruct * n)()
     for i, r in enumerate(crop):
         if r is None:
             continue
         vals = tuple(r)
         if len(vals) != 4 or any(isinstance(v, bool) or not isinstance(v, numbers.Integral) for v in vals):
-            raise ValueError("crop[%d]: expected None or four integers (x, y, width, height), got %r" % (i, r))
+            raise ValueError("%s[%d]: expected None or four integers (x, y, width, height), got %r" % (name, i, r))
         if any(v < 0 or v > 0xFFFFFFFF for v in vals):
-            raise ValueError("crop[%d]: x, y, width and height must be 0 .. 2**32 - 1, got %r" % (i, vals))
+            raise ValueError("%s[%d]: x, y, width and height must be 0 .. 2**32 - 1, got %r" % (name, i, vals))
         table[i].x, table[i].y, table[i].width, table[i].height = (int(v) for v in vals)
     return table
 
@@ -168,6 +273,39 @@ def resize_table(resize, n, name="resize"):
             raise ValueError("%s[%d]: exactly one of h and w is zero: %r" % (name, i, hw))
         table[i].height, table[i].width = int(hw[0]), int(hw[1])
     return table
+
+
+def box_table(box, n):
+    """The b200jpg_box table of BatchDecoder(box=...): n entries, each None (the default box) or (x0, y0, x1, y1) as finite real
+    numbers, Pillow's Image.resize(box=...) order. Raises ValueError; the boxes themselves are checked against the frames by the
+    batch."""
+    import math
+    import numbers
+    if len(box) != n:
+        raise ValueError("box: %d boxes for %d frames" % (len(box), n))
+    table = (native.BoxStruct * n)()
+    for i, b in enumerate(box):
+        if b is None:
+            continue
+        vals = tuple(b) if isinstance(b, (tuple, list)) else None
+        if vals is None or len(vals) != 4 or any(isinstance(v, bool) or not isinstance(v, numbers.Real) for v in vals):
+            raise ValueError("box[%d]: expected None or four numbers (x0, y0, x1, y1), got %r" % (i, b))
+        if not all(math.isfinite(v) for v in vals):
+            raise ValueError("box[%d]: every coordinate must be finite, got %r" % (i, vals))
+        if vals[0] < 0 or vals[1] < 0 or vals[2] < vals[0] or vals[3] < vals[1]:
+            raise ValueError("box[%d]: expected 0 <= x0 <= x1 and 0 <= y0 <= y1, got %r" % (i, vals))
+        table[i].x0, table[i].y0, table[i].x1, table[i].y1 = (float(v) for v in vals)
+    return table
+
+
+def reducing_gap_value(gap):
+    """The reducing_gap of b200jpg_batch_create_resample: 0.0 for None, else a real number of at least 1.0. Raises ValueError."""
+    import numbers
+    if gap is None:
+        return 0.0
+    if isinstance(gap, bool) or not isinstance(gap, numbers.Real) or not gap >= 1.0:
+        raise ValueError("reducing_gap must be None or a number >= 1.0, got %r" % (gap,))
+    return float(gap)
 
 
 def resample_filter(name):
@@ -362,7 +500,8 @@ class BatchDecoder:
     """One batch of codestreams: parse + pack on construction, then upload() / decode() on a CUDA stream."""
 
     def __init__(self, frames, device=-1, tolerate_bad=False, ctx=None, color_transform=True, upsample=True, downscale=1,
-                 exif_orientation=False, crop=None, resize=None, resample="bilinear", mode=None, reconstruction="reference", draft=None):
+                 exif_orientation=False, crop=None, resize=None, resample="bilinear", mode=None, reconstruction="reference", draft=None,
+                 box=None, reducing_gap=None, window=None):
         """downscale = 2, 4 or 8 decodes every frame at ceil(W / k) x ceil(H / k) (B200JPG_FLAG_DOWNSCALE_k): each 8x8 block is
         inverse transformed straight to (8/k) x (8/k) samples, the k x k box average of its IDCT, and the rest of the
         reconstruction runs on the smaller frame. geometry(), frame_view() and plane_views() give the reduced sizes. Not to be
@@ -425,7 +564,21 @@ class BatchDecoder:
         rectangles are given in output_size(data, downscale=k, exif_orientation=...). A frame whose k is 1 is decoded
         exactly as without a draft; status(i) is unchanged. A draft needs reconstruction="libjpeg-turbo" (else NativeError,
         B200JPG_ERR_NOT_IMPLEMENTED); a wrong length, an entry that is not two non-negative integers or exactly one zero in an
-        entry raises ValueError."""
+        entry raises ValueError.
+
+        box, reducing_gap and window (b200jpg_batch_create_resample, DESIGN §19) are the rest of Pillow's Image.resize, for frames
+        with a `resize` entry. box is one entry per frame: None, or Pillow's (x0, y0, x1, y1) in floats, in the coordinates of the
+        image the resize takes (after draft, downscaling, Exif orientation and the crop). reducing_gap is None or a number >= 1.0
+        for the whole batch, Pillow's reducing_gap: Image.reduce() runs first when the box is at least twice `gap` times the
+        target. window is one entry per frame: None, or (x, y, width, height) -- the order of `crop` -- a rectangle of the resized
+        h x w image. The frame is then written as, byte for byte,
+            Image.fromarray(C).resize((w, h), filter, box=box, reducing_gap=gap).crop((x, y, x + width, y + height))
+        of its image C without the size, and output_shape() and the destinations of decode_into() are the window's (height, width),
+        so a Resize(256) + CenterCrop(224) batch fills one [N, 3, 224, 224] tensor. Only the part of C the resize reads is
+        reconstructed. thumbnail_args(), fit_args() and resize_center_crop_args() give the entries of Pillow's thumbnail(),
+        ImageOps.fit() and torchvision's Resize + CenterCrop. A box or window on a frame without a size, a box outside C, a window
+        outside h x w, or a reduce box that is empty raises NativeError (B200JPG_ERR_INVALID_PARAMETER); a wrong length, an entry
+        of the wrong form, a box that is not finite or has x1 < x0 or y1 < y0 and a reducing_gap below 1.0 raise ValueError."""
         if not isinstance(mode, (str, type(None))) or mode not in native.MODE_FLAGS:
             raise ValueError('mode must be None, "RGB" or "L", got %r' % (mode,))
         if not isinstance(reconstruction, str) or reconstruction not in native.RECONSTRUCTION_FLAGS:
@@ -435,6 +588,9 @@ class BatchDecoder:
         rects = None if crop is None else crop_table(crop, len(frames))
         sizes = None if resize is None else resize_table(resize, len(frames))
         drafts = None if draft is None else resize_table(draft, len(frames), "draft")
+        boxes = None if box is None else box_table(box, len(frames))
+        windows = None if window is None else crop_table(window, len(frames), "window")
+        gap = reducing_gap_value(reducing_gap)
         filt = resample_filter(resample)
         self.ctx = ctx or Context(device)
         self._keep = []
@@ -460,7 +616,10 @@ class BatchDecoder:
         flags |= native.MODE_FLAGS[mode]
         self.reconstruction = reconstruction
         flags |= native.RECONSTRUCTION_FLAGS[reconstruction]
-        if drafts is None:
+        if boxes is not None or windows is not None or gap > 0.0:
+            rc = lib.b200jpg_batch_create_resample(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, drafts, rects, sizes, boxes,
+                                                   windows, filt, gap, ctypes.byref(self.handle))
+        elif drafts is None:
             rc = lib.b200jpg_batch_create_resize(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, rects, sizes, filt, ctypes.byref(self.handle))
         else:
             rc = lib.b200jpg_batch_create_draft(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, drafts, rects, sizes, filt,

@@ -46,6 +46,11 @@ class SizeStruct(ctypes.Structure):
     _fields_ = [("width", ctypes.c_uint32), ("height", ctypes.c_uint32)]
 
 
+class BoxStruct(ctypes.Structure):
+    """b200jpg_box: a source box of b200jpg_batch_create_resample, Pillow's (x0, y0, x1, y1); all zero = the default box."""
+    _fields_ = [("x0", ctypes.c_double), ("y0", ctypes.c_double), ("x1", ctypes.c_double), ("y1", ctypes.c_double)]
+
+
 SAMPLE_F32, SAMPLE_F16, SAMPLE_BF16 = 1, 2, 3
 FLAG_NO_COLOR_TRANSFORM, FLAG_NO_UPSAMPLE = 1, 2
 DOWNSCALE_FLAGS = {1: 0x0, 2: 0x4, 4: 0x8, 8: 0xC}  # B200JPG_FLAG_DOWNSCALE_k
@@ -86,8 +91,14 @@ def _load():
         "b200jpg_batch_create_draft": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.c_uint,
                                              ctypes.POINTER(SizeStruct), ctypes.POINTER(RectStruct), ctypes.POINTER(SizeStruct), i32,
                                              ctypes.POINTER(vp)]),
+        "b200jpg_batch_create_resample": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.c_uint,
+                                                ctypes.POINTER(SizeStruct), ctypes.POINTER(RectStruct), ctypes.POINTER(SizeStruct),
+                                                ctypes.POINTER(BoxStruct), ctypes.POINTER(RectStruct), i32, ctypes.c_double,
+                                                ctypes.POINTER(vp)]),
         "b200jpg_draft_scale": (i32, [vp, ctypes.c_size_t, ctypes.c_uint32, ctypes.c_uint32]),
         "b200jpg_resample_coefficients": (i32, [ctypes.c_uint32, ctypes.c_uint32, i32, vp, vp, u64, ctypes.POINTER(ctypes.c_uint32)]),
+        "b200jpg_resample_coefficients_box": (i32, [ctypes.c_uint32, ctypes.c_float, ctypes.c_float, ctypes.c_uint32, i32, vp, vp, u64,
+                                                    ctypes.POINTER(ctypes.c_uint32)]),
         "b200jpg_batch_destroy": (None, [vp]),
         "b200jpg_batch_frame_info": (i32, [vp, i32, ctypes.POINTER(FrameInfoStruct)]),
         "b200jpg_batch_output_extent": (i32, [vp, i32, i32, ctypes.POINTER(ctypes.c_uint32), ctypes.POINTER(ctypes.c_uint32)]),
@@ -144,6 +155,7 @@ ABI_SYMBOLS = [
     "b200jpg_selftest_table_cache", "b200jpg_microbench_int32", "b200jpg_exif_orientation", "b200jpg_batch_frame_orientation",
     "b200jpg_batch_create_crop", "b200jpg_output_size", "b200jpg_batch_create_resize", "b200jpg_resample_coefficients",
     "b200jpg_batch_output_components", "b200jpg_colorspace", "b200jpg_batch_create_draft", "b200jpg_draft_scale",
+    "b200jpg_batch_create_resample", "b200jpg_resample_coefficients_box",
 ]
 
 
