@@ -18,6 +18,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <tuple>
 #include <type_traits>
 #include <vector>
 
@@ -132,16 +133,25 @@ struct ScanClass {
     uint64_t dev_scans = 0, dev_intervals = 0, dev_interval_end = 0, dev_clean_off = 0;
 };
 
-struct ReconGroup {
+// What the frames of one reconstruction group share: component count, chroma factors and path, and the parts of their plans that
+// change the launches or the store kind
+struct GroupKey {
     uint32_t ncomp = 0, subx = 1, suby = 1;
     ReconPath path = ReconPath::Tiled;
     int orientation = 1;  // B200JPG_FLAG_EXIF_ORIENTATION: the frames' orientation; 2..8 store through rewritten descriptors
-    bool cropped = false; // b200jpg_batch_create_crop: the frames' tiles cover their rectangles, clipped stores (FrameRecon::clip_*)
-    bool resized = false; // b200jpg_batch_create_resize: cropped frames stored as uint8 into the scratch, never converted
-    OutMode mode = OutMode::Coded;  // B200JPG_FLAG_OUTPUT_RGB / _L: the frames' slots are described (rewritten descriptors)
+    bool cropped = false; // the frames' tiles cover their rectangles, clipped stores (FrameRecon::clip_*)
+    bool resized = false; // cropped frames stored as uint8 into the scratch, never converted
+    bool described = false;  // the frames store through rewritten descriptors (FramePlan::described)
+    OutMode mode = OutMode::Coded;  // B200JPG_FLAG_OUTPUT_RGB / _L
+    uint32_t scale = 1;   // the frames' factor k (ReconLaunch::downscale)
+    auto fields() const { return std::tie(ncomp, subx, suby, path, orientation, cropped, resized, described, mode, scale); }
+    bool operator==(const GroupKey &o) const { return fields() == o.fields(); }
+};
+
+struct ReconGroup {
+    GroupKey key;
     std::vector<FrameRecon> frames;
     uint32_t max_bw0 = 0, max_bh0 = 0, max_bwc = 0, max_bhc = 0;
-    uint32_t scale = 1;   // the frames' factor k (b200jpg_batch::scale)
     uint64_t dev_frames = 0;
 };
 
@@ -204,19 +214,50 @@ Ratio draft_ratio(const b200jpg_frame_info &fi, int c, uint32_t k) {
     return {hmax * (8 / k) / (fi.hs[c] * s), vmax * (8 / k) / (fi.vs[c] * s)};
 }
 
-// component c as it leaves the decoder, decoded at scale 1/k (B200JPG_FLAG_DOWNSCALE_k or the frame's draft: b200jpg_batch::scale):
-// the frame size W' x H' = ceil(W / k) x ceil(H / k), or without upsampling its own ceil(W' / subx) x ceil(H' / suby); width and
-// height swapped for the Exif orientations 5..8 (`orientation`: the one the frame leaves with, 1 for the extent the kernels decode);
-// the rectangle's size for a frame with a crop (`crop`, given in those output coordinates and checked against them; never together
-// with B200JPG_FLAG_NO_UPSAMPLE); the target size of a resized frame (`size`)
-Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags, uint64_t k, int orientation, const b200jpg_rect *crop = nullptr,
-                  const b200jpg_size *size = nullptr) {
-    if (size) return {size->width, size->height};
-    if (crop) return {crop->width, crop->height};
+// What live frame i of a batch is asked for and how it is decoded (b200jpg_batch::plan), filled once by the planning steps of
+// batch_create_impl and read by every later step and both decode calls. A JPEG XT residual codestream's record is its frame's, with
+// its own ncomp (parse_residual checks that they agree), so that the two stay in one reconstruction group.
+struct FramePlan {
+    // frame_plan (B200JPG_FLAG_OUTPUT_RGB / _L, DESIGN §14): the path, the components the reconstruction covers and the components the
+    // frame leaves with. Without a mode bit: recon_path and the frame's own components.
+    ReconPath path = ReconPath::Tiled;
+    uint32_t ncomp = 0;      // components reconstructed, from component 0 on
+    uint32_t out_ncomp = 0;  // components written
+    OutMode mode = OutMode::Coded;
+    uint32_t k = 1;          // decoded at 1/k: B200JPG_FLAG_DOWNSCALE_k, or the frame's draft (admit_drafts)
+    int orientation = 1;     // the Exif orientation the frame leaves with: its own with B200JPG_FLAG_EXIF_ORIENTATION, else 1
+    // admit_crops: C, a rectangle of the oriented output at 1/k -- the caller's, or the whole output for a resized frame and under
+    // B200JPG_FLAG_LIBJPEG_TURBO -- trimmed by plan_resample to the part the resize reads
+    bool cropped = false;
+    b200jpg_rect crop{};
+    // admit_sizes / admit_boxes (DESIGN §19): the target W_t x H_t, Pillow's source box and the window ({0, ..}: the defaults); the
+    // frame leaves with the window's extent, or the target's; rs: its index into b200jpg_batch::rs_frames (plan_resample)
+    bool resized = false;
+    b200jpg_size target{};
+    b200jpg_box box{};
+    b200jpg_rect window{};
+    int rs = -1;
+    // oriented, cropped (so resized) or written in an output mode: the reconstruction stores through the frame's destinations
+    // rewritten into decoded coordinates (rewrite_frame), in place of the packed slot it takes otherwise
+    bool described = false;
+};
+
+// component c as it leaves the decoder, decoded at scale 1/k: the frame size W' x H' = ceil(W / k) x ceil(H / k), or without
+// upsampling its own ceil(W' / subx) x ceil(H' / suby) -- the extent the kernels decode
+Extent decoded_extent(const b200jpg_frame_info &fi, int c, unsigned flags, uint64_t k) {
     uint64_t w = (fi.width + k - 1) / k, h = (fi.height + k - 1) / k;
     if (flags & B200JPG_FLAG_NO_UPSAMPLE) w = (w + fi.subx[c] - 1) / fi.subx[c], h = (h + fi.suby[c] - 1) / fi.suby[c];
-    if (orientation >= 5) return {h, w};
     return {w, h};
+}
+
+// ... and as the frame of plan p leaves: width and height swapped for the Exif orientations 5..8; the size of C for a cropped frame
+// (C is given in those output coordinates and checked against them; never together with B200JPG_FLAG_NO_UPSAMPLE); the window's or
+// the target's size for a resized one
+Extent out_extent(const b200jpg_frame_info &fi, int c, unsigned flags, const FramePlan &p) {
+    if (p.resized) return rect_empty(p.window) ? Extent{p.target.width, p.target.height} : Extent{p.window.width, p.window.height};
+    if (p.cropped) return {p.crop.width, p.crop.height};
+    const Extent e = decoded_extent(fi, c, flags, p.k);
+    return p.orientation >= 5 ? Extent{e.h, e.w} : e;
 }
 
 // A destination described in output coordinates (data d, pixel stride p, row stride r) as seen from the decoded coordinates
@@ -291,10 +332,10 @@ struct b200jpg_batch {
     unsigned flags = 0;  // B200JPG_FLAG_*
     std::vector<ParsedFrame> frames;
     std::vector<int> parse_status;
-    // [n] the factor k every frame is decoded at, 1/k: B200JPG_FLAG_DOWNSCALE_k, or a live frame's draft (admit_drafts). Every
-    // extent, plane layout and path decision of a frame reads it here
-    std::vector<uint32_t> scale;
-    int n_user = 0;                       // frames of the caller; [n_user, n) are residual codestreams of JPEG XT frames
+    // [n] every live frame's request and plan (FramePlan): every extent, plane layout, path and store decision of a frame reads it
+    // here -- its factor k included (DESIGN §17)
+    std::vector<FramePlan> plan;
+    int n_user = 0;                      // frames of the caller; [n_user, n) are residual codestreams of JPEG XT frames
     std::vector<int> xt_child, xt_parent;  // [n_user] index of a frame's residual frame or -1; [n] the reverse
     std::vector<uint64_t> out_off, out_bytes;
     uint64_t out_total = 0;
@@ -349,23 +390,15 @@ struct b200jpg_batch {
     b200jpg_plane *h_planes = nullptr, *d_planes = nullptr;
     cudaEvent_t ev_planes[kPlaneSlots] = {};
     int plane_slot = 0;
-    // some live frame leaves with an Exif orientation other than 1 or with a crop: its group stores through rewritten descriptors
+    // some live frame is described (FramePlan::described): its group stores through rewritten descriptors
     bool rewritten = false;
-    std::vector<b200jpg_rect> crop;  // [n_user] b200jpg_batch_create_crop's rectangles, {0, 0, 0, 0}: the whole frame
-    // b200jpg_batch_create_resize: [n_user] target sizes ({0, 0}: not resized) and the filter; per resized frame its resample
-    // descriptor, its caller frame and its tables (h bounds, h coefficients, v bounds, v coefficients). The descriptor table of
-    // a decode holds 4 * (n + resized frames) entries: the destinations of resized frame r at 4 * (n + r)
-    std::vector<b200jpg_size> size;
+    // resized frames: the filter and the reducing_gap (<= 0: None) of the batch; per resized frame its resample descriptor and its
+    // tables (h bounds, h coefficients, v bounds, v coefficients). The descriptor table of a decode holds 4 * (n + resized frames)
+    // entries: the destinations of resized frame r at 4 * (n + r)
     int resample = 0;
-    // b200jpg_batch_create_resample (DESIGN §19): [n_user] the target sizes W_t x H_t (`size` holds the window's extent then), the
-    // source boxes and the windows ({0, ..}: the defaults), and the reducing_gap (<= 0: None)
-    std::vector<b200jpg_size> target;
-    std::vector<b200jpg_box> box;
-    std::vector<b200jpg_rect> window;
     double gap = 0.0;
     std::vector<ResampleFrame> rs_frames;
-    std::vector<int> rs_user, rs_index;  // [resized] caller frame; [n_user] index into rs_frames or -1
-    uint32_t rs_plain = 0;  // resized frames [rs_plain, ..) are grey frames of B200JPG_FLAG_OUTPUT_RGB (ResampleLaunch::n_plain)
+    uint32_t rs_plain = 0; // resized frames [rs_plain, ..) are grey frames of B200JPG_FLAG_OUTPUT_RGB (ResampleLaunch::n_plain)
     std::vector<std::array<std::vector<int32_t>, 4>> rs_tables;
     uint64_t dev_rs_frames = 0;
     uint32_t rs_max_rows = 0, rs_max_reduce_rows = 0;
@@ -377,27 +410,6 @@ struct b200jpg_batch {
     bool timing = false;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // start, after a0, after a1, after b
 };
-
-// the Exif orientation frame i leaves the decoder with: its own (a JPEG XT residual codestream: its frame's, so that the two stay
-// in one reconstruction group) with B200JPG_FLAG_EXIF_ORIENTATION, else 1
-static int applied_orientation(const b200jpg_batch &b, int i) {
-    if (!(b.flags & B200JPG_FLAG_EXIF_ORIENTATION)) return 1;
-    return b.frames[b.xt_parent[i] >= 0 ? b.xt_parent[i] : i].orientation;
-}
-
-// the rectangle of the output frame i leaves as (a JPEG XT residual codestream: its frame's), nullptr for the whole frame
-static const b200jpg_rect *crop_of(const b200jpg_batch &b, int i) {
-    const int u = b.xt_parent[i] >= 0 ? b.xt_parent[i] : i;
-    if (b.crop.empty() || u >= b.n_user || rect_empty(b.crop[u])) return nullptr;
-    return &b.crop[u];
-}
-
-// the target size of frame i (a JPEG XT residual codestream: its frame's), nullptr for a frame that is not resized
-static const b200jpg_size *size_of(const b200jpg_batch &b, int i) {
-    const int u = b.xt_parent[i] >= 0 ? b.xt_parent[i] : i;
-    if (b.size.empty() || u >= b.n_user || size_empty(b.size[u])) return nullptr;
-    return &b.size[u];
-}
 
 extern "C" {
 
@@ -507,8 +519,10 @@ int b200jpg_output_size(const uint8_t *data, size_t len, unsigned flags, uint32_
     ParsedFrame pf;
     const int rc = parse_one(data, len, pf);
     if (rc != 0) return rc;
-    const Extent e = out_extent(pf.info, 0, flags & ~B200JPG_FLAG_NO_UPSAMPLE, downscale_of(flags),
-                                (flags & B200JPG_FLAG_EXIF_ORIENTATION) ? pf.orientation : 1);
+    FramePlan p;
+    p.k = downscale_of(flags);
+    p.orientation = (flags & B200JPG_FLAG_EXIF_ORIENTATION) ? pf.orientation : 1;
+    const Extent e = out_extent(pf.info, 0, flags & ~B200JPG_FLAG_NO_UPSAMPLE, p);
     *width = (uint32_t)e.w;
     *height = (uint32_t)e.h;
     return B200JPG_OK;
@@ -690,7 +704,7 @@ static void attach_residuals(b200jpg_batch &b, Codestreams &cs, bool device_inde
     const int n_user = b.n_user;
     b.xt_child.assign(n_user, -1);
     for (int i = 0; i < n_user; i++) {
-        if (b.parse_status[i] == 0 && !b.size.empty() && !size_empty(b.size[i]) && b.frames[i].info.precision != 8) {
+        if (b.parse_status[i] == 0 && !size_empty(b.plan[i].target) && b.frames[i].info.precision != 8) {
             b.parse_status[i] = B200JPG_ERR_NOT_IMPLEMENTED;  // never written unresized
             cs.err[i] = "only 8-bit frames are resized";
             continue;
@@ -738,6 +752,7 @@ static void attach_residuals(b200jpg_batch &b, Codestreams &cs, bool device_inde
     for (int i = 0; i < n_user; i++)  // push_back may have moved the frames: take the addresses again
         if (b.xt_child[i] >= 0) cs.data[b.xt_child[i]] = b.frames[i].xt.resi.data();
     b.n = (int)b.frames.size();
+    b.plan.resize(b.n);
     b.xt_parent.assign(b.n, -1);
     for (int i = 0; i < n_user; i++)
         if (b.xt_child[i] >= 0) b.xt_parent[b.xt_child[i]] = i;
@@ -849,8 +864,8 @@ static ReconPath turbo_path(const b200jpg_frame_info &fi, int ncomp, uint32_t k)
 
 static ReconPath recon_path(const b200jpg_batch &b, int i) {
     const b200jpg_frame_info &fi = b.frames[i].info;
-    const bool scaled = b.scale[i] > 1;
-    if (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) return turbo_path(fi, fi.ncomp, b.scale[i]);
+    const bool scaled = b.plan[i].k > 1;
+    if (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) return turbo_path(fi, fi.ncomp, b.plan[i].k);
     if (b.xt_parent[i] >= 0 || (i < b.n_user && b.xt_child[i] >= 0)) return ReconPath::Generic;
     if (b.flags & B200JPG_FLAG_NO_UPSAMPLE) return scaled ? ReconPath::Scaled : ReconPath::Generic;  // planes of every component, then one sample -> one output value
     if (fi.precision != 8) return scaled ? ReconPath::Scaled : ReconPath::Generic;  // 12-bit frames: int32 planes, 16-bit samples out
@@ -861,38 +876,26 @@ static ReconPath recon_path(const b200jpg_batch &b, int i) {
     return scaled ? ReconPath::Scaled : ReconPath::Tiled;
 }
 
-// What live frame i reconstructs and what it writes (B200JPG_FLAG_OUTPUT_RGB / _L, DESIGN §14): the path, the components the
-// reconstruction covers and the components the frame leaves with. Without a mode bit: recon_path and the frame's own components.
-struct FramePlan {
-    ReconPath path;
-    uint32_t ncomp;      // components reconstructed, from component 0 on
-    uint32_t out_ncomp;  // components written
-    OutMode mode;
-};
-
-static FramePlan frame_plan(const b200jpg_batch &b, int i) {
-    if (b.xt_parent[i] >= 0) {  // a JPEG XT residual codestream stays in its frame's group: the frame's plan
-        FramePlan p = frame_plan(b, b.xt_parent[i]);
-        p.ncomp = b.frames[i].info.ncomp;  // (the frame's own: parse_residual checks that they agree)
-        return p;
-    }
+// The plan of the caller's live frame i as far as its factor k decides it (right after admit_drafts): the path, the components,
+// the output mode and the orientation; the admission steps add the request
+static void frame_plan(b200jpg_batch &b, int i) {
     const b200jpg_frame_info &fi = b.frames[i].info;
-    FramePlan p{recon_path(b, i), fi.ncomp, fi.ncomp, OutMode::Coded};
-    const bool xt = i < b.n_user && b.xt_child[i] >= 0;
+    FramePlan &p = b.plan[i];
+    p.path = recon_path(b, i);
+    p.ncomp = p.out_ncomp = fi.ncomp;
+    p.orientation = (b.flags & B200JPG_FLAG_EXIF_ORIENTATION) ? b.frames[i].orientation : 1;
+    const bool xt = b.xt_child[i] >= 0;
     if ((b.flags & B200JPG_FLAG_OUTPUT_L) && fi.ncomp == 3) {
         p.out_ncomp = 1;
         if (fi.ycbcr && !xt) {
             // luma alone: a grey frame over component 0 on the MCU-padded block grid; libjpeg's JCS_GRAYSCALE for YCbCr input
             p.ncomp = 1;
-            if (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) {  // the turbo kernels over component 0
-                p.path = turbo_path(fi, 1, b.scale[i]);
-                return p;
-            }
-            if (b.scale[i] > 1) p.path = ReconPath::Scaled;
+            if (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) p.path = turbo_path(fi, 1, p.k);  // the turbo kernels over component 0
+            else if (p.k > 1) p.path = ReconPath::Scaled;
             else p.path = (fi.precision != 8 || fi.subx[0] != 1 || fi.suby[0] != 1) ? ReconPath::Generic : ReconPath::Tiled;
         } else {  // RGB-coded and JPEG XT frames: the L formula after the colour transformation (merge) and clamp, in the generic kernels
             p.mode = OutMode::Luma;
-            if (!(b.flags & B200JPG_FLAG_LIBJPEG_TURBO)) p.path = b.scale[i] > 1 ? ReconPath::Scaled : ReconPath::Generic;
+            if (!(b.flags & B200JPG_FLAG_LIBJPEG_TURBO)) p.path = p.k > 1 ? ReconPath::Scaled : ReconPath::Generic;
         }
     }
     if ((b.flags & B200JPG_FLAG_OUTPUT_RGB) && fi.ncomp == 1) {
@@ -904,9 +907,9 @@ static FramePlan frame_plan(const b200jpg_batch &b, int i) {
         p.out_ncomp = rgb ? 3 : 1;
         p.mode = rgb ? OutMode::CmykRgb : OutMode::CmykLuma;
         if (b.flags & B200JPG_FLAG_LIBJPEG_TURBO) p.path = ReconPath::TurboGeneric;
-        else p.path = b.scale[i] > 1 ? ReconPath::Scaled : ReconPath::Generic;
+        else p.path = p.k > 1 ? ReconPath::Scaled : ReconPath::Generic;
     }
-    return p;
+    p.described = p.orientation != 1 || p.mode != OutMode::Coded;  // (admit_crops adds the cropped frames)
 }
 
 // Coefficient, sample and output layout of the live frames; returns the sample plane offsets. The sample planes a frame gets
@@ -924,10 +927,10 @@ static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
     for (int i = 0; i < n; i++) {
         if (b.parse_status[i] != 0) continue;
         const b200jpg_frame_info &fi = b.frames[i].info;
-        const FramePlan plan = frame_plan(b, i);
+        const FramePlan &plan = b.plan[i];
         const ReconPath path = plan.path;
         const int first_plane = (path == ReconPath::Generic || path == ReconPath::Scaled || path == ReconPath::TurboGeneric) ? 0 : (path == ReconPath::Tiled ? 1 : fi.ncomp);
-        const uint32_t k = b.scale[i];
+        const uint32_t k = plan.k;
         uint64_t samples = 0;
         for (int c = 0; c < fi.ncomp; c++) {  // every component is entropy decoded; only the reconstructed ones get sample planes
             const uint64_t elems = (uint64_t)fi.blocks_w[c] * fi.blocks_h[c] * 64;
@@ -943,7 +946,7 @@ static std::vector<std::array<uint64_t, 4>> lay_out_planes(b200jpg_batch &b) {
             }
         }
         for (uint32_t c = 0; c < plan.out_ncomp; c++) {
-            const Extent e = out_extent(fi, (int)c, b.flags, k, 1, crop_of(b, i), size_of(b, i));  // the components one after the other (w * h: any orientation)
+            const Extent e = out_extent(fi, (int)c, b.flags, plan);  // the components one after the other
             samples += e.w * e.h;
         }
         b.out_off[i] = out_cur;
@@ -1159,43 +1162,29 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         if (b.parse_status[i] != 0) continue;
         const b200jpg_frame_info &fi = b.frames[i].info;
         const int xt_res = (i < b.n_user) ? b.xt_child[i] : -1;  // JPEG XT: this frame's residual frame
-        const FramePlan plan = frame_plan(b, i);
+        const FramePlan &plan = b.plan[i];
         const ReconPath path = plan.path;
-        const uint32_t nc = plan.ncomp;
+        const uint32_t nc = plan.ncomp, k = plan.k;
         const bool generic = path == ReconPath::Generic || path == ReconPath::Scaled || path == ReconPath::TurboGeneric;
         uint32_t sx = nc > 1 ? fi.subx[1] : 1, sy = nc > 1 ? fi.suby[1] : 1;
-        if (nc > 1 && path == ReconPath::Turbo) sx = draft_ratio(fi, 1, b.scale[i]).x, sy = draft_ratio(fi, 1, b.scale[i]).y;
+        if (nc > 1 && path == ReconPath::Turbo) sx = draft_ratio(fi, 1, k).x, sy = draft_ratio(fi, 1, k).y;
         if (generic) sx = sy = 0;  // one group per component count: the generic kernels read the factors per frame
         // oriented frames (B200JPG_FLAG_EXIF_ORIENTATION, 2..8) form groups of their own, one per orientation: their destinations
-        // are rewritten descriptors, whose store kind is chosen per group
-        const int orientation = applied_orientation(b, i);
-        // cropped frames too: their launches are sized by the tiles the rectangles cover, and they always store clipped
-        const b200jpg_rect *crop = crop_of(b, i);
-        // resized frames too (every one of them is cropped, admit_sizes): they store into the scratch, unconverted
-        const bool resized = size_of(b, i) != nullptr;
-        // and the frames of an output mode, keyed by it, their slots described like those of oriented frames. A resized grey frame
-        // of B200JPG_FLAG_OUTPUT_RGB writes its one channel into the scratch: the resample pass replicates it
-        const OutMode mode = (resized && plan.mode == OutMode::Replicate) ? OutMode::Coded : plan.mode;
-        if (orientation != 1 || crop || plan.mode != OutMode::Coded) b.rewritten = true;
-        // and the frames of one scale: a group's launches take its factor k (ReconLaunch::downscale)
-        const uint32_t k = b.scale[i];
+        // are rewritten descriptors, whose store kind is chosen per group. Cropped frames too: their launches are sized by the tiles
+        // the rectangles cover, and they always store clipped. Resized frames too (every one of them is cropped, admit_crops): they
+        // store into the scratch, unconverted. And the frames of an output mode, keyed by it, and of one scale: a group's launches
+        // take its factor k. A resized grey frame of B200JPG_FLAG_OUTPUT_RGB writes its one channel into the scratch: the resample
+        // pass replicates it
+        const OutMode mode = (plan.resized && plan.mode == OutMode::Replicate) ? OutMode::Coded : plan.mode;
+        const GroupKey key{nc, sx, sy, path, plan.orientation, plan.cropped, plan.resized, plan.described, mode, k};
+        b.rewritten = b.rewritten || plan.described;
         ReconGroup *g = nullptr;
         for (auto &gg : b.groups)
-            if (gg.ncomp == nc && gg.subx == sx && gg.suby == sy && gg.path == path && gg.orientation == orientation && gg.cropped == (crop != nullptr) &&
-                gg.resized == resized && gg.mode == mode && gg.scale == k)
-                g = &gg;
+            if (gg.key == key) g = &gg;
         if (!g) {
             b.groups.emplace_back();
             g = &b.groups.back();
-            g->ncomp = nc;
-            g->mode = mode;
-            g->subx = sx;
-            g->suby = sy;
-            g->path = path;
-            g->orientation = orientation;
-            g->cropped = crop != nullptr;
-            g->resized = resized;
-            g->scale = k;
+            g->key = key;
         }
         FrameRecon fr{};
         const bool drafted = k > 1 && (path == ReconPath::TurboGeneric || path == ReconPath::Turbo);
@@ -1224,7 +1213,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         }
         fr.fancy = k < 8;  // libjpeg-turbo upsamples by replication at 1/8 (min_DCT_scaled_size == 1)
         fr.out_base = b.out_off[i];
-        const Extent reduced = out_extent(fi, 0, b.flags & ~B200JPG_FLAG_NO_UPSAMPLE, k, 1);  // W' x H' (the full size at k = 1)
+        const Extent reduced = decoded_extent(fi, 0, b.flags & ~B200JPG_FLAG_NO_UPSAMPLE, k);  // W' x H' (the full size at k = 1)
         fr.width = (uint32_t)reduced.w;
         fr.height = (uint32_t)reduced.h;
         if (b.xt_parent[i] >= 0) fr.width = fr.height = 0;  // a residual codestream: planes only, its frame's reconstruction reads them
@@ -1248,10 +1237,10 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         fr.ch = (uint32_t)(sy ? (reduced.h + sy - 1) / sy : reduced.h);
         fr.status_idx = (uint32_t)i;
         fr.precision = fi.precision;
-        if (crop) {
+        if (plan.cropped) {
             // the tiles of the path that cover the clip rectangle, from tile (tx0, ty0) on; the launch grid is sized by the largest
             // such range of the group and every CTA runs tile (tx0 + bx, ty0 + by) exactly as the uncropped decode does
-            const Clip cl = crop_to_decoded(orientation, *crop, reduced.w, reduced.h);
+            const Clip cl = crop_to_decoded(plan.orientation, plan.crop, reduced.w, reduced.h);
             const ReconTile t = recon_tile(path);
             const uint32_t bpx = (drafted && path == ReconPath::Turbo) ? 8 / k : 8;  // output pixels per tile block: a drafted luma block's
             const uint32_t tw = bpx * t.bw, th = bpx * t.bh;
@@ -1286,7 +1275,7 @@ static void form_recon_groups(b200jpg_batch &b, const std::vector<std::array<uin
         if (generic) {  // the largest block grid of any component: the extent of the generic (or scaled) IDCT launch
             for (uint32_t c = 0; c < nc; c++)
                 if ((uint64_t)fi.blocks_w[c] * fi.blocks_h[c] > (uint64_t)g->max_bwc * g->max_bhc) g->max_bwc = fi.blocks_w[c], g->max_bhc = fi.blocks_h[c];
-        } else if (nc > 1 && !crop) {  // (a cropped Tiled frame: its chroma block range above)
+        } else if (nc > 1 && !plan.cropped) {  // (a cropped Tiled frame: its chroma block range above)
             g->max_bwc = std::max(g->max_bwc, fi.blocks_w[1]);
             g->max_bhc = std::max(g->max_bhc, fi.blocks_h[1]);
         }
@@ -1414,65 +1403,49 @@ static int stage_and_allocate(b200jpg_batch &b, const Codestreams &cs, const std
     return B200JPG_OK;
 }
 
-// b200jpg_batch_create_crop's rectangles: kept for the live frames (a failed frame's is ignored), each checked against the frame's
-// uncropped output extent; returns 0 or the status the call fails with
+// The live frames' rectangles C (a failed frame's request is ignored): b200jpg_batch_create_crop's (nullptr: none), each checked
+// against the frame's uncropped output extent, else the whole output for a frame with a target size, so that the reconstruction
+// writes C through the cropped path, and for every frame under B200JPG_FLAG_LIBJPEG_TURBO, so that turbo_generic_kernel needs only
+// the clipped strided store kinds, whatever the destination. A cropped frame is described. Returns 0 or the status the call fails with.
 static int admit_crops(b200jpg_batch &b, const b200jpg_rect *rects) {
-    b.crop.assign(rects, rects + b.n_user);
     for (int i = 0; i < b.n_user; i++) {
-        b200jpg_rect &r = b.crop[i];
-        if (b.parse_status[i] != 0) r = b200jpg_rect{0, 0, 0, 0};
-        if (rect_empty(r)) continue;
-        const Extent e = out_extent(b.frames[i].info, 0, b.flags, b.scale[i], applied_orientation(b, i));
+        FramePlan &p = b.plan[i];
+        b200jpg_rect r = rects ? rects[i] : b200jpg_rect{0, 0, 0, 0};
+        const bool whole = !size_empty(p.target) || (b.flags & B200JPG_FLAG_LIBJPEG_TURBO);
+        if (b.parse_status[i] != 0 || (rect_empty(r) && !whole)) continue;
+        const Extent e = out_extent(b.frames[i].info, 0, b.flags, p);
+        if (rect_empty(r)) r = b200jpg_rect{0, 0, (uint32_t)e.w, (uint32_t)e.h};
         if (r.width == 0 || r.height == 0 || (uint64_t)r.x + r.width > e.w || (uint64_t)r.y + r.height > e.h)
             return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": crop rectangle (" + std::to_string(r.x) + ", " +
                                                                   std::to_string(r.y) + ", " + std::to_string(r.width) + ", " + std::to_string(r.height) +
                                                                   ") is empty or leaves the " + std::to_string(e.w) + " x " + std::to_string(e.h) + " output");
+        p.crop = r;
+        p.cropped = p.described = true;
     }
     return B200JPG_OK;
 }
 
-// b200jpg_batch_create_resize's sizes: kept for the live frames (a failed frame's is ignored). A resized frame without a rectangle is
-// cropped to its whole output, so that the reconstruction writes C through the cropped path; returns 0 or the status the call fails
-// with (a size whose bitmaps could never be allocated)
-static int admit_sizes(b200jpg_batch &b, const b200jpg_size *sizes) {
-    b.size.assign(sizes, sizes + b.n_user);
-    if (b.crop.empty()) b.crop.assign(b.n_user, b200jpg_rect{0, 0, 0, 0});
+// b200jpg_batch_create_resize's sizes (in the records since batch creation began: attach_residuals reads them), for the live frames
+// (a failed frame's is ignored); returns 0 or the status the call fails with (a size whose bitmaps could never be allocated)
+static int admit_sizes(b200jpg_batch &b) {
     for (int i = 0; i < b.n_user; i++) {
-        b200jpg_size &s = b.size[i];
-        if (b.parse_status[i] != 0) s = b200jpg_size{0, 0};
-        if (size_empty(s)) continue;
-        const b200jpg_frame_info &fi = b.frames[i].info;
-        if (s.width > (1u << 24) || s.height > (1u << 24) || (uint64_t)s.width * s.height * frame_plan(b, i).out_ncomp > (1ull << 34))
+        FramePlan &p = b.plan[i];
+        const b200jpg_size &s = p.target;
+        if (b.parse_status[i] != 0 || size_empty(s)) continue;
+        if (s.width > (1u << 24) || s.height > (1u << 24) || (uint64_t)s.width * s.height * p.out_ncomp > (1ull << 34))
             return b.ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "frame " + std::to_string(i) + ": target size " + std::to_string(s.width) + " x " +
                                                               std::to_string(s.height) + " is too large to allocate");
-        if (rect_empty(b.crop[i])) {
-            const Extent e = out_extent(fi, 0, b.flags, b.scale[i], applied_orientation(b, i));
-            b.crop[i] = b200jpg_rect{0, 0, (uint32_t)e.w, (uint32_t)e.h};
-        }
+        p.resized = true;
     }
-    b.target = b.size;
-    b.box.assign(b.n_user, b200jpg_box{0, 0, 0, 0});
-    b.window.assign(b.n_user, b200jpg_rect{0, 0, 0, 0});
     return B200JPG_OK;
 }
 
-// b200jpg_batch_create_draft's requests (nullptr: none): every frame's factor k, B200JPG_FLAG_DOWNSCALE_k or, for a live caller's
+// b200jpg_batch_create_draft's requests (nullptr: none): every caller's frame's factor k, B200JPG_FLAG_DOWNSCALE_k or, for a live
 // frame with a request, Pillow's draft scale (a failed frame's request is ignored)
 static void admit_drafts(b200jpg_batch &b, const b200jpg_size *drafts) {
-    b.scale.assign(b.n, downscale_of(b.flags));
-    for (int i = 0; drafts && i < b.n_user; i++)
-        if (b.parse_status[i] == 0 && !size_empty(drafts[i])) b.scale[i] = draft_scale_of(b.frames[i].info, drafts[i].width, drafts[i].height);
-}
-
-// B200JPG_FLAG_LIBJPEG_TURBO: every live frame without a rectangle is cropped to its whole output, as admit_sizes does for
-// resized frames. Its slot is then described (rewritten descriptors), and turbo_generic_kernel needs only the clipped strided
-// store kinds, whatever the destination.
-static void crop_whole_frames(b200jpg_batch &b) {
-    if (b.crop.empty()) b.crop.assign(b.n_user, b200jpg_rect{0, 0, 0, 0});
     for (int i = 0; i < b.n_user; i++) {
-        if (b.parse_status[i] != 0 || !rect_empty(b.crop[i])) continue;
-        const Extent e = out_extent(b.frames[i].info, 0, b.flags, b.scale[i], applied_orientation(b, i));
-        b.crop[i] = b200jpg_rect{0, 0, (uint32_t)e.w, (uint32_t)e.h};
+        b.plan[i].k = downscale_of(b.flags);
+        if (drafts && b.parse_status[i] == 0 && !size_empty(drafts[i])) b.plan[i].k = draft_scale_of(b.frames[i].info, drafts[i].width, drafts[i].height);
     }
 }
 
@@ -1488,17 +1461,17 @@ static double filter_support(int resample) {
 
 // Image.resize's reduce step for resized frame i (DESIGN §19), in double as Pillow's Python computes it: the factors, the reduce
 // box rb in C (x0, y0, x1, y1; Image._get_safe_box) and the box the resampler then takes, in the reduced image's coordinates (C's
-// when the frame does not reduce). C is the frame's rectangle b.crop[i], untrimmed.
+// when the frame does not reduce). C is the frame's rectangle FramePlan::crop, untrimmed.
 struct ReducePlan {
     uint64_t fx = 1, fy = 1;
     int64_t rb[4] = {0, 0, 0, 0};
     double box[4];
 };
 static ReducePlan reduce_plan(const b200jpg_batch &b, int i) {
-    const b200jpg_rect &c = b.crop[i];
-    const b200jpg_size &t = b.target[i];
+    const b200jpg_rect &c = b.plan[i].crop;
+    const b200jpg_size &t = b.plan[i].target;
     ReducePlan p;
-    const b200jpg_box &bx = b.box[i];
+    const b200jpg_box &bx = b.plan[i].box;
     const double box[4] = {bx.x0, bx.y0, bx.x1, bx.y1}, whole[4] = {0.0, 0.0, (double)c.width, (double)c.height};
     memcpy(p.box, box_empty(bx) ? whole : box, sizeof(p.box));
     if (b.gap <= 0.0) return p;
@@ -1517,19 +1490,19 @@ static ReducePlan reduce_plan(const b200jpg_batch &b, int i) {
 }
 
 // b200jpg_batch_create_resample's boxes and windows (nullptr: none), checked for the live frames (a failed frame's are ignored)
-// against C (the frame's rectangle, set by admit_sizes) and the target size; a window replaces the frame's output extent
-// (`size`), the target staying in `target` (admit_sizes sets `target`, `box` and `window`; without sizes they stay empty and any
-// box or window is refused). Returns 0 or the status the call fails with.
+// against C (the frame's rectangle, set by admit_crops) and the target size; a frame without a target size refuses both (a window
+// replaces the frame's output extent: out_extent). Returns 0 or the status the call fails with.
 static int admit_boxes(b200jpg_batch &b, const b200jpg_box *boxes, const b200jpg_rect *windows) {
     for (int i = 0; i < b.n_user; i++) {
         if (b.parse_status[i] != 0) continue;
+        FramePlan &p = b.plan[i];
         const b200jpg_box bx = boxes ? boxes[i] : b200jpg_box{0, 0, 0, 0};
         const b200jpg_rect wn = windows ? windows[i] : b200jpg_rect{0, 0, 0, 0};
         const std::string at = "frame " + std::to_string(i) + ": ";
         if (!box_empty(bx) || !rect_empty(wn)) {
-            if (b.target.empty() || size_empty(b.target[i])) return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "a box or window needs a target size");
-            const b200jpg_rect &c = b.crop[i];
-            const b200jpg_size &t = b.target[i];
+            if (!p.resized) return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "a box or window needs a target size");
+            const b200jpg_rect &c = p.crop;
+            const b200jpg_size &t = p.target;
             if (!box_empty(bx)) {
                 const std::string desc = "box (" + std::to_string(bx.x0) + ", " + std::to_string(bx.y0) + ", " + std::to_string(bx.x1) + ", " +
                                          std::to_string(bx.y1) + ")";
@@ -1546,10 +1519,10 @@ static int admit_boxes(b200jpg_batch &b, const b200jpg_box *boxes, const b200jpg
                                                                       std::to_string(wn.width) + ", " + std::to_string(wn.height) +
                                                                       ") is empty or leaves the " + std::to_string(t.width) + " x " +
                                                                       std::to_string(t.height) + " image");
-            b.box[i] = bx;
-            if (!rect_empty(wn)) b.window[i] = wn, b.size[i] = b200jpg_size{wn.width, wn.height};
+            p.box = bx;
+            p.window = wn;
         }
-        if (b.target.empty() || size_empty(b.target[i]) || b.gap <= 0.0) continue;
+        if (!p.resized || b.gap <= 0.0) continue;
         const ReducePlan rp = reduce_plan(b, i);
         if (rp.fx * rp.fy >= (1ull << 24))
             return b.ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, at + "reduce factors " + std::to_string(rp.fx) + " x " + std::to_string(rp.fy) +
@@ -1589,26 +1562,26 @@ static void plan_axis(uint32_t in, const float *box, uint32_t out, uint32_t w0, 
 // channel: the vertical pass replicates it. Each frame's rectangle shrinks to the part of C its tables (or its reduce box) read,
 // which is all of C without a box, a window and a reduce (DESIGN §19): the reconstruction covers no more.
 static void plan_resample(b200jpg_batch &b) {
-    b.rs_index.assign(b.n_user, -1);
+    std::vector<int> rs_user;  // [resized] caller frame
     for (int rgb = 0; rgb < 2; rgb++) {
         for (int i = 0; i < b.n_user; i++)
-            if (b.parse_status[i] == 0 && size_of(b, i) && (frame_plan(b, i).mode == OutMode::Replicate) == (rgb == 1)) {
-                b.rs_index[i] = (int)b.rs_user.size();
-                b.rs_user.push_back(i);
+            if (b.parse_status[i] == 0 && b.plan[i].resized && (b.plan[i].mode == OutMode::Replicate) == (rgb == 1)) {
+                b.plan[i].rs = (int)rs_user.size();
+                rs_user.push_back(i);
             }
-        if (rgb == 0) b.rs_plain = (uint32_t)b.rs_user.size();
+        if (rgb == 0) b.rs_plain = (uint32_t)rs_user.size();
     }
-    const int nr = (int)b.rs_user.size();
+    const int nr = (int)rs_user.size();
     b.rs_frames.assign(nr, ResampleFrame{});
     b.rs_tables.assign(nr, {});
     for_frames(nr, 16, [&](int r) {
-        const int i = b.rs_user[r];
-        b200jpg_rect &c = b.crop[i];  // C, trimmed below to what the resize reads
-        const b200jpg_size &s = b.target[i];
-        const b200jpg_rect &wn = b.window[i];
+        const int i = rs_user[r];
+        FramePlan &plan = b.plan[i];  // C has the components the reconstruction stores
+        b200jpg_rect &c = plan.crop;  // C, trimmed below to what the resize reads
+        const b200jpg_size &s = plan.target;
+        const b200jpg_rect &wn = plan.window;
         ResampleFrame &f = b.rs_frames[r];
         auto &t = b.rs_tables[r];
-        const FramePlan plan = frame_plan(b, i);  // C has the components the reconstruction stores
         const ReducePlan rp = reduce_plan(b, i);
         const bool reduces = rp.fx > 1 || rp.fy > 1;
         f.fx = (uint32_t)rp.fx, f.fy = (uint32_t)rp.fy;
@@ -1616,7 +1589,7 @@ static void plan_resample(b200jpg_batch &b) {
         const uint32_t sw = reduces ? (uint32_t)((rp.rb[2] - rp.rb[0] + rp.fx - 1) / rp.fx) : c.width;
         const uint32_t sh = reduces ? (uint32_t)((rp.rb[3] - rp.rb[1] + rp.fy - 1) / rp.fy) : c.height;
         const float fb[4] = {(float)rp.box[0], (float)rp.box[1], (float)rp.box[2], (float)rp.box[3]};  // Pillow's "(ffff)"
-        const bool plain = !reduces && box_empty(b.box[i]);  // DESIGN §13's tables, computed as they always were
+        const bool plain = !reduces && box_empty(plan.box);  // DESIGN §13's tables, computed as they always were
         f.pass = (s.width != sw || fb[0] != 0.0f || fb[2] != (float)s.width ? kPassH : 0u) |
                  (s.height != sh || fb[1] != 0.0f || fb[3] != (float)s.height ? kPassV : 0u);
         f.tw = rect_empty(wn) ? s.width : wn.width, f.th = rect_empty(wn) ? s.height : wn.height;
@@ -1713,7 +1686,9 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
     b.ctx = ctx;
     b.n = b.n_user = n;
     b.flags = flags;
-    if (sizes) b.size.assign(sizes, sizes + n), b.resample = resample;  // (attach_residuals refuses 12-bit frames with a size)
+    b.plan.assign(n, FramePlan{});
+    for (int i = 0; sizes && i < n; i++) b.plan[i].target = sizes[i];  // (attach_residuals refuses 12-bit frames with a size)
+    if (sizes) b.resample = resample, b.gap = reducing_gap;  // (gap <= 0: None)
     Codestreams cs;
     cs.data.assign(frames, frames + n);
     cs.len.assign(lens, lens + n);
@@ -1726,15 +1701,15 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
     std::vector<std::vector<TableSet>> frame_tables;
     if (int rc = admit_frames(b, cs, tolerate_bad != 0, frame_tables)) return rc;
     admit_drafts(b, drafts);
-    if (rects)
-        if (int rc = admit_crops(b, rects)) return rc;
-    if (sizes)
-        if (int rc = admit_sizes(b, sizes)) return rc;
-    if (sizes) b.gap = reducing_gap;  // (<= 0: None)
+    for (int i = 0; i < n; i++)
+        if (b.parse_status[i] == 0) frame_plan(b, i);
+    if (int rc = admit_crops(b, rects)) return rc;
+    if (int rc = admit_sizes(b)) return rc;
     if (boxes || windows || b.gap > 0.0)
         if (int rc = admit_boxes(b, boxes, windows)) return rc;
-    if (flags & B200JPG_FLAG_LIBJPEG_TURBO) crop_whole_frames(b);
     plan_resample(b);  // (before the reconstruction groups: it trims the rectangles of resized frames)
+    for (int i = n; i < b.n; i++)  // JPEG XT residual codestreams: their frames' records, their own components
+        if (b.parse_status[i] == 0) b.plan[i] = b.plan[b.xt_parent[i]], b.plan[i].ncomp = b.frames[i].info.ncomp;
     const std::vector<uint64_t> byte_off = lay_out_codestreams(b, cs.len);
     const std::vector<std::array<uint64_t, 4>> sample_base = lay_out_planes(b);
     form_scan_classes(b, frame_tables, byte_off);
@@ -1797,8 +1772,8 @@ int b200jpg_batch_output_extent(const b200jpg_batch *b, int i, int c, uint32_t *
     if (!b || i < 0 || i >= b->n_user || !width || !height) return B200JPG_ERR_INVALID_PARAMETER;
     if (b->parse_status[i] != 0) return b->parse_status[i];
     const b200jpg_frame_info &fi = b->frames[i].info;
-    if (c < 0 || c >= (int)frame_plan(*b, i).out_ncomp) return B200JPG_ERR_INVALID_PARAMETER;
-    const Extent e = out_extent(fi, c, b->flags, b->scale[i], applied_orientation(*b, i), crop_of(*b, i), size_of(*b, i));
+    if (c < 0 || c >= (int)b->plan[i].out_ncomp) return B200JPG_ERR_INVALID_PARAMETER;
+    const Extent e = out_extent(fi, c, b->flags, b->plan[i]);
     *width = (uint32_t)e.w;
     *height = (uint32_t)e.h;
     return B200JPG_OK;
@@ -1807,7 +1782,7 @@ int b200jpg_batch_output_extent(const b200jpg_batch *b, int i, int c, uint32_t *
 int b200jpg_batch_output_components(const b200jpg_batch *b, int i) {
     if (!b || i < 0 || i >= b->n_user) return B200JPG_ERR_INVALID_PARAMETER;
     if (b->parse_status[i] != 0) return b->parse_status[i];
-    return (int)frame_plan(*b, i).out_ncomp;
+    return (int)b->plan[i].out_ncomp;
 }
 
 int b200jpg_batch_frame_orientation(const b200jpg_batch *b, int i) {
@@ -2061,71 +2036,76 @@ static int stage_planes(b200jpg_batch *b, void *stream, const std::function<void
 // Frame i's destinations, described in its output coordinates, rewritten into the decoded coordinates the kernels walk, in place:
 // translated by its crop rectangle into the uncropped output (translate_plane), then oriented (orient_plane); planar[i] cleared
 // unless every component then has bytes_per_pixel == size. Returns false when a pixel stride does not fit (only a caller's
-// descriptor can do that). nc: the descriptors the reconstruction stores through (frame_plan's output components, or C's in the
+// descriptor can do that). nc: the descriptors the reconstruction stores through (the plan's output components, or C's in the
 // scratch).
 static bool rewrite_frame(const b200jpg_batch *b, int i, b200jpg_plane *pl, uint64_t size, std::vector<char> &planar, uint32_t nc) {
-    const b200jpg_frame_info &fi = b->frames[i].info;
-    const int o = applied_orientation(*b, i);
-    const b200jpg_rect *crop = crop_of(*b, i);
+    const FramePlan &p = b->plan[i];
     for (uint32_t c = 0; c < nc; c++) {
-        const Extent d = out_extent(fi, c, b->flags, b->scale[i], 1);
-        if (crop) translate_plane(pl[c], *crop);
-        if (!orient_plane(pl[c], o, d.w, d.h)) return false;
+        const Extent d = decoded_extent(b->frames[i].info, c, b->flags, p.k);
+        if (p.cropped) translate_plane(pl[c], p.crop);
+        if (!orient_plane(pl[c], p.orientation, d.w, d.h)) return false;
         if ((uint64_t)pl[c].bytes_per_pixel != size) planar[(size_t)i] = 0;
     }
     return true;
 }
 
-// The reconstruction's destination of resized frame i: its C in the scratch, an interleaved uint8 bitmap, rewritten like a cropped
-// frame's slot (rewrite_frame)
-static void scratch_planes(const b200jpg_batch *b, int i, b200jpg_plane *pl, std::vector<char> &planar) {
-    const ResampleFrame &f = b->rs_frames[(size_t)b->rs_index[i]];
-    for (uint32_t c = 0; c < f.ncomp; c++) {
-        pl[c].data = b->d_scratch + f.c_src + c;
-        pl[c].bytes_per_pixel = (int32_t)f.ncomp;
-        pl[c].bytes_per_row = f.c_pitch;
+// Live frame i's destinations q, described in its output coordinates (a caller's, or its packed slot's), made the ones its
+// reconstruction stores through, in place: a resized frame's C in the scratch, an interleaved uint8 bitmap (its own destinations go
+// to the resample pass: stage_frame_planes), rewritten like a cropped frame's; another described frame's rewritten (rewrite_frame),
+// planar[i] decided on those; an undescribed frame's as they are. size: the bytes of a sample in q. Returns false as rewrite_frame.
+static bool place_frame(const b200jpg_batch *b, int i, b200jpg_plane *q, uint64_t size, std::vector<char> &planar) {
+    const FramePlan &p = b->plan[i];
+    if (p.resized) {
+        const ResampleFrame &f = b->rs_frames[(size_t)p.rs];
+        for (uint32_t c = 0; c < f.ncomp; c++) {
+            q[c].data = b->d_scratch + f.c_src + c;
+            q[c].bytes_per_pixel = (int32_t)f.ncomp;
+            q[c].bytes_per_row = f.c_pitch;
+        }
+        return rewrite_frame(b, i, q, 1, planar, f.ncomp);  // (a scratch row always fits the pixel stride)
     }
-    rewrite_frame(b, i, pl, 1, planar, f.ncomp);  // a scratch row always fits the pixel stride
+    if (!p.described) return true;
+    planar[(size_t)i] = 1;
+    return rewrite_frame(b, i, q, size, planar, p.out_ncomp);
 }
 
-// b200jpg_batch_decode of a batch with oriented or cropped frames: each such frame's packed slot in out_dev, seen as an interleaved
-// bitmap of the oriented (cropped) extent (B200JPG_FLAG_NO_UPSAMPLE: plane after plane), rewritten for its crop and orientation and
-// staged like the table of b200jpg_batch_decode_into. A resized frame: its scratch, and its slot as the resample pass's
-// destination at 4 * (n + r), in output coordinates. planar[i] as for that table.
-static int stage_slot_planes(b200jpg_batch *b, uint8_t *out_dev, void *stream, std::vector<char> &planar) {
+// The descriptor table of a decode (staged: stage_planes): every live frame's placed destinations q (place_frame), and the
+// destinations of resized frame r, as given in `planes`, at 4 * (n + r) for the resample pass ([4 * n_user] each)
+static int stage_frame_planes(b200jpg_batch *b, const b200jpg_plane *q, const b200jpg_plane *planes, void *stream) {
     return stage_planes(b, stream, [&](b200jpg_plane *table) {
-        for (size_t r = 0; r < b->rs_frames.size(); r++) {
-            const int i = b->rs_user[r];
-            const ResampleFrame &f = b->rs_frames[r];
-            scratch_planes(b, i, table + 4 * (size_t)i, planar);
-            const uint32_t no = frame_plan(*b, i).out_ncomp;
-            for (uint32_t c = 0; c < no; c++) {
-                b200jpg_plane &p = table[4 * (size_t)f.plane + c];
-                p.data = out_dev + b->out_off[i] + c;
-                p.bytes_per_pixel = (int32_t)no;
-                p.bytes_per_row = (int64_t)f.tw * no;
-            }
-        }
         for (int i = 0; i < b->n_user; i++) {
-            if (b->parse_status[i] != 0 || size_of(*b, i)) continue;
-            const uint32_t no = frame_plan(*b, i).out_ncomp;
-            const b200jpg_frame_info &fi = b->frames[i].info;
-            if (applied_orientation(*b, i) == 1 && !crop_of(*b, i) && frame_plan(*b, i).mode == OutMode::Coded) continue;
-            const int o = applied_orientation(*b, i);
-            const int64_t size = fi.precision > 8 ? 2 : 1;
-            const bool planes = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
-            uint64_t before = 0;
-            b200jpg_plane *pl = table + 4 * (size_t)i;
-            for (uint32_t c = 0; c < no; c++) {
-                const Extent e = out_extent(fi, (int)c, b->flags, b->scale[i], o, crop_of(*b, i));
-                pl[c].data = out_dev + b->out_off[i] + (planes ? before : (uint64_t)c) * size;
-                pl[c].bytes_per_pixel = (int32_t)(planes ? size : no * size);
-                pl[c].bytes_per_row = (int64_t)e.w * pl[c].bytes_per_pixel;
-                before += e.w * e.h;
-            }
-            rewrite_frame(b, i, pl, (uint64_t)size, planar, no);  // a slot's row stride always fits the pixel stride
+            const FramePlan &p = b->plan[i];
+            if (b->parse_status[i] != 0) continue;
+            memcpy(table + 4 * (size_t)i, q + 4 * (size_t)i, sizeof(b200jpg_plane) * p.out_ncomp);
+            if (p.resized) memcpy(table + 4 * ((size_t)b->n + p.rs), planes + 4 * (size_t)i, sizeof(b200jpg_plane) * p.out_ncomp);
         }
     });
+}
+
+// b200jpg_batch_decode of a batch with described frames: each such frame's packed slot in out_dev, described as a caller of
+// b200jpg_batch_decode_into would: an interleaved bitmap of its output extent (B200JPG_FLAG_NO_UPSAMPLE: plane after plane), placed
+// and staged as that call's table is (never checked like it). planar[i] as for that table.
+static int stage_slot_planes(b200jpg_batch *b, uint8_t *out_dev, void *stream, std::vector<char> &planar) {
+    std::vector<b200jpg_plane> slots(4 * (size_t)b->n_user), q(slots.size());
+    for (int i = 0; i < b->n_user; i++) {
+        const FramePlan &p = b->plan[i];
+        if (b->parse_status[i] != 0 || !p.described) continue;
+        const b200jpg_frame_info &fi = b->frames[i].info;
+        const int64_t size = fi.precision > 8 ? 2 : 1;
+        const bool planes = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
+        uint64_t before = 0;
+        b200jpg_plane *pl = &slots[4 * (size_t)i];
+        for (uint32_t c = 0; c < p.out_ncomp; c++) {
+            const Extent e = out_extent(fi, (int)c, b->flags, p);
+            pl[c].data = out_dev + b->out_off[i] + (planes ? before : (uint64_t)c) * size;
+            pl[c].bytes_per_pixel = (int32_t)(planes ? size : p.out_ncomp * size);
+            pl[c].bytes_per_row = (int64_t)e.w * pl[c].bytes_per_pixel;
+            before += e.w * e.h;
+        }
+        std::copy_n(pl, 4, &q[4 * (size_t)i]);
+        place_frame(b, i, &q[4 * (size_t)i], (uint64_t)size, planar);  // (a slot's row stride always fits the pixel stride)
+    }
+    return stage_frame_planes(b, q.data(), slots.data(), stream);
 }
 
 // planes_dev: b200jpg_batch_decode_into's descriptor table (device), planar[i]: every component of frame i has
@@ -2133,13 +2113,13 @@ static int stage_slot_planes(b200jpg_batch *b, uint8_t *out_dev, void *stream, s
 static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b200jpg_plane *planes_dev = nullptr,
                      const std::vector<char> *planar = nullptr, const b200jpg_convert *convert = nullptr) {
     NvtxRange nvtx("b200jpg reconstruction: IDCT + upsampling + colour");
-    // into the packed slots with oriented or cropped frames: those frames' slots as rewritten descriptors, built for this call's out_dev
+    // into the packed slots with described frames: those frames' slots as descriptors, built for this call's out_dev; the groups of
+    // the other frames store into out_dev
     std::vector<char> slot_planar;
-    const b200jpg_plane *slot_planes = nullptr;
     if (!planes_dev && b->rewritten) {
         slot_planar.assign((size_t)b->n, 1);
         if (int rc = stage_slot_planes(b, out_dev, stream, slot_planar)) return rc;
-        slot_planes = b->d_planes;
+        planes_dev = b->d_planes, planar = &slot_planar;
     }
     cudaError_t me = cudaMemsetAsync(b->d_status + b->n, 0, sizeof(uint32_t) * 2 * (size_t)b->n, (cudaStream_t)stream);
     if (me != cudaSuccess) return b->ctx->fail_cuda(me, "flag reset");
@@ -2151,12 +2131,12 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.max_bh0 = g.max_bh0;
         l.max_bwc = g.max_bwc;
         l.max_bhc = g.max_bhc;
-        l.ncomp = g.ncomp;
-        l.subx = g.subx;
-        l.suby = g.suby;
-        l.path = g.path;
-        l.mode = g.mode;
-        l.downscale = (int)g.scale;
+        l.ncomp = g.key.ncomp;
+        l.subx = g.key.subx;
+        l.suby = g.key.suby;
+        l.path = g.key.path;
+        l.mode = g.key.mode;
+        l.downscale = (int)g.key.scale;
         l.planes_out = (b->flags & B200JPG_FLAG_NO_UPSAMPLE) != 0;
         l.coef = b->d_coef;
         l.samples16 = b->d_samples16;
@@ -2166,19 +2146,16 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.narrow_flags = b->d_status + 2 * (size_t)b->n;
         l.narrow_list = b->d_status + 3 * (size_t)b->n;
         l.out = out_dev;
-        l.planes = planes_dev;
+        l.planes = (out_dev && !g.key.described) ? nullptr : planes_dev;
         l.convert = convert;
-        const std::vector<char> *group_planar = planar;
-        const bool described = g.orientation != 1 || g.cropped || g.mode != OutMode::Coded;  // (by stage_slot_planes)
-        if (slot_planes && described) l.planes = slot_planes, group_planar = &slot_planar;
-        if (g.resized) l.convert = nullptr;  // C leaves as uint8; the resample pass converts
+        if (g.key.resized) l.convert = nullptr;  // C leaves as uint8; the resample pass converts
         l.planar = l.planes != nullptr;
         if (l.planes)
-            for (const FrameRecon &fr : g.frames) l.planar = l.planar && (*group_planar)[fr.status_idx];
+            for (const FrameRecon &fr : g.frames) l.planar = l.planar && (*planar)[fr.status_idx];
         // oriented frames into anything but planar destinations: the staged store kinds, runs of eight samples along x or y; cropped
         // frames into any destination: the same kinds with the clip (the generic kernels: the strided kinds with the clip)
-        l.runs = described && l.planes && (!l.planar || g.cropped);
-        l.clip = g.cropped;
+        l.runs = g.key.described && l.planes && (!l.planar || g.key.cropped);
+        l.clip = g.key.cropped;
         int launches = 0;
         // grid.y carries the frame index: at most 65535 frames per launch. A generic group that is cut runs the IDCT of ALL its
         // frames first: a JPEG XT frame reads the planes of its residual frame, which may sit in another part
@@ -2207,7 +2184,7 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         rl.input = b->d_input;
         rl.scratch = b->d_scratch;
         rl.inter = b->d_inter;
-        rl.planes = planes_dev ? planes_dev : slot_planes;
+        rl.planes = planes_dev;
         rl.convert = convert;
         rl.n_plain = std::min(rl.n_frames, b->rs_plain > first ? b->rs_plain - first : 0u);
         int launches = 0;
@@ -2267,23 +2244,21 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
         else return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "unknown sample type " + std::to_string(convert->type));
         int ncomp = 0;  // the components some live frame is written with
         for (int i = 0; i < b->n_user; i++)
-            if (b->parse_status[i] == 0) ncomp = std::max(ncomp, (int)frame_plan(*b, i).out_ncomp);
+            if (b->parse_status[i] == 0) ncomp = std::max(ncomp, (int)b->plan[i].out_ncomp);
         for (int c = 0; c < ncomp; c++)
             if (!std::isfinite(convert->scale[c]) || !std::isfinite(convert->bias[c]))
                 return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "component " + std::to_string(c) + ": scale and bias must be finite");
     }
     std::vector<char> planar((size_t)b->n, 1);
-    // a batch with oriented or cropped frames: the table as staged, those frames' descriptors rewritten once here (rewrite_frame)
-    std::vector<b200jpg_plane> rewritten(b->rewritten ? 4 * (size_t)b->n_user : 0);
+    std::vector<b200jpg_plane> q(planes, planes + 4 * (size_t)b->n_user);  // placed once here (place_frame)
     for (int i = 0; i < b->n_user; i++) {
         if (b->parse_status[i] != 0) continue;
         const b200jpg_frame_info &fi = b->frames[i].info;
         const uint64_t size = convert ? element : (fi.precision > 8 ? 2 : 1);
-        const int orientation = applied_orientation(*b, i);
-        const FramePlan plan = frame_plan(*b, i);
+        const FramePlan &plan = b->plan[i];
         for (int c = 0; c < (int)plan.out_ncomp; c++) {
             const b200jpg_plane &p = planes[4 * i + c];
-            const auto [w, h] = out_extent(fi, c, b->flags, b->scale[i], orientation, crop_of(*b, i), size_of(*b, i));  // the rules hold in (cropped, resized) output coordinates
+            const auto [w, h] = out_extent(fi, c, b->flags, plan);  // the rules hold in (cropped, resized) output coordinates
             const uint64_t bpp = magnitude(p.bytes_per_pixel), bpr = magnitude(p.bytes_per_row);
             const std::string at = "frame " + std::to_string(i) + " component " + std::to_string(c) + ": ";
             if (!p.data) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "no destination");
@@ -2300,27 +2275,10 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
                 return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "not device memory of the batch's device");
             if ((uint64_t)p.bytes_per_pixel != size) planar[(size_t)i] = 0;
         }
-        if (b->rewritten) {
-            b200jpg_plane *q = rewritten.data() + 4 * (size_t)i;
-            memcpy(q, planes + 4 * (size_t)i, sizeof(b200jpg_plane) * plan.out_ncomp);
-            if (size_of(*b, i)) {  // the reconstruction stores into the scratch; the caller's descriptors go to the resample pass
-                scratch_planes(b, i, q, planar);
-            } else if (orientation != 1 || crop_of(*b, i)) {  // the kernels store through the rewritten descriptors: planar is decided on those
-                planar[(size_t)i] = 1;
-                if (!rewrite_frame(b, i, q, size, planar, plan.out_ncomp))
-                    return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) +
-                                                                           ": |bytes_per_row| does not fit the pixel stride of the transposed frame");
-            }
-        }
+        if (!place_frame(b, i, &q[4 * (size_t)i], size, planar))
+            return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": |bytes_per_row| does not fit the pixel stride of the transposed frame");
     }
-    const b200jpg_plane *src = b->rewritten ? rewritten.data() : planes;
-    const int rc = stage_planes(b, stream, [&](b200jpg_plane *table) {
-        for (int i = 0; i < b->n_user; i++)
-            if (b->parse_status[i] == 0) memcpy(table + 4 * (size_t)i, src + 4 * (size_t)i, sizeof(b200jpg_plane) * frame_plan(*b, i).out_ncomp);
-        for (size_t r = 0; r < b->rs_frames.size(); r++)  // the caller's descriptors of resized frames: the resample pass's, as given
-            memcpy(table + 4 * (size_t)b->rs_frames[r].plane, planes + 4 * (size_t)b->rs_user[r], sizeof(b200jpg_plane) * frame_plan(*b, b->rs_user[r]).out_ncomp);
-    });
-    if (rc) return rc;
+    if (int rc = stage_frame_planes(b, q.data(), planes, stream)) return rc;
     return run_decode(b, nullptr, stream, b->d_planes, &planar, convert);
 }
 

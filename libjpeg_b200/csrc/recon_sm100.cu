@@ -1971,7 +1971,7 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
 
 template <int K>
 static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches) {
-    if (l.path == ReconPath::Turbo || l.path == ReconPath::TurboGeneric) {  // (every frame of such a group is cropped: crop_whole_frames)
+    if (l.path == ReconPath::Turbo || l.path == ReconPath::TurboGeneric) {  // (every frame of such a group is cropped: admit_crops)
         if constexpr (kClipKind<K>) return launch_turbo<(kFloatKind<K> ? kStoreStridedF : kStoreStrided) | kStoreClip>(l, s, launches);
         return (int)cudaErrorInvalidValue;
     }

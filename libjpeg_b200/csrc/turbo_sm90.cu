@@ -14,7 +14,7 @@
 //                              ratios after the IDCT
 //   turbo_cmyk_*kernel         turbo_generic_kernel and its draft form for the 8-bit Adobe CMYK / YCCK frames of an output mode
 //                              (DESIGN §18): four components read, Pillow's conversion (cmyk_sm90.cuh), three or one stored
-// Every frame of a flagged batch is cropped (abi.cpp: crop_whole_frames), so both kinds store through described destinations with
+// Every frame of a flagged batch is cropped (abi.cpp: admit_crops), so both kinds store through described destinations with
 // the clip.
 #include <cuda_runtime.h>
 

@@ -616,14 +616,8 @@ class BatchDecoder:
         flags |= native.MODE_FLAGS[mode]
         self.reconstruction = reconstruction
         flags |= native.RECONSTRUCTION_FLAGS[reconstruction]
-        if boxes is not None or windows is not None or gap > 0.0:
-            rc = lib.b200jpg_batch_create_resample(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, drafts, rects, sizes, boxes,
-                                                   windows, filt, gap, ctypes.byref(self.handle))
-        elif drafts is None:
-            rc = lib.b200jpg_batch_create_resize(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, rects, sizes, filt, ctypes.byref(self.handle))
-        else:
-            rc = lib.b200jpg_batch_create_draft(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, drafts, rects, sizes, filt,
-                                                ctypes.byref(self.handle))
+        rc = lib.b200jpg_batch_create_resample(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, drafts, rects, sizes, boxes, windows,
+                                               filt, gap, ctypes.byref(self.handle))
         native.check(rc, self.ctx.handle)
         self.ctx._batch_opened()
         self._keep = []  # the batch holds its own pinned copy

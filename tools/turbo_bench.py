@@ -8,7 +8,7 @@ all of them. Cases, each for reconstruction="reference" and "libjpeg-turbo" on t
   fp16     decode_into an fp16 [N, 3, H, W] tensor with the ImageNet map
   rrc224   RandomResizedCrop rectangles (seeded), resized to fp16 [N, 3, 224, 224] with the ImageNet map
 and, for the reference reconstruction only, packed / fp16 with every frame cropped to its whole output (`packed_whole`,
-`fp16_whole`): the cost of the described, clipped store that every turbo frame takes (crop_whole_frames), on upright packed and
+`fp16_whole`): the cost of the described, clipped store that every turbo frame takes (admit_crops), on upright packed and
 planar destinations.
 The entropy / reconstruction split comes from the batch's event timing in a step of its own. With --out, one packed turbo step
 per workload runs again under torch.profiler (CUDA activities) for the times of turbo_idct_kernel, turbo_reconstruct_kernel and
