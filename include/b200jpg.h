@@ -240,6 +240,14 @@ typedef struct b200jpg_size {
 #define B200JPG_RESAMPLE_BICUBIC 3
 #define B200JPG_RESAMPLE_BOX 4
 #define B200JPG_RESAMPLE_HAMMING 5
+/* OpenCV's cv2.resize(C, (W_t, H_t), interpolation=INTER_LINEAR / INTER_AREA) instead of Pillow's resampler: 0x100 | cv2's own
+ * constant (DESIGN §20). Every function that takes `resample` accepts them; with either, R below is cv2.resize of C, byte for
+ * byte (OpenCV 4.13), and boxes and a reducing_gap are refused: B200JPG_ERR_INVALID_PARAMETER for the call, the frame named,
+ * tolerate_bad or not. Windows, sizes, modes, orientation, drafts and the float map are as for Pillow's filters. An INTER_AREA
+ * frame that shrinks by integer factors fx, fy with 255 fx fy >= 2^31 (OpenCV's int block sums overflow) is
+ * B200JPG_ERR_NOT_IMPLEMENTED for the call. */
+#define B200JPG_RESAMPLE_CV_LINEAR 0x101
+#define B200JPG_RESAMPLE_CV_AREA 0x103
 /* b200jpg_batch_create_crop with a target size per frame (no counterpart in the reference). Let C be what the batch writes for the
  * caller's frame i without a size: O[y : y + height, x : x + width] of b200jpg_batch_create_crop (O itself without a rectangle),
  * uint8, [h, w, ncomp]. With sizes[i] = {W_t, H_t}, frame i is written as R(C), bit for bit, where R is Pillow's convolution
@@ -328,11 +336,21 @@ B200JPG_API int b200jpg_draft_scale(const uint8_t *data, size_t len, uint32_t wi
  * only, no device): bounds[2 j] is the first source index and bounds[2 j + 1] the number of taps of output j, coeffs[j * ksize + t]
  * the int32 coefficient of tap t (zero behind the taps). *ksize receives the row length. The tables are written when bounds and
  * coeffs are both non-NULL: bounds needs 2 * out_size entries and coeffs `capacity` >= out_size * ksize entries, else the call
- * returns B200JPG_ERR_INVALID_PARAMETER. Also B200JPG_ERR_INVALID_PARAMETER: a zero size, an unknown filter or a NULL ksize. */
+ * returns B200JPG_ERR_INVALID_PARAMETER. Also B200JPG_ERR_INVALID_PARAMETER: a zero size, an unknown filter or a NULL ksize.
+ * For B200JPG_RESAMPLE_CV_LINEAR / _CV_AREA the tables are OpenCV's (DESIGN §20), of the horizontal axis, or of the vertical one
+ * with B200JPG_CV_TABLE_VERTICAL or-ed into `resample`:
+ *   - INTER_LINEAR, and INTER_AREA on an axis that upscales or with B200JPG_CV_TABLE_LINEAR (the other axis upscales): ksize = 2,
+ *     bounds[2 j] and bounds[2 j + 1] the two source indices of output j (clamped to the axis), coeffs[2 j], coeffs[2 j + 1] their
+ *     int16 weights (11 fractional bits);
+ *   - INTER_AREA otherwise: bounds as for Pillow's filters (first source index, taps), coeffs[j * ksize + t] the bits of the float
+ *     weight of tap t (computeResizeAreaTab). The batch sums blocks instead where both axes shrink by integer factors. */
+#define B200JPG_CV_TABLE_VERTICAL 0x1000
+#define B200JPG_CV_TABLE_LINEAR 0x2000
 B200JPG_API int b200jpg_resample_coefficients(uint32_t in_size, uint32_t out_size, int resample, int32_t *bounds, int32_t *coeffs,
                                               uint64_t capacity, uint32_t *ksize);
 /* b200jpg_resample_coefficients for the source box [in0, in1) of b200jpg_batch_create_resample, as Pillow's C resampler takes it in
- * floats (tests only, host only). Also B200JPG_ERR_INVALID_PARAMETER: a box that is not 0 <= in0 <= in1 <= in_size. */
+ * floats (tests only, host only). Also B200JPG_ERR_INVALID_PARAMETER: a box that is not 0 <= in0 <= in1 <= in_size, and the
+ * OpenCV filters, which take no box. */
 B200JPG_API int b200jpg_resample_coefficients_box(uint32_t in_size, float in0, float in1, uint32_t out_size, int resample, int32_t *bounds,
                                                   int32_t *coeffs, uint64_t capacity, uint32_t *ksize);
 /* The uncropped output size W_o x H_o of one codestream under `flags` (B200JPG_FLAG_DOWNSCALE_k, and width and height swapped for

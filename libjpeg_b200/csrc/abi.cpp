@@ -8,6 +8,7 @@
 
 #include <algorithm>
 #include <array>
+#include <cfloat>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -181,6 +182,7 @@ bool rect_empty(const b200jpg_rect &r) { return r.x == 0 && r.y == 0 && r.width 
 bool size_empty(const b200jpg_size &s) { return s.width == 0 && s.height == 0; }
 bool box_empty(const b200jpg_box &b) { return b.x0 == 0.0 && b.y0 == 0.0 && b.x1 == 0.0 && b.y1 == 0.0; }
 bool resample_known(int r) { return r >= B200JPG_RESAMPLE_LANCZOS && r <= B200JPG_RESAMPLE_HAMMING; }  // PIL's values 1 .. 5
+bool resample_cv(int r) { return r == B200JPG_RESAMPLE_CV_LINEAR || r == B200JPG_RESAMPLE_CV_AREA; }  // OpenCV's (DESIGN §20)
 
 // Pillow's draft scale (JpegImageFile.draft) of a frame of codestream size W x H for a request of width x height (both >= 1): the
 // largest k of 8, 4, 2, 1 with k <= min(W / width, H / height), 1 when none fits
@@ -402,6 +404,7 @@ struct b200jpg_batch {
     std::vector<std::array<std::vector<int32_t>, 4>> rs_tables;
     uint64_t dev_rs_frames = 0;
     uint32_t rs_max_rows = 0, rs_max_reduce_rows = 0;
+    uint32_t rs_cv_kinds = 0;  // OpenCV's filters: kCvLinear / kCvArea / kCvBlocks of the resized frames (ResampleLaunch::cv_kinds)
     uint64_t rs_max_pixels = 0;
     uint8_t *d_scratch = nullptr, *d_inter = nullptr;  // C of every resized frame; the horizontal pass's rows
     uint64_t scratch_bytes = 0, inter_bytes = 0;
@@ -538,11 +541,13 @@ int b200jpg_draft_scale(const uint8_t *data, size_t len, uint32_t width, uint32_
 // the tables of resample_coefficients copied out (b200jpg_resample_coefficients / _box)
 static int coefficients_out(uint32_t in_size, const float *box, uint32_t out_size, int resample, int32_t *bounds, int32_t *coeffs,
                             uint64_t capacity, uint32_t *ksize) {
-    if (!ksize || in_size == 0 || out_size == 0 || !resample_known(resample)) return B200JPG_ERR_INVALID_PARAMETER;
+    const bool cv = !box && resample_cv(resample & ~(B200JPG_CV_TABLE_VERTICAL | B200JPG_CV_TABLE_LINEAR));
+    if (!ksize || in_size == 0 || out_size == 0 || !(resample_known(resample) || cv)) return B200JPG_ERR_INVALID_PARAMETER;
     std::vector<int32_t> b, k;
     uint32_t ks = 0;
     try {
-        if (int rc = resample_coefficients(in_size, box, out_size, resample, b, k, ks)) return rc;
+        if (int rc = cv ? cv_resample_coefficients(in_size, out_size, resample, b, k, ks) : resample_coefficients(in_size, box, out_size, resample, b, k, ks))
+            return rc;
     } catch (const std::bad_alloc &) {
         return B200JPG_ERR_OUT_OF_MEMORY;
     }
@@ -1489,9 +1494,30 @@ static ReducePlan reduce_plan(const b200jpg_batch &b, int i) {
     return p;
 }
 
+// Which rule of DESIGN §20 cv2.resize applies to resized frame i (C, the frame's untrimmed rectangle, to its target), as OpenCV
+// decides it: 0 for the copy (same size), 1 for INTER_LINEAR; for INTER_AREA 2 where both axes shrink by integer factors
+// (|scale - round(scale)| < DBL_EPSILON), 3 where both scales are >= 1 otherwise, 4 where either axis grows.
+struct CvPlan {
+    int rule = 0;
+    uint64_t fx = 1, fy = 1;  // rule 2's factors
+};
+static CvPlan cv_plan(const b200jpg_batch &b, int i) {
+    const b200jpg_rect &c = b.plan[i].crop;
+    const b200jpg_size &t = b.plan[i].target;
+    CvPlan p;
+    if (c.width == t.width && c.height == t.height) return p;
+    if (b.resample == B200JPG_RESAMPLE_CV_LINEAR) return p.rule = 1, p;
+    const double sx = 1.0 / ((double)t.width / c.width), sy = 1.0 / ((double)t.height / c.height);
+    if (sx < 1.0 || sy < 1.0) return p.rule = 4, p;
+    const double ix = std::nearbyint(sx), iy = std::nearbyint(sy);
+    if (std::fabs(sx - ix) < DBL_EPSILON && std::fabs(sy - iy) < DBL_EPSILON) return p.rule = 2, p.fx = (uint64_t)ix, p.fy = (uint64_t)iy, p;
+    return p.rule = 3, p;
+}
+
 // b200jpg_batch_create_resample's boxes and windows (nullptr: none), checked for the live frames (a failed frame's are ignored)
 // against C (the frame's rectangle, set by admit_crops) and the target size; a frame without a target size refuses both (a window
-// replaces the frame's output extent: out_extent). Returns 0 or the status the call fails with.
+// replaces the frame's output extent: out_extent). Under OpenCV's filters a box is refused and so are rule 2's blocks whose int
+// sums could overflow (DESIGN §20). Returns 0 or the status the call fails with.
 static int admit_boxes(b200jpg_batch &b, const b200jpg_box *boxes, const b200jpg_rect *windows) {
     for (int i = 0; i < b.n_user; i++) {
         if (b.parse_status[i] != 0) continue;
@@ -1503,6 +1529,8 @@ static int admit_boxes(b200jpg_batch &b, const b200jpg_box *boxes, const b200jpg
             if (!p.resized) return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "a box or window needs a target size");
             const b200jpg_rect &c = p.crop;
             const b200jpg_size &t = p.target;
+            if (!box_empty(bx) && resample_cv(b.resample))
+                return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, at + "OpenCV's resize takes no source box");
             if (!box_empty(bx)) {
                 const std::string desc = "box (" + std::to_string(bx.x0) + ", " + std::to_string(bx.y0) + ", " + std::to_string(bx.x1) + ", " +
                                          std::to_string(bx.y1) + ")";
@@ -1521,6 +1549,12 @@ static int admit_boxes(b200jpg_batch &b, const b200jpg_box *boxes, const b200jpg
                                                                       std::to_string(t.height) + " image");
             p.box = bx;
             p.window = wn;
+        }
+        if (p.resized && resample_cv(b.resample)) {  // rule 2's int sums: 255 fx fy below 2^31
+            const CvPlan cp = cv_plan(b, i);
+            if (cp.rule == 2 && 255ull * cp.fx * cp.fy >= (1ull << 31))
+                return b.ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, at + "area blocks of " + std::to_string(cp.fx) + " x " + std::to_string(cp.fy) +
+                                                                    " pixels overflow OpenCV's int sums");
         }
         if (!p.resized || b.gap <= 0.0) continue;
         const ReducePlan rp = reduce_plan(b, i);
@@ -1556,6 +1590,52 @@ static void plan_axis(uint32_t in, const float *box, uint32_t out, uint32_t w0, 
     for (uint32_t j = 0; j < wn; j++) bounds[2 * j] = bounds[2 * j + 1] > 0 ? bounds[2 * j] - (int32_t)lo : 0;
 }
 
+// One axis of a frame under OpenCV's rules 1, 3 and 4 (DESIGN §20): the table of `table` (b200jpg_resample_coefficients' encoding;
+// `pairs`: the two-tap tables of rules 1 / 4) restricted to the window's outputs [w0, w0 + wn), rebased to the source range [lo, hi)
+// it reads.
+static void plan_cv_axis(uint32_t in, uint32_t out, uint32_t w0, uint32_t wn, int table, bool pairs, std::vector<int32_t> &bounds,
+                         std::vector<int32_t> &coef, uint32_t &ksize, uint32_t &lo, uint32_t &hi) {
+    cv_resample_coefficients(in, out, table, bounds, coef, ksize);  // (the arguments are valid: the call cannot fail)
+    if (w0 != 0 || wn != out) {
+        bounds.erase(bounds.begin() + 2 * ((size_t)w0 + wn), bounds.end());
+        bounds.erase(bounds.begin(), bounds.begin() + 2 * (size_t)w0);
+        coef.erase(coef.begin() + ((size_t)w0 + wn) * ksize, coef.end());
+        coef.erase(coef.begin(), coef.begin() + (size_t)w0 * ksize);
+    }
+    lo = in, hi = 0;
+    for (uint32_t j = 0; j < wn; j++) {
+        const uint32_t a = bounds[2 * j], e = pairs ? bounds[2 * j + 1] + 1 : a + bounds[2 * j + 1];
+        if (e > a) lo = std::min(lo, a), hi = std::max(hi, e);
+    }
+    if (lo >= hi) lo = 0, hi = 1;
+    for (uint32_t j = 0; j < wn; j++) {
+        bounds[2 * j] = std::max<int32_t>(bounds[2 * j] - (int32_t)lo, 0);
+        if (pairs) bounds[2 * j + 1] -= (int32_t)lo;
+    }
+}
+
+// A resized frame under OpenCV's filters: the blocks of rule 2 (and the copy) read C from the window's first block on; rules 1, 3
+// and 4 run the two passes over what their tables read.
+static void plan_cv_frame(const b200jpg_batch &b, int i, ResampleFrame &f, std::array<std::vector<int32_t>, 4> &t, b200jpg_rect &c) {
+    const CvPlan cp = cv_plan(b, i);
+    const b200jpg_size &s = b.plan[i].target;
+    const b200jpg_rect &wn = b.plan[i].window;
+    const uint32_t wx = rect_empty(wn) ? 0 : wn.x, wy = rect_empty(wn) ? 0 : wn.y;
+    if (cp.rule == 0 || cp.rule == 2) {
+        f.fx = (uint32_t)cp.fx, f.fy = (uint32_t)cp.fy;
+        c.x += wx * f.fx, c.y += wy * f.fy, c.width = f.tw * f.fx, c.height = f.th * f.fy;
+        f.w = c.width, f.h = c.height;
+        return;
+    }
+    f.pass = kPassH | kPassV | (cp.rule == 3 ? kPassArea : 0u);
+    const int table = b.resample | (cp.rule == 4 ? B200JPG_CV_TABLE_LINEAR : 0);
+    uint32_t x0, x1, y0, y1;
+    plan_cv_axis(c.width, s.width, wx, f.tw, table, cp.rule != 3, t[0], t[1], f.h_ksize, x0, x1);
+    plan_cv_axis(c.height, s.height, wy, f.th, table | B200JPG_CV_TABLE_VERTICAL, cp.rule != 3, t[2], t[3], f.v_ksize, y0, y1);
+    f.w = x1 - x0, f.h = y1 - y0;
+    c.x += x0, c.y += y0, c.width = f.w, c.height = f.h;
+}
+
 // The resample descriptors and tables of the resized frames (tables built on host threads, one frame each) and the layout of the
 // scratch (C: c_h rows of align16(c_w * ncomp) bytes per frame, then R where the frame reduces) and of the intermediate (rows y0 ..
 // y1 - 1 of tw * ncomp bytes, for frames with a horizontal pass). The grey frames of B200JPG_FLAG_OUTPUT_RGB come last, with one
@@ -1582,6 +1662,19 @@ static void plan_resample(b200jpg_batch &b) {
         const b200jpg_rect &wn = plan.window;
         ResampleFrame &f = b.rs_frames[r];
         auto &t = b.rs_tables[r];
+        f.ncomp = plan.mode == OutMode::Replicate ? plan.ncomp : plan.out_ncomp;
+        f.plane = (uint32_t)(b.n + r);
+        if (resample_cv(b.resample)) {  // (DESIGN §20)
+            f.tw = rect_empty(wn) ? s.width : wn.width, f.th = rect_empty(wn) ? s.height : wn.height;
+            f.fx = f.fy = 1;
+            plan_cv_frame(b, i, f, t, c);
+            f.c_w = c.width, f.c_h = c.height;
+            f.c_pitch = f.src_pitch = (uint32_t)align_up((uint64_t)f.w * f.ncomp, 16);
+            f.y0 = 0, f.y1 = f.h;
+            if (f.src_pitch <= kResampleRowSmem) f.stage |= kStageRow;
+            if ((f.pass & kPassH) && align_up(t[1].size() * sizeof(int32_t), 16) <= kResampleCoefSmem) f.stage |= kStageCoef;
+            return;
+        }
         const ReducePlan rp = reduce_plan(b, i);
         const bool reduces = rp.fx > 1 || rp.fy > 1;
         f.fx = (uint32_t)rp.fx, f.fy = (uint32_t)rp.fy;
@@ -1598,7 +1691,6 @@ static void plan_resample(b200jpg_batch &b) {
         plan_axis(sw, plain ? nullptr : fbh, s.width, wn.x, f.tw, b.resample, f.pass & kPassH, t[0], t[1], f.h_ksize, x0, x1);
         plan_axis(sh, plain ? nullptr : fbv, s.height, wn.y, f.th, b.resample, f.pass & kPassV, t[2], t[3], f.v_ksize, y0, y1);
         f.w = x1 - x0, f.h = y1 - y0;
-        f.ncomp = plan.mode == OutMode::Replicate ? plan.ncomp : plan.out_ncomp;
         f.src_pitch = (uint32_t)align_up((uint64_t)f.w * f.ncomp, 16);
         if (reduces) {  // R's blocks x0 .. x1 - 1, y0 .. y1 - 1: the pixels of C they cover (the last ones partial only at rb's edges)
             const uint64_t cx = rp.rb[0] + (uint64_t)x0 * rp.fx, cy = rp.rb[1] + (uint64_t)y0 * rp.fy;
@@ -1610,22 +1702,23 @@ static void plan_resample(b200jpg_batch &b) {
         }
         f.c_w = c.width, f.c_h = c.height;
         f.c_pitch = (uint32_t)align_up((uint64_t)f.c_w * f.ncomp, 16);
-        f.plane = (uint32_t)(b.n + r);
         f.y0 = 0, f.y1 = f.h;
         if (f.src_pitch <= kResampleRowSmem) f.stage |= kStageRow;
         if ((f.pass & kPassH) && align_up(t[1].size() * sizeof(int32_t), 16) <= kResampleCoefSmem) f.stage |= kStageCoef;
     });
+    const bool cv = resample_cv(b.resample);
     for (ResampleFrame &f : b.rs_frames) {
         f.c_src = f.src = b.scratch_bytes;
         b.scratch_bytes = align_up(b.scratch_bytes + (uint64_t)f.c_pitch * f.c_h, 256);
-        if (f.fx > 1 || f.fy > 1) {  // R behind C
+        if (cv) b.rs_cv_kinds |= !f.pass ? kCvBlocks : (f.pass & kPassArea) ? kCvArea : kCvLinear;
+        if (!cv && (f.fx > 1 || f.fy > 1)) {  // R behind C
             f.src = b.scratch_bytes;
             b.scratch_bytes = align_up(b.scratch_bytes + (uint64_t)f.src_pitch * f.h, 256);
             b.rs_max_reduce_rows = std::max(b.rs_max_reduce_rows, f.h);
         }
         if (f.pass & kPassH) {
             f.inter = b.inter_bytes;
-            b.inter_bytes = align_up(b.inter_bytes + (uint64_t)(f.y1 - f.y0) * f.tw * f.ncomp, 256);
+            b.inter_bytes = align_up(b.inter_bytes + (uint64_t)(f.y1 - f.y0) * f.tw * f.ncomp * (cv ? 4 : 1), 256);  // (cv: int32 / float)
             b.rs_max_rows = std::max(b.rs_max_rows, f.y1 - f.y0);
         }
         b.rs_max_pixels = std::max(b.rs_max_pixels, (uint64_t)f.tw * f.th);
@@ -1661,8 +1754,10 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
         if ((sizes[i].width == 0) != (sizes[i].height == 0))
             return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": target size " + std::to_string(sizes[i].width) + " x " +
                                                                 std::to_string(sizes[i].height) + " has exactly one zero side");
-        if (!size_empty(sizes[i]) && !resample_known(resample))
+        if (!size_empty(sizes[i]) && !resample_known(resample) && !resample_cv(resample))
             return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": unknown resample filter " + std::to_string(resample));
+        if (!size_empty(sizes[i]) && resample_cv(resample) && reducing_gap > 0.0)
+            return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": OpenCV's resize takes no reducing_gap");
         any_size = any_size || !size_empty(sizes[i]);
     }
     if (!any_size) sizes = nullptr;  // all {0, 0}: exactly the batch of b200jpg_batch_create_crop
@@ -1705,7 +1800,7 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
         if (b.parse_status[i] == 0) frame_plan(b, i);
     if (int rc = admit_crops(b, rects)) return rc;
     if (int rc = admit_sizes(b)) return rc;
-    if (boxes || windows || b.gap > 0.0)
+    if (boxes || windows || b.gap > 0.0 || resample_cv(b.resample))
         if (int rc = admit_boxes(b, boxes, windows)) return rc;
     plan_resample(b);  // (before the reconstruction groups: it trims the rectangles of resized frames)
     for (int i = n; i < b.n; i++)  // JPEG XT residual codestreams: their frames' records, their own components
@@ -2187,6 +2282,8 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         rl.planes = planes_dev;
         rl.convert = convert;
         rl.n_plain = std::min(rl.n_frames, b->rs_plain > first ? b->rs_plain - first : 0u);
+        rl.resample = b->resample;
+        rl.cv_kinds = b->rs_cv_kinds;
         int launches = 0;
         int rc = launch_resample(rl, stream, &launches);
         if (rc != 0) return b->ctx->fail_cuda((cudaError_t)rc, "resample kernel launch");

@@ -410,6 +410,14 @@ struct ResampleFrame {
 };
 constexpr uint32_t kStageRow = 1, kStageCoef = 2;
 constexpr uint32_t kPassH = 1, kPassV = 2;
+// OpenCV's filters (DESIGN §20) reuse the descriptor: a frame with kPassH | kPassV runs cv_resample_h_kernel into an intermediate
+// of 4 bytes per sample and cv_resample_v_kernel, with rule 3's float tables where kPassArea is set and the two-tap int16 tables of
+// rules 1 / 4 otherwise (bounds: the two rebased source indices); a frame with no pass bit sums fx x fy blocks of the source
+// (rule 2; 1 x 1 for a copy) in cv_area_block_kernel.
+constexpr uint32_t kPassArea = 4;
+int cv_resample_coefficients(uint32_t in_size, uint32_t out_size, int table, std::vector<int32_t> &bounds, std::vector<int32_t> &coef,
+                             uint32_t &ksize);
+constexpr uint32_t kCvLinear = 1, kCvArea = 2, kCvBlocks = 4;  // ResampleLaunch::cv_kinds: the frame kinds of a cv batch
 constexpr uint32_t kResampleRowSmem = 16 * 1024, kResampleCoefSmem = 32 * 1024;  // the shared buffers of resample_h_kernel
 constexpr uint32_t kResampleRows = 8;                                            // rows of the intermediate per CTA
 constexpr uint32_t kReduceRows = 4;                                              // rows of R per reduce_kernel CTA
@@ -426,6 +434,8 @@ struct ResampleLaunch {
     const b200jpg_convert *convert;  // host; null: uint8 destinations
     uint32_t n_plain;             // frames [n_plain, n_frames) are grey frames of B200JPG_FLAG_OUTPUT_RGB: one channel in the scratch and
                                   // the intermediate, each resampled value stored to three destinations
+    int resample;                 // the batch's B200JPG_RESAMPLE_*: OpenCV's filters take the cv kernels
+    uint32_t cv_kinds;            // kCvLinear / kCvArea / kCvBlocks: which cv kernels some frame needs
 };
 int launch_resample(const ResampleLaunch &l, void *stream, int *launches);
 

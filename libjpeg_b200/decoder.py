@@ -309,7 +309,8 @@ def reducing_gap_value(gap):
 
 
 def resample_filter(name):
-    """B200JPG_RESAMPLE_* of a filter name: "box", "bilinear", "hamming", "bicubic" or "lanczos". Raises ValueError."""
+    """B200JPG_RESAMPLE_* of a filter name: Pillow's "box", "bilinear", "hamming", "bicubic" or "lanczos", or OpenCV's
+    "cv2-linear" or "cv2-area" (INTER_LINEAR / INTER_AREA, DESIGN §20). Raises ValueError."""
     if not isinstance(name, str) or name not in native.RESAMPLE:
         raise ValueError("resample must be one of %s, got %r" % (", ".join(sorted(native.RESAMPLE)), name))
     return native.RESAMPLE[name]
@@ -524,7 +525,8 @@ class BatchDecoder:
         resize (b200jpg_batch_create_resize) is one (h, w) for every frame, or one entry per frame: None, or (h, w). The frame's
         output -- after downscaling, Exif orientation and the crop -- is then resized to h x w with `resample`, one of "box",
         "bilinear", "hamming", "bicubic" and "lanczos": bit for bit what PIL's Image.resize((w, h), filter) gives for that uint8
-        image (DESIGN §13), and a float destination of decode_into() receives the resized samples through its map.
+        image (DESIGN §13), and a float destination of decode_into() receives the resized samples through its map; OpenCV's
+        "cv2-linear" and "cv2-area" are described below.
         output_shape(), geometry(), frame_view() and the destinations of decode_into() are then h x w, so one [N, C, h, w] tensor
         takes frames of any size. status(i) is the frame's status without the size; a 12-bit frame with a size is
         B200JPG_ERR_NOT_IMPLEMENTED, and a size with upsample=False raises NativeError (B200JPG_ERR_NOT_IMPLEMENTED). A wrong length,
@@ -578,7 +580,16 @@ class BatchDecoder:
         reconstructed. thumbnail_args(), fit_args() and resize_center_crop_args() give the entries of Pillow's thumbnail(),
         ImageOps.fit() and torchvision's Resize + CenterCrop. A box or window on a frame without a size, a box outside C, a window
         outside h x w, or a reduce box that is empty raises NativeError (B200JPG_ERR_INVALID_PARAMETER); a wrong length, an entry
-        of the wrong form, a box that is not finite or has x1 < x0 or y1 < y0 and a reducing_gap below 1.0 raise ValueError."""
+        of the wrong form, a box that is not finite or has x1 < x0 or y1 < y0 and a reducing_gap below 1.0 raise ValueError.
+
+        resample="cv2-linear" or "cv2-area" (B200JPG_RESAMPLE_CV_LINEAR / _CV_AREA, DESIGN §20) resizes as OpenCV does instead of
+        Pillow: the frame is written, byte for byte, as
+            cv2.resize(C, (w, h), interpolation=cv2.INTER_LINEAR or cv2.INTER_AREA)[y:y + height, x:x + width]
+        of OpenCV 4.13, with C the frame's image without the size and (x, y, width, height) the window (the whole h x w image
+        without one). With reconstruction="libjpeg-turbo", C of a YCbCr or grey frame is cv2.imdecode(data, IMREAD_COLOR)
+        in RGB order (IMREAD_GRAYSCALE under mode "L"), so an OpenCV loader's pixels come out unchanged; a BGR tensor is a
+        decode_into() with the planes in the other order. cv2.resize has no box and no reducing_gap: either with a cv2 filter
+        raises NativeError (B200JPG_ERR_INVALID_PARAMETER)."""
         if not isinstance(mode, (str, type(None))) or mode not in native.MODE_FLAGS:
             raise ValueError('mode must be None, "RGB" or "L", got %r' % (mode,))
         if not isinstance(reconstruction, str) or reconstruction not in native.RECONSTRUCTION_FLAGS:

@@ -59,6 +59,8 @@ MODE_FLAGS = {None: 0x0, "RGB": 0x20, "L": 0x40}  # B200JPG_FLAG_OUTPUT_RGB / _L
 RECONSTRUCTION_FLAGS = {"reference": 0x0, "libjpeg-turbo": 0x80}  # B200JPG_FLAG_LIBJPEG_TURBO
 COLORSPACES = [None, "L", "YCbCr", "RGB", "CMYK", "YCCK"]  # B200JPG_COLORSPACE_UNKNOWN .. _YCCK, named after PIL's modes
 RESAMPLE = {"lanczos": 1, "bilinear": 2, "bicubic": 3, "box": 4, "hamming": 5}  # B200JPG_RESAMPLE_*, PIL's values
+# B200JPG_RESAMPLE_CV_*: OpenCV's cv2.resize, 0x100 | cv2.INTER_LINEAR / cv2.INTER_AREA (DESIGN §20)
+RESAMPLE.update({"cv2-linear": 0x101, "cv2-area": 0x103})
 
 
 def library_path():
