@@ -20,6 +20,7 @@
  *                            YCbCrTrafo::YCbCr2RGB                      colortrafo/ycbcrtrafo.cpp:679
  *   b200jpg_batch_decode_into  the same, into per-component ImageBitMaps interface/imagebitmap.hpp:104-109
  *   b200jpg_batch_decode_into_ex  the same, samples converted to float32 / float16 / bfloat16 on the way out (no counterpart)
+ *   b200jpg_batch_decode_into_table  the same, every sample looked up in a per-component table (no counterpart)
  *   b200jpg_last_error       JPEG::LastError                            interface/jpeg.cpp:962
  *
  * Error codes are the reference's (interface/parameters.hpp:1156-1228).
@@ -328,6 +329,24 @@ B200JPG_API int b200jpg_batch_create_resample(b200jpg_ctx *ctx, const uint8_t *c
                                               unsigned flags, const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes,
                                               const b200jpg_box *boxes, const b200jpg_rect *windows, int resample, double reducing_gap,
                                               b200jpg_batch **batch);
+/* The flips of b200jpg_batch_create_flip, or-ed into one entry per frame. */
+#define B200JPG_FLIP_H 1
+#define B200JPG_FLIP_V 2
+/* b200jpg_batch_create_resample with a flip per frame (DESIGN §21; no counterpart in the reference), torchvision's
+ * RandomHorizontalFlip / RandomVerticalFlip and PIL's FLIP_LEFT_RIGHT / FLIP_TOP_BOTTOM. The flip is the last geometric step:
+ * draft / downscale -> mode -> orientation -> crop -> resize -> window -> flip -> float map. Let O be what frame i is written as
+ * without it ([h, w, C]); with flips[i] it is written as O[:, ::-1] (B200JPG_FLIP_H), O[::-1, :] (B200JPG_FLIP_V) or O[::-1, ::-1]
+ * (both), for every destination kind; with B200JPG_FLAG_NO_UPSAMPLE every plane is flipped at its own extent. Rectangles, sizes,
+ * boxes and windows keep their coordinates (those of the unflipped image). A flip changes no extent, out_bytes / out_offset,
+ * status or b200jpg_batch_frame_orientation (the Exif value). A flipped frame without a size is planned as the frame of the
+ * composed orientation, its rectangle mirrored, and joins that orientation's reconstruction group; a resized frame's resample
+ * pass stores mirrored, with the launches of the unflipped batch. flips == NULL, or every entry 0: exactly
+ * b200jpg_batch_create_resample. An entry with any other bit set is B200JPG_ERR_INVALID_PARAMETER for the call, tolerate_bad or not,
+ * the frame named in the message. The flip of a frame that fails to parse is ignored. */
+B200JPG_API int b200jpg_batch_create_flip(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad,
+                                          unsigned flags, const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes,
+                                          const b200jpg_box *boxes, const b200jpg_rect *windows, int resample, double reducing_gap,
+                                          const uint8_t *flips, b200jpg_batch **batch);
 /* Pillow's draft scale of one codestream for a requested width x height (host only): s = min(W / width, H / height) in integer
  * division over the codestream's own W x H (before any Exif orientation), and the largest k of 8, 4, 2, 1 with k <= s, or 1 when
  * none fits. Returns k, or the negative parse error of the codestream; a zero width or height is B200JPG_ERR_INVALID_PARAMETER. */
@@ -443,6 +462,19 @@ typedef struct b200jpg_convert {
  * kernel launches. */
 B200JPG_API int b200jpg_batch_decode_into_ex(b200jpg_batch *batch, const b200jpg_plane *planes, const b200jpg_convert *convert,
                                              void *stream);
+/* Per-component sample tables (DESIGN §22; host memory): every 8-bit sample v of output component c that
+ * b200jpg_batch_decode_into would write is written as table[c][v], stored as float32, or rounded to nearest even into float16
+ * (overflow -> inf, subnormals kept) or bfloat16, as b200jpg_convert's results are. A table holds any per-sample map exactly:
+ * torchvision's ToTensor() + Normalize(mean, std) (three roundings, two divisions), gamma or sRGB curves, dequantisation. */
+typedef struct b200jpg_convert_table {
+    int32_t type; /* B200JPG_SAMPLE_* */
+    float table[B200JPG_MAX_COMPONENTS][256];
+} b200jpg_convert_table;
+/* b200jpg_batch_decode_into_ex with the map replaced by `table`: the same descriptor rules, positions written and kernel launches
+ * (the tables ride the call's one descriptor copy). B200JPG_ERR_INVALID_PARAMETER, with nothing launched: a NULL table or an
+ * unknown type; B200JPG_ERR_NOT_IMPLEMENTED: a batch with a live 12-bit frame. */
+B200JPG_API int b200jpg_batch_decode_into_table(b200jpg_batch *batch, const b200jpg_plane *planes, const b200jpg_convert_table *table,
+                                                void *stream);
 /* Only one of the two stages (profiling / roofline measurements / parity of the intermediate). */
 B200JPG_API int b200jpg_batch_decode_entropy(b200jpg_batch *batch, void *stream);
 B200JPG_API int b200jpg_batch_reconstruct(b200jpg_batch *batch, uint8_t *out_dev, void *stream);

@@ -5,4 +5,4 @@ shim, see ``include/``).  This Python package is the thin host layer used by the
 ctypes bindings of the C ABI, with PyTorch supplying device memory and streams only.
 """
 from .native import NativeError, lib, library_path  # noqa: F401
-from .decoder import BatchDecoder, FrameInfo, parse  # noqa: F401
+from .decoder import BatchDecoder, FrameInfo, parse, sample_table  # noqa: F401

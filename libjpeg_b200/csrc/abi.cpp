@@ -239,6 +239,10 @@ struct FramePlan {
     b200jpg_box box{};
     b200jpg_rect window{};
     int rs = -1;
+    // the caller's B200JPG_FLIP_H / _V (DESIGN §21). A frame without a size has it folded into `orientation` (frame_plan) and
+    // `crop` (admit_crops); a resized frame's resample pass stores through its destinations mirrored over the window
+    // (stage_frame_planes): the flip stays behind the resize, with which it does not commute
+    uint8_t flip = 0;
     // oriented, cropped (so resized) or written in an output mode: the reconstruction stores through the frame's destinations
     // rewritten into decoded coordinates (rewrite_frame), in place of the packed slot it takes otherwise
     bool described = false;
@@ -312,6 +316,28 @@ Clip crop_to_decoded(int o, const b200jpg_rect &r, uint64_t w, uint64_t h) {
     case 8: return {W - v1, u0, W - v0, u1};
     default: return {u0, v0, u1, v1};
     }
+}
+
+// The orientation that writes F(T_o(D)), for the Exif orientation o (T_o: DESIGN §11) and the flip F (B200JPG_FLIP_H / _V bits,
+// DESIGN §21): the dihedral product, kFlipOrientation[o - 1][F]
+constexpr uint8_t kFlipOrientation[8][4] = {{1, 2, 4, 3}, {2, 1, 3, 4}, {3, 4, 2, 1}, {4, 3, 1, 2},
+                                            {5, 6, 8, 7}, {6, 5, 7, 8}, {7, 8, 6, 5}, {8, 7, 5, 6}};
+
+// The rectangle r of an image of extent w x h as the rectangle of the flipped image that holds the same samples
+b200jpg_rect flip_rect(const b200jpg_rect &r, uint32_t flip, uint64_t w, uint64_t h) {
+    b200jpg_rect m = r;
+    if (flip & B200JPG_FLIP_H) m.x = (uint32_t)(w - r.x - r.width);
+    if (flip & B200JPG_FLIP_V) m.y = (uint32_t)(h - r.y - r.height);
+    return m;
+}
+
+// A destination of a tw x th image made the destination of its flipped image: (x, y) goes where (tw - 1 - x, y) (B200JPG_FLIP_H)
+// and (x, th - 1 - y) (B200JPG_FLIP_V) went, as orient_plane mirrors for the orientations 2 and 4
+void flip_plane(b200jpg_plane &pl, uint32_t flip, uint64_t tw, uint64_t th) {
+    uint64_t a = reinterpret_cast<uintptr_t>(pl.data);
+    if (flip & B200JPG_FLIP_H) a += (uint64_t)((int64_t)(tw - 1) * pl.bytes_per_pixel), pl.bytes_per_pixel = -pl.bytes_per_pixel;
+    if (flip & B200JPG_FLIP_V) a += (uint64_t)((int64_t)(th - 1) * pl.bytes_per_row), pl.bytes_per_row = -pl.bytes_per_row;
+    pl.data = reinterpret_cast<void *>((uintptr_t)a);
 }
 
 // body(i) for every frame i < n, on at most max_threads host threads
@@ -388,7 +414,10 @@ struct b200jpg_batch {
     // b200jpg_batch_decode_into: the descriptor table [4 * n], staged in a ring of kPlaneSlots pinned copies and copied on the
     // call's stream; ev_planes[k] is recorded behind the copy out of slot k, which is rewritten only after it. With several
     // slots the host may run that many calls ahead of the device.
+    // Behind the table, 256-byte aligned, each slot has room for the 4 KB of sample tables of b200jpg_batch_decode_into_table, which
+    // ride the same copy.
     static constexpr int kPlaneSlots = 3;
+    static constexpr uint64_t kTableBytes = sizeof(float) * B200JPG_MAX_COMPONENTS * 256;
     b200jpg_plane *h_planes = nullptr, *d_planes = nullptr;
     cudaEvent_t ev_planes[kPlaneSlots] = {};
     int plane_slot = 0;
@@ -409,6 +438,8 @@ struct b200jpg_batch {
     uint8_t *d_scratch = nullptr, *d_inter = nullptr;  // C of every resized frame; the horizontal pass's rows
     uint64_t scratch_bytes = 0, inter_bytes = 0;
     size_t n_planes() const { return 4 * ((size_t)n + rs_frames.size()); }
+    uint64_t table_offset() const { return align_up(sizeof(b200jpg_plane) * n_planes(), 256); }  // of the sample tables in a slot
+    uint64_t slot_bytes() const { return table_offset() + kTableBytes; }
     int last_launches = 0;
     bool timing = false;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};  // start, after a0, after a1, after b
@@ -667,8 +698,8 @@ void b200jpg_batch_destroy(b200jpg_batch *b) {
     if (b->d_spec) b->ctx->put(1, b->d_spec, b->sz_spec);
     if (b->d_dcplane) b->ctx->put(1, b->d_dcplane, b->coef_elems / 64 * sizeof(int16_t));
     b->ctx->put(1, b->d_status, b->sz_status);
-    b->ctx->put(0, b->h_planes, sizeof(b200jpg_plane) * b->n_planes() * b200jpg_batch::kPlaneSlots);
-    b->ctx->put(1, b->d_planes, sizeof(b200jpg_plane) * b->n_planes());
+    b->ctx->put(0, b->h_planes, b->slot_bytes() * b200jpg_batch::kPlaneSlots);
+    b->ctx->put(1, b->d_planes, b->slot_bytes());
     if (b->d_scratch) b->ctx->put(1, b->d_scratch, b->scratch_bytes);
     if (b->d_inter) b->ctx->put(1, b->d_inter, b->inter_bytes);
     for (auto &e : b->ev_planes)
@@ -889,6 +920,7 @@ static void frame_plan(b200jpg_batch &b, int i) {
     p.path = recon_path(b, i);
     p.ncomp = p.out_ncomp = fi.ncomp;
     p.orientation = (b.flags & B200JPG_FLAG_EXIF_ORIENTATION) ? b.frames[i].orientation : 1;
+    if (size_empty(p.target)) p.orientation = kFlipOrientation[p.orientation - 1][p.flip];  // (DESIGN §21)
     const bool xt = b.xt_child[i] >= 0;
     if ((b.flags & B200JPG_FLAG_OUTPUT_L) && fi.ncomp == 3) {
         p.out_ncomp = 1;
@@ -1424,7 +1456,8 @@ static int admit_crops(b200jpg_batch &b, const b200jpg_rect *rects) {
             return b.ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": crop rectangle (" + std::to_string(r.x) + ", " +
                                                                   std::to_string(r.y) + ", " + std::to_string(r.width) + ", " + std::to_string(r.height) +
                                                                   ") is empty or leaves the " + std::to_string(e.w) + " x " + std::to_string(e.h) + " output");
-        p.crop = r;
+        // a flip without a size is in the orientation (frame_plan): r, given in the unflipped image, as a rectangle of the flipped one
+        p.crop = size_empty(p.target) ? flip_rect(r, p.flip, e.w, e.h) : r;
         p.cropped = p.described = true;
     }
     return B200JPG_OK;
@@ -1727,10 +1760,18 @@ static void plan_resample(b200jpg_batch &b) {
 
 static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
                              const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes, const b200jpg_box *boxes,
-                             const b200jpg_rect *windows, int resample, double reducing_gap, b200jpg_batch **out) {
+                             const b200jpg_rect *windows, int resample, double reducing_gap, const uint8_t *flips, b200jpg_batch **out) {
     NvtxRange nvtx("b200jpg batch_create: parse + pack");
     if (!out || !frames || !lens || n <= 0) return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "invalid batch arguments");
     *out = nullptr;
+    bool any_flip = false;
+    for (int i = 0; flips && i < n; i++) {
+        if (flips[i] & ~(B200JPG_FLIP_H | B200JPG_FLIP_V))
+            return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": flip " + std::to_string(flips[i]) +
+                                                                " has a bit other than B200JPG_FLIP_H and B200JPG_FLIP_V");
+        any_flip = any_flip || flips[i] != 0;
+    }
+    if (!any_flip) flips = nullptr;  // all zero: exactly the batch of b200jpg_batch_create_resample
     if (std::isnan(reducing_gap) || (reducing_gap > 0.0 && reducing_gap < 1.0))
         return ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "reducing_gap " + std::to_string(reducing_gap) + " is NaN or below 1.0");
     bool any_box = false;
@@ -1783,6 +1824,7 @@ static int batch_create_impl(b200jpg_ctx *ctx, const uint8_t *const *frames, con
     b.flags = flags;
     b.plan.assign(n, FramePlan{});
     for (int i = 0; sizes && i < n; i++) b.plan[i].target = sizes[i];  // (attach_residuals refuses 12-bit frames with a size)
+    for (int i = 0; flips && i < n; i++) b.plan[i].flip = flips[i];    // (read by frame_plan, admit_crops and the descriptor table)
     if (sizes) b.resample = resample, b.gap = reducing_gap;  // (gap <= 0: None)
     Codestreams cs;
     cs.data.assign(frames, frames + n);
@@ -1845,9 +1887,17 @@ int b200jpg_batch_create_draft(b200jpg_ctx *ctx, const uint8_t *const *frames, c
 int b200jpg_batch_create_resample(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
                                   const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes, const b200jpg_box *boxes,
                                   const b200jpg_rect *windows, int resample, double reducing_gap, b200jpg_batch **out) {
+    return b200jpg_batch_create_flip(ctx, frames, lens, n, tolerate_bad, flags, drafts, rects, sizes, boxes, windows, resample, reducing_gap,
+                                     nullptr, out);
+}
+
+int b200jpg_batch_create_flip(b200jpg_ctx *ctx, const uint8_t *const *frames, const size_t *lens, int n, int tolerate_bad, unsigned flags,
+                              const b200jpg_size *drafts, const b200jpg_rect *rects, const b200jpg_size *sizes, const b200jpg_box *boxes,
+                              const b200jpg_rect *windows, int resample, double reducing_gap, const uint8_t *flips, b200jpg_batch **out) {
     if (!ctx) return B200JPG_ERR_INVALID_PARAMETER;
     try {  // no exception crosses the C ABI
-        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, drafts, rects, sizes, boxes, windows, resample, reducing_gap, out);
+        return batch_create_impl(ctx, frames, lens, n, tolerate_bad, flags, drafts, rects, sizes, boxes, windows, resample, reducing_gap, flips,
+                                 out);
     } catch (const std::bad_alloc &) {
         if (out) *out = nullptr;
         return ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "out of host memory while preparing the batch");
@@ -2094,20 +2144,22 @@ static int run_entropy(b200jpg_batch *b, void *stream) {
 }
 
 // The descriptor table [b->n_planes()] that fill(table) writes (on zeros: residual codestreams and failed frames have no destination) to
-// b->d_planes on `stream`, staged in the next slot of the pinned ring (b200jpg_batch::kPlaneSlots)
-static int stage_planes(b200jpg_batch *b, void *stream, const std::function<void(b200jpg_plane *)> &fill) {
+// b->d_planes on `stream`, staged in the next slot of the pinned ring (b200jpg_batch::kPlaneSlots); with `table` (the 4 KB of
+// b200jpg_batch_decode_into_table) also the sample tables, at b->table_offset() of the slot, in the same copy
+static int stage_planes(b200jpg_batch *b, void *stream, const std::function<void(b200jpg_plane *)> &fill, const float *table = nullptr) {
     const size_t bytes = sizeof(b200jpg_plane) * b->n_planes();
+    const uint64_t slot_bytes = b->slot_bytes();
     cudaError_t ce = cudaSuccess;
     constexpr int kSlots = b200jpg_batch::kPlaneSlots;
     if (!b->d_planes) {  // everything is allocated before any of it is kept: a failure leaves the batch as it was
-        b200jpg_plane *h = (b200jpg_plane *)b->ctx->get(0, bytes * kSlots, &ce), *d = nullptr;
+        b200jpg_plane *h = (b200jpg_plane *)b->ctx->get(0, slot_bytes * kSlots, &ce), *d = nullptr;
         cudaEvent_t ev[kSlots] = {};
-        if (ce == cudaSuccess) d = (b200jpg_plane *)b->ctx->get(1, bytes, &ce);
+        if (ce == cudaSuccess) d = (b200jpg_plane *)b->ctx->get(1, slot_bytes, &ce);
         for (int k = 0; k < kSlots && ce == cudaSuccess; k++) ce = cudaEventCreateWithFlags(&ev[k], cudaEventDisableTiming);
         if (ce != cudaSuccess) {
             const std::string why = cudaGetErrorString(ce);
-            b->ctx->put(0, h, bytes * kSlots);
-            b->ctx->put(1, d, bytes);
+            b->ctx->put(0, h, slot_bytes * kSlots);
+            b->ctx->put(1, d, slot_bytes);
             for (auto &e : ev)
                 if (e) cudaEventDestroy(e);
             return b->ctx->fail(B200JPG_ERR_OUT_OF_MEMORY, "descriptor table allocation failed: " + why);
@@ -2118,10 +2170,12 @@ static int stage_planes(b200jpg_batch *b, void *stream, const std::function<void
     const int slot = b->plane_slot;
     ce = cudaEventSynchronize(b->ev_planes[slot]);  // the copy kSlots calls ago has read this slot (at once when never recorded)
     if (ce != cudaSuccess) return b->ctx->fail_cuda(ce, "descriptor table");
-    b200jpg_plane *stage = b->h_planes + b->n_planes() * slot;
+    uint8_t *base = reinterpret_cast<uint8_t *>(b->h_planes) + slot_bytes * slot;
+    b200jpg_plane *stage = reinterpret_cast<b200jpg_plane *>(base);
     memset(stage, 0, bytes);
     fill(stage);
-    ce = cudaMemcpyAsync(b->d_planes, stage, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream);
+    if (table) memcpy(base + b->table_offset(), table, b200jpg_batch::kTableBytes);
+    ce = cudaMemcpyAsync(b->d_planes, stage, table ? slot_bytes : bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream);
     if (ce == cudaSuccess) ce = cudaEventRecord(b->ev_planes[slot], (cudaStream_t)stream);
     b->plane_slot = (slot + 1) % kSlots;
     if (ce != cudaSuccess) return b->ctx->fail_cuda(ce, "descriptor table upload");
@@ -2165,16 +2219,21 @@ static bool place_frame(const b200jpg_batch *b, int i, b200jpg_plane *q, uint64_
 }
 
 // The descriptor table of a decode (staged: stage_planes): every live frame's placed destinations q (place_frame), and the
-// destinations of resized frame r, as given in `planes`, at 4 * (n + r) for the resample pass ([4 * n_user] each)
-static int stage_frame_planes(b200jpg_batch *b, const b200jpg_plane *q, const b200jpg_plane *planes, void *stream) {
+// destinations of resized frame r, as given in `planes`, at 4 * (n + r) for the resample pass ([4 * n_user] each), mirrored over
+// the window's tw x th for a flipped frame (flip_plane); the sample tables behind them (stage_planes)
+static int stage_frame_planes(b200jpg_batch *b, const b200jpg_plane *q, const b200jpg_plane *planes, void *stream, const float *table = nullptr) {
     return stage_planes(b, stream, [&](b200jpg_plane *table) {
         for (int i = 0; i < b->n_user; i++) {
             const FramePlan &p = b->plan[i];
             if (b->parse_status[i] != 0) continue;
             memcpy(table + 4 * (size_t)i, q + 4 * (size_t)i, sizeof(b200jpg_plane) * p.out_ncomp);
-            if (p.resized) memcpy(table + 4 * ((size_t)b->n + p.rs), planes + 4 * (size_t)i, sizeof(b200jpg_plane) * p.out_ncomp);
+            if (!p.resized) continue;
+            b200jpg_plane *rs = table + 4 * ((size_t)b->n + p.rs);
+            memcpy(rs, planes + 4 * (size_t)i, sizeof(b200jpg_plane) * p.out_ncomp);
+            const ResampleFrame &f = b->rs_frames[(size_t)p.rs];
+            for (uint32_t c = 0; p.flip && c < p.out_ncomp; c++) flip_plane(rs[c], p.flip, f.tw, f.th);
         }
-    });
+    }, table);
 }
 
 // b200jpg_batch_decode of a batch with described frames: each such frame's packed slot in out_dev, described as a caller of
@@ -2204,9 +2263,10 @@ static int stage_slot_planes(b200jpg_batch *b, uint8_t *out_dev, void *stream, s
 }
 
 // planes_dev: b200jpg_batch_decode_into's descriptor table (device), planar[i]: every component of frame i has
-// bytes_per_pixel == sample size (element size with `convert`, the float map of b200jpg_batch_decode_into_ex)
+// bytes_per_pixel == sample size (element size with `convert`, the float map of b200jpg_batch_decode_into_ex); table: with
+// `convert`, the sample tables of b200jpg_batch_decode_into_table (device)
 static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b200jpg_plane *planes_dev = nullptr,
-                     const std::vector<char> *planar = nullptr, const b200jpg_convert *convert = nullptr) {
+                     const std::vector<char> *planar = nullptr, const b200jpg_convert *convert = nullptr, const float *table = nullptr) {
     NvtxRange nvtx("b200jpg reconstruction: IDCT + upsampling + colour");
     // into the packed slots with described frames: those frames' slots as descriptors, built for this call's out_dev; the groups of
     // the other frames store into out_dev
@@ -2243,7 +2303,8 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         l.out = out_dev;
         l.planes = (out_dev && !g.key.described) ? nullptr : planes_dev;
         l.convert = convert;
-        if (g.key.resized) l.convert = nullptr;  // C leaves as uint8; the resample pass converts
+        l.table = table;
+        if (g.key.resized) l.convert = nullptr, l.table = nullptr;  // C leaves as uint8; the resample pass converts
         l.planar = l.planes != nullptr;
         if (l.planes)
             for (const FrameRecon &fr : g.frames) l.planar = l.planar && (*planar)[fr.status_idx];
@@ -2281,6 +2342,7 @@ static int run_recon(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b20
         rl.inter = b->d_inter;
         rl.planes = planes_dev;
         rl.convert = convert;
+        rl.table = table;
         rl.n_plain = std::min(rl.n_frames, b->rs_plain > first ? b->rs_plain - first : 0u);
         rl.resample = b->resample;
         rl.cv_kinds = b->rs_cv_kinds;
@@ -2300,7 +2362,7 @@ static int ensure_events(b200jpg_batch *b) {
 }
 
 static int run_decode(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b200jpg_plane *planes_dev = nullptr,
-                      const std::vector<char> *planar = nullptr, const b200jpg_convert *convert = nullptr) {
+                      const std::vector<char> *planar = nullptr, const b200jpg_convert *convert = nullptr, const float *table = nullptr) {
     b->last_launches = 0;
     b->status_fetched = false;
     if (b->timing) {
@@ -2310,7 +2372,7 @@ static int run_decode(b200jpg_batch *b, uint8_t *out_dev, void *stream, const b2
     int rc = run_entropy(b, stream);
     if (rc) return rc;
     if (b->timing) cudaEventRecord(b->ev[1], (cudaStream_t)stream);
-    rc = run_recon(b, out_dev, stream, planes_dev, planar, convert);
+    rc = run_recon(b, out_dev, stream, planes_dev, planar, convert, table);
     if (rc) return rc;
     if (b->timing) cudaEventRecord(b->ev[2], (cudaStream_t)stream);
     return B200JPG_OK;
@@ -2329,23 +2391,15 @@ int b200jpg_batch_decode_into(b200jpg_batch *b, const b200jpg_plane *planes, voi
     return b200jpg_batch_decode_into_ex(b, planes, nullptr, stream);
 }
 
-int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, const b200jpg_convert *convert, void *stream) {
-    if (!b || !planes) return B200JPG_ERR_INVALID_PARAMETER;
-    if (!b->uploaded) return b->ctx->fail(B200JPG_ERR_OBJECT_DOESNT_EXIST, "batch has not been uploaded");
-    cudaSetDevice(b->ctx->device);
-    // the map and every descriptor of every live frame are checked before anything is enqueued
-    uint64_t element = 0;  // float destinations: the element size replaces the sample size
-    if (convert) {
-        if (convert->type == B200JPG_SAMPLE_F32) element = 4;
-        else if (convert->type == B200JPG_SAMPLE_F16 || convert->type == B200JPG_SAMPLE_BF16) element = 2;
-        else return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "unknown sample type " + std::to_string(convert->type));
-        int ncomp = 0;  // the components some live frame is written with
-        for (int i = 0; i < b->n_user; i++)
-            if (b->parse_status[i] == 0) ncomp = std::max(ncomp, (int)b->plan[i].out_ncomp);
-        for (int c = 0; c < ncomp; c++)
-            if (!std::isfinite(convert->scale[c]) || !std::isfinite(convert->bias[c]))
-                return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "component " + std::to_string(c) + ": scale and bias must be finite");
-    }
+// the bytes of one float element of B200JPG_SAMPLE_* `type`; 0 for an unknown type
+static uint64_t element_size(int32_t type) {
+    return type == B200JPG_SAMPLE_F32 ? 4 : ((type == B200JPG_SAMPLE_F16 || type == B200JPG_SAMPLE_BF16) ? 2 : 0);
+}
+
+// b200jpg_batch_decode_into(_ex, _table) once the map is checked: every descriptor of every live frame is checked before anything
+// is enqueued, then placed, staged (with the sample tables of `table`, host) and decoded into
+static int decode_into_checked(b200jpg_batch *b, const b200jpg_plane *planes, const b200jpg_convert *convert, const float *table, void *stream) {
+    const uint64_t element = convert ? element_size(convert->type) : 0;  // float destinations: the element size replaces the sample size
     std::vector<char> planar((size_t)b->n, 1);
     std::vector<b200jpg_plane> q(planes, planes + 4 * (size_t)b->n_user);  // placed once here (place_frame)
     for (int i = 0; i < b->n_user; i++) {
@@ -2375,8 +2429,39 @@ int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, 
         if (!place_frame(b, i, &q[4 * (size_t)i], size, planar))
             return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "frame " + std::to_string(i) + ": |bytes_per_row| does not fit the pixel stride of the transposed frame");
     }
-    if (int rc = stage_frame_planes(b, q.data(), planes, stream)) return rc;
-    return run_decode(b, nullptr, stream, b->d_planes, &planar, convert);
+    if (int rc = stage_frame_planes(b, q.data(), planes, stream, table)) return rc;
+    const float *table_dev = table ? reinterpret_cast<const float *>(reinterpret_cast<uint8_t *>(b->d_planes) + b->table_offset()) : nullptr;
+    return run_decode(b, nullptr, stream, b->d_planes, &planar, convert, table_dev);
+}
+
+int b200jpg_batch_decode_into_ex(b200jpg_batch *b, const b200jpg_plane *planes, const b200jpg_convert *convert, void *stream) {
+    if (!b || !planes) return B200JPG_ERR_INVALID_PARAMETER;
+    if (!b->uploaded) return b->ctx->fail(B200JPG_ERR_OBJECT_DOESNT_EXIST, "batch has not been uploaded");
+    cudaSetDevice(b->ctx->device);
+    if (convert) {
+        if (!element_size(convert->type)) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "unknown sample type " + std::to_string(convert->type));
+        int ncomp = 0;  // the components some live frame is written with
+        for (int i = 0; i < b->n_user; i++)
+            if (b->parse_status[i] == 0) ncomp = std::max(ncomp, (int)b->plan[i].out_ncomp);
+        for (int c = 0; c < ncomp; c++)
+            if (!std::isfinite(convert->scale[c]) || !std::isfinite(convert->bias[c]))
+                return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "component " + std::to_string(c) + ": scale and bias must be finite");
+    }
+    return decode_into_checked(b, planes, convert, nullptr, stream);
+}
+
+int b200jpg_batch_decode_into_table(b200jpg_batch *b, const b200jpg_plane *planes, const b200jpg_convert_table *table, void *stream) {
+    if (!b || !planes) return B200JPG_ERR_INVALID_PARAMETER;
+    if (!b->uploaded) return b->ctx->fail(B200JPG_ERR_OBJECT_DOESNT_EXIST, "batch has not been uploaded");
+    cudaSetDevice(b->ctx->device);
+    if (!table) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "no sample table");
+    if (!element_size(table->type)) return b->ctx->fail(B200JPG_ERR_INVALID_PARAMETER, "unknown sample type " + std::to_string(table->type));
+    for (int i = 0; i < b->n_user; i++)
+        if (b->parse_status[i] == 0 && b->frames[i].info.precision > 8)
+            return b->ctx->fail(B200JPG_ERR_NOT_IMPLEMENTED, "frame " + std::to_string(i) + ": 12-bit samples have no 256-entry sample table");
+    b200jpg_convert convert{};  // the element type; the tables replace the map
+    convert.type = table->type;
+    return decode_into_checked(b, planes, &convert, &table->table[0][0], stream);
 }
 
 int b200jpg_batch_decode_entropy(b200jpg_batch *b, void *stream) {

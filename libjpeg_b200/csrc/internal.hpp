@@ -353,6 +353,9 @@ struct ReconLaunch {
     // b200jpg_batch_decode_into_ex: the samples leave as float32 / float16 / bfloat16 through this map (host memory, passed to
     // the kernels by value); null: as integers
     const b200jpg_convert *convert;
+    // b200jpg_batch_decode_into_table: with `convert` (its type), every sample v of output component c leaves as table[256 c + v]
+    // (device); null: through the map
+    const float *table;
 };
 
 // How the reconstruction kernels store a block (the destination kind of the launch, chosen per group from the descriptors):
@@ -365,23 +368,31 @@ struct ReconLaunch {
 // interleaved slot as 24-byte runs of pixels; whatever has no contiguous axis, one store per sample.
 // kStoreClip, or-ed into kStoreRuns / kStoreRunsF / kStoreStrided / kStoreStridedF (groups of cropped frames): the CTAs run the tiles
 // from FrameRecon::tx0 / ty0 on and store only inside the frame's clip rectangle; kBaseKind strips it.
-enum StoreKind : int { kStoreCanvas = 0, kStorePlanar = 1, kStoreStrided = 2, kStorePlanarF = 3, kStoreStridedF = 4, kStoreRuns = 5, kStoreRunsF = 6, kStoreClip = 8 };
+// kStoreTable, or-ed into the float kinds (b200jpg_batch_decode_into_table): every sample leaves through FloatDst::table in place of
+// the map. A bit of its own, so that the lookup is compiled out of the affine instances: in the 4:2:0 kernels it costs registers.
+enum StoreKind : int { kStoreCanvas = 0, kStorePlanar = 1, kStoreStrided = 2, kStorePlanarF = 3, kStoreStridedF = 4, kStoreRuns = 5, kStoreRunsF = 6, kStoreClip = 8,
+                       kStoreTable = 16 };
 template <int k>
-constexpr int kBaseKind = k & ~kStoreClip;
+constexpr int kBaseKind = k & ~(kStoreClip | kStoreTable);
 template <int k>
 constexpr bool kClipKind = (k & kStoreClip) != 0;
 template <int k>
+constexpr bool kTableKind = (k & kStoreTable) != 0;
+template <int k>
 constexpr bool kFloatKind = kBaseKind<k> == kStorePlanarF || kBaseKind<k> == kStoreStridedF || kBaseKind<k> == kStoreRunsF;
 
-// the destination argument of the float kinds: the descriptors plus the map, both in the kernel's parameter bank
+// the destination argument of the float kinds: the descriptors plus the map, both in the kernel's parameter bank, and the
+// per-component sample tables of b200jpg_batch_decode_into_table (device, 256 floats per component; null: the map), a
+// launch-uniform switch like the element type
 struct FloatDst {
     const b200jpg_plane *planes;
     int32_t type;
     float scale[B200JPG_MAX_COMPONENTS], bias[B200JPG_MAX_COMPONENTS];
+    const float *table;
 };
 int launch_recon(const ReconLaunch &l, void *stream, int *launches);
 // turbo_sm90.cu: a Turbo or TurboGeneric group, every frame cropped (ReconLaunch::clip), K = kStoreStrided or kStoreStridedF with
-// kStoreClip
+// kStoreClip, the latter also with kStoreTable
 template <int K>
 int launch_turbo(const ReconLaunch &l, void *stream, int *launches);
 
@@ -432,6 +443,7 @@ struct ResampleLaunch {
     uint8_t *inter;
     const b200jpg_plane *planes;  // device
     const b200jpg_convert *convert;  // host; null: uint8 destinations
+    const float *table;           // device, with `convert`: the sample tables (FloatDst::table), the kernels' kTable instances
     uint32_t n_plain;             // frames [n_plain, n_frames) are grey frames of B200JPG_FLAG_OUTPUT_RGB: one channel in the scratch and
                                   // the intermediate, each resampled value stored to three destinations
     int resample;                 // the batch's B200JPG_RESAMPLE_*: OpenCV's filters take the cv kernels

@@ -521,9 +521,11 @@ using StoreDst = std::conditional_t<K == kStoreCanvas, uint8_t *, std::condition
 __device__ __forceinline__ const b200jpg_plane *planes_of(const b200jpg_plane *p) { return p; }
 __device__ __forceinline__ const b200jpg_plane *planes_of(const FloatDst &d) { return d.planes; }
 
-// ---- float elements: convert_bits / convert_int / pick4 / store_elem (store_sm90.cuh)
-// byte k of a packed word of four 8-bit samples as 0x4B0000vv: bytes 4..7 of the permute are those of 0x4B000000
-__device__ __forceinline__ float convert_byte(uint32_t w, int k, float s, float b) {
+// ---- float elements: convert_bits / map_int / table_at / pick4 / store_elem (store_sm90.cuh)
+// byte k of a packed word of four 8-bit samples as 0x4B0000vv: bytes 4..7 of the permute are those of 0x4B000000; with the
+// sample tables t, the byte alone (bytes 4..7 of the permute are zero) indexes component c's table
+__device__ __forceinline__ float convert_byte(uint32_t w, int k, const float *t, uint32_t c, float s, float b) {
+    if (t) return table_at(t, c, __byte_perm(w, 0u, 0x4440u | (uint32_t)k));
     return convert_bits(__byte_perm(w, 0x4B000000u, 0x7440u | (uint32_t)k), s, b);
 }
 __device__ __forceinline__ uint32_t pack2(int type, float lo, float hi) {
@@ -539,7 +541,7 @@ __device__ __forceinline__ uint32_t pack2(int type, float lo, float hi) {
 template <int K>
 __device__ __forceinline__ void store_row_f(int type, const b200jpg_plane *p, uint8_t *o, const float (&y)[8], int xmax) {
     const bool f32 = type == B200JPG_SAMPLE_F32;
-    if (K == kStorePlanarF && xmax == 7 && (reinterpret_cast<uintptr_t>(o) & 15u) == 0) {
+    if (kBaseKind<K> == kStorePlanarF && xmax == 7 && (reinterpret_cast<uintptr_t>(o) & 15u) == 0) {
         uint4 *o4 = reinterpret_cast<uint4 *>(o);
         if (f32) {
             o4[0] = make_uint4(__float_as_uint(y[0]), __float_as_uint(y[1]), __float_as_uint(y[2]), __float_as_uint(y[3]));
@@ -549,7 +551,7 @@ __device__ __forceinline__ void store_row_f(int type, const b200jpg_plane *p, ui
         }
         return;
     }
-    const int64_t s = (K == kStorePlanarF) ? (f32 ? 4 : 2) : p->bytes_per_pixel;
+    const int64_t s = (kBaseKind<K> == kStorePlanarF) ? (f32 ? 4 : 2) : p->bytes_per_pixel;
 #pragma unroll
     for (int x = 0; x < 8; x++)
         if (x <= xmax) store_elem(type, o + x * s, y[x]);
@@ -578,7 +580,7 @@ __device__ __forceinline__ void store_row(const D &out, int c, const b200jpg_pla
     if constexpr (kFloatKind<K>) {
         float y[8];
 #pragma unroll
-        for (int x = 0; x < 8; x++) y[x] = convert_byte((x < 4) ? w0 : w1, x & 3, out.scale[c], out.bias[c]);
+        for (int x = 0; x < 8; x++) y[x] = convert_byte((x < 4) ? w0 : w1, x & 3, table_of<kTableKind<K>>(out), (uint32_t)c, out.scale[c], out.bias[c]);
         store_row_f<K>(out.type, p, o, y, xmax);
     } else {
         store_row8<K>(p, o, w0, w1, xmax);
@@ -602,10 +604,10 @@ __device__ __forceinline__ void put_run8(uint8_t *o, uint32_t w0, uint32_t w1) {
     for (int k = 0; k < 8; k++) o[k] = (uint8_t)byte_of(k < 4 ? w0 : w1, k & 3);
 }
 // the same converted to float elements of `type`: 16-byte stores when aligned
-__device__ __forceinline__ void put_run_f(int type, uint8_t *o, uint32_t w0, uint32_t w1, float s, float b) {
+__device__ __forceinline__ void put_run_f(int type, uint8_t *o, uint32_t w0, uint32_t w1, const float *t, uint32_t c, float s, float b) {
     float y[8];
 #pragma unroll
-    for (int k = 0; k < 8; k++) y[k] = convert_byte(k < 4 ? w0 : w1, k & 3, s, b);
+    for (int k = 0; k < 8; k++) y[k] = convert_byte(k < 4 ? w0 : w1, k & 3, t, c, s, b);
     const bool f32 = type == B200JPG_SAMPLE_F32;
     if ((reinterpret_cast<uintptr_t>(o) & 15u) == 0) {
         uint4 *o4 = reinterpret_cast<uint4 *>(o);
@@ -624,7 +626,7 @@ __device__ __forceinline__ void put_run_f(int type, uint8_t *o, uint32_t w0, uin
 
 template <int K, typename D>
 __device__ __forceinline__ void put_run(const D &out, int c, uint8_t *o, uint32_t w0, uint32_t w1) {
-    if constexpr (kBaseKind<K> == kStoreRunsF) put_run_f(out.type, o, w0, w1, pick4(out.scale, c), pick4(out.bias, c));
+    if constexpr (kBaseKind<K> == kStoreRunsF) put_run_f(out.type, o, w0, w1, table_of<kTableKind<K>>(out), (uint32_t)c, pick4(out.scale, c), pick4(out.bias, c));
     else put_run8(o, w0, w1);
 }
 
@@ -738,7 +740,7 @@ __device__ __forceinline__ void store_staged(const D &out, const b200jpg_plane *
 #pragma unroll 1
                 for (int x = xmin; x <= xmax; x++) {
                     const uint32_t v = byte_of((uint32_t)st[(8 * y + 2 * c + (x >> 2)) * NT], x & 3);
-                    if constexpr (KB == kStoreRunsF) store_elem(out.type, at(x, y), convert_bits(0x4B000000u | v, pick4(out.scale, c), pick4(out.bias, c)));
+                    if constexpr (KB == kStoreRunsF) store_elem(out.type, at(x, y), map_int(table_of<kTableKind<K>>(out), c, (int)v, pick4(out.scale, c), pick4(out.bias, c)));
                     else *at(x, y) = (uint8_t)v;
                 }
         }
@@ -1685,7 +1687,7 @@ __device__ __forceinline__ void store_mode_pixel(StoreDst<K> out, uint32_t statu
     for (uint32_t c = 0; c < no; c++) {
         const int u = kRgb ? w[c] : v;
         if constexpr (KB == kStoreStridedF) {
-            store_elem(out.type, plane_at(out.planes + 4u * status_idx + c, x, y), convert_int(u, pick4(out.scale, c), pick4(out.bias, c)));
+            store_elem(out.type, plane_at(out.planes + 4u * status_idx + c, x, y), map_int(table_of<kTableKind<K>>(out), c, u, pick4(out.scale, c), pick4(out.bias, c)));
         } else {
             uint8_t *o = plane_at(out + 4u * status_idx + c, x, y);
             if (deep) *reinterpret_cast<uint16_t *>(o) = (uint16_t)u;
@@ -1772,7 +1774,7 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
                     const uint8_t m = (uint8_t)clamp_to(clamp_to(v[c], 255) + ((clamp_to(res[c], 4095) + 8) >> 4) - 128, 255);
                     if constexpr (KB == kStoreCanvas) o[nc * x + c] = m;
                     else if constexpr (KB == kStoreStridedF)
-                        store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, X + x, Y + y), convert_int(m, pick4(out.scale, c), pick4(out.bias, c)));
+                        store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, X + x, Y + y), map_int(table_of<kTableKind<K>>(out), c, m, pick4(out.scale, c), pick4(out.bias, c)));
                     else *plane_at(out + 4u * f.status_idx + c, X + x, Y + y) = m;
                 }
             }
@@ -1814,7 +1816,7 @@ generic_reconstruct_kernel(const FrameRecon *__restrict__ frames, const int32_t 
                     if (deep) o16[nc * x + c] = (uint16_t)w;
                     else o8[nc * x + c] = (uint8_t)w;
                 } else if constexpr (KB == kStoreStridedF) {
-                    store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, X + x, Y + y), convert_int((int)w, pick4(out.scale, c), pick4(out.bias, c)));
+                    store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, X + x, Y + y), map_int(table_of<kTableKind<K>>(out), c, (int)w, pick4(out.scale, c), pick4(out.bias, c)));
                 } else {
                     uint8_t *o = plane_at(out + 4u * f.status_idx + c, X + x, Y + y);
                     if (deep) *reinterpret_cast<uint16_t *>(o) = (uint16_t)w;
@@ -1845,8 +1847,8 @@ planes_out_kernel(const FrameRecon *__restrict__ frames, const int32_t *__restri
         if constexpr (K == kStoreCanvas) {
             if (f.precision > 8) reinterpret_cast<uint16_t *>(out + f.out_base)[before + i] = (uint16_t)v;
             else out[f.out_base + before + i] = (uint8_t)v;
-        } else if constexpr (K == kStoreStridedF) {
-            store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, (int)x, (int)y), convert_int(v, pick4(out.scale, c), pick4(out.bias, c)));
+        } else if constexpr (kBaseKind<K> == kStoreStridedF) {
+            store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, (int)x, (int)y), map_int(table_of<kTableKind<K>>(out), c, v, pick4(out.scale, c), pick4(out.bias, c)));
         } else {
             uint8_t *o = plane_at(out + 4u * f.status_idx + c, (int)x, (int)y);
             if (f.precision > 8) *reinterpret_cast<uint16_t *>(o) = (uint16_t)v;
@@ -1867,6 +1869,7 @@ static StoreDst<K> dst_of(const ReconLaunch &l) {
         d.planes = l.planes;
         d.type = l.convert->type;
         for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) d.scale[c] = l.convert->scale[c], d.bias[c] = l.convert->bias[c];
+        d.table = l.table;
         return d;
     } else {
         return l.planes;
@@ -1972,11 +1975,11 @@ static int launch_recon_generic(const ReconLaunch &l, cudaStream_t s, int *launc
 template <int K>
 static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches) {
     if (l.path == ReconPath::Turbo || l.path == ReconPath::TurboGeneric) {  // (every frame of such a group is cropped: admit_crops)
-        if constexpr (kClipKind<K>) return launch_turbo<(kFloatKind<K> ? kStoreStridedF : kStoreStrided) | kStoreClip>(l, s, launches);
+        if constexpr (kClipKind<K>) return launch_turbo<(kFloatKind<K> ? kStoreStridedF : kStoreStrided) | kStoreClip | (K & kStoreTable)>(l, s, launches);
         return (int)cudaErrorInvalidValue;
     }
     if (l.path == ReconPath::Generic || l.path == ReconPath::Scaled)
-        return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : ((kFloatKind<K> ? kStoreStridedF : kStoreStrided) | (K & kStoreClip))>(l, s, launches);
+        return launch_recon_generic<K == kStoreCanvas ? kStoreCanvas : ((kFloatKind<K> ? kStoreStridedF : kStoreStrided) | (K & (kStoreClip | kStoreTable)))>(l, s, launches);
     if (l.path == ReconPath::Fused420) return launch_recon420<K>(l, s, launches);
     if (l.path == ReconPath::Scaled420) return launch_recon420_scaled<K>(l, s, launches);
     int n = 0;  // ReconPath::Tiled
@@ -2021,6 +2024,11 @@ static int launch_recon_kind(const ReconLaunch &l, cudaStream_t s, int *launches
 int launch_recon(const ReconLaunch &l, void *stream, int *launches) {
     cudaStream_t s = (cudaStream_t)stream;
     if (!l.planes) return launch_recon_kind<kStoreCanvas>(l, s, launches);
+    if (l.convert && l.table) {  // (b200jpg_batch_decode_into_table)
+        if (l.clip) return launch_recon_kind<kStoreRunsF | kStoreClip | kStoreTable>(l, s, launches);
+        if (l.runs) return launch_recon_kind<kStoreRunsF | kStoreTable>(l, s, launches);
+        return l.planar ? launch_recon_kind<kStorePlanarF | kStoreTable>(l, s, launches) : launch_recon_kind<kStoreStridedF | kStoreTable>(l, s, launches);
+    }
     if (l.clip) return l.convert ? launch_recon_kind<kStoreRunsF | kStoreClip>(l, s, launches) : launch_recon_kind<kStoreRuns | kStoreClip>(l, s, launches);
     if (l.runs) return l.convert ? launch_recon_kind<kStoreRunsF>(l, s, launches) : launch_recon_kind<kStoreRuns>(l, s, launches);
     if (l.convert) return l.planar ? launch_recon_kind<kStorePlanarF>(l, s, launches) : launch_recon_kind<kStoreStridedF>(l, s, launches);

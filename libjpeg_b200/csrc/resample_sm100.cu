@@ -135,7 +135,7 @@ __global__ void __launch_bounds__(256) resample_h_kernel(const ResampleFrame *__
     }
 }
 
-template <bool kFloat>
+template <bool kFloat, bool kTable = false>
 __global__ void __launch_bounds__(256) resample_v_kernel(const ResampleFrame *__restrict__ frames, const uint8_t *__restrict__ input,
                                                          const uint8_t *__restrict__ scratch, const uint8_t *__restrict__ inter, FloatDst out) {
     const ResampleFrame &f = frames[blockIdx.y];
@@ -171,14 +171,14 @@ __global__ void __launch_bounds__(256) resample_v_kernel(const ResampleFrame *__
     for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) {
         if (c >= (int)nc) break;
         uint8_t *o = plane_at(out.planes + 4u * f.plane + c, (int)x, (int)y);
-        if constexpr (kFloat) store_elem(out.type, o, convert_int(acc[c], pick4(out.scale, c), pick4(out.bias, c)));
+        if constexpr (kFloat) store_elem(out.type, o, map_int(table_of<kTable>(out), c, acc[c], pick4(out.scale, c), pick4(out.bias, c)));
         else *o = (uint8_t)acc[c];
     }
 }
 
 // resample_v_kernel for the grey frames of B200JPG_FLAG_OUTPUT_RGB: one channel in the scratch and the intermediate, each resampled
 // value stored through the frame's three destinations, each with its own component's map
-template <bool kFloat>
+template <bool kFloat, bool kTable = false>
 __global__ void __launch_bounds__(256) resample_v_rgb_kernel(const ResampleFrame *__restrict__ frames, const uint8_t *__restrict__ input,
                                                              const uint8_t *__restrict__ scratch, const uint8_t *__restrict__ inter, FloatDst out) {
     const ResampleFrame &f = frames[blockIdx.y];
@@ -203,7 +203,7 @@ __global__ void __launch_bounds__(256) resample_v_rgb_kernel(const ResampleFrame
 #pragma unroll
     for (int c = 0; c < 3; c++) {
         uint8_t *o = plane_at(out.planes + 4u * f.plane + c, (int)x, (int)y);
-        if constexpr (kFloat) store_elem(out.type, o, convert_int(v, out.scale[c], out.bias[c]));
+        if constexpr (kFloat) store_elem(out.type, o, map_int(table_of<kTable>(out), c, v, out.scale[c], out.bias[c]));
         else *o = (uint8_t)v;
     }
 }
@@ -263,19 +263,19 @@ __device__ __forceinline__ int clamp255(int v) { return v < 0 ? 0 : (v > 255 ? 2
 
 // the value of output (x, y), channel c, stored through the frame's destinations: three for the grey frames of
 // B200JPG_FLAG_OUTPUT_RGB (kRgb), each with its own component's map
-template <bool kFloat, bool kRgb>
+template <bool kFloat, bool kRgb, bool kTable>
 __device__ __forceinline__ void cv_store(const ResampleFrame &f, const FloatDst &out, uint32_t x, uint32_t y, int c, int v) {
 #pragma unroll
     for (int k = 0; k < (kRgb ? 3 : 1); k++) {
         const int oc = kRgb ? k : c;
         uint8_t *o = plane_at(out.planes + 4u * f.plane + oc, (int)x, (int)y);
-        if constexpr (kFloat) store_elem(out.type, o, convert_int(v, pick4(out.scale, oc), pick4(out.bias, oc)));
+        if constexpr (kFloat) store_elem(out.type, o, map_int(table_of<kTable>(out), oc, v, pick4(out.scale, oc), pick4(out.bias, oc)));
         else *o = (uint8_t)v;
     }
 }
 
 // one thread per output pixel, all channels; the taps go down a column of the intermediate (rows y0 .. y1 - 1 of the source)
-template <bool kArea, bool kFloat, bool kRgb>
+template <bool kArea, bool kFloat, bool kRgb, bool kTable = false>
 __global__ void __launch_bounds__(256) cv_resample_v_kernel(const ResampleFrame *__restrict__ frames, const uint8_t *__restrict__ input,
                                                             const uint8_t *__restrict__ inter, FloatDst out) {
     const ResampleFrame &f = frames[blockIdx.y];
@@ -302,20 +302,20 @@ __global__ void __launch_bounds__(256) cv_resample_v_kernel(const ResampleFrame 
         }
 #pragma unroll
         for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++)
-            if (c < (int)nc) cv_store<kFloat, kRgb>(f, out, x, y, c, clamp255(__float2int_rn(acc[c])));
+            if (c < (int)nc) cv_store<kFloat, kRgb, kTable>(f, out, x, y, c, clamp255(__float2int_rn(acc[c])));
     } else {  // (((b0 (T0 >> 4)) >> 16) + ((b1 (T1 >> 4)) >> 16) + 2) >> 2, clamped
         const int32_t *t0 = T + (uint64_t)__ldg(vb + 2 * y) * pitch, *t1 = T + (uint64_t)__ldg(vb + 2 * y + 1) * pitch;
         const int b0 = __ldg(kk), b1 = __ldg(kk + 1);
 #pragma unroll
         for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++)
             if (c < (int)nc)
-                cv_store<kFloat, kRgb>(f, out, x, y, c, clamp255((((b0 * (__ldg(t0 + c) >> 4)) >> 16) + ((b1 * (__ldg(t1 + c) >> 4)) >> 16) + 2) >> 2));
+                cv_store<kFloat, kRgb, kTable>(f, out, x, y, c, clamp255((((b0 * (__ldg(t0 + c) >> 4)) >> 16) + ((b1 * (__ldg(t1 + c) >> 4)) >> 16) + 2) >> 2));
     }
 }
 
 // rule 2: output (x, y) is the fx x fy block of the (trimmed) C at (x fx, y fy): (s + 2) >> 2 for 2 x 2 blocks, else
 // rint((float)s * (1.0f / (fx fy))); 1 x 1 blocks copy. The planning keeps 255 fx fy below 2^31.
-template <bool kFloat, bool kRgb>
+template <bool kFloat, bool kRgb, bool kTable = false>
 __global__ void __launch_bounds__(256) cv_area_block_kernel(const ResampleFrame *__restrict__ frames, const uint8_t *__restrict__ scratch,
                                                             FloatDst out) {
     const ResampleFrame &f = frames[blockIdx.y];
@@ -338,21 +338,21 @@ __global__ void __launch_bounds__(256) cv_area_block_kernel(const ResampleFrame 
     const float inv = __fdiv_rn(1.0f, (float)(fx * fy));
 #pragma unroll
     for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++)
-        if (c < (int)nc) cv_store<kFloat, kRgb>(f, out, x, y, c, half ? (s[c] + 2) >> 2 : clamp255(__float2int_rn(__fmul_rn((float)s[c], inv))));
+        if (c < (int)nc) cv_store<kFloat, kRgb, kTable>(f, out, x, y, c, half ? (s[c] + 2) >> 2 : clamp255(__float2int_rn(__fmul_rn((float)s[c], inv))));
 }
 
-template <bool kFloat, bool kRgb>
+template <bool kFloat, bool kRgb, bool kTable = false>
 void launch_cv_v(const ResampleLaunch &l, const ResampleFrame *frames, uint32_t n, uint32_t gv, const FloatDst &d, cudaStream_t s, int &launches) {
     if (l.cv_kinds & kCvLinear) {
-        cv_resample_v_kernel<false, kFloat, kRgb><<<dim3(gv, n), 256, 0, s>>>(frames, l.input, l.inter, d);
+        cv_resample_v_kernel<false, kFloat, kRgb, kTable><<<dim3(gv, n), 256, 0, s>>>(frames, l.input, l.inter, d);
         launches++;
     }
     if (l.cv_kinds & kCvArea) {
-        cv_resample_v_kernel<true, kFloat, kRgb><<<dim3(gv, n), 256, 0, s>>>(frames, l.input, l.inter, d);
+        cv_resample_v_kernel<true, kFloat, kRgb, kTable><<<dim3(gv, n), 256, 0, s>>>(frames, l.input, l.inter, d);
         launches++;
     }
     if (l.cv_kinds & kCvBlocks) {
-        cv_area_block_kernel<kFloat, kRgb><<<dim3(gv, n), 256, 0, s>>>(frames, l.scratch, d);
+        cv_area_block_kernel<kFloat, kRgb, kTable><<<dim3(gv, n), 256, 0, s>>>(frames, l.scratch, d);
         launches++;
     }
 }
@@ -479,14 +479,17 @@ int launch_resample(const ResampleLaunch &l, void *stream, int *launches) {
         if (l.convert) {
             d.type = l.convert->type;
             for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) d.scale[c] = l.convert->scale[c], d.bias[c] = l.convert->bias[c];
+            d.table = l.table;
         }
         const uint32_t n_rgb = l.n_frames - l.n_plain;
         if (l.n_plain) {
-            if (l.convert) launch_cv_v<true, false>(l, l.frames, l.n_plain, gv, d, s, n);
+            if (l.table) launch_cv_v<true, false, true>(l, l.frames, l.n_plain, gv, d, s, n);
+            else if (l.convert) launch_cv_v<true, false>(l, l.frames, l.n_plain, gv, d, s, n);
             else launch_cv_v<false, false>(l, l.frames, l.n_plain, gv, d, s, n);
         }
         if (n_rgb) {
-            if (l.convert) launch_cv_v<true, true>(l, l.frames + l.n_plain, n_rgb, gv, d, s, n);
+            if (l.table) launch_cv_v<true, true, true>(l, l.frames + l.n_plain, n_rgb, gv, d, s, n);
+            else if (l.convert) launch_cv_v<true, true>(l, l.frames + l.n_plain, n_rgb, gv, d, s, n);
             else launch_cv_v<false, true>(l, l.frames + l.n_plain, n_rgb, gv, d, s, n);
         }
         if (launches) *launches = n;
@@ -504,16 +507,19 @@ int launch_resample(const ResampleLaunch &l, void *stream, int *launches) {
     if (l.convert) {
         d.type = l.convert->type;
         for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) d.scale[c] = l.convert->scale[c], d.bias[c] = l.convert->bias[c];
+        d.table = l.table;
     }
     const uint32_t n_rgb = l.n_frames - l.n_plain;
     if (l.n_plain) {
-        if (l.convert) resample_v_kernel<true><<<dim3(gv, l.n_plain), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);
+        if (l.table) resample_v_kernel<true, true><<<dim3(gv, l.n_plain), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);
+        else if (l.convert) resample_v_kernel<true><<<dim3(gv, l.n_plain), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);
         else resample_v_kernel<false><<<dim3(gv, l.n_plain), 256, 0, s>>>(l.frames, l.input, l.scratch, l.inter, d);
         n++;
     }
     if (n_rgb) {
         const ResampleFrame *rgb = l.frames + l.n_plain;
-        if (l.convert) resample_v_rgb_kernel<true><<<dim3(gv, n_rgb), 256, 0, s>>>(rgb, l.input, l.scratch, l.inter, d);
+        if (l.table) resample_v_rgb_kernel<true, true><<<dim3(gv, n_rgb), 256, 0, s>>>(rgb, l.input, l.scratch, l.inter, d);
+        else if (l.convert) resample_v_rgb_kernel<true><<<dim3(gv, n_rgb), 256, 0, s>>>(rgb, l.input, l.scratch, l.inter, d);
         else resample_v_rgb_kernel<false><<<dim3(gv, n_rgb), 256, 0, s>>>(rgb, l.input, l.scratch, l.inter, d);
         n++;
     }

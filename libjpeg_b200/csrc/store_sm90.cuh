@@ -18,6 +18,24 @@ __device__ __forceinline__ float convert_bits(uint32_t bits, float s, float b) {
     return __fadd_rn(__fmul_rn(__fsub_rn(__uint_as_float(bits), 8388608.f), s), b);
 }
 __device__ __forceinline__ float convert_int(int v, float s, float b) { return convert_bits(0x4B000000u | (uint32_t)v, s, b); }
+// b200jpg_batch_decode_into_table: entry v of component c of the sample tables t (device, 256 floats per component), through the
+// non-coherent path -- the 4 KB stay in L1 for the launch
+__device__ __forceinline__ float table_at(const float *t, uint32_t c, uint32_t v) {
+    float y;
+    asm("ld.global.nc.f32 %0, [%1];" : "=f"(y) : "l"(t + 256u * c + v));
+    return y;
+}
+// the sample tables of a float destination d (FloatDst) in a launch whose kind has them (kTable: kStoreTable), else null, so that
+// the lookup is compiled out of the affine instances
+template <bool kTable, class D>
+__device__ __forceinline__ const float *table_of(const D &d) {
+    if constexpr (kTable) return d.table;
+    else return nullptr;
+}
+// the float element of the 8-bit sample v of component c: its table entry when the call has tables, else the map
+__device__ __forceinline__ float map_int(const float *t, uint32_t c, int v, float s, float b) {
+    return t ? table_at(t, c, (uint32_t)v) : convert_int(v, s, b);
+}
 // scale[c] / bias[c] of a component index known only at run time (a select chain: the parameter bank is not indexed)
 __device__ __forceinline__ float pick4(const float (&a)[B200JPG_MAX_COMPONENTS], uint32_t c) {
     return c == 0 ? a[0] : (c == 1 ? a[1] : (c == 2 ? a[2] : a[3]));

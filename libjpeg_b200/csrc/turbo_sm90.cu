@@ -359,7 +359,7 @@ __device__ __forceinline__ void turbo_reconstruct(const FrameRecon *__restrict__
         for (uint32_t c = 0; c < kMaxOut; c++) {
             if (c >= no) break;
             uint8_t *o = reinterpret_cast<uint8_t *>(data[c] + (uint64_t)((int64_t)x * bpp[c]) + (uint64_t)((int64_t)y * bpr[c]));
-            if constexpr (kFloatKind<K>) store_elem(out.type, o, convert_int(v[c], pick4(out.scale, c), pick4(out.bias, c)));
+            if constexpr (kFloatKind<K>) store_elem(out.type, o, map_int(table_of<kTableKind<K>>(out), c, v[c], pick4(out.scale, c), pick4(out.bias, c)));
             else *o = (uint8_t)v[c];
         }
     }
@@ -418,7 +418,7 @@ __device__ __forceinline__ void turbo_generic(const FrameRecon *__restrict__ fra
     for (uint32_t c = 0; c < 3; c++) {
         if (c >= no) break;
         if constexpr (kFloatKind<K>)
-            store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, x, y), convert_int(v[c], pick4(out.scale, c), pick4(out.bias, c)));
+            store_elem(out.type, plane_at(out.planes + 4u * f.status_idx + c, x, y), map_int(table_of<kTableKind<K>>(out), c, v[c], pick4(out.scale, c), pick4(out.bias, c)));
         else
             *plane_at(out + 4u * f.status_idx + c, x, y) = (uint8_t)v[c];
     }
@@ -491,6 +491,7 @@ int launch_turbo(const ReconLaunch &l, void *stream, int *launches) {
         out.planes = l.planes;
         out.type = l.convert->type;
         for (int c = 0; c < B200JPG_MAX_COMPONENTS; c++) out.scale[c] = l.convert->scale[c], out.bias[c] = l.convert->bias[c];
+        out.table = l.table;
     } else {
         out = l.planes;
     }
@@ -525,5 +526,6 @@ int launch_turbo(const ReconLaunch &l, void *stream, int *launches) {
 
 template int launch_turbo<kStoreStrided | kStoreClip>(const ReconLaunch &, void *, int *);
 template int launch_turbo<kStoreStridedF | kStoreClip>(const ReconLaunch &, void *, int *);
+template int launch_turbo<kStoreStridedF | kStoreClip | kStoreTable>(const ReconLaunch &, void *, int *);
 
 }  // namespace b200jpg

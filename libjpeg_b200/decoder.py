@@ -247,6 +247,31 @@ def crop_table(crop, n, name="crop"):
     return table
 
 
+def flip_table(hflip, vflip, n):
+    """The flips of b200jpg_batch_create_flip for BatchDecoder(hflip=..., vflip=...): each of hflip and vflip is None, one bool
+    for every frame, or a sequence of n bools. None when no frame is flipped (the batch of b200jpg_batch_create_resample). Raises
+    ValueError for a wrong length or a value that is not a bool."""
+    def is_bool(v):
+        return isinstance(v, (bool, np.bool_))
+
+    table = (ctypes.c_uint8 * n)()
+    for name, arg, bit in (("hflip", hflip, native.FLIP_H), ("vflip", vflip, native.FLIP_V)):
+        if arg is None:
+            continue
+        if is_bool(arg):
+            arg = [arg] * n
+        elif isinstance(arg, (str, bytes)) or not hasattr(arg, "__len__"):
+            raise ValueError("%s must be None, a bool or one bool per frame, got %r" % (name, arg))
+        if len(arg) != n:
+            raise ValueError("%s: %d entries for %d frames" % (name, len(arg), n))
+        for i, v in enumerate(arg):
+            if not is_bool(v):
+                raise ValueError("%s[%d]: expected a bool, got %r" % (name, i, v))
+            if v:
+                table[i] |= bit
+    return table if any(table) else None
+
+
 def resize_table(resize, n, name="resize"):
     """The b200jpg_size table of BatchDecoder(resize=...) (or of `name`=..., draft): one (h, w) for every frame, or n entries each
     None or (h, w), as non-negative integers; (0, 0) leaves a frame unresized (undrafted). Raises ValueError."""
@@ -351,6 +376,47 @@ def destination_dtype(dst):
         for t in entry or ():
             return getattr(t, "dtype", None)
     return None
+
+
+def table_args(dtype, table, ncomp=1):
+    """The b200jpg_convert_table of a decode_into call into `dtype` tensors with `table`, a [C, 256] float32 tensor or array
+    (ncomp <= C <= 4, ncomp: the most output components a live frame of the batch has): row c maps the samples of output
+    component c. Raises TypeError for an integer destination or a table that is not float32, ValueError for a table of another
+    shape or with fewer rows than the batch's components."""
+    floats = _sample_types()
+    if dtype not in floats:
+        raise TypeError("a sample table needs a float32, float16 or bfloat16 destination, not %s" % dtype)
+    if hasattr(table, "detach"):
+        table = table.detach().cpu().numpy()
+    a = np.asarray(table)
+    if a.dtype != np.float32:
+        raise TypeError("the sample table must be float32, got %s" % a.dtype)
+    if a.ndim != 2 or a.shape[1] != 256 or not 1 <= a.shape[0] <= 4:
+        raise ValueError("the sample table must be [C, 256] with C <= 4, got %s" % (a.shape,))
+    if a.shape[0] < ncomp:
+        raise ValueError("the sample table has %d rows, but frames of the batch are written with %d components: one row per "
+                         "component" % (a.shape[0], ncomp))
+    t = native.ConvertTableStruct()
+    t.type = floats[dtype]
+    ctypes.memmove(ctypes.addressof(t.table), np.ascontiguousarray(a).ctypes.data, a.nbytes)
+    return t
+
+
+def sample_table(fn, ncomp=3):
+    """The [ncomp, 256] float32 sample table of decode_into(..., table=...) that a per-sample transform gives: fn runs once on the
+    [ncomp, 1, 256] uint8 CPU tensor of every sample value (each component's row is arange(256)) and returns a tensor of the same
+    shape, whose values become the table. For torchvision's ToTensor() + Normalize(mean, std):
+        sample_table(lambda t: TF.normalize(t.float().div(255), mean, std))
+    fn must act sample by sample (component c of sample v -> one value): a transform that mixes samples, like a blur or a
+    resize, has no table."""
+    import torch
+    if isinstance(ncomp, bool) or not isinstance(ncomp, int) or not 1 <= ncomp <= 4:
+        raise ValueError("ncomp must be 1 .. 4, got %r" % (ncomp,))
+    x = torch.arange(256, dtype=torch.uint8).view(1, 1, 256).expand(ncomp, 1, 256).contiguous()
+    y = torch.as_tensor(fn(x)).detach().cpu()  # (fn may return a CUDA tensor, or one that requires grad)
+    if tuple(y.shape) != (ncomp, 1, 256):
+        raise ValueError("fn must return a [%d, 1, 256] tensor, got %s" % (ncomp, tuple(y.shape)))
+    return y.reshape(ncomp, 256).to(torch.float32).numpy()
 
 
 def convert_args(dtype, scale=None, bias=None, ncomp=4):
@@ -502,7 +568,7 @@ class BatchDecoder:
 
     def __init__(self, frames, device=-1, tolerate_bad=False, ctx=None, color_transform=True, upsample=True, downscale=1,
                  exif_orientation=False, crop=None, resize=None, resample="bilinear", mode=None, reconstruction="reference", draft=None,
-                 box=None, reducing_gap=None, window=None):
+                 box=None, reducing_gap=None, window=None, hflip=None, vflip=None):
         """downscale = 2, 4 or 8 decodes every frame at ceil(W / k) x ceil(H / k) (B200JPG_FLAG_DOWNSCALE_k): each 8x8 block is
         inverse transformed straight to (8/k) x (8/k) samples, the k x k box average of its IDCT, and the rest of the
         reconstruction runs on the smaller frame. geometry(), frame_view() and plane_views() give the reduced sizes. Not to be
@@ -589,7 +655,16 @@ class BatchDecoder:
         without one). With reconstruction="libjpeg-turbo", C of a YCbCr or grey frame is cv2.imdecode(data, IMREAD_COLOR)
         in RGB order (IMREAD_GRAYSCALE under mode "L"), so an OpenCV loader's pixels come out unchanged; a BGR tensor is a
         decode_into() with the planes in the other order. cv2.resize has no box and no reducing_gap: either with a cv2 filter
-        raises NativeError (B200JPG_ERR_INVALID_PARAMETER)."""
+        raises NativeError (B200JPG_ERR_INVALID_PARAMETER).
+
+        hflip and vflip (b200jpg_batch_create_flip, DESIGN §21) are None, one bool for every frame, or one bool per frame:
+        torchvision's RandomHorizontalFlip / RandomVerticalFlip with the coin already tossed. The flip is the last geometric step,
+        after the resize and the window: a frame whose output without it is O ([h, w, C]) is written as O[:, ::-1] with hflip,
+        O[::-1, :] with vflip and O[::-1, ::-1] with both, so hflip(img.crop(box).resize(size)) fills the batch tensor with no pass
+        of its own. crop, box and window keep the coordinates of the unflipped image; output_shape(), status() and orientation()
+        do not change. A frame without a size is reconstructed mirrored (the flip composed with its Exif orientation); a resized
+        frame's resample pass stores mirrored, with the launches of the unflipped batch. A wrong length or a value that is not a
+        bool raises ValueError."""
         if not isinstance(mode, (str, type(None))) or mode not in native.MODE_FLAGS:
             raise ValueError('mode must be None, "RGB" or "L", got %r' % (mode,))
         if not isinstance(reconstruction, str) or reconstruction not in native.RECONSTRUCTION_FLAGS:
@@ -603,6 +678,7 @@ class BatchDecoder:
         windows = None if window is None else crop_table(window, len(frames), "window")
         gap = reducing_gap_value(reducing_gap)
         filt = resample_filter(resample)
+        flips = flip_table(hflip, vflip, len(frames))
         self.ctx = ctx or Context(device)
         self._keep = []
         n = len(frames)
@@ -627,8 +703,8 @@ class BatchDecoder:
         flags |= native.MODE_FLAGS[mode]
         self.reconstruction = reconstruction
         flags |= native.RECONSTRUCTION_FLAGS[reconstruction]
-        rc = lib.b200jpg_batch_create_resample(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, drafts, rects, sizes, boxes, windows,
-                                               filt, gap, ctypes.byref(self.handle))
+        rc = lib.b200jpg_batch_create_flip(self.ctx.handle, ptrs, lens, n, int(tolerate_bad), flags, drafts, rects, sizes, boxes, windows,
+                                           filt, gap, flips, ctypes.byref(self.handle))
         native.check(rc, self.ctx.handle)
         self.ctx._batch_opened()
         self._keep = []  # the batch holds its own pinned copy
@@ -744,7 +820,7 @@ class BatchDecoder:
             self._geometry = geo
         return self._geometry
 
-    def decode_into(self, dst, stream=None, scale=None, bias=None):
+    def decode_into(self, dst, stream=None, scale=None, bias=None, table=None):
         """decode() into caller-described tensors: dst[i] holds one 2-D CUDA tensor per component of frame i ([H, W], or
         each component's own size with upsample=False), so a [N, C, H, W] batch tensor can be passed as it is, an NHWC
         tensor t as t.permute(0, 3, 1, 2), BGR as [t[i, ..., 2], t[i, ..., 1], t[i, ..., 0]]. uint8 for 8-bit frames,
@@ -755,16 +831,29 @@ class BatchDecoder:
             y = float32(float32(v * scale[c]) + bias[c]), then rounded to nearest even into float16 / bfloat16
         which is what t.float() * scale + bias followed by .half() / .bfloat16() gives. c is the output component (R, G, B
         after the colour transformation). scale and bias are a scalar or one value per component (defaults 1 and 0),
-        rounded to float32. ImageNet-style normalisation (x / 255 - mean) / std is scale = 1 / (255 * std),
-        bias = -mean / std."""
+        rounded to float32. scale = 1 / (255 * std), bias = -mean / std is close to ImageNet-style normalisation but not equal
+        to it: torchvision's ToTensor() + Normalize(mean, std) computes v / 255, then - mean, then / std, three roundings, and differs
+        from the map in the last bit for many (v, c).
+
+        table (b200jpg_batch_decode_into_table, DESIGN §22), a [C, 256] float32 tensor or array with C <= 4, replaces the map: every
+        8-bit sample v of output component c is written as table[c][v], stored as float32 or rounded to nearest even into float16 /
+        bfloat16 as above. sample_table(fn) builds it from any per-sample transform, so ToTensor() + Normalize() is matched bit
+        for bit. A table with fewer rows than the batch's output components, or with scale or bias, raises ValueError, with an integer destination TypeError; a batch with a live 12-bit
+        frame raises NativeError (B200JPG_ERR_NOT_IMPLEMENTED)."""
+        if table is not None and (scale is not None or bias is not None):
+            raise ValueError("a sample table replaces scale and bias: pass one or the other")
         geo = self.geometry()
-        table = plane_table(geo, dst)
+        planes = plane_table(geo, dst)
         ncomp = max([len(g[0]) for g in geo if g is not None] or [1])
+        if table is not None:
+            conv = table_args(destination_dtype(dst), table, ncomp)
+            native.check(lib.b200jpg_batch_decode_into_table(self.handle, planes, ctypes.byref(conv), self._stream_ptr(stream)), self.ctx.handle)
+            return dst
         conv = convert_args(destination_dtype(dst), scale, bias, ncomp)
         if conv is None:
-            native.check(lib.b200jpg_batch_decode_into(self.handle, table, self._stream_ptr(stream)), self.ctx.handle)
+            native.check(lib.b200jpg_batch_decode_into(self.handle, planes, self._stream_ptr(stream)), self.ctx.handle)
         else:
-            native.check(lib.b200jpg_batch_decode_into_ex(self.handle, table, ctypes.byref(conv), self._stream_ptr(stream)), self.ctx.handle)
+            native.check(lib.b200jpg_batch_decode_into_ex(self.handle, planes, ctypes.byref(conv), self._stream_ptr(stream)), self.ctx.handle)
         return dst
 
     def decode_entropy(self, stream=None):

@@ -36,6 +36,11 @@ class ConvertStruct(ctypes.Structure):
     _fields_ = [("type", ctypes.c_int32), ("scale", ctypes.c_float * 4), ("bias", ctypes.c_float * 4)]
 
 
+class ConvertTableStruct(ctypes.Structure):
+    """b200jpg_convert_table: element type (SAMPLE_*) and the per-component sample tables y = table[c][v] of a float destination."""
+    _fields_ = [("type", ctypes.c_int32), ("table", (ctypes.c_float * 256) * 4)]
+
+
 class RectStruct(ctypes.Structure):
     """b200jpg_rect: a crop rectangle of b200jpg_batch_create_crop, in output coordinates; all zero = the whole frame."""
     _fields_ = [("x", ctypes.c_uint32), ("y", ctypes.c_uint32), ("width", ctypes.c_uint32), ("height", ctypes.c_uint32)]
@@ -61,6 +66,7 @@ COLORSPACES = [None, "L", "YCbCr", "RGB", "CMYK", "YCCK"]  # B200JPG_COLORSPACE_
 RESAMPLE = {"lanczos": 1, "bilinear": 2, "bicubic": 3, "box": 4, "hamming": 5}  # B200JPG_RESAMPLE_*, PIL's values
 # B200JPG_RESAMPLE_CV_*: OpenCV's cv2.resize, 0x100 | cv2.INTER_LINEAR / cv2.INTER_AREA (DESIGN §20)
 RESAMPLE.update({"cv2-linear": 0x101, "cv2-area": 0x103})
+FLIP_H, FLIP_V = 1, 2  # B200JPG_FLIP_H / _V of b200jpg_batch_create_flip
 
 
 def library_path():
@@ -97,6 +103,10 @@ def _load():
                                                 ctypes.POINTER(SizeStruct), ctypes.POINTER(RectStruct), ctypes.POINTER(SizeStruct),
                                                 ctypes.POINTER(BoxStruct), ctypes.POINTER(RectStruct), i32, ctypes.c_double,
                                                 ctypes.POINTER(vp)]),
+        "b200jpg_batch_create_flip": (i32, [vp, ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), i32, i32, ctypes.c_uint,
+                                            ctypes.POINTER(SizeStruct), ctypes.POINTER(RectStruct), ctypes.POINTER(SizeStruct),
+                                            ctypes.POINTER(BoxStruct), ctypes.POINTER(RectStruct), i32, ctypes.c_double,
+                                            ctypes.POINTER(ctypes.c_uint8), ctypes.POINTER(vp)]),
         "b200jpg_draft_scale": (i32, [vp, ctypes.c_size_t, ctypes.c_uint32, ctypes.c_uint32]),
         "b200jpg_resample_coefficients": (i32, [ctypes.c_uint32, ctypes.c_uint32, i32, vp, vp, u64, ctypes.POINTER(ctypes.c_uint32)]),
         "b200jpg_resample_coefficients_box": (i32, [ctypes.c_uint32, ctypes.c_float, ctypes.c_float, ctypes.c_uint32, i32, vp, vp, u64,
@@ -118,6 +128,7 @@ def _load():
         "b200jpg_batch_decode": (i32, [vp, vp, vp]),
         "b200jpg_batch_decode_into": (i32, [vp, ctypes.POINTER(PlaneStruct), vp]),
         "b200jpg_batch_decode_into_ex": (i32, [vp, ctypes.POINTER(PlaneStruct), ctypes.POINTER(ConvertStruct), vp]),
+        "b200jpg_batch_decode_into_table": (i32, [vp, ctypes.POINTER(PlaneStruct), ctypes.POINTER(ConvertTableStruct), vp]),
         "b200jpg_batch_decode_entropy": (i32, [vp, vp]),
         "b200jpg_batch_reconstruct": (i32, [vp, vp, vp]),
         "b200jpg_batch_frame_status": (i32, [vp, i32]),
@@ -157,7 +168,8 @@ ABI_SYMBOLS = [
     "b200jpg_selftest_table_cache", "b200jpg_microbench_int32", "b200jpg_exif_orientation", "b200jpg_batch_frame_orientation",
     "b200jpg_batch_create_crop", "b200jpg_output_size", "b200jpg_batch_create_resize", "b200jpg_resample_coefficients",
     "b200jpg_batch_output_components", "b200jpg_colorspace", "b200jpg_batch_create_draft", "b200jpg_draft_scale",
-    "b200jpg_batch_create_resample", "b200jpg_resample_coefficients_box",
+    "b200jpg_batch_create_resample", "b200jpg_resample_coefficients_box", "b200jpg_batch_create_flip",
+    "b200jpg_batch_decode_into_table",
 ]
 
 
